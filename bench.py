@@ -2,9 +2,9 @@
 """bench.py — residuals/sec per Levenberg-Marquardt iteration of the continuous-time IMU-camera calibration solve.
 
 Contract (see DESIGN.md "Measurement"):
-  python bench.py --gpus N --steps K --warmup W [--impl reference] [--config 4]
+  python bench.py --gpus N --steps K --warmup W [--impl reference] [--config 4] [--dump-outputs DIR]
   * workload  = BASELINE.json configs[3]: ExtendedUnified, 3000 frames x 144 corners, 1 kHz IMU (the config the metric's
-                target is quoted on; fits one B200).  N > 1 shards the residuals by time slice, NCCL all-reduce of the
+                target is quoted on; fits one H100).  N > 1 shards the residuals by time slice, NCCL all-reduce of the
                 packed J^T J / J^T r buffer (strong scaling).
   * step      = ONE full LM iteration from the same initial state: residual + analytic Jacobian evaluation fused with the
                 J^T J / J^T r reduction, Jacobi scaling, damped banded+bordered LDL^T solve, manifold update, candidate
@@ -14,6 +14,9 @@ Contract (see DESIGN.md "Measurement"):
   * roofline  = the dominant kernel (vision residual/Jacobian kernel) timed alone with CUDA events on its stream.
   * cpu_baseline / --impl reference = the CPU restatement of the reference Ceres path (oracle/), all host threads, on a
                 bounded sample of the same workload (the real reference cannot be built offline: Ceres/Theia/Eigen absent).
+  * --dump-outputs DIR = after the timed steps, what the last timed step computed (the state a caller of lm_iterations reads
+                back: spline knots, T_i_c, line delay, the step's costs) as DIR/<name>.npy in float64.  The inputs are generated
+                from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -52,7 +55,7 @@ def algorithmic_bytes(ds, n_frames, n_corners, n_imu, n_cells):
 
 
 class ClockSampler:
-    """SM clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe: the same fields as the nvidia-smi clocks line).
+    """SM clocks / throttle reasons sampled DURING the timed region (the same fields as the nvidia-smi clocks line).
     Read through NVML inside this process (nvidia_ml_py, one handle opened before the timed region), ONE sample per step taken by the
     timing loop itself between two steps -- while the L2-flush fill of the next step keeps the GPU under load, outside the CUDA-event
     bracket of either step.  Every out-of-band sampler perturbed the number it was meant to vouch for: a freshly started `nvidia-smi -lms`
@@ -170,6 +173,18 @@ def run_reference(args, cfg):
             "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}, "gpu_launches": 0}
 
 
+def dump_outputs(path, handles, summaries):
+    """Writes what the last timed step left in each handle (one prefix per handle when there are several) as float64 .npy files."""
+    os.makedirs(path, exist_ok=True)
+    for k, (a, s) in enumerate(zip(handles, summaries)):
+        pre = f"seq{k}_" if len(handles) > 1 else ""
+        so3, r3, ba, bg = a.get_knots()
+        out = {"so3_knots": so3, "r3_knots": r3, "accel_bias_knots": ba, "gyro_bias_knots": bg, "T_i_c": a.get_T_i_c(),
+               "line_delay": np.array([a.get_line_delay()]), "costs": np.array([s.initial_cost, s.final_cost])}
+        for name, v in out.items():
+            np.save(os.path.join(path, pre + name + ".npy"), np.asarray(v, dtype=np.float64))
+
+
 def run_batch_of_eight(args):
     """BASELINE configs[4]: 8 independent calibration sequences (mixed camera models), replicas only — rank r owns sequences
     r, r+N, ...; no data-path collective.  step = one LM iteration on every owned sequence; value = all residuals / max-rank time."""
@@ -198,22 +213,25 @@ def run_batch_of_eight(args):
         if world > 1:
             dist.barrier(); torch.cuda.synchronize()
     sampler = ClockSampler(local) if rank == 0 else None
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=f"cuda:{local}")   # > L2 (126 MB): every round starts cold
-    total_ms, launches = 0.0, 0
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=f"cuda:{local}")   # > L2 (50 MB): every round starts cold
+    total_ms, launches, last = 0.0, 0, []
     for i in range(args.warmup + args.steps):       # warm-up rounds run exactly like timed ones, they are just not recorded
         if i == args.warmup and sampler: sampler.samples.clear()
         reset(); flush.fill_(float(i))
         if sampler: sampler.sample()                # under load (the fill is running), outside the wall-clock bracket of any round
         sync()
         t0 = time.perf_counter()
-        n_l = 0
+        n_l, last = 0, []
         for a in handles:
-            n_l += a.lm_iterations(1, FLAGS).gpu_launches     # each call ends with a stream synchronisation
+            last.append(a.lm_iterations(1, FLAGS))          # each call ends with a stream synchronisation
+            n_l += last[-1].gpu_launches
         torch.cuda.synchronize()
         if i >= args.warmup:
             total_ms += 1e3 * (time.perf_counter() - t0); launches += n_l
     sync()
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0 and world == 1:
+        dump_outputs(args.dump_outputs, handles, last)
     tot_res = nres
     if world > 1:
         t = torch.tensor([total_ms, float(nres)], dtype=torch.float64, device=f"cuda:{local}")
@@ -241,6 +259,7 @@ def main():
     ap.add_argument("--cpu-baseline-steps", type=int, default=3)
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step computed to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.config == 5:
@@ -285,7 +304,7 @@ def main():
     if world > 1:
         t = torch.tensor([nres_local], dtype=torch.int64, device=f"cuda:{local}"); dist.all_reduce(t); nres = int(t.item())
     so3, r3, ba, bg = api.get_knots(); T0 = api.get_T_i_c(); ld0 = api.get_line_delay()
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=f"cuda:{local}")   # 256 MiB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=f"cuda:{local}")   # 256 MiB > 50 MB L2
 
     def reset():
         api.set_knots(so3, r3, ba, bg); api.set_T_i_c(T0); api.set_line_delay(ld0)
@@ -324,6 +343,8 @@ def main():
     barrier()
     clocks = sampler.stop() if sampler else None
     gc.enable()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, [api], [summ])
     total_ms = float(np.sum(step_ms))
     if world > 1:
         t = torch.tensor([total_ms], dtype=torch.float64, device=f"cuda:{local}"); dist.all_reduce(t, op=dist.ReduceOp.MAX); total_ms = float(t.item())
@@ -338,45 +359,23 @@ def main():
     nv, na, ng = api.num_residuals()
     n_frames_local = len(ds["frame_t"]) if world == 1 else None
     jac_s, lin_s = summ.seconds_jacobian, summ.seconds_linear_solve
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback"
+    hbm_peak = 3350.0                               # GB/s, H100 SXM data sheet; a data-sheet ceiling, not a measured one
     roof = None
     if world == 1:
         ncells = len({(int(s // int(cfg.dt_so3_s * 1e9))) for s in ((api.imu_used()[0] * 1e9).astype(np.int64) - int(ds["frame_t"].min() * 1e9))})
         b_vis, b_imu = algorithmic_bytes(ds, len(ds["frame_t"]), nv // 2, na // 3, ncells)
         ach = b_vis / (ms_vis * 1e-3) / 1e9
-        # FP64 work of the vision kernel against the MEASURED FP64 ceilings of this chip (tools/fp64_peaks.cu -> profiles/r2_fp64_peaks.json):
-        # DMMA (mma.sync m8n8k4 f64) and DFMA share ONE FP64 pipe on B200 (mixed microbenchmark: DMMA 32.3 + DFMA 4.0 TF concurrently
-        # vs 37.1 / 33.9 alone), so the floor is the SUM of both instruction streams' pipe time, not the max.
-        rows = nv
-        dmma_flops = (rows / 4.0) * 21 * 512                      # 21 block products per 4 tile rows, 512 flop each
-        simt_instr_per_corner = 1170.0                            # FP64 SIMT warp-instructions per 32 corners (ncu: 15.8 M per 13 500 chunks)
-        simt_flops = (rows / 2.0) * simt_instr_per_corner * 2     # counted as FMAs
-        fp = {}
-        try:
-            fp = json.load(open(os.path.join(ROOT, "profiles", "r2_fp64_peaks.json")))
-        except Exception:
-            pass
-        dmma_peak = float(fp.get("dmma_m8n8k4_tflops_21acc", 37.0)); dfma_peak = float(fp.get("dfma_tflops", 34.0))
-        pipe_floor_ms = 1e3 * (dmma_flops / (dmma_peak * 1e12) + simt_flops / (dfma_peak * 1e12))
-        traffic, traffic_src = None, None
-        try:   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel from the committed ncu --set full capture (config 4 only)
-            if args.config == 4:
-                nc = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_summary.json")))["eval_tmem_kernel<6>"]
-                traffic = nc["dram_bytes_read"] + nc["dram_bytes_write"]; traffic_src = "profiles/r2_ncu_summary.json (ncu --set full, one launch)"
-        except Exception:
-            pass
-        roof = {"kernel": "vision_tmem_kernel<MODEL> (residual + analytic Jacobian + J^T J tile: persistent 12-warp CTAs, accumulators parked in TMEM)", "bound": "hbm", "achieved": ach,
-                "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+        # FP64 tensor-core work of the vision kernel (the J^T J tile products, counted from shapes) against the data-sheet FP64
+        # tensor-core rate of the H100 SXM; the SIMT FP64 work of the residual / Jacobian rows comes on top of it
+        dmma_flops = (nv / 4.0) * 21 * 512                        # 21 block products per 4 tile rows, 512 flop each
+        dmma_peak = 67.0
+        tensor_floor_ms = 1e3 * dmma_flops / (dmma_peak * 1e12)
+        roof = {"kernel": "eval_tmem_kernel<MODEL>, vision items (residual + analytic Jacobian + J^T J tile: persistent 6-warp CTAs, accumulators parked in shared memory)", "bound": "hbm", "achieved": ach,
+                "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "peak_source": "H100 SXM data sheet",
                 "algorithmic_bytes_per_launch": b_vis, "launch_ms": ms_vis,
-                "note": "arithmetic intensity >> FP64 ridge: the kernel is bound by the FP64 pipe (DMMA + DFMA share it), not by HBM (DESIGN.md); see fp64",
-                "fp64": {"tensor_tflops_issued": dmma_flops / (ms_vis * 1e-3) / 1e12, "simt_tflops_issued": simt_flops / (ms_vis * 1e-3) / 1e12,
-                         "measured_peak_dmma_tflops": dmma_peak, "measured_peak_dfma_tflops": dfma_peak, "peak_source": "profiles/r2_fp64_peaks.json (tools/fp64_peaks.cu on B200)" if fp else "nominal",
-                         "fp64_pipe_floor_ms": pipe_floor_ms, "frac_of_fp64_pipe": pipe_floor_ms / ms_vis},
+                "note": "arithmetic intensity >> FP64 ridge: the kernel is bound by FP64 issue, not by HBM; see fp64",
+                "fp64": {"tensor_tflops_issued": dmma_flops / (ms_vis * 1e-3) / 1e12, "peak_dmma_tflops": dmma_peak, "peak_source": "H100 SXM data sheet",
+                         "tensor_floor_ms": tensor_floor_ms, "frac_of_tensor_peak": tensor_floor_ms / ms_vis},
                 "imu_kernel": {"launch_ms": ms_imu, "algorithmic_bytes_per_launch": b_imu, "achieved": b_imu / (ms_imu * 1e-3) / 1e9},
                 "cost_only_eval_ms": ms_cost, "jacobian_eval_ms_in_step": 1e3 * jac_s / max(1, summ.jacobian_evaluations),
                 "linear_solve_ms_in_step": 1e3 * lin_s / max(1, summ.iterations)}

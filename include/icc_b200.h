@@ -1,11 +1,11 @@
-/* icc_b200.h — C-ABI of the B200-native continuous-time IMU-camera calibration solver.
+/* icc_b200.h — C-ABI of the H100-native continuous-time IMU-camera calibration solver.
  *
  * Drop-in boundary for the ONE hot path of urbste/OpenImuCameraCalibrator: everything below
  * OpenICC::core::ImuCameraCalibrator (include/OpenCameraCalibrator/core/imu_camera_calibrator.h:29-118)
  * and SplineTrajectoryEstimator<6> (core/spline_trajectory_estimator.h:31-218), i.e. what the reference
  * delegates to Ceres autodiff + sparse Cholesky + Theia camera projections.  The reference has no FFI layer;
  * each entry point cites the C++ member it replaces.  Plain pointers and sizes only, no torch / C++ types.
- * All arithmetic is FP64; all device work is hand-written sm_100a CUDA; there is NO CPU fallback:
+ * All arithmetic is FP64; all device work is hand-written sm_90a CUDA; there is NO CPU fallback:
  * every compute entry point fails with ICC_ERR_NO_DEVICE when no CUDA device is usable.
  *
  * Threading: one host thread per handle; one handle per GPU; handles are independent.

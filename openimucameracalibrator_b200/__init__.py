@@ -1,4 +1,4 @@
-"""openimucameracalibrator_b200 — B200-native (sm_100a) continuous-time IMU-camera calibration solver.
+"""openimucameracalibrator_b200 — H100-native (sm_90a) continuous-time IMU-camera calibration solver.
 
 Drop-in for the one hot path of urbste/OpenImuCameraCalibrator: the spline batch optimisation behind
 `applications/continuous_time_imu_to_camera_calibration.cc`.  The compute lives in `libicc_b200.so` (hand-written CUDA

@@ -4,7 +4,7 @@
 //                                           (src/io/write_camera_calibration.cc:33-133) -- what every other tool reads back
 //   <save_path_calib_dataset>.calibdata     the calibration dataset (views + board points)
 // The calibration itself -- CameraCalibrator::CalibrateCameraFromJson / RunCalibration (src/core/camera_calibrator.cc:131-389) --
-// runs on the B200 through icc_calibrate_camera; PrintResult (:391-458) is reproduced on stdout.
+// runs on the GPU through icc_calibrate_camera; PrintResult (:391-458) is reproduced on stdout.
 //
 // Deliberate differences: the .calibdata file is the JSON pose dataset this repository's tools exchange ({"views": {"<name>":
 // {"q_wc": [w,x,y,z], "p_wc": [...], "timestamp_s": t, "mean_reproj_error": e}}, "tracks": {...}}), not Theia's cereal binary

@@ -1,7 +1,7 @@
 // Drop-in host program for applications/continuous_time_imu_to_camera_calibration.cc of urbste/OpenImuCameraCalibrator:
 // same gflags names (app :38-80), same input files (UBJSON corners, camera / telemetry / init / bias / IMU-intrinsics /
 // spline-weighting JSON), same result JSON keys (app :247-332) and the two PLY files (app :335-364); everything between
-// "files parsed" and "results written" runs on the B200 through the C-ABI of include/icc_b200.h.
+// "files parsed" and "results written" runs on the GPU through the C-ABI of include/icc_b200.h.
 //
 // One deliberate difference: --input_pose_dataset.  The reference reads Theia's cereal-binary .calibdata
 // (theia::ReadReconstruction, app :95-97), which cannot be parsed without Theia.  This program reads the same content as

@@ -1,6 +1,6 @@
 // Drop-in host program for applications/estimate_camera_poses_from_checkerboard.cc of urbste/OpenImuCameraCalibrator
 // (SURVEY.md §8(f) row f1): same gflags names (app :34-41), same inputs (UBJSON corner file, camera calibration JSON); every
-// view's board pose is estimated on the B200 through icc_estimate_board_poses (PoseEstimator::EstimatePosesFromJson,
+// view's board pose is estimated on the GPU through icc_estimate_board_poses (PoseEstimator::EstimatePosesFromJson,
 // src/core/pose_estimator.cc:92-191).
 //
 // One deliberate difference: --output_pose_dataset is written as the JSON pose dataset that this repository's

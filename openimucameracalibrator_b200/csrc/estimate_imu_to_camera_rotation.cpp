@@ -1,7 +1,7 @@
 // Drop-in host program for applications/estimate_imu_to_camera_rotation.cc of urbste/OpenImuCameraCalibrator (SURVEY.md §8(f)
 // row f3): same gflags names (app :30-53), same telemetry / bias JSON inputs, same output JSON keys (app :175-185:
 // gyro_bias, gyro_to_camera_rotation{w,x,y,z}, time_offset_gyro_to_cam) -- the file the hot CLI reads as
-// --gyro_to_cam_initial_calibration.  The estimation runs on the B200 through icc_estimate_imu_to_camera_rotation
+// --gyro_to_cam_initial_calibration.  The estimation runs on the GPU through icc_estimate_imu_to_camera_rotation
 // (ImuToCameraRotationEstimator::EstimateCameraImuRotation, src/core/imu_to_camera_rotation_estimator.cc:116-274).
 //
 // One deliberate difference: --input_pose_calibration_dataset is the JSON pose dataset of this repository

@@ -1,4 +1,4 @@
-// C-ABI + host logic of the B200 calibration solver (see include/icc_b200.h for the boundary contract).
+// C-ABI + host logic of the H100 calibration solver (see include/icc_b200.h for the boundary contract).
 //
 // Host side mirrors, in its own structure, what the reference does on one thread before/around ceres::Solve:
 //   ImuCameraCalibrator::BatchInitSpline / InitializeGravity / Optimize   src/core/imu_camera_calibrator.cc:21-168
@@ -165,7 +165,7 @@ struct icc_handle {
   cudaStream_t stream = nullptr;
   EvalAux aux{};            // second stream + fork/join events: vision and IMU kernels of one evaluation run concurrently
   bool aux_ok = false;
-  int sm_count = 148;
+  int sm_count = 132;
   StateBufs st[2]; int cur = 0;
   HostBuf<unsigned char> small_pinned; DevBuf<int> d_idrange;
   void* arena_small(size_t bytes) { if (small_pinned.size() < bytes) small_pinned.resize(std::max<size_t>(bytes, 256), true); return small_pinned.pinned ? small_pinned.data() : nullptr; }
@@ -613,7 +613,7 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
 // =================================================================================================================
 extern "C" {
 
-const char* icc_version(void) { return "icc_b200 0.1 (sm_100a, fp64)"; }
+const char* icc_version(void) { return "icc_b200 0.1 (sm_90a, fp64)"; }
 
 void icc_default_solver_options(icc_solver_options* o) {
   o->function_tolerance = 1e-4; o->parameter_tolerance = 1e-7; o->gradient_tolerance = 1e-10;
@@ -1095,7 +1095,7 @@ icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
     CU(upload_staged(h, h->d_iwork, iw)); P.iwork = h->d_iwork.p; P.n_iwork = (int)iw.size();
     CU(upload_staged(h, h->d_cells, h->cells)); P.cells = h->d_cells.p;
     {
-      // Schedule of the persistent TMEM evaluation kernel (icc_eval_tmem.cu).  Both streams -- the corners of the non-empty frames and
+      // Schedule of the persistent evaluation kernel (icc_eval_tmem.cu).  Both streams -- the corners of the non-empty frames and
       // the samples of the knot-interval cells, units padded to a multiple of 4 = one m8n8k4 k-step -- are walked with the kernel's own
       // chunk rule (a chunk = up to 32 stream positions from at most two consecutive units) and cut into even per-warp runs.
       struct Walk { std::vector<int> pos, unit; int total = 0; };
@@ -1651,7 +1651,7 @@ icc_status icc_estimate_imu_to_camera_rotation(icc_handle* h, int n_views, const
   for (int d = 0; d < 3; ++d) Q.bias_in[d] = bias_in ? bias_in[d] : 0.0;
   // the bracket shrinks by the golden ratio per step whatever the data says, so the step count is known up to rounding
   int n_it = 0; { const double g = (1.0 + std::sqrt(5.0)) / 2.0; double a = -1.0, b = 1.0, c = b - (b - a) / g, d = a + (b - a) / g; while (std::fabs(c - d) > Q.tolerance && n_it < 200) { b = d; c = b - (b - a) / g; d = a + (b - a) / g; ++n_it; } }
-  launch_golden_section(Q, 1.0, n_it + 2, h->sm_count > 0 ? h->sm_count : 148, h->stream);
+  launch_golden_section(Q, 1.0, n_it + 2, h->sm_count > 0 ? h->sm_count : 132, h->stream);
   RotInitState S;
   CU(cudaMemcpyAsync(&S, d_state.p, sizeof S, cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
@@ -1720,7 +1720,7 @@ icc_status icc_spline_error_weighting(icc_handle* h, int n, const double* times,
   bool cuda_ok = true;
   auto removed = [&](double dt) -> double {      // signal_energy((1 - H) * Xhat)
     double e = 0.0;
-    launch_sew_residual_energy(n, d_xhat.p, fscale, dt, d_acc.p + 1, h->sm_count > 0 ? h->sm_count : 148, h->stream);
+    launch_sew_residual_energy(n, d_xhat.p, fscale, dt, d_acc.p + 1, h->sm_count > 0 ? h->sm_count : 132, h->stream);
     if (cudaMemcpyAsync(&e, d_acc.p + 1, sizeof(double), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess || cudaStreamSynchronize(h->stream) != cudaSuccess) cuda_ok = false;
     return e / (double)n;
   };

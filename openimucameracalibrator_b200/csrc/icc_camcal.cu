@@ -1,4 +1,4 @@
-// Camera intrinsic calibration (sm_100a): bundle adjustment of every view pose + ONE shared intrinsic vector (SURVEY.md §8(f) row f4).
+// Camera intrinsic calibration (sm_90a): bundle adjustment of every view pose + ONE shared intrinsic vector (SURVEY.md §8(f) row f4).
 //
 // Replaces what the reference delegates to theia::BundleAdjustViews (Ceres, DENSE/SPARSE_SCHUR, autodiff, CPU threads) in
 //   CameraCalibrator::RunCalibration            src/core/camera_calibrator.cc:131-219   (three stages, Huber 1.345)

@@ -1,7 +1,7 @@
 // Device camera-model "plugin surface": project a camera-frame point to pixels and return the analytic 2x3 Jacobian.
 //
 // Replaces theia::XCameraModel::CameraToPixelCoordinates<T>(intr, pt3, px) (pyTheiaSfM@69c3d37, external to
-// /root/reference) as dispatched at include/OpenCameraCalibrator/basalt_spline/ceres_calib_split_residuals.h:366-389,
+// the reference's repository) as dispatched at include/OpenCameraCalibrator/basalt_spline/ceres_calib_split_residuals.h:366-389,
 // where the derivative came from Ceres Jets.  Intrinsic index order = Theia's InternalParametersIndex (see icc_b200.h).
 // Return value = Theia's `bool` (false => the reference writes the constant 1e10 residual, quirk q12).
 #pragma once

@@ -1,4 +1,4 @@
-// Device-side FP64 Lie / spline helpers for the B200 calibration kernels.
+// Device-side FP64 Lie / spline helpers for the calibration kernels.
 //
 // What these replace in the reference (each evaluated there through ceres::Jet autodiff on CPU threads):
 //   SO3 exp/log/product      third_party/Sophus/sophus/so3.hpp:247-290,326-339,584-620  (same branches, eps = 1e-10)

@@ -1,4 +1,4 @@
-// Residual + analytic Jacobian evaluation kernels (sm_100a), fused with the J^T J / J^T r reduction.
+// Residual + analytic Jacobian evaluation kernels (sm_90a), fused with the J^T J / J^T r reduction.
 //
 // Replaces, for every board-corner observation and every accelerometer / gyroscope sample in parallel, what the
 // reference evaluates per residual block through ceres::DynamicAutoDiffCostFunction on CPU threads:
@@ -527,7 +527,7 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
   DeviceProblem P = P_in;
   if (S.board) P.board = S.board;   // the board points belong to the state (parameter blocks under SplineOptimFlags::POINTS)
   static int sm_count = 0;
-  if (!sm_count) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev); if (sm_count <= 0) sm_count = 148; }
+  if (!sm_count) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev); if (sm_count <= 0) sm_count = 132; }
   const size_t sm_vis = WARPS * sizeof(WarpCtx) + WARPS * 48 * LDJ * sizeof(double);
   const size_t sm_vis_k = WARPS * sizeof(WarpCtx) + WARPS * 56 * LDJ * sizeof(double);
   const size_t sm_imu_nb = WARPS * sizeof(WarpCtx) + WARPS * 40 * LDJ * sizeof(double);
@@ -542,7 +542,7 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
     if (e) return 1;
     attr_done = true;
   }
-  // Jacobian evaluations of the standard column sets run as items of the persistent TMEM-parked kernel (icc_eval_tmem.cu), which owns
+  // Jacobian evaluations of the standard column sets run as items of the persistent shared-memory-parking kernel (icc_eval_tmem.cu), which owns
   // every SM (one CTA each); whatever is not eligible (camera intrinsics / bias knots / IMU intrinsics free) follows on the same stream.
   const bool legacy_vision = getenv("ICC_VISION_LEGACY") != nullptr;   // A/B switch for profiling only (read per call)
   // size test: the persistent kernel pays off once every warp has a few chunks (BASELINE config 4: 7.6 vision / 1.8 IMU chunks per warp);

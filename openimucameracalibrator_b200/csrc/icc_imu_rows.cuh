@@ -6,7 +6,7 @@
 // right increments of the six SO(3) knots, the six R^3 knots and gravity (the column set of the hot CLI's stage 1 with the biases
 // fixed: the wider column sets -- bias knots, IMU intrinsics, time offset -- stay on imu_kernel of icc_eval.cu).
 // __host__ __device__ so that tests/test_host_device_math.py can check exactly this code against finite differences on the CPU;
-// the TMEM IMU kernel (icc_imu_tmem.cu) inlines it unchanged.
+// the persistent IMU items (icc_imu_tmem.cu) inlines it unchanged.
 //
 // As in icc_vision_rows.cuh: the three rows of a triple share one pass through the knot recursion (three independent dependency
 // chains per lane, shared window loads and per-increment coefficients), increment rotations are applied in Rodrigues form about

@@ -1,13 +1,13 @@
-// Accelerometer + gyroscope residuals, analytic Jacobians and J^T J / J^T r reduction: the IMU items of the persistent, TMEM-parked evaluation kernel (icc_eval_tmem.cu, sm_100a).
+// Accelerometer + gyroscope residuals, analytic Jacobians and J^T J / J^T r reduction: the IMU items of the persistent, shared-memory-parking evaluation kernel (icc_eval_tmem.cu, sm_90a).
 //
 // Same arithmetic contract as imu_kernel<true, 0> of icc_eval.cu (reference: AccelerationCostFunctorSplit<6> / GyroCostFunctorSplit<6>,
 // basalt_spline/ceres_calib_split_residuals.h:52-93,133-169, under Ceres autodiff + LieLocalParameterization) for the column set of
 // the hot CLI's stage 1 with fixed biases; the wider column sets (bias knots, IMU intrinsics, time offset) stay on imu_kernel.
 // Machine mapping = icc_vision_tmem.cu:
-//  * one persistent CTA per SM, 12 warps at <= 168 registers; the 15 + 6 FP64 tensor-core accumulator fragments of the two tiles
-//    (accelerometer 40 columns, gyroscope 24) are parked in tensor memory (tcgen05.st / tcgen05.ld) during the SIMT passes;
+//  * one persistent CTA per SM; the 15 + 6 FP64 tensor-core accumulator fragments of the two tiles (accelerometer 40 columns,
+//    gyroscope 24) are parked in the warp's shared-memory park (icc_park.cuh) during the SIMT passes;
 //  * the three rows of a sensor are evaluated in ONE pass (icc_imu_rows.cuh): row 0 goes to the warp's shared-memory tile, rows 1
-//    and 2 are parked in TMEM (43 / 38 doubles) and expanded into the same tile after the previous row has been contracted;
+//    and 2 are parked (43 / 38 doubles) and expanded into the same tile after the previous row has been contracted;
 //  * the samples of all knot-interval cells form ONE packed stream (cells padded to a multiple of 4 = one m8n8k4 k-step) cut into
 //    equal runs of 32-lane chunks, one run per warp: a 50-sample cell (1 kHz, dt = 0.05 s) no longer costs two passes with 18 of 32
 //    lanes idle in the second; a chunk may straddle two cells (two staged windows, lanes pick theirs).
@@ -15,14 +15,15 @@
 #include "icc_imu_rows.cuh"
 #include "icc_kernels.h"
 #include "icc_tile_common.cuh"
-#include "icc_tmem_gen.cuh"
+#include "icc_park.cuh"
 
 namespace icc {
 namespace tmi {
 
-constexpr int IW = 12;                       // warps per CTA
+constexpr int IW = 6;                        // warps per CTA
 constexpr int LDT = TILE_LD, TCOLS = TILE_COLS;
-constexpr int TM_ACCA = 0, TM_ACCG = 60, TM_PARK = 84;
+constexpr int TM_ACCA = 0, TM_ACCG = 30, TM_PARK = 42;   // park offsets in doubles per lane
+static_assert(TM_PARK + ACC_PARK <= PARK_DOUBLES && TM_PARK + GYR_PARK <= PARK_DOUBLES, "park layout");
 
 struct ImuSlot {
   ImuWin win[2];
@@ -61,13 +62,13 @@ __device__ __noinline__ void stage_cell(ImuSlot* slot, int w, ImuCellP C, ImuSta
 }
 
 // accelerometer tile part (rows [4 k0, 4 k1) of the chunk belong to one cell): rows 0, 1, 2 contracted one after the other
-ICC_D void accel_part(const NeLayout& L, const ImuConst& K, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, uint32_t ta, int lane) {
+ICC_D void accel_part(const NeLayout& L, const ImuConst& K, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, double* ta, int lane) {
   double acc[30];
   if (first) {
 #pragma unroll
     for (int i = 0; i < 30; ++i) acc[i] = 0.0;
   } else {
-    tmem_ld_d30(ta + TM_ACCA, acc);
+    park_ld(ta + 32 * TM_ACCA, acc);
   }
   tile_syrk<5>(tile, k0, k1, acc);
   const bool mine = lane >= 4 * k0 && lane < 4 * k1;
@@ -76,8 +77,8 @@ ICC_D void accel_part(const NeLayout& L, const ImuConst& K, double* __restrict__
     __syncwarp();
     {
       double so3[18], tail[7];                                   // tail = [q (4) | r1 | r2 | u_r3]
-      tmem_ld_d18(ta + TM_PARK + (k == 1 ? 0 : 36), so3);
-      tmem_ld_d7(ta + TM_PARK + 72, tail);
+      park_ld(ta + 32 * (TM_PARK + (k == 1 ? 0 : 18)), so3);
+      park_ld(ta + 32 * (TM_PARK + 36), tail);
       if (mine) imu_accel_row_expand(so3, q4(tail[0], tail[1], tail[2], tail[3]), k == 1 ? tail[4] : tail[5], tail[6], K, k, tile + lane, LDT);
     }
     __syncwarp();
@@ -85,16 +86,16 @@ ICC_D void accel_part(const NeLayout& L, const ImuConst& K, double* __restrict__
   }
   __syncwarp();
   if (last) tile_flush<5, 4>(L, gidx, acc);
-  else tmem_st_d30(ta + TM_ACCA, acc);
+  else park_st(ta + 32 * TM_ACCA, acc);
 }
 
-ICC_D void gyro_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, uint32_t ta, int lane) {
+ICC_D void gyro_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, double* ta, int lane) {
   double acc[12];
   if (first) {
 #pragma unroll
     for (int i = 0; i < 12; ++i) acc[i] = 0.0;
   } else {
-    tmem_ld_d12(ta + TM_ACCG, acc);
+    park_ld(ta + 32 * TM_ACCG, acc);
   }
   tile_syrk<3>(tile, k0, k1, acc);
   const bool mine = lane >= 4 * k0 && lane < 4 * k1;
@@ -103,8 +104,8 @@ ICC_D void gyro_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
     __syncwarp();
     {
       double so3[18], tail[2];
-      tmem_ld_d18(ta + TM_PARK + (k == 1 ? 0 : 36), so3);
-      tmem_ld_d2(ta + TM_PARK + 72, tail);
+      park_ld(ta + 32 * (TM_PARK + (k == 1 ? 0 : 18)), so3);
+      park_ld(ta + 32 * (TM_PARK + 36), tail);
       if (mine) {
         double* row = tile + lane;
 #pragma unroll
@@ -119,7 +120,7 @@ ICC_D void gyro_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
   }
   __syncwarp();
   if (last) tile_flush<3, 2>(L, gidx, acc);
-  else tmem_st_d12(ta + TM_ACCG, acc);
+  else park_st(ta + 32 * TM_ACCG, acc);
 }
 
 ICC_D void init_const(ImuConst* K, const DeviceProblem& P, const DeviceState& S) {
@@ -135,7 +136,7 @@ ICC_D void init_const(ImuConst* K, const DeviceProblem& P, const DeviceState& S)
 }
 
 // One item = one contiguous run of 32-lane chunks of the packed IMU sample stream, processed by one warp.
-ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst* K, ImuSlot* slot, double* __restrict__ tile, uint32_t ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
+ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst* K, ImuSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
   const bool lock = rounds > 0;
   ImuStageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.ba = S.ba; A.bg = S.bg; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_g = P.col_g;
   const double dto = S.glob[G_TOFF];          // time-offset increment [s] (0 unless the extension has been optimised)
@@ -186,14 +187,12 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst
 #pragma unroll
           for (int cc = 0; cc < ACC_PARK; ++cc) park[cc] = 0.0;
         }
-        tmem_st_d43(ta + TM_PARK, park);
+        park_st(ta + 32 * TM_PARK, park);
       }
-      tmem_wait_st();
       __syncwarp();
 #pragma unroll 1
       for (int part = 0; part < (nB ? 2 : 1); ++part)
         accel_part(L, *K, tile, part ? nA >> 2 : 0, part ? n >> 2 : nA >> 2, part ? true : fresh, part ? lastB : lastA, slot->gidxA[part ? cur ^ 1 : cur], ta, lane);
-      tmem_wait_st();
       __syncwarp();
       // ---- gyroscope ------------------------------------------------------------------------------------------------------
       if (lock) asm volatile("bar.sync %0, %1;" :: "r"(bar_id + 6), "r"(bar_n) : "memory");
@@ -213,16 +212,14 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst
 #pragma unroll
           for (int cc = 0; cc < GYR_PARK; ++cc) park[cc] = 0.0;
         }
-        tmem_st_d38(ta + TM_PARK, park);
+        park_st(ta + 32 * TM_PARK, park);
       }
-      tmem_wait_st();
       __syncwarp();
 #pragma unroll 1
       for (int part = 0; part < (nB ? 2 : 1); ++part)
         gyro_part(L, tile, part ? nA >> 2 : 0, part ? n >> 2 : nA >> 2, part ? true : fresh, part ? lastB : lastA, slot->gidxG[part ? cur ^ 1 : cur], ta, lane);
       fresh = false;
       if (nB) { ++c; cur ^= 1; endC = endB; }
-      tmem_wait_st();
       __syncwarp();
       pos += n;
     }

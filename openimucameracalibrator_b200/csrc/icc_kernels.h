@@ -25,7 +25,7 @@ struct DeviceState {
 };
 
 struct VisionWork { int frame, c_begin, c_end, pad; };
-// Packed corner stream of the TMEM vision kernel (icc_vision_tmem.cu): the non-empty frames are laid end to end, each padded to a
+// Packed corner stream of the persistent vision items (icc_vision_tmem.cu): the non-empty frames are laid end to end, each padded to a
 // multiple of four corners (one tensor-core k-step), and the stream is cut into one item per warp at 32-lane chunk boundaries, so
 // a chunk may take its first lanes from the end of one frame and the rest from the start of the next.
 struct VisFrame { int poff, c0, cn, s_so3, s_r3, pad; double u_so3, u_r3; };   // poff = padded stream offset; entry [n] is a sentinel
@@ -90,7 +90,7 @@ enum { SC_MODEL_CHANGE = 0, SC_STEP_SQ = 1, SC_X_SQ = 2, SC_CAND_COST = 3, SC_OK
 // `aux` (optional): a second stream + two events; the IMU kernel then runs concurrently with the vision kernel (fork / join
 // around the pair on `st`), which fills the partial last wave of either kernel.
 struct EvalAux { cudaStream_t stream; cudaEvent_t fork, join; };
-// Persistent TMEM-parked Jacobian evaluation, vision + IMU items in one launch (icc_eval_tmem.cu); non-zero on a launch error.
+// Persistent Jacobian evaluation, vision + IMU items in one launch (icc_eval_tmem.cu); non-zero on a launch error.
 // P.vitems[k] / P.iitems[k] is the run of global warp k; the two item types go out as two launches of the same kernel.
 int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st);
 int eval_tmem_warps();

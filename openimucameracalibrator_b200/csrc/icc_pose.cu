@@ -1,4 +1,4 @@
-// Per-view board pose estimation (sm_100a): the step that fills the pose dataset the hot CLI consumes (SURVEY.md §8(f) row f1).
+// Per-view board pose estimation (sm_90a): the step that fills the pose dataset the hot CLI consumes (SURVEY.md §8(f) row f1).
 //
 // Replaces, for every view in parallel, what the reference runs serially on the CPU in
 //   PoseEstimator::EstimatePosesFromJson      src/core/pose_estimator.cc:92-191

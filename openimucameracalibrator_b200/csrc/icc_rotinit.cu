@@ -1,4 +1,4 @@
-// IMU-to-camera rotation + time-offset initialiser (sm_100a): the step that produces `gyro_to_cam_calibration.json`, i.e. the
+// IMU-to-camera rotation + time-offset initialiser (sm_90a): the step that produces `gyro_to_cam_calibration.json`, i.e. the
 // T_i_c_init rotation and the time offset the hot CLI starts from (SURVEY.md §8(f) row f3).
 //
 // Replaces what the reference runs serially on the CPU in

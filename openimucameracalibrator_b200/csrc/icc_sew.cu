@@ -1,4 +1,4 @@
-// Spline Error Weighting (sm_100a): knot spacing + spline-fit variance from the spectrum of an IMU stream, i.e. the
+// Spline Error Weighting (sm_90a): knot spacing + spline-fit variance from the spectrum of an IMU stream, i.e. the
 // `spline_error_weighting_json` the hot CLI requires (SURVEY.md §8(f) row f2).
 //
 // Replaces python/sew.py:knot_spacing_and_variance (python/sew.py:86-147,150-234) as driven by python/get_sew_for_dataset.py:38-48:

@@ -1,4 +1,4 @@
-// Damped normal-equation solve + manifold update kernels (sm_100a).
+// Damped normal-equation solve + manifold update kernels (sm_90a).
 //
 // Replaces what ceres::Solve does between two Jacobian evaluations for the reference's spline problem
 // (SplineTrajectoryEstimator::Optimize, include/OpenCameraCalibrator/core/spline_trajectory_estimator.impl.h:254-276):
@@ -986,7 +986,7 @@ SolvePlan make_plan(const DeviceProblem& P) {
   static const int forced_chunks = env_int("ICC_SOLVER_CHUNKS", 0), leaf_cols = env_int("ICC_SOLVER_LEAF", 0);
   int Pn = 1;
   if (nk > 0 && kd > 0) {
-    // P = 2^k chunks give a complete elimination tree of k-1 reduction levels; measured on B200: ~0.45 us per leaf column
+    // P = 2^k chunks give a complete elimination tree of k-1 reduction levels
     // (forward + backward) against ~25 us per level  =>  pick the k that minimises the sum while leaves keep >= kd+1 columns
     double best = 1e300;
     for (int k = 0; k <= 7; ++k) {
@@ -1043,7 +1043,7 @@ size_t solve_workspace_doubles(const DeviceProblem& P) {
 
 void launch_compute_scale(const DeviceProblem& P, double* scale, int jacobi, double* scal, cudaStream_t st) {
   const int n = P.nk + P.nb;
-  int grid = (n + 255) / 256; if (grid > 148) grid = 148; if (grid < 1) grid = 1;
+  int grid = (n + 255) / 256; if (grid > 132) grid = 132; if (grid < 1) grid = 1;
   scale_kernel<<<grid, 256, 0, st>>>(P, scale, jacobi, scal);
   count_launch();
 }
@@ -1072,7 +1072,7 @@ int launch_solve(const DeviceProblem& P, const double* scale, SolveParams sp, do
     launch_pdl(backsub_kernel<true>, pl.P, NT, sC, st, P, pl, 0, workspace, (const double*)scal); count_launch();
   }
   const int n = P.nk + P.nb;
-  int grid = (n + 255) / 256; if (grid > 148) grid = 148; if (grid < 1) grid = 1;
+  int grid = (n + 255) / 256; if (grid > 132) grid = 132; if (grid < 1) grid = 1;
   launch_pdl(finish_kernel, grid, 256, 0, st, P, pl, scale, sp, workspace, delta, scal); count_launch();
   return cudaGetLastError() == cudaSuccess ? 0 : 2;
 }

@@ -1,4 +1,4 @@
-// Device helpers shared by the TMEM-parked residual kernels (icc_vision_tmem.cu, icc_imu_tmem.cu): the FP64 tensor-core symmetric
+// Device helpers shared by the persistent residual kernels (icc_vision_tmem.cu, icc_imu_tmem.cu): the FP64 tensor-core symmetric
 // rank-k update of a column-major shared-memory tile, and the scatter of the finished fragments into the packed banded + bordered
 // normal equations.
 #pragma once

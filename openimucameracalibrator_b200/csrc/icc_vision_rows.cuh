@@ -3,7 +3,7 @@
 // Reference: RSReprojectionCostFunctorSplit<6>::operator() (basalt_spline/ceres_calib_split_residuals.h:319-402) under
 // ceres::DynamicAutoDiffCostFunction x LieLocalParameterization; here the Jacobian is closed form (derivation: header of
 // icc_device_math.cuh).  Kept __host__ __device__ so that tests/test_host_device_math.py can compile exactly this code for the
-// CPU and check it against finite differences; the TMEM vision kernel (icc_vision_tmem.cu) inlines it unchanged.
+// CPU and check it against finite differences; the persistent vision items (icc_vision_tmem.cu) inlines it unchanged.
 //
 // What is new against the per-row recursion of icc_spline_chain.cuh (still used by the IMU kernels):
 //  * the x and the y row run through the SO(3) knot recursion TOGETHER (two independent dependency chains per lane, shared

@@ -1,17 +1,14 @@
-// Rolling-shutter reprojection residuals + analytic Jacobians + J^T J / J^T r reduction: the vision items of the persistent, TMEM-parked evaluation kernel (icc_eval_tmem.cu, sm_100a).
+// Rolling-shutter reprojection residuals + analytic Jacobians + J^T J / J^T r reduction: the vision items of the persistent, shared-memory-parking evaluation kernel (icc_eval_tmem.cu, sm_90a).
 //
 // Same arithmetic contract as vision_kernel<1> of icc_eval.cu (reference: RSReprojectionCostFunctorSplit<6>::operator(),
 // basalt_spline/ceres_calib_split_residuals.h:319-402, under Ceres autodiff + LieLocalParameterization), re-mapped to the machine:
 //
-//  * ONE persistent CTA per SM, 12 warps at <= 168 registers (three warps per scheduler instead of the two that 255 registers
-//    allowed).  What made 255 registers necessary was the co-existence of the 21 FP64 tensor-core accumulator fragments (84
-//    registers, live for a whole frame) with the per-corner spline chain.  Here the fragments are PARKED IN TENSOR MEMORY
-//    (tcgen05.st / tcgen05.ld, lane-private 32x32b shape; SASS STTM / LDTM) while a warp is in its SIMT phase, and only live in
-//    registers during the DMMA phases.  TMEM is otherwise idle on this path (tcgen05.mma has no FP64 kind), costs no shared
-//    memory and no L1, and 512 columns hold 12 warps x (84 accumulator + 72 row) columns.
+//  * ONE persistent CTA per SM.  The 21 FP64 tensor-core accumulator fragments (42 doubles per lane, live for a whole frame)
+//    would otherwise co-exist with the per-corner spline chain; here they are PARKED in the warp's lane-private shared-memory
+//    park (icc_park.cuh) while the warp is in its SIMT phase, and only live in registers during the DMMA phases.
 //  * Both rows of a corner are evaluated in ONE pass (icc_vision_rows.cuh): the x row goes to the warp's shared-memory tile, the
-//    y row (36 doubles, R^3 block factored) is parked in TMEM and expanded into the same tile after the x rows have been
-//    contracted.  Nothing of the spline chain survives a tensor-core phase, so nothing spills.
+//    y row (36 doubles, R^3 block factored) is parked and expanded into the same tile after the x rows have been contracted.
+//    Nothing of the spline chain survives a tensor-core phase, so nothing spills.
 //  * The corners of all frames form ONE packed stream (frames padded to a multiple of 4 = one m8n8k4 k-step) that is cut into
 //    equal runs of 32-lane chunks, one run per warp: no partial last wave, no half-empty chunk at the end of a 144-corner frame.
 //    A chunk may straddle two frames (two staged knot windows, lanes pick theirs); the k-steps of the first frame finish its
@@ -21,15 +18,15 @@
 #pragma once
 #include "icc_kernels.h"
 #include "icc_tile_common.cuh"
-#include "icc_tmem_gen.cuh"
+#include "icc_park.cuh"
 #include "icc_vision_rows.cuh"
 
 namespace icc {
 namespace tmv {
 
-constexpr int VW = 12;                 // warps per CTA
+constexpr int VW = 6;                  // warps per CTA
 constexpr int LDT = TILE_LD, TCOLS = TILE_COLS;   // 44 tile columns used
-constexpr int TM_ACC = 0, TM_YROW = 84;
+constexpr int TM_ACC = 0, TM_YROW = 42;          // park offsets in doubles per lane
 constexpr int NBLK = 21;               // upper block triangle of 6 x 6 blocks of 8 columns
 
 struct WarpSlot {
@@ -66,15 +63,15 @@ __device__ __noinline__ void stage_frame(WarpSlot* slot, int w, VisFrame F, Stag
 }
 
 // One tile part: rows [4 k0, 4 k1) of the chunk belong to one frame.
-//   first: the frame's tile starts here (accumulators zero) -- otherwise they are fetched from TMEM;
+//   first: the frame's tile starts here (accumulators zero) -- otherwise they are fetched from the park;
 //   last:  the frame's tile (or the item) ends here: scatter -- otherwise park the accumulators.
-ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, uint32_t ta, int lane) {
+ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, double* ta, int lane) {
   double acc[2 * NBLK];
   if (first) {
 #pragma unroll
     for (int i = 0; i < 2 * NBLK; ++i) acc[i] = 0.0;
   } else {
-    tmem_ld_d42(ta + TM_ACC, acc);
+    park_ld(ta + 32 * TM_ACC, acc);
   }
   tile_syrk<6>(tile, k0, k1, acc);                       // x rows
   __syncwarp();
@@ -82,12 +79,12 @@ ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
     const bool mine = lane >= 4 * k0 && lane < 4 * k1;
     double* yrow = tile + lane;
     double h[18];
-    tmem_ld_d18(ta + TM_YROW, h);
+    park_ld(ta + 32 * TM_YROW, h);
     if (mine) {
 #pragma unroll
       for (int c = 0; c < 18; ++c) yrow[c * LDT] = h[c];
     }
-    tmem_ld_d18(ta + TM_YROW + 36, h);            // [m_t 0..2 | Dp 3..5 | om 6..8 | ld 9 | r 10 | cc 11..16 | pad]
+    park_ld(ta + 32 * (TM_YROW + 18), h);       // [m_t 0..2 | Dp 3..5 | om 6..8 | ld 9 | r 10 | cc 11..16 | pad]
     if (mine) {
 #pragma unroll
       for (int j = 0; j < 6; ++j) {
@@ -105,7 +102,7 @@ ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
   if (last) {
     tile_flush<6, 4>(L, gidx, acc);
   } else {
-    tmem_st_d42(ta + TM_ACC, acc);
+    park_st(ta + 32 * TM_ACC, acc);
   }
 }
 
@@ -121,7 +118,7 @@ ICC_D void init_const(VisConst* K, const DeviceProblem& P, const DeviceState& S,
 
 // One item = one contiguous run of 32-lane chunks of the packed corner stream, processed by one warp.
 template <int MODEL>
-ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, uint32_t ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
+ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
   StageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_tic = P.col_tic; A.col_ld = P.col_ld;
   {
     int f = it.vf0, pos = it.pos_begin, cur = 0;
@@ -164,9 +161,8 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst
 #pragma unroll
           for (int c = 0; c < YR_N; ++c) yr[c] = 0.0;
         }
-        tmem_st_d36(ta + TM_YROW, yr);
+        park_st(ta + 32 * TM_YROW, yr);
       }
-      tmem_wait_st();
       __syncwarp();
       // ---- tensor-core passes: the rows of the frame that ends first, then (straddling chunk) the rows of the next frame --------
 #pragma unroll 1
@@ -178,7 +174,6 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst
       }
       fresh = false;
       if (nB) { ++f; cur ^= 1; endF = endB; }
-      tmem_wait_st();
       pos += n;
     }
   }

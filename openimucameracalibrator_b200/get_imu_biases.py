@@ -1,6 +1,6 @@
 """Drop-in for python/get_imu_biases.py of urbste/OpenImuCameraCalibrator: same command line (--input_json_path, --output_path,
 --gravity_const, --remove_sec), same telemetry JSON in, same bias JSON out ({"gyro_bias": {x,y,z}, "accl_bias": {x,y,z}}), which is what
-the hot CLI reads as --imu_bias_file and estimate_imu_to_camera_rotation as --imu_bias_estimate.  The stream reductions run on the B200
+the hot CLI reads as --imu_bias_file and estimate_imu_to_camera_rotation as --imu_bias_estimate.  The stream reductions run on the GPU
 through icc_estimate_imu_biases; there is no CPU fallback.
 
     python -m openimucameracalibrator_b200.get_imu_biases --input_json_path telemetry.json --output_path imu_bias.json

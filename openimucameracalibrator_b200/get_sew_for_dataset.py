@@ -1,7 +1,7 @@
 """Drop-in for python/get_sew_for_dataset.py of urbste/OpenImuCameraCalibrator (SURVEY.md §8(f) row f2): same command line
 (--input_json_path, --output_path, --q_so3, --q_r3), same telemetry JSON in (accelerometer, gyroscope, timestamps_ns, camera_fps),
 same spline_error_weighting JSON out ({"so3": {knot_spacing, weighting_factor, quality_factor}, "r3": {...}, "camera_fps"}), which is
-what the hot CLI reads as --spline_error_weighting_json.  The spectra and the knot-spacing searches run on the B200 through
+what the hot CLI reads as --spline_error_weighting_json.  The spectra and the knot-spacing searches run on the GPU through
 icc_spline_error_weighting (python/sew.py:knot_spacing_and_variance); there is no CPU fallback.
 
     python -m openimucameracalibrator_b200.get_sew_for_dataset --input_json_path telemetry.json --output_path sew.json

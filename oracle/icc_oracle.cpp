@@ -231,7 +231,7 @@ void lp_jacobian_se3(const double* T7, double J[7][6]) {
   for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) J[4 + i][j] = R.m[i][j];
 }
 
-// ceres::HomogeneousVectorParameterization(4) (Ceres 2.1 local_parameterization.cc; not in /root/reference -- restated):
+// ceres::HomogeneousVectorParameterization(4) (Ceres 2.1 local_parameterization.cc; not in the reference's repository -- restated):
 // Householder vector v, beta with (I - beta v v^T) x = |x| e_4 (internal::ComputeHouseholderVector); Jacobian = |x| / 2 x the first
 // three columns of H; Plus(x, d) = |x| H [sin(|d|/2) d / |d| ; cos(|d|/2)]  (Hartley & Zisserman A6.9.2-3).
 void householder4(const double* x, double v[4], double& beta) {
@@ -720,7 +720,7 @@ double mean_reproj_error(Oracle& o) {
 
 // -------------------------------------------------------------------------------------------------------------
 // Ceres inner iterations (Ruhe & Wedin "Algorithm II" as implemented by ceres::internal::CoordinateDescentMinimizer; Ceres is
-// not in /root/reference -- restated from the Ceres 2.1 sources as published):
+// not in the reference's repository -- restated from the Ceres 2.1 sources as published):
 //   * ordering (inner_iteration_ordering unset): recursive independent sets of the Hessian graph of the parameter blocks
 //     (vertices by increasing degree, greedy), reversed -- CoordinateDescentMinimizer::CreateOrdering;
 //   * for every set in order, every parameter block of the set is minimised ALONE over the residual blocks that depend on it,

@@ -10,7 +10,7 @@
 //   * uniform B-spline blending matrices  ~ include/OpenCameraCalibrator/basalt_spline/spline_common.h:67-133
 //   * cumulative SO(3) / R^3 spline eval  ~ include/OpenCameraCalibrator/basalt_spline/ceres_spline_helper.h:69-220
 //   * IMU triad model                     ~ include/OpenCameraCalibrator/utils/types.h:226-246,304-307
-//   * camera projections                  ~ TheiaSfM camera models (pyTheiaSfM@69c3d37, NOT in /root/reference):
+//   * camera projections                  ~ TheiaSfM camera models (pyTheiaSfM@69c3d37, NOT in the reference's repository):
 //                                           restated from the published model equations; call sites
 //                                           basalt_spline/ceres_calib_split_residuals.h:247-270,366-389
 //

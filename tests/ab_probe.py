@@ -1,4 +1,4 @@
-"""Developer probe (not a test): legacy vs TMEM vision kernel on the BASELINE configs -- parity of cost / gradient / LM step and timings."""
+"""Developer probe (not a test): legacy vs persistent vision kernel on the BASELINE configs -- parity of cost / gradient / LM step and timings."""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))

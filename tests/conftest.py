@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -38,7 +38,7 @@ def gpu_factory(cuda_lib):
 @pytest.fixture(params=["sized", "tmem_always"])
 def eval_path(request, monkeypatch):
     """Both Jacobian evaluation paths of launch_eval: the size-selected default (small problems: one warp per frame / cell) and the
-    persistent TMEM-parked kernel forced on (ICC_TMEM_ALWAYS), so that the small parity cases also pin the kernel BASELINE config 4 uses."""
+    persistent shared-memory-parking kernel forced on (ICC_TMEM_ALWAYS), so that the small parity cases also pin the kernel BASELINE config 4 uses."""
     if request.param == "tmem_always":
         monkeypatch.setenv("ICC_TMEM_ALWAYS", "1")
     else:

@@ -1,10 +1,10 @@
 """Golden vectors for the static IMU bias step, produced by the REFERENCE'S OWN code: python/get_imu_biases.py of
-urbste/OpenImuCameraCalibrator is plain NumPy, so its unmodified main() is run here (in the build container, where /root/reference
-is mounted) on deterministic telemetry files and inputs + outputs are committed as tests/golden/imu_bias_*.npz.
+urbste/OpenImuCameraCalibrator is plain NumPy, so its unmodified main() is run here (from a checkout of the reference named by
+$ICC_REFERENCE_ROOT) on deterministic telemetry files and inputs + outputs are committed as tests/golden/imu_bias_*.npz.
 
 The script imports matplotlib (plots that are commented out) and the container has none: an empty stand-in module is registered for
 the import to succeed -- no line of the reference is changed or skipped.
-Run from the repo root:  python tests/golden/make_imu_bias_golden.py
+Run from the repo root:  ICC_REFERENCE_ROOT=<reference checkout> python tests/golden/make_imu_bias_golden.py
 """
 import json
 import os
@@ -15,7 +15,7 @@ import types
 
 import numpy as np
 
-REF_PY = "/root/reference/python"
+REF_PY = os.path.join(os.environ["ICC_REFERENCE_ROOT"], "python")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

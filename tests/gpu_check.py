@@ -1,6 +1,6 @@
 """Ad-hoc GPU vs oracle comparison (developer tool; the real parity tests live in test_*.py)."""
-import sys, time, numpy as np
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests')
+import os, sys, time, numpy as np
+_root = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, _root); sys.path.insert(0, os.path.join(_root, 'tests'))
 from oracle_api import new_oracle
 from openimucameracalibrator_b200 import synthetic as syn, _capi as capi, calibrator
 from openimucameracalibrator_b200 import camera_models as cm

@@ -65,7 +65,7 @@ void hm_so3_chain(const double* knots, double u, const double* m_theta, double* 
   for (int c = 0; c < 18; ++c) rows[c] = Jt[c * LDJ];
   q_out[0] = ch.q.x; q_out[1] = ch.q.y; q_out[2] = ch.q.z; q_out[3] = ch.q.w;
 }
-// Both rows [J | r] of one corner exactly as the TMEM vision kernel computes them (icc_vision_rows.cuh): window staging
+// Both rows [J | r] of one corner exactly as the persistent vision kernel computes them (icc_vision_rows.cuh): window staging
 // (stage_frame_increment), vision_corner_rows (x row direct, y row in the parked layout), vision_yrow_expand.
 //   so3 = 6 x (x,y,z,w), r3 = 6 x 3, T_ic = (qx,qy,qz,qw,tx,ty,tz), rows = 2 x 44 (row-major), returns 1 when the projection succeeded
 int hm_vision_rows(int model, const double* intr10, int fov, const double* so3, const double* r3, double u_so3, double u_r3, const double* T_ic, double ld,
@@ -82,7 +82,7 @@ int hm_vision_rows(int model, const double* intr10, int fov, const double* so3, 
   return r0 == 1e10 ? 0 : 1;
 }
 void hm_sincos_small(double x, double* s, double* c) { sincos_small(x, s, c); }
-// The three accelerometer rows (3 x 40) and the three gyroscope rows (3 x 24) of one IMU sample exactly as the TMEM IMU kernel computes them
+// The three accelerometer rows (3 x 40) and the three gyroscope rows (3 x 24) of one IMU sample exactly as the persistent IMU kernel computes them
 // (icc_imu_rows.cuh): imu_accel_rows / imu_gyro_rows, then the parked rows expanded the way accel_part / gyro_part of icc_imu_tmem.cu do.
 //   Ma, Mg row-major 3x3; knots as in hm_vision_rows; ba, bg = 3 x 3 bias knots
 void hm_imu_rows(const double* so3, const double* r3, const double* ba, const double* bg, double u_so3, double u_r3, double u_ba, double u_bg, const double* Ma, const double* Mg,

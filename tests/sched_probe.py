@@ -1,4 +1,4 @@
-"""Developer probe (not a test): schedule variants of the unified TMEM evaluation kernel on BASELINE config 4 / 3."""
+"""Developer probe (not a test): schedule variants of the unified persistent evaluation kernel on BASELINE config 4 / 3."""
 import sys, os, subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 code = r'''

@@ -1,4 +1,4 @@
-"""Developer probe (not a test): lockstep groups / stagger of the TMEM evaluation kernel on config 4.  python tests/stagger_probe.py"""
+"""Developer probe (not a test): lockstep groups / stagger of the persistent evaluation kernel on config 4.  python tests/stagger_probe.py"""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,5 +1,5 @@
 """Residual sharding on real GPUs: 2 ranks over NCCL evaluate their time slices, all-reduce the packed normal equations on
-the solver stream and must follow exactly the single-GPU LM path.  Needs >= 2 visible GPUs (gpurun --gpus 2)."""
+the solver stream and must follow exactly the single-GPU LM path.  Needs >= 2 visible GPUs."""
 import os
 import sys
 
@@ -40,7 +40,7 @@ def test_two_gpu_sharded_lm_matches_single_gpu(tmp_path, gpu_factory, native):
     import torch
     import torch.multiprocessing as mp
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     from helpers import F_STAGE1, rel
     from openimucameracalibrator_b200 import _capi as capi, synthetic as syn
     port = 29600 + (os.getpid() % 2000)
@@ -60,7 +60,7 @@ def test_cli_gpus_flag_matches_single_gpu(tmp_path):
     import subprocess
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
     from openimucameracalibrator_b200 import camera_models as cm, io_formats as iof, synthetic as syn
     from test_cli_formats import _args

@@ -208,7 +208,7 @@ def test_device_so3_spline_chain_and_knot_jacobian(hm, spread):
     assert np.isfinite(q).all() and np.isfinite(rows).all() and np.isfinite(du)
 
 
-# ---- the joint x/y rows of the TMEM vision kernel ------------------------------------------------------------------------------------------
+# ---- the joint x/y rows of the persistent vision kernel ------------------------------------------------------------------------------------------
 _B6 = np.array([[1, -5, 10, -10, 5, -1], [26, -50, 20, 20, -20, 5], [66, 0, -60, 0, 30, -10], [26, 50, 20, -20, -20, 10], [1, 5, 10, 10, 5, -5], [0, 0, 0, 0, 0, 1]]) / 120.0
 
 

@@ -4,7 +4,7 @@ inner_iterations -- CoordinateDescentMinimizer over recursive independent sets +
 The CUDA product runs plain Levenberg-Marquardt.  What these tests pin: the refinement really is a descent step of the same
 objective, it heads for the SAME minimiser (so parity "at the true optimum" -- SURVEY §7 -- is the meaningful comparison), and at
 the reference's loose function_tolerance = 1e-4 BOTH stopping points sit further from that minimiser than they sit from each other
-times a small factor: the reference's own stopping point is not defined to 1e-4 (profiles/r2_inner_iterations.json has the
+times a small factor: the reference's own stopping point is not defined to 1e-4 (tools/inner_iteration_study.py prints the
 numbers for BASELINE configs 1-3)."""
 import ctypes as C
 
@@ -47,7 +47,7 @@ def test_reference_tolerance_leaves_the_stopping_point_undetermined_at_1e_4():
     """BASELINE config 1 with the reference's own tolerances: the stopping points with and without inner iterations differ by a few
     1e-3 relative in T_i_c (1-2 mm of the weakly observable lever arm) -- an order of magnitude above the north-star's 1e-4, while
     the GPU path reproduces the plain path to 1e-8 (tests/test_gpu_lm.py).  The numbers for configs 1-3, next to the tight-tolerance
-    runs, are in profiles/r2_inner_iterations.json (tools/inner_iteration_study.py)."""
+    runs, come from tools/inner_iteration_study.py."""
     ds = syn.make_dataset(syn.CONFIGS[1])
     a, _ = _oracle(ds, False); b, lib = _oracle(ds, True)
     sa, sb = a.optimize(50, F_STAGE1), b.optimize(50, F_STAGE1)

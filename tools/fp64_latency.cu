@@ -1,5 +1,5 @@
 // Microbenchmark: dependent-issue latencies (cycles) of the FP64 / shuffle / shared-memory / DMMA instructions that sit on the
-// solver's pivot and back-substitution recurrences.  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_latency fp64_latency.cu
+// solver's pivot and back-substitution recurrences.  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_latency fp64_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N 4096

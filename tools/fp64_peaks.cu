@@ -1,11 +1,11 @@
-// Microbenchmark: MEASURED FP64 throughput ceilings of one B200 -- the denominators of the "honest second roofline" of the
-// residual / solver kernels (bench.py reads profiles/r2_fp64_peaks.json produced from this tool's output):
+// Microbenchmark: measured FP64 throughput ceilings of one GPU -- the denominators of a second roofline of the residual / solver
+// kernels next to the data-sheet figures bench.py divides by:
 //   * DFMA (SIMT FP64 pipe): every thread runs 8 independent FMA chains;
-//   * DMMA (mma.sync.m8n8k4.f64, the only FP64 tensor shape sm_100a has; tcgen05.mma has no f64 kind): every warp runs 8 / 21
+//   * DMMA (mma.sync.m8n8k4.f64, the FP64 tensor shape the kernels use): every warp runs 8 / 21
 //     independent accumulator fragments (21 = the vision tile's upper block triangle);
 //   * both together (alternating warps), to see whether the two pipes overlap.
-// Timed with CUDA events over a grid that fills all SMs (148 x 8 CTAs x 256 threads), best of 5.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peaks fp64_peaks.cu && ./fp64_peaks > gpurun_out/fp64_peaks.json
+// Timed with CUDA events over a grid that fills all SMs (SM count x 8 CTAs x 256 threads), best of 5.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peaks fp64_peaks.cu && ./fp64_peaks > fp64_peaks.json
 #include <cstdio>
 #include <cuda_runtime.h>
 

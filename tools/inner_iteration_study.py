@@ -5,8 +5,8 @@ Runs the CPU oracle three ways on BASELINE configs (both stages of the hot CLI: 
   plain   : the LM path the CUDA product follows (function_tolerance 1e-4, parameter_tolerance 1e-7 -- impl.h:263-264),
   inner   : the same with Ceres' inner iterations restated (oracle/icc_oracle.cpp: inner_iterations),
   optimum : plain LM with tolerances 1e-12 (the true minimiser both paths head for).
-Prints one JSON line per config; profiles/r2_inner_iterations.json keeps the committed run.
-usage: python tools/inner_iteration_study.py 1 2 3 > profiles/r2_inner_iterations.json"""
+Prints one JSON line per config.
+usage: python tools/inner_iteration_study.py 1 2 3"""
 import ctypes as C, json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))

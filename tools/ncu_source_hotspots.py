@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Source lines of one kernel ranked by warp-stall samples, from an `ncu --set full --import-source on` report:
     ncu -i X.ncu-rep --page source --csv --print-source cuda,sass --kernel-name regex:NAME --launch-count 1 > src.csv
-    python tools/ncu_source_hotspots.py src.csv [top N] > profiles/rK_hotspots_NAME.txt
+    python tools/ncu_source_hotspots.py src.csv [top N] > hotspots_NAME.txt
 (the sample attributed to the instruction after a barrier is the time spent waiting AT the barrier)."""
 import collections, csv, sys
 rows = list(csv.reader(open(sys.argv[1])))

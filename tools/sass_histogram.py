@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-kernel SASS opcode histogram of the device objects of libicc_b200.so (cuobjdump -sass): makes the claims of DESIGN.md checkable
-from the repository -- FP64 tensor-core MMAs (DMMA) in the evaluation / solver kernels, tensor-memory parking (LDTM / STTM) and the TMEM
-allocator (UTCATOMSWS) in eval_tmem_kernel, no library kernels, no HMMA / UTC*MMA (tcgen05.mma has no FP64 kind).
-usage: python tools/sass_histogram.py > profiles/r2_sass_opcodes.txt"""
+from the repository -- FP64 tensor-core MMAs (DMMA) in the evaluation / solver kernels, shared-memory parking (LDS / STS) in
+eval_tmem_kernel, no local-memory spills (LDL / STL), no library kernels, no HMMA.
+usage: python tools/sass_histogram.py"""
 import collections, glob, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KEY = ["DMMA", "DFMA", "DMUL", "DADD", "LDTM", "STTM", "UTCATOMSWS", "REDG", "RED", "ATOMG", "LDS", "STS", "LDG", "STG", "LDL", "STL", "SHFL", "BAR", "MUFU", "HMMA", "UTCHMMA", "UTCQMMA", "UTMALDG", "UBLKCP"]
