@@ -10,6 +10,7 @@
 #include "../../include/icc_b200.h"
 #include "icc_camera.cuh"
 #include "icc_kernels.h"
+#include "icc_trust_region.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -515,7 +516,6 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
   auto mark = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, h->stream); ev.push_back(e); return (int)ev.size() - 1; };
   std::vector<std::pair<int, int>> jac_spans, lin_spans;
   double sc[SC_COUNT];
-  double x_cost = 0.0;
   auto jac = [&]() -> icc_status {
     const int a = mark();
     icc_status r = eval_jacobian(h, h->st[h->cur].view(), nullptr);
@@ -537,20 +537,21 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
     return ICC_OK;
   };
   if (n == 0) { if (out) *out = S; return ICC_OK; }
-  double radius = h->opt.initial_trust_region_radius, decrease_factor = 2.0;
-  int invalid = 0;
-  bool ne_valid = false, first = true;
-  S.termination = 0;
-  for (int it = 0; it < max_iters; ++it) {
+  TrOptions to;
+  to.function_tolerance = h->opt.function_tolerance; to.parameter_tolerance = h->opt.parameter_tolerance; to.gradient_tolerance = h->opt.gradient_tolerance;
+  to.initial_radius = h->opt.initial_trust_region_radius; to.max_radius = h->opt.max_trust_region_radius; to.min_radius = h->opt.min_trust_region_radius;
+  to.min_relative_decrease = h->opt.min_relative_decrease; to.min_diagonal = h->opt.min_lm_diagonal; to.max_diagonal = h->opt.max_lm_diagonal;
+  to.max_iterations = max_iters; to.max_invalid = h->opt.max_consecutive_invalid_steps; to.check_convergence = check_convergence ? 1 : 0;
+  TrustRegion T = tr_start(to);
+  while (tr_continue(T)) {
     // The Jacobian / normal equations are (re)built lazily at the top of the iteration that needs them, so that n
     // iterations cost n linear solves + n cost evaluations + one Jacobian evaluation per accepted step (and the first).
-    bool fresh_jacobian = false;
-    if (!ne_valid) {
+    const bool fresh_jacobian = T.jacobian_stale != 0;
+    if (fresh_jacobian) {
       rc = jac(); if (rc != ICC_OK) return rc;
-      rc = after_jacobian(first); if (rc != ICC_OK) return rc;
-      ne_valid = true; fresh_jacobian = true;
+      rc = after_jacobian(T.iterations == 0); if (rc != ICC_OK) return rc;
     }
-    SolveParams sp; sp.radius = radius; sp.min_diag = h->opt.min_lm_diagonal; sp.max_diag = h->opt.max_lm_diagonal; sp.jacobi_scaling = h->opt.jacobi_scaling;
+    SolveParams sp; sp.radius = T.radius; sp.min_diag = to.min_diagonal; sp.max_diag = to.max_diagonal; sp.jacobi_scaling = h->opt.jacobi_scaling;
     const int a = mark();
     { const int se = launch_solve(P, h->d_scale.p, sp, h->d_ws.p, h->d_delta.p, h->d_scal.p, h->stream);
       if (se == 1) return fail(h, ICC_ERR_UNSUPPORTED, "the border (bias knots + globals) is too wide for the solver's shared-memory plans");
@@ -563,40 +564,20 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
     rc = read_scalars(); if (rc != ICC_OK) return rc;
     trace.lap("run_lm: iteration");
     if (fresh_jacobian) {
-      x_cost = sc[SC_X_COST];
-      if (first) { S.initial_cost = x_cost; first = false; if (!std::isfinite(x_cost)) return fail(h, ICC_ERR_NUMERIC, "non-finite initial cost"); }
+      if (T.iterations == 0 && !std::isfinite(sc[SC_X_COST])) return fail(h, ICC_ERR_NUMERIC, "non-finite initial cost");
       // Ceres tests the gradient right after the Jacobian evaluation; the step computed above is simply discarded
-      if (check_convergence && sc[SC_GRAD_MAX] <= h->opt.gradient_tolerance) { S.termination = 3; break; }
+      if (!tr_jacobian(T, sc[SC_X_COST], sc[SC_GRAD_MAX])) break;
     }
-    ++S.iterations; ++S.cost_evaluations;
-    const double model_change = sc[SC_MODEL_CHANGE];
-    if (sc[SC_OK] == 0.0 || !(model_change > 0.0)) {          // invalid step (HandleInvalidStep)
-      if (++invalid >= h->opt.max_consecutive_invalid_steps) { S.termination = 4; break; }
-      radius /= decrease_factor; decrease_factor *= 2.0;
-      if (radius < h->opt.min_trust_region_radius) { S.termination = 4; break; }   // Ceres tests MinTrustRegionRadiusReached after every iteration
-      continue;
-    }
-    invalid = 0;
-    const double step_norm = std::sqrt(sc[SC_STEP_SQ]), x_norm = std::sqrt(sc[SC_X_SQ]);
-    double cand_cost = sc[SC_CAND_COST];
-    if (!std::isfinite(cand_cost)) cand_cost = 1.7976931348623157e308;
-    if (check_convergence && step_norm <= h->opt.parameter_tolerance * (x_norm + h->opt.parameter_tolerance)) { S.termination = 2; break; }
-    const double cost_change = x_cost - cand_cost;
-    if (check_convergence && std::fabs(cost_change) <= h->opt.function_tolerance * x_cost) { S.termination = 1; break; }
-    const double rel = cost_change / model_change;
-    if (rel > h->opt.min_relative_decrease) {               // HandleSuccessfulStep
-      ++S.successful_steps;
+    if (tr_step(T, sc[SC_OK] != 0.0, sc[SC_MODEL_CHANGE], std::sqrt(sc[SC_STEP_SQ]), std::sqrt(sc[SC_X_SQ])) && tr_candidate(T, sc[SC_CAND_COST])) {
       h->cur = cand; h->state_dirty_host = true; h->glob_host_current = false;
-      x_cost = cand_cost; ne_valid = false;
-      radius = radius / std::max(1.0 / 3.0, 1.0 - std::pow(2.0 * rel - 1.0, 3));
-      radius = std::min(h->opt.max_trust_region_radius, radius);
-      decrease_factor = 2.0;
-    } else {                                                  // StepRejected
-      radius /= decrease_factor; decrease_factor *= 2.0;
-      if (radius < h->opt.min_trust_region_radius) { S.termination = 4; break; }
     }
   }
-  if (first) { rc = jac(); if (rc != ICC_OK) return rc; rc = after_jacobian(true); if (rc != ICC_OK) return rc; rc = read_scalars(); if (rc != ICC_OK) return rc; x_cost = sc[SC_X_COST]; S.initial_cost = x_cost; }
+  S.termination = T.termination; S.iterations = S.cost_evaluations = T.iterations; S.successful_steps = T.successful;
+  S.initial_cost = T.initial_cost; S.final_cost = T.cost;
+  if (max_iters <= 0) {   // no iteration ran: the costs at x
+    rc = jac(); if (rc != ICC_OK) return rc; rc = after_jacobian(true); if (rc != ICC_OK) return rc; rc = read_scalars(); if (rc != ICC_OK) return rc;
+    S.initial_cost = S.final_cost = sc[SC_X_COST];
+  }
   if (P.col_pts >= 0 && S.successful_steps > 0) {   // both state buffers carry the accepted points again (runs without POINTS never copy them)
     const StateBufs& a = h->st[h->cur]; StateBufs& b = h->st[1 - h->cur];
     CU(cudaMemcpyAsync(b.pts.p, a.pts.p, a.pts.n * sizeof(double4), cudaMemcpyDeviceToDevice, h->stream));
@@ -604,7 +585,6 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
     CU(cudaMemcpyAsync(b.pjac.p, a.pjac.p, a.pjac.n * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
   }
   CU(cudaStreamSynchronize(h->stream));
-  S.final_cost = x_cost;
   auto span_s = [&](const std::vector<std::pair<int, int>>& v) { double tot = 0; for (auto& p : v) { float ms = 0; cudaEventElapsedTime(&ms, ev[p.first], ev[p.second]); tot += ms; } return tot * 1e-3; };
   S.seconds_jacobian = span_s(jac_spans); S.seconds_linear_solve = span_s(lin_spans);
   for (auto e : ev) cudaEventDestroy(e);
@@ -1894,59 +1874,38 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int W, int H, int nv, 
   // theia::BundleAdjustViews: Levenberg-Marquardt with Ceres' trust-region logic; one device->host read-back per iteration
   auto bundle_adjust = [&](unsigned mask, bool pose_free, int stage) -> icc_status {
     Q.intr_mask = mask; Q.pose_free = pose_free ? 1 : 0;
-    double radius = 1e4, decrease_factor = 2.0, x_cost = 0.0, sc[CC_SCAL_COUNT];
-    int invalid = 0; bool ne_valid = false, first = true;
-    int term = 0, iters = 0;
     if (Q.n_active == 0 || (mask == 0u && !pose_free)) { if (stage >= 0) S.termination[stage] = 3; return ICC_OK; }
-    for (int it = 0; it < o.max_num_iterations; ++it) {
-      bool fresh = false;
-      if (!ne_valid) {
+    TrOptions to = ceres_default_options();   // theia::BundleAdjustmentOptions: the Ceres defaults but for these
+    to.function_tolerance = o.function_tolerance; to.parameter_tolerance = o.parameter_tolerance; to.gradient_tolerance = o.gradient_tolerance;
+    to.max_iterations = o.max_num_iterations;
+    TrustRegion T = tr_start(to);
+    double sc[CC_SCAL_COUNT];
+    while (tr_continue(T)) {
+      const bool fresh = T.jacobian_stale != 0;
+      if (fresh) {
         CU(cudaMemsetAsync(d_sys.p, 0, (CC_PACK + 1) * sizeof(double), st));
         launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, st);
-        ne_valid = true; fresh = true;
       }
       CU(cudaMemsetAsync(d_red.p, 0, 66 * sizeof(double), st));
       CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
-      launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, first ? 1 : 0, radius, 1e-6, 1e32, d_dk.p, d_scal.p, st);
+      launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, T.iterations == 0 ? 1 : 0, T.radius, to.min_diagonal, to.max_diagonal, d_dk.p, d_scal.p, st);
       launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, st);
       CU(cudaMemcpyAsync(sc, d_scal.p, sizeof sc, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
       if (fresh) {
-        x_cost = sc[CC_X_COST];
-        if (first) { if (stage == 0) S.initial_cost = x_cost; if (!std::isfinite(x_cost)) return fail(h, ICC_ERR_NUMERIC, "non-finite initial cost"); }
-        if (sc[CC_GRAD_MAX] <= o.gradient_tolerance) { term = 3; first = false; break; }
+        if (T.iterations == 0 && !std::isfinite(sc[CC_X_COST])) return fail(h, ICC_ERR_NUMERIC, "non-finite initial cost");
+        if (!tr_jacobian(T, sc[CC_X_COST], sc[CC_GRAD_MAX])) break;
       }
-      first = false;
-      ++iters;
-      const double model_change = 0.5 * (sc[CC_D_DELTA] - sc[CC_G_DELTA]);
-      if (sc[CC_FAIL] != 0.0 || !(model_change > 0.0)) {
-        if (++invalid >= 5) { term = 4; break; }
-        radius /= decrease_factor; decrease_factor *= 2.0;
-        continue;
-      }
-      invalid = 0;
-      const double step_norm = std::sqrt(sc[CC_STEP_SQ]), x_norm = std::sqrt(sc[CC_X_SQ]);
-      double cand_cost = sc[CC_CAND_COST];
-      if (!std::isfinite(cand_cost)) cand_cost = 1.7976931348623157e308;
-      if (step_norm <= o.parameter_tolerance * (x_norm + o.parameter_tolerance)) { term = 2; break; }
-      const double cost_change = x_cost - cand_cost;
-      if (std::fabs(cost_change) <= o.function_tolerance * x_cost) { term = 1; break; }   // Ceres returns before accepting this step
-      const double rel = cost_change / model_change;
-      if (rel > 1e-3) {
-        cur = 1 - cur; x_cost = cand_cost; ne_valid = false;
-        radius = std::min(1e16, radius / std::max(1.0 / 3.0, 1.0 - std::pow(2.0 * rel - 1.0, 3)));
-        decrease_factor = 2.0;
-      } else {
-        radius /= decrease_factor; decrease_factor *= 2.0;
-        if (radius < 1e-32) { term = 4; break; }
-      }
+      if (tr_step(T, sc[CC_FAIL] == 0.0, 0.5 * (sc[CC_D_DELTA] - sc[CC_G_DELTA]), std::sqrt(sc[CC_STEP_SQ]), std::sqrt(sc[CC_X_SQ])) && tr_candidate(T, sc[CC_CAND_COST]))
+        cur = 1 - cur;
     }
     // both state copies must agree on everything outside the last step (inactive views never move; the intrinsics / poses of
     // a rejected candidate are stale): bring the spare copy back to the current state
     CU(cudaMemcpyAsync(d_q[1 - cur].p, d_q[cur].p, 4 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
     CU(cudaMemcpyAsync(d_c[1 - cur].p, d_c[cur].p, 3 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
     CU(cudaMemcpyAsync(d_k[1 - cur].p, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (stage >= 0) { S.final_cost[stage] = x_cost; S.iterations[stage] = iters; S.termination[stage] = term; } else S.init_iterations = iters;
+    if (stage == 0) S.initial_cost = T.initial_cost;
+    if (stage >= 0) { S.final_cost[stage] = T.cost; S.iterations[stage] = T.iterations; S.termination[stage] = T.termination; } else S.init_iterations = T.iterations;
     return ICC_OK;
   };
   auto finish = [&](bool success) -> icc_status {

@@ -36,7 +36,6 @@ namespace {
 
 using simu::Dual;
 using simu::LmState;
-using simu::LmOptions;
 
 constexpr int kMult = 10;          // threshold multipliers 1..10 (static_imu_calibrator.cc:83)
 constexpr int kThreads = 256;
@@ -206,7 +205,7 @@ struct AccFitArgs {
   int ns, use_means;
   double g_mag;
   double x0[9];
-  LmOptions o;
+  TrOptions o;
   double* out;             // per multiplier: x[9], initial cost, final cost, iterations, termination, successful steps
 };
 constexpr int kAccOut = 14, kSums = 55;   // 45 (upper triangle of J^T J) + 9 (J^T r) + cost
@@ -280,7 +279,7 @@ __global__ void __launch_bounds__(kThreads) acc_fit_kernel(AccFitArgs A) {
   if (threadIdx.x == 0) {
     double* o = A.out + (size_t)m * kAccOut;
     for (int p = 0; p < 9; ++p) o[p] = L.x[p];
-    o[9] = L.initial_cost; o[10] = L.cost; o[11] = L.iterations; o[12] = L.termination; o[13] = L.successful;
+    o[9] = L.T.initial_cost; o[10] = L.T.cost; o[11] = L.T.iterations; o[12] = L.T.termination; o[13] = L.T.successful;
   }
 }
 
@@ -448,7 +447,7 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
       interval_mean_kernel<<<((int)all.size() + 127) / 128, 128, 0, st>>>((int)all.size(), d_all.p, d_acc.p, 0, none, d_means.p); count_launch();
     }
     A.acc = d_acc.p; A.kept = d_all.p; A.means = d_means.p; A.ns = o.interval_n_samples; A.use_means = o.acc_use_means ? 1 : 0; A.g_mag = o.g_mag;
-    memcpy(A.x0, x0, sizeof x0); A.o = simu::ceres_default_options(); A.out = d_fit.p;
+    memcpy(A.x0, x0, sizeof x0); A.o = ceres_default_options(); A.out = d_fit.p;
     acc_fit_kernel<<<kMult, kThreads, 0, st>>>(A); count_launch();
     SCU(cudaMemcpyAsync(fit_out.data(), d_fit.p, fit_out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
     SCU(cudaStreamSynchronize(st));
@@ -543,13 +542,13 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
     };
     icc_status rc = eval(x); if (rc != ICC_OK) return rc;
     LmState L;
-    simu::lm_start(L, simu::ceres_default_options(), np, x, cost, H, g);
+    simu::lm_start(L, ceres_default_options(), np, x, cost, H, g);
     while (simu::lm_propose(L)) {
       rc = eval(L.xc); if (rc != ICC_OK) return rc;
       simu::lm_consider(L, cost, H, g);
     }
     for (int p = 0; p < 12; ++p) x[p] = L.x[p];
-    S.gyro_initial_cost = L.initial_cost; S.gyro_final_cost = L.cost; S.gyro_iterations = L.iterations; S.gyro_termination = L.termination;
+    S.gyro_initial_cost = L.T.initial_cost; S.gyro_final_cost = L.T.cost; S.gyro_iterations = L.T.iterations; S.gyro_termination = L.T.termination;
   }
   for (int p = 0; p < 9; ++p) gyr_out[p] = x[p];
   for (int d = 0; d < 3; ++d) bias_out[d] = gbias[d] + x[9 + d];                                  // :320-331

@@ -15,6 +15,7 @@
 // multiplication.
 #pragma once
 #include "icc_device_math.cuh"
+#include "icc_trust_region.cuh"
 
 namespace icc {
 namespace simu {
@@ -160,61 +161,41 @@ ICC_HD void transition_residual(const T P[16], const double g0[3], const double 
   for (int i = 0; i < 3; ++i) r[i] = ((R[i] * cst<T>(g0[0]) + R[3 + i] * cst<T>(g0[1])) + R[6 + i] * cst<T>(g0[2])) - cst<T>(g1[i]);
 }
 
-// ---- Levenberg-Marquardt with Ceres' TrustRegionMinimizer semantics (the same schedule as the oracle's lm_solve) ---------------
-// Dense, up to 12 unknowns; inactive unknowns (i >= n) stay at zero.  Usage:
-//   lm_start(L, cost, H, g);  while (lm_propose(L)) { evaluate at L.xc -> (c, Hc, gc); lm_consider(L, c, Hc, gc); }
-struct LmOptions {
-  double function_tolerance, gradient_tolerance, parameter_tolerance, initial_radius, max_radius, min_radius, min_relative_decrease,
-      min_diagonal, max_diagonal;
-  int max_iterations, max_invalid;
-};
-ICC_HD LmOptions ceres_default_options() {   // ceres::Solver::Options defaults (Ceres 2.1, solver.h)
-  LmOptions o;
-  o.function_tolerance = 1e-6; o.gradient_tolerance = 1e-10; o.parameter_tolerance = 1e-8; o.initial_radius = 1e4; o.max_radius = 1e16;
-  o.min_radius = 1e-32; o.min_relative_decrease = 1e-3; o.min_diagonal = 1e-6; o.max_diagonal = 1e32; o.max_iterations = 50; o.max_invalid = 5;
-  return o;
-}
-
+// ---- Levenberg-Marquardt: the dense step of Ceres' LevenbergMarquardtStrategy under the shared trust-region controller ----------
+// Up to 12 unknowns; inactive unknowns (i >= n) stay at zero.  Usage:
+//   lm_start(L, options, n, x0, cost, H, g);  while (lm_propose(L)) { evaluate at L.xc -> (c, Hc, gc); lm_consider(L, c, Hc, gc); }
 struct LmState {
-  LmOptions o;
+  TrustRegion T;   // T.cost is the cost at x
   int n;
-  double x[12], xc[12], scale[12], diag[12], H[12][12], g[12], cost, initial_cost, model_change, radius, decrease_factor;
-  int iterations, successful, invalid, termination;   // termination: -1 running, icc_summary codes otherwise
-  int reuse_diagonal, check_gradient;
+  double x[12], xc[12], scale[12], H[12][12], g[12];
 };
 
 ICC_HD double lm_grad_max(const LmState& L) { double m = 0.0; for (int i = 0; i < L.n; ++i) m = fmax(m, fabs(L.g[i])); return m; }
 
-ICC_HD void lm_start(LmState& L, const LmOptions& o, int n, const double x0[12], double cost, const double H[12][12], const double g[12]) {
-  L.o = o; L.n = n;
+ICC_HD void lm_start(LmState& L, const TrOptions& o, int n, const double x0[12], double cost, const double H[12][12], const double g[12]) {
+  L.T = tr_start(o); L.T.cost = cost;   // handed to tr_jacobian with the gradient by the first lm_propose
+  L.n = n;
   for (int i = 0; i < 12; ++i) {
-    L.x[i] = i < n ? x0[i] : 0.0; L.xc[i] = L.x[i]; L.g[i] = i < n ? g[i] : 0.0; L.diag[i] = 0.0;
+    L.x[i] = i < n ? x0[i] : 0.0; L.xc[i] = L.x[i]; L.g[i] = i < n ? g[i] : 0.0;
     for (int j = 0; j < 12; ++j) L.H[i][j] = (i < n && j < n) ? H[i][j] : 0.0;
     L.scale[i] = i < n ? 1.0 / (1.0 + ::sqrt(L.H[i][i])) : 0.0;     // Jacobi scaling, fixed at the first evaluation
   }
-  L.cost = cost; L.initial_cost = cost; L.model_change = 0.0; L.radius = o.initial_radius; L.decrease_factor = 2.0;
-  L.iterations = 0; L.successful = 0; L.invalid = 0; L.termination = -1; L.reuse_diagonal = 0; L.check_gradient = 1;
-}
-
-ICC_HD void lm_shrink(LmState& L) {
-  L.radius = L.radius / L.decrease_factor; L.decrease_factor *= 2.0; L.reuse_diagonal = 1;
-  if (L.radius < L.o.min_radius) L.termination = 4;
 }
 
 // Runs iterations until a candidate L.xc needs its cost (returns true) or the minimiser stops (returns false).
 ICC_HD bool lm_propose(LmState& L) {
   const int n = L.n;
-  while (L.termination < 0) {
-    if (L.iterations >= L.o.max_iterations) { L.termination = 0; break; }
-    if (L.check_gradient) { L.check_gradient = 0; if (lm_grad_max(L) <= L.o.gradient_tolerance) { L.termination = 3; break; } }
-    ++L.iterations;
+  TrustRegion& T = L.T;
+  while (tr_continue(T)) {
+    // x and its Jacobian came with the evaluation that accepted them (or lm_start's); the gradient test comes after the iteration limit
+    if (T.jacobian_stale && !tr_jacobian(T, T.cost, lm_grad_max(L))) break;
     double A[12][12], y[12];
     for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) A[i][j] = (i < n && j < n) ? L.H[i][j] * L.scale[i] * L.scale[j] : (i == j ? 1.0 : 0.0);
-    if (!L.reuse_diagonal) for (int i = 0; i < n; ++i) L.diag[i] = fmin(fmax(A[i][i], L.o.min_diagonal), L.o.max_diagonal);
     double Hs_y[12], gs[12];
     for (int i = 0; i < 12; ++i) { gs[i] = i < n ? L.scale[i] * L.g[i] : 0.0; y[i] = -gs[i]; }
+    // LM diagonal, clamped; Ceres reuses it after a failed step, which is the same value: H and the scaling have not changed
     double M[12][12];
-    for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) M[i][j] = A[i][j] + ((i == j && i < n) ? L.diag[i] / L.radius : 0.0);
+    for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) M[i][j] = A[i][j] + ((i == j && i < n) ? fmin(fmax(A[i][i], T.o.min_diagonal), T.o.max_diagonal) / T.radius : 0.0);
     bool ok = true;
     {   // Cholesky solve M y = -gs
       for (int j = 0; j < 12; ++j) {
@@ -231,36 +212,16 @@ ICC_HD bool lm_propose(LmState& L) {
     double yg = 0.0, yHy = 0.0;
     for (int i = 0; i < n; ++i) { double s = 0.0; for (int j = 0; j < n; ++j) s += A[i][j] * y[j]; Hs_y[i] = s; }
     for (int i = 0; i < n; ++i) { yg += y[i] * gs[i]; yHy += y[i] * Hs_y[i]; }
-    L.model_change = -yg - 0.5 * yHy;
-    if (!ok || !(L.model_change > 0.0)) {
-      if (++L.invalid >= L.o.max_invalid) { L.termination = 4; break; }
-      lm_shrink(L);
-      continue;
-    }
-    L.invalid = 0;
     double step_sq = 0.0, x_sq = 0.0;
     for (int i = 0; i < n; ++i) { const double dx = y[i] * L.scale[i]; L.xc[i] = L.x[i] + dx; step_sq += dx * dx; x_sq += L.x[i] * L.x[i]; }
-    const double x_norm = ::sqrt(x_sq);
-    if (::sqrt(step_sq) <= L.o.parameter_tolerance * (x_norm + L.o.parameter_tolerance)) { L.termination = 2; break; }
-    return true;
+    if (tr_step(T, ok, -yg - 0.5 * yHy, ::sqrt(step_sq), ::sqrt(x_sq))) return true;
   }
   return false;
 }
 
 ICC_HD void lm_consider(LmState& L, double c, const double H[12][12], const double g[12]) {
-  if (!(c <= 1.7976931348623157e308)) c = 1.7976931348623157e308;   // non-finite candidate cost: a failed step
-  const double change = L.cost - c;
-  if (fabs(change) <= L.o.function_tolerance * L.cost) { L.termination = 1; return; }
-  const double rho = change / L.model_change;
-  if (rho > L.o.min_relative_decrease) {
-    ++L.successful;
-    for (int i = 0; i < L.n; ++i) { L.x[i] = L.xc[i]; L.g[i] = g[i]; for (int j = 0; j < L.n; ++j) L.H[i][j] = H[i][j]; }
-    L.cost = c;
-    L.radius = fmin(L.o.max_radius, L.radius / fmax(1.0 / 3.0, 1.0 - ::pow(2.0 * rho - 1.0, 3.0)));
-    L.decrease_factor = 2.0; L.reuse_diagonal = 0; L.check_gradient = 1;
-  } else {
-    lm_shrink(L);
-  }
+  if (!tr_candidate(L.T, c)) return;
+  for (int i = 0; i < L.n; ++i) { L.x[i] = L.xc[i]; L.g[i] = g[i]; for (int j = 0; j < L.n; ++j) L.H[i][j] = H[i][j]; }
 }
 
 }  // namespace simu

@@ -1994,7 +1994,7 @@ CamCalStage camcal_bundle_adjust(CamCal& C, unsigned mask, bool pose_free, const
     }
     double model_change = 0.0; const bool solved = dense_cholesky_solve(n, A, b);
     if (solved) { double gd = 0, dd = 0; for (int i = 0; i < n; ++i) { gd += g[i] * b[i]; dd += D[i] * b[i] * b[i]; } model_change = 0.5 * (dd - gd); }
-    if (!solved || !(model_change > 0.0)) { if (++invalid >= 5) { R.termination = 4; break; } radius /= decrease_factor; decrease_factor *= 2.0; continue; }
+    if (!solved || !(model_change > 0.0)) { if (++invalid >= 5) { R.termination = 4; break; } radius /= decrease_factor; decrease_factor *= 2.0; if (radius < 1e-32) { R.termination = 4; break; } continue; }
     invalid = 0;
     std::vector<double> ext = C.ext; double k[10]; memcpy(k, C.k, sizeof k);
     double step_sq = 0, x_sq = 0;

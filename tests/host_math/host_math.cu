@@ -8,6 +8,7 @@
 #include "../../openimucameracalibrator_b200/csrc/icc_rotinit_math.cuh"
 #include "../../openimucameracalibrator_b200/csrc/icc_small_linalg.cuh"
 #include "../../openimucameracalibrator_b200/csrc/icc_points_math.cuh"
+#include "../../openimucameracalibrator_b200/csrc/icc_trust_region.cuh"
 
 using namespace icc;
 
@@ -132,3 +133,24 @@ void hm_quat_from_columns(const double* R9 /* row-major */, double* q) {
 // ceres::HomogeneousVectorParameterization(4) of a board point exactly as icc_points.cu uses it (icc_points_math.cuh)
 extern "C" void hm_points_prepare(const double* x4, double* board4, double* jac12) { icc::points_prepare(x4, board4, jac12); }
 extern "C" void hm_points_plus(const double* x4, const double* d3, double* out4) { icc::points_plus(x4, d3, out4); }
+
+// ---- the trust-region controller of every LM driver (icc_trust_region.cuh), on an opaque buffer of hm_tr_size() bytes ------------------
+//   d = function, parameter, gradient tolerance, initial, max, min radius, min relative decrease; i = max iterations, max invalid, check convergence
+//   state = radius, decrease factor, cost, initial cost, invalid, iterations, successful, termination, jacobian stale
+extern "C" {
+int hm_tr_size() { return (int)sizeof(icc::TrustRegion); }
+void hm_tr_start(void* t, const double* d, const int* i) {
+  icc::TrOptions o = icc::ceres_default_options();
+  o.function_tolerance = d[0]; o.parameter_tolerance = d[1]; o.gradient_tolerance = d[2]; o.initial_radius = d[3]; o.max_radius = d[4]; o.min_radius = d[5];
+  o.min_relative_decrease = d[6]; o.max_iterations = i[0]; o.max_invalid = i[1]; o.check_convergence = i[2];
+  *(icc::TrustRegion*)t = icc::tr_start(o);
+}
+int hm_tr_continue(void* t) { return icc::tr_continue(*(icc::TrustRegion*)t) ? 1 : 0; }
+int hm_tr_jacobian(void* t, double cost, double grad_max) { return icc::tr_jacobian(*(icc::TrustRegion*)t, cost, grad_max) ? 1 : 0; }
+int hm_tr_step(void* t, int valid, double model_change, double step_norm, double x_norm) { return icc::tr_step(*(icc::TrustRegion*)t, valid != 0, model_change, step_norm, x_norm) ? 1 : 0; }
+int hm_tr_candidate(void* t, double cand_cost) { return icc::tr_candidate(*(icc::TrustRegion*)t, cand_cost) ? 1 : 0; }
+void hm_tr_state(const void* t, double* s) {
+  const icc::TrustRegion& T = *(const icc::TrustRegion*)t;
+  s[0] = T.radius; s[1] = T.decrease_factor; s[2] = T.cost; s[3] = T.initial_cost; s[4] = T.invalid; s[5] = T.iterations; s[6] = T.successful; s[7] = T.termination; s[8] = T.jacobian_stale;
+}
+}

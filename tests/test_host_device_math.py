@@ -1,7 +1,8 @@
 """The product's own __host__ __device__ math (csrc/icc_camera.cuh, csrc/icc_device_math.cuh -- the functions every CUDA kernel
 inlines) compiled for the CPU and checked without a GPU: camera projections against the independent NumPy models, both closed-form
 Jacobians (point 2x3, intrinsics 2xK) against central finite differences for all seven models, SO(3) exp / log / Jr^-1 identities, and
-the spline blending polynomials against the reference's blending matrices (SURVEY.md §8(a2) known answers) and their own derivatives."""
+the spline blending polynomials against the reference's blending matrices (SURVEY.md §8(a2) known answers) and their own derivatives,
+and the trust-region controller of every LM driver (csrc/icc_trust_region.cuh) against a Python statement of Ceres' rules."""
 import ctypes
 import os
 import subprocess
@@ -20,7 +21,7 @@ DP = ctypes.POINTER(ctypes.c_double)
 
 @pytest.fixture(scope="module")
 def hm():
-    hdrs = [os.path.join(HERE, "..", "openimucameracalibrator_b200", "csrc", f) for f in ("icc_camera.cuh", "icc_device_math.cuh", "icc_spline_chain.cuh", "icc_vision_rows.cuh", "icc_imu_rows.cuh", "icc_rotinit_math.cuh", "icc_small_linalg.cuh", "icc_points_math.cuh")]
+    hdrs = [os.path.join(HERE, "..", "openimucameracalibrator_b200", "csrc", f) for f in ("icc_camera.cuh", "icc_device_math.cuh", "icc_spline_chain.cuh", "icc_vision_rows.cuh", "icc_imu_rows.cuh", "icc_rotinit_math.cuh", "icc_small_linalg.cuh", "icc_points_math.cuh", "icc_trust_region.cuh")]
     if not os.path.exists(OUT) or any(os.path.getmtime(f) > os.path.getmtime(OUT) for f in [SRC] + hdrs):
         os.makedirs(os.path.dirname(OUT), exist_ok=True)
         subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-O2", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-o", OUT, SRC])
@@ -449,3 +450,184 @@ def test_device_homogeneous_point_parameterization(hm):
             assert np.abs(J[:, i] - fd).max() <= 1e-8 * np.linalg.norm(x), (x, i, J[:, i], fd)
         if x[:3] @ x[:3] > np.finfo(float).eps:                                # (Ceres' own shortcut for x on the w axis takes H = I there)
             assert np.abs(J.T @ x).max() <= 1e-14 * (x @ x)                   # the tangent columns are orthogonal to x
+
+
+# ---- the trust-region controller shared by every LM driver (icc_trust_region.cuh) ---------------------------------------------------------
+class _TrRules:
+    """Ceres 2.1 TrustRegionMinimizer step control, independent statement: the state the controller must hold after every call."""
+
+    def __init__(self, ftol, ptol, gtol, r0, rmax, rmin, eta, max_it, max_invalid, check):
+        self.o = dict(ftol=ftol, ptol=ptol, gtol=gtol, rmax=rmax, rmin=rmin, eta=eta, max_it=max_it, max_invalid=max_invalid, check=check)
+        self.radius, self.nu, self.cost, self.initial_cost, self.mc = r0, 2.0, 0.0, 0.0, 0.0
+        self.invalid = self.iterations = self.successful = 0
+        self.term, self.stale = -1, 1
+
+    def state(self):
+        return [self.radius, self.nu, self.cost, self.initial_cost, self.invalid, self.iterations, self.successful, self.term, self.stale]
+
+    def _shrink(self):
+        self.radius /= self.nu; self.nu *= 2.0
+        if self.radius < self.o["rmin"]:
+            self.term = 4
+
+    def cont(self):
+        if self.term < 0 and self.iterations >= self.o["max_it"]:
+            self.term = 0
+        return self.term < 0
+
+    def jacobian(self, cost, gmax):
+        self.cost = cost; self.stale = 0
+        if self.iterations == 0:
+            self.initial_cost = cost
+        if self.o["check"] and gmax <= self.o["gtol"]:
+            self.term = 3
+        return self.term < 0
+
+    def step(self, valid, mc, sn, xn):
+        self.iterations += 1
+        if not valid or not mc > 0.0:
+            self.invalid += 1
+            if self.invalid >= self.o["max_invalid"]:
+                self.term = 4
+            else:
+                self._shrink()
+            return False
+        self.invalid, self.mc = 0, mc
+        if self.o["check"] and sn <= self.o["ptol"] * (xn + self.o["ptol"]):
+            self.term = 2
+            return False
+        return True
+
+    def candidate(self, c):
+        c = c if np.isfinite(c) else np.finfo(float).max
+        change = self.cost - c
+        if self.o["check"] and abs(change) <= self.o["ftol"] * self.cost:
+            self.term = 1
+            return False
+        rho = change / self.mc
+        if not rho > self.o["eta"]:
+            self._shrink()
+            return False
+        self.successful += 1; self.cost = c; self.nu = 2.0; self.stale = 1
+        self.radius = min(self.o["rmax"], self.radius / max(1.0 / 3.0, 1.0 - (2.0 * rho - 1.0) ** 3))
+        return True
+
+
+class _Tr:
+    """The product's controller and _TrRules driven in lockstep; every call must return the same and leave the same state."""
+
+    def __init__(self, hm, ftol=1e-6, ptol=1e-8, gtol=1e-10, r0=1e4, rmax=1e16, rmin=1e-32, eta=1e-3, max_it=50, max_invalid=5, check=1):
+        self.hm, self.buf = hm, ctypes.create_string_buffer(hm.hm_tr_size())
+        d = np.array([ftol, ptol, gtol, r0, rmax, rmin, eta]); i = np.array([max_it, max_invalid, check], dtype=np.int32)
+        hm.hm_tr_start(self.buf, d.ctypes.data_as(DP), i.ctypes.data_as(ctypes.POINTER(ctypes.c_int)))
+        self.ref = _TrRules(ftol, ptol, gtol, r0, rmax, rmin, eta, max_it, max_invalid, check)
+        self._check(True, True)
+
+    def state(self):
+        s = np.zeros(9); self.hm.hm_tr_state(self.buf, s.ctypes.data_as(DP))
+        return s
+
+    def _check(self, got, want):
+        assert bool(got) == want and list(self.state()) == self.ref.state(), (bool(got), want, list(self.state()), self.ref.state())
+        return want
+
+    def cont(self):
+        return self._check(self.hm.hm_tr_continue(self.buf), self.ref.cont())
+
+    def jacobian(self, cost, gmax):
+        return self._check(self.hm.hm_tr_jacobian(self.buf, ctypes.c_double(cost), ctypes.c_double(gmax)), self.ref.jacobian(cost, gmax))
+
+    def step(self, valid, mc, sn=1.0, xn=1.0):
+        return self._check(self.hm.hm_tr_step(self.buf, ctypes.c_int(int(valid)), ctypes.c_double(mc), ctypes.c_double(sn), ctypes.c_double(xn)), self.ref.step(valid, mc, sn, xn))
+
+    def candidate(self, c):
+        return self._check(self.hm.hm_tr_candidate(self.buf, ctypes.c_double(c)), self.ref.candidate(c))
+
+    def get(self, name):
+        return self.state()[["radius", "nu", "cost", "initial_cost", "invalid", "iterations", "successful", "termination", "stale"].index(name)]
+
+
+def test_trust_region_invalid_steps_shrink_and_stop_at_max_invalid(hm):
+    t = _Tr(hm)
+    assert t.cont() and t.jacobian(10.0, 1.0)
+    for k in range(4):
+        assert not t.step(False, 1.0) and t.cont()
+        assert t.get("radius") == 1e4 / 2.0 ** ((k + 1) * (k + 2) // 2) and t.get("nu") == 2.0 ** (k + 2)   # r / 2, / 4, / 8, ...
+    assert not t.step(True, -1.0) and not t.cont()            # no model decrease: the fifth invalid step in a row
+    assert t.get("termination") == 4 and t.get("iterations") == 5 and t.get("successful") == 0 and t.get("radius") == 1e4 / 1024.0
+
+
+def test_trust_region_min_radius_after_invalid_and_after_rejected_steps(hm):
+    t = _Tr(hm, r0=1.0, rmin=0.3)
+    assert t.cont() and t.jacobian(10.0, 1.0)
+    assert not t.step(False, 1.0) and t.get("radius") == 0.5 and t.cont()
+    assert not t.step(False, 1.0) and t.get("radius") == 0.125 and not t.cont() and t.get("termination") == 4 and t.get("invalid") == 2
+    t = _Tr(hm, r0=1.0, rmin=0.3)
+    assert t.cont() and t.jacobian(10.0, 1.0)
+    assert t.step(True, 1.0) and not t.candidate(10.5) and t.get("radius") == 0.5 and t.cont()   # cost went up: rejected
+    assert t.step(True, 1.0) and not t.candidate(np.nan) and t.get("radius") == 0.125 and not t.cont() and t.get("termination") == 4
+    assert t.get("successful") == 0 and t.get("cost") == 10.0
+
+
+def test_trust_region_accepted_steps_grow_the_radius_up_to_max_radius(hm):
+    t = _Tr(hm, r0=1.0, rmax=5.0)
+    assert t.cont() and t.jacobian(10.0, 1.0)
+    assert t.step(True, 2.0) and t.candidate(8.0)              # rho = 1: radius x 3
+    assert t.get("radius") == 3.0 and t.get("stale") == 1 and t.get("cost") == 8.0 and t.get("successful") == 1
+    assert t.cont() and t.jacobian(8.0, 1.0) and t.step(True, 2.0) and t.candidate(6.0)
+    assert t.get("radius") == 5.0 and t.get("nu") == 2.0       # 9 capped at max_radius
+    assert t.cont() and t.jacobian(6.0, 1.0) and t.step(True, 2.0) and t.candidate(5.5)   # rho = 0.25: radius / max(1/3, 1.125)
+    assert t.get("radius") == 5.0 / 1.125 and t.get("initial_cost") == 10.0
+
+
+def test_trust_region_gradient_stop_on_the_first_jacobian(hm):
+    t = _Tr(hm)
+    assert t.cont() and not t.jacobian(3.0, 1e-11) and not t.cont()
+    assert t.get("termination") == 3 and t.get("iterations") == 0 and t.get("initial_cost") == 3.0 and t.get("cost") == 3.0
+
+
+def test_trust_region_function_and_parameter_tolerance_stops_accept_nothing(hm):
+    t = _Tr(hm, ftol=1e-6)
+    assert t.cont() and t.jacobian(1.0, 1.0) and t.step(True, 1e-3)
+    assert not t.candidate(1.0 - 5e-7) and not t.cont()
+    assert t.get("termination") == 1 and t.get("successful") == 0 and t.get("cost") == 1.0 and t.get("iterations") == 1
+    t = _Tr(hm, ptol=1e-8)
+    assert t.cont() and t.jacobian(1.0, 1.0) and t.step(True, 0.5) and t.candidate(0.5)
+    assert t.cont() and t.jacobian(0.5, 1.0) and not t.step(True, 0.1, sn=1e-8 * 2.0, xn=2.0) and not t.cont()
+    assert t.get("termination") == 2 and t.get("successful") == 1 and t.get("cost") == 0.5 and t.get("iterations") == 2
+
+
+def test_trust_region_without_convergence_tests(hm):
+    """icc_lm_iterations' fixed-count runs: no gradient, parameter or function stop; the iteration limit, invalid steps and the
+    minimum radius still stop the run."""
+    t = _Tr(hm, max_it=4, check=0)
+    assert t.cont() and t.jacobian(1.0, 0.0)
+    assert t.step(True, 1.0, sn=0.0) and not t.candidate(1.0) and t.cont()   # zero step, unchanged cost: rejected
+    assert t.step(True, 1.0, sn=0.0) and t.candidate(0.0) and t.cont()
+    assert t.jacobian(0.0, 0.0) and t.step(True, 1.0) and not t.candidate(0.0) and t.cont()
+    assert not t.step(False, 1.0) and not t.cont() and t.get("termination") == 0 and t.get("iterations") == 4
+    t = _Tr(hm, check=0, max_invalid=2)
+    assert t.cont() and t.jacobian(1.0, 0.0) and not t.step(False, 0.0) and t.cont() and not t.step(True, np.nan) and not t.cont()
+    assert t.get("termination") == 4
+    t = _Tr(hm, check=0, r0=1.0, rmin=0.4)
+    assert t.cont() and t.jacobian(1.0, 0.0) and t.step(True, 1.0) and not t.candidate(2.0) and t.cont()
+    assert t.step(True, 1.0) and not t.candidate(2.0) and not t.cont() and t.get("termination") == 4
+
+
+@pytest.mark.filterwarnings("ignore::RuntimeWarning")             # the rules overflow to inf on huge candidate costs, as the C++ does
+def test_trust_region_random_sequences_follow_the_rules(hm):
+    """Random mixes of invalid, rejected, accepted and converged steps, the controller against the rules after every call."""
+    rng = np.random.default_rng(5)
+    for trial in range(300):
+        t = _Tr(hm, ftol=10.0 ** rng.uniform(-8, -2), ptol=10.0 ** rng.uniform(-10, -4), r0=10.0 ** rng.uniform(-2, 4), rmax=10.0 ** rng.uniform(0, 6),
+                rmin=10.0 ** rng.uniform(-8, -1), max_it=int(rng.integers(0, 30)), max_invalid=int(rng.integers(1, 6)), check=int(rng.integers(0, 2)))
+        cost = rng.uniform(1.0, 10.0)
+        while t.cont():
+            if t.get("stale") and not t.jacobian(cost, 10.0 ** rng.uniform(-12, 0)):
+                break
+            mc = rng.choice([-1.0, 0.0, np.nan, rng.uniform(0.0, 0.5) * cost])
+            if t.step(rng.uniform() > 0.15, mc, 10.0 ** rng.uniform(-12, 0), rng.uniform(0, 10)):
+                c = rng.choice([cost * (1 + rng.normal(0, 1e-7)), cost - mc * rng.uniform(-1, 2), np.inf, np.nan])
+                if t.candidate(c):
+                    cost = c
+        assert t.get("termination") in (0, 1, 2, 3, 4)
