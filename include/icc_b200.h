@@ -398,6 +398,49 @@ icc_status icc_static_imu_calibration(icc_handle* h, int n, const double* t_s, c
  * many (start, end) sample index pairs (inclusive).  `buf` NULL returns the required length in *len; otherwise *len is its capacity. */
 icc_status icc_get_static_imu_intervals(const icc_handle* h, int32_t* buf, int32_t* len);
 
+/* ---- upstream: Allan variance noise characterisation of a static IMU log ----------------------------------------------------------------
+ * AllanVarianceFitter::RunFit (src/core/allan_variance_fitter.cc; imu_utils) behind applications/fit_allan_variance.cc.  Channels are
+ * 0-2 accelerometer x, y, z (m/s^2, used as given) and 3-5 gyroscope x, y, z (rad/s, scaled by 57.3 * 3600 to deg/h as pushRadPerSec
+ * does).  With dt the mean timestamp difference, freq = 1/dt and theta = cumsum(x) / freq, the overlapping Allan variance
+ *   sigma2(m) = sum_{k < n-2m} (theta[k+2m] - 2 theta[k+m] + theta[k])^2 / (2 (dt m)^2 (n - 2m)),   tau(m) = dt m,
+ * is computed at the reference's cluster sizes m (n_clusters log-spaced values up to the largest power of two <= n/2, rounded up,
+ * consecutive duplicates dropped).  Each channel then fits log10(Q^2/tau^2 + N^2/tau + B^2 + K^2 tau + R^2 tau^2) to log10(sigma2)
+ * with Ceres' DOGLEG strategy and default options from the reference's least-squares initial values; the accelerometer fit drops
+ * the points below tau = 1 s that raise the running maximum of sigma2 (FitAllanAcc::checkData).  params: [Q, N, B, K, R] per channel.
+ * Deviation: the reference divides by zero for n < 3 or n_clusters < 2; here those return ICC_ERR_INVALID_ARGUMENT. */
+typedef struct icc_allan_options {
+  int32_t n_clusters;                /* log-spaced cluster sizes before deduplication; 10000 (fit_allan_variance.cc:41) */
+  int32_t reserved;
+} icc_allan_options;
+typedef struct icc_allan_noise {     /* the quantities the reference prints per channel */
+  double mean;                       /* gyroscope: mean rate in deg/s (getAvgValue() / 3600); accelerometer: mean in m/s^2 */
+  double bias_instability;           /* min of the fitted deviation over the fitted taus (from 1000): rad/s (/ (57.3 * 3600)) or m/s^2 */
+  double bias_instability_tau;       /* the tau of that minimum [s] */
+  double bias_b;                     /* gyroscope: getB() / (57.3 * 3600) = |B| / 0.6642824703 / (57.3 * 3600) rad/s; 0 for the accelerometer */
+  double white_noise_n;              /* gyroscope: sqrt(freq) getN() 60 / 57.3 = sqrt(freq) |N| / 57.3 rad/s; 0 for the accelerometer */
+  double white_noise;                /* sqrt(freq) sqrt(model(tau = 1)): rad/s (/ (57.3 * 3600)) or m/s^2 */
+} icc_allan_noise;
+typedef struct icc_allan_summary {
+  int32_t n_samples;
+  int32_t n_factors;                 /* F: distinct cluster sizes */
+  int32_t n_fit_points;              /* points in the fit (F, or fewer for the accelerometer) */
+  int32_t iterations, successful_steps;
+  int32_t termination;               /* icc_summary.termination codes */
+  int32_t gpu_launches;              /* kernel launches of the whole call */
+  int32_t reserved;
+  double freq, period;               /* 1 / mean dt [Hz], mean dt [s] */
+  double init_coeffs[5];             /* the signed least-squares solution initValue prints ("C ..."); the fit starts from |C| */
+  double initial_cost, final_cost;
+  double seconds_total;              /* host wall clock of the whole call (all channels) */
+} icc_allan_summary;
+void icc_default_allan_options(icc_allan_options* o);
+icc_status icc_allan_variance(icc_handle* h, int n, const double* t_s, const double* accel_xyz, const double* gyro_xyz,
+                              const icc_allan_options* options /* nullable */, double params[30] /* 6 x 5 */, icc_allan_noise noise[6],
+                              icc_allan_summary summary[6]);
+/* Curves of the last icc_allan_variance for one channel (0-5): factors, tau [s], sigma2 and the fitted deviation sqrt(model(tau)) at
+ * every factor.  `factors` NULL returns F in *len; otherwise *len is the capacity of each array. */
+icc_status icc_get_allan_curves(const icc_handle* h, int channel, int32_t* factors, double* tau, double* sigma2, double* fit_deviation, int32_t* len);
+
 /* Device blocks of destroyed handles are cached process-wide for the next job; this returns them to the CUDA driver. */
 void icc_trim_device_cache(void);
 

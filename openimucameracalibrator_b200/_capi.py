@@ -92,6 +92,34 @@ class StaticImuSummary(C.Structure):
         return d
 
 
+class AllanOptions(C.Structure):
+    """icc_allan_options (include/icc_b200.h); icc_default_allan_options fills in the reference's defaults."""
+    _fields_ = [("n_clusters", C.c_int32), ("reserved", C.c_int32)]
+
+
+class AllanNoise(C.Structure):
+    _fields_ = [("mean", C.c_double), ("bias_instability", C.c_double), ("bias_instability_tau", C.c_double), ("bias_b", C.c_double),
+                ("white_noise_n", C.c_double), ("white_noise", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class AllanSummary(C.Structure):
+    _fields_ = [("n_samples", C.c_int32), ("n_factors", C.c_int32), ("n_fit_points", C.c_int32), ("iterations", C.c_int32),
+                ("successful_steps", C.c_int32), ("termination", C.c_int32), ("gpu_launches", C.c_int32), ("reserved", C.c_int32),
+                ("freq", C.c_double), ("period", C.c_double), ("init_coeffs", C.c_double * 5), ("initial_cost", C.c_double),
+                ("final_cost", C.c_double), ("seconds_total", C.c_double)]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        d["init_coeffs"] = list(self.init_coeffs)
+        return d
+
+
+ALLAN_CHANNELS = ("acc_x", "acc_y", "acc_z", "gyr_x", "gyr_y", "gyr_z")
+ALLAN_PARAMS = ("Q", "N", "B", "K", "R")
+
 ALLREDUCE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p)
 
 
@@ -295,6 +323,31 @@ class CApi:
         for _ in range(10):
             c = int(buf[k]); out.append(buf[k + 1:k + 1 + 2 * c].reshape(c, 2).astype(np.int64)); k += 1 + 2 * c
         return out
+
+    # ---- upstream: Allan variance noise characterisation (src/core/allan_variance_fitter.cc) ------------------------------------
+    def allan_variance(self, t_s, accel, gyro, n_clusters=None):
+        """-> dict(params (6, 5) [Q, N, B, K, R], noise [6 dicts], summary [6 dicts]); channels ALLAN_CHANNELS."""
+        t = _f64(t_s); a = _f64(accel).reshape(-1, 3); g = _f64(gyro).reshape(-1, 3)
+        assert a.shape == g.shape and a.shape[0] == t.size
+        o = AllanOptions()
+        f = self._fn("default_allan_options"); f.restype = None; f.argtypes = [C.POINTER(AllanOptions)]
+        f(C.byref(o))
+        if n_clusters is not None:
+            o.n_clusters = int(n_clusters)
+        p, z, s = np.zeros(30), (AllanNoise * 6)(), (AllanSummary * 6)()
+        self._call("allan_variance", [C.c_int, c_double_p, c_double_p, c_double_p, C.POINTER(AllanOptions), c_double_p, C.POINTER(AllanNoise),
+                                      C.POINTER(AllanSummary)], t.size, _dp(t), _dp(a), _dp(g), C.byref(o), _dp(p), z, s)
+        return dict(params=p.reshape(6, 5), noise=[x.as_dict() for x in z], summary=[x.as_dict() for x in s])
+
+    def allan_curves(self, channel):
+        """Curves of the last allan_variance for channel 0-5: dict(factors, tau, sigma2, fit_deviation)."""
+        args = [C.c_int, c_int32_p, c_double_p, c_double_p, c_double_p, C.POINTER(C.c_int32)]
+        n = C.c_int32()
+        self._call("get_allan_curves", args, int(channel), None, None, None, None, C.byref(n))
+        f = np.zeros(max(n.value, 1), dtype=np.int32); t, s2, d = (np.zeros(max(n.value, 1)) for _ in range(3))
+        self._call("get_allan_curves", args, int(channel), f.ctypes.data_as(c_int32_p), _dp(t), _dp(s2), _dp(d), C.byref(n))
+        k = n.value
+        return dict(factors=f[:k].astype(np.int64), tau=t[:k], sigma2=s2[:k], fit_deviation=d[:k])
 
     # ---- upstream row f2: spline error weighting (python/sew.py:knot_spacing_and_variance) ------------------------------------
     def spline_error_weighting(self, times_s, signal_xyz, quality, min_dt=0.0, max_dt=0.0, want_spectrum=False):

@@ -275,3 +275,24 @@ class StaticImuCalibrator:
     def getGyroCalib(self):
         """-> (gyr_params[9], bias[3])"""
         return self._gyr.copy(), self._gyr_bias.copy()
+
+
+class AllanVarianceFitter:
+    """OpenICC::core::AllanVarianceFitter (include/OpenCameraCalibrator/core/allan_variance_fitter.h) on the CUDA C-ABI: constructed from
+    the telemetry (timestamps [s], accelerometer [m/s^2] and gyroscope [rad/s] as (n, 3)) and the number of clusters; RunFit runs
+    icc_allan_variance.  Afterwards `params` (6, 5) holds [Q, N, B, K, R] per channel (acc x, y, z, gyr x, y, z), `noise` and `summary`
+    the derived quantities and fit statistics per channel, and curves(c) the sigma^2 curve and its fit."""
+
+    def __init__(self, timestamps_s, accelerometer, gyroscope, nr_clusters: int = 10000, device: int = 0):
+        self._api = CApi(load_library(), "icc_", device)
+        self._data = (timestamps_s, accelerometer, gyroscope)
+        self.nr_clusters = nr_clusters
+        self.params = self.noise = self.summary = None
+
+    def RunFit(self) -> bool:
+        r = self._api.allan_variance(*self._data, n_clusters=self.nr_clusters)
+        self.params, self.noise, self.summary = r["params"], r["noise"], r["summary"]
+        return True
+
+    def curves(self, channel: int) -> dict:
+        return self._api.allan_curves(channel)

@@ -8,6 +8,7 @@
 // Everything numerical per LM iteration runs on the GPU (icc_eval.cu, icc_solver.cu); the host only sequences launches
 // and applies the trust-region accept/reject logic to a few scalars read back per iteration.  There is no CPU fallback.
 #include "../../include/icc_b200.h"
+#include "icc_allan_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_kernels.h"
 #include "icc_trust_region.cuh"
@@ -31,6 +32,10 @@ namespace icc {   // icc_static_imu.cu
 void default_static_imu_options(icc_static_imu_options* o);
 icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_static_imu_options& o,
                                 double acc_out[9], double gyr_out[9], double bias_out[3], icc_static_imu_summary& S, std::vector<int32_t>& intervals, std::string& err);
+// icc_allan.cu
+void default_allan_options(icc_allan_options* o);
+icc_status allan_variance(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options& o,
+                          double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6], allan::Curves& curves, std::string& err);
 }  // namespace icc
 
 namespace {
@@ -197,6 +202,7 @@ struct icc_handle {
   std::vector<int> perm;           // canonical tangent index -> solver index
   int launches_at_start = 0;
   std::vector<int32_t> static_imu_intervals;   // kept static intervals of the last icc_static_imu_calibration
+  allan::Curves allan_curves;                  // curves of the last icc_allan_variance
 };
 
 namespace {
@@ -2069,6 +2075,38 @@ icc_status icc_get_static_imu_intervals(const icc_handle* h, int32_t* buf, int32
   if (!buf) { *len = need; return ICC_OK; }
   if (*len < need) return ICC_ERR_INVALID_ARGUMENT;
   std::copy(h->static_imu_intervals.begin(), h->static_imu_intervals.end(), buf);
+  *len = need;
+  return ICC_OK;
+}
+
+// ---- upstream: Allan variance noise characterisation (icc_allan.cu) -----------------------------------------------------------------
+void icc_default_allan_options(icc_allan_options* o) { if (o) default_allan_options(o); }
+
+icc_status icc_allan_variance(icc_handle* h, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options* opt,
+                              double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6]) {
+  if (!h || !t || !acc || !gyr || !params || !noise || !summary) return ICC_ERR_INVALID_ARGUMENT;
+  icc_allan_options o; default_allan_options(&o);
+  if (opt) o = *opt;
+  if (n < 3 || o.n_clusters < 2) return fail(h, ICC_ERR_INVALID_ARGUMENT, "icc_allan_variance needs n >= 3 samples and n_clusters >= 2");
+  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+  CU(cudaSetDevice(h->device));
+  h->allan_curves = allan::Curves();
+  std::string err;
+  const icc_status rc = allan_variance(h->stream, n, t, acc, gyr, o, params, noise, summary, h->allan_curves, err);
+  if (rc != ICC_OK) { h->allan_curves = allan::Curves(); return fail(h, rc, err); }
+  return ICC_OK;
+}
+
+icc_status icc_get_allan_curves(const icc_handle* h, int channel, int32_t* factors, double* tau, double* sigma2, double* fit_deviation, int32_t* len) {
+  if (!h || !len || channel < 0 || channel >= 6) return ICC_ERR_INVALID_ARGUMENT;
+  const allan::Curves& C = h->allan_curves;
+  const int32_t need = (int32_t)C.factors.size();
+  if (!factors) { *len = need; return ICC_OK; }
+  if (*len < need || !tau || !sigma2 || !fit_deviation) return ICC_ERR_INVALID_ARGUMENT;
+  std::copy(C.factors.begin(), C.factors.end(), factors);
+  std::copy(C.tau.begin(), C.tau.end(), tau);
+  std::copy(C.sigma2[channel].begin(), C.sigma2[channel].end(), sigma2);
+  std::copy(C.fit_deviation[channel].begin(), C.fit_deviation[channel].end(), fit_deviation);
   *len = need;
   return ICC_OK;
 }

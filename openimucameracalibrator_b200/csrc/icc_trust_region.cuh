@@ -85,4 +85,95 @@ __host__ __device__ __forceinline__ bool tr_candidate(TrustRegion& T, double can
   return true;
 }
 
+// ---- Ceres 2.1 DoglegStrategy (TRADITIONAL_DOGLEG) under the same minimiser ------------------------------------------------------
+// A restatement written from the documented behaviour of Ceres 2.1 (dogleg_strategy.cc), not from its source.  The iteration, the
+// tolerances and the invalid-step limit are the TrustRegion above; only the radius schedule differs, and the strategy keeps the
+// regularisation mu of its Gauss-Newton solve and whether the Gauss-Newton and Cauchy vectors of the current Jacobian can be reused:
+//   Dogleg D = dl_start(options);
+//   while (tr_continue(D.T)) {
+//     if (D.T.jacobian_stale) { evaluate J at x; if (!tr_jacobian(D.T, cost, max|g|)) break; }
+//     if (!D.reuse) { diagonal, gradient, Cauchy alpha; while (D.mu < kDoglegMaxMu && !solve with D.mu) D.mu *= kDoglegMuIncrease; }
+//     step = dl_dogleg_step(...);  if (dl_step(D, solved, model_change, |step|, |x|) && dl_candidate(D, candidate cost)) x <- candidate;
+//   }
+struct Dogleg {
+  TrustRegion T;       // T.radius is the dogleg radius; T.decrease_factor is unused
+  double mu;           // Gauss-Newton regularisation: (J^T J + mu diag(D^2)) y = J^T r
+  double step_norm;    // norm of the last dogleg step in the D-scaled space (dl_dogleg_step)
+  int reuse;           // the Gauss-Newton and Cauchy vectors belong to the current Jacobian (after a rejected step)
+};
+constexpr double kDoglegMinMu = 1e-8, kDoglegMaxMu = 1.0, kDoglegMuIncrease = 10.0;
+
+__host__ __device__ __forceinline__ Dogleg dl_start(const TrOptions& o) {
+  Dogleg D; D.T = tr_start(o); D.mu = kDoglegMinMu; D.step_norm = 0.0; D.reuse = 0;
+  return D;
+}
+
+// The traditional dogleg step in the D-scaled space from the scaled gradient g, the scaled Gauss-Newton step gn and the Cauchy
+// factor alpha: gn inside the radius; else the gradient step cut at the radius when the Cauchy point lies outside; else the point
+// of the segment Cauchy point -> gn on the boundary.  Writes step / D (the Jacobi-scaled coordinates); returns the scaled norm.
+template <int N>
+__host__ __device__ __forceinline__ double dl_dogleg_step(const double g[N], const double gn[N], const double diag[N], double alpha, double radius,
+                                                          double step[N]) {
+  double gg = 0.0, nn = 0.0, gb = 0.0;
+  for (int i = 0; i < N; ++i) { gg += g[i] * g[i]; nn += gn[i] * gn[i]; gb += g[i] * gn[i]; }
+  const double g_norm = sqrt(gg), gn_norm = sqrt(nn);
+  if (gn_norm <= radius) {
+    for (int i = 0; i < N; ++i) step[i] = gn[i] / diag[i];
+    return gn_norm;
+  }
+  if (g_norm * alpha >= radius) {
+    for (int i = 0; i < N; ++i) step[i] = (-(radius / g_norm) * g[i]) / diag[i];
+    return radius;
+  }
+  // a = -alpha g (inside), b = gn (outside): beta in [0, 1] with |a + beta (b - a)| = radius
+  const double b_dot_a = -alpha * gb;
+  const double a_sq = (alpha * g_norm) * (alpha * g_norm);
+  const double bma_sq = (a_sq - 2.0 * b_dot_a) + gn_norm * gn_norm;
+  const double c = b_dot_a - a_sq;
+  const double d = sqrt(c * c + bma_sq * (radius * radius - a_sq));
+  const double beta = c <= 0.0 ? (d - c) / bma_sq : (radius * radius - a_sq) / (d + c);
+  double s2 = 0.0;
+  for (int i = 0; i < N; ++i) { const double v = (-alpha * (1.0 - beta)) * g[i] + beta * gn[i]; s2 += v * v; step[i] = v / diag[i]; }
+  return sqrt(s2);
+}
+
+// A step without a solved Gauss-Newton system or without a positive model decrease is invalid: mu x 10 and a fresh solve (the
+// radius stays); max_invalid in a row stop the run.  A valid step faces the parameter tolerance.  True when the candidate cost
+// decides the step (dl_candidate).
+__host__ __device__ __forceinline__ bool dl_step(Dogleg& D, bool valid, double model_change, double step_norm, double x_norm) {
+  TrustRegion& T = D.T;
+  ++T.iterations;
+  if (!valid || !(model_change > 0.0)) {
+    if (++T.invalid >= T.o.max_invalid) T.termination = 4;
+    else { D.mu *= kDoglegMuIncrease; D.reuse = 0; }
+    return false;
+  }
+  T.invalid = 0; T.model_change = model_change;
+  if (T.o.check_convergence && step_norm <= T.o.parameter_tolerance * (x_norm + T.o.parameter_tolerance)) { T.termination = 2; return false; }
+  return true;
+}
+
+// Function tolerance, then accept when rho > min_relative_decrease or reject.  Rejected: radius / 2, the Gauss-Newton and Cauchy
+// vectors are reused.  Accepted: rho < 0.25 halves the radius, rho > 0.75 makes it at least 3 |step|, mu / 5 (not below its
+// minimum).  The run stops when the radius falls below min_radius.  True when accepted.
+__host__ __device__ __forceinline__ bool dl_candidate(Dogleg& D, double cand_cost) {
+  TrustRegion& T = D.T;
+  if (!(fabs(cand_cost) <= 1.7976931348623157e308)) cand_cost = 1.7976931348623157e308;
+  const double cost_change = T.cost - cand_cost;
+  if (T.o.check_convergence && fabs(cost_change) <= T.o.function_tolerance * T.cost) { T.termination = 1; return false; }
+  const double rho = cost_change / T.model_change;
+  if (!(rho > T.o.min_relative_decrease)) {
+    T.radius *= 0.5; D.reuse = 1;
+    if (T.radius < T.o.min_radius) T.termination = 4;
+    return false;
+  }
+  ++T.successful; T.cost = cand_cost;
+  if (rho < 0.25) T.radius *= 0.5;
+  if (rho > 0.75) T.radius = fmax(T.radius, 3.0 * D.step_norm);
+  if (T.radius < T.o.min_radius) T.termination = 4;
+  D.mu = fmax(kDoglegMinMu, 2.0 * D.mu / kDoglegMuIncrease);
+  D.reuse = 0; T.jacobian_stale = 1;
+  return true;
+}
+
 }  // namespace icc

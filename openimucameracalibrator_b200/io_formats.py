@@ -209,3 +209,28 @@ def imu_intrinsics_document(acc_params, gyr_params, gyr_bias) -> dict:
 def write_imu_intrinsics_json(path: str, acc_params, gyr_params, gyr_bias) -> None:
     with open(path, "w") as f:
         json.dump(imu_intrinsics_document(acc_params, gyr_params, gyr_bias), f, indent=4)
+
+
+def allan_variance_document(result: dict, curves: list) -> dict:
+    """The --output_json document of bin/fit_allan_variance: per channel (acc_x .. gyr_z) the curve (factors, tau [s], sigma2, fitted
+    deviation), the fitted [Q, N, B, K, R], the derived noise quantities and the fit statistics.  `result` is CApi.allan_variance's,
+    `curves` the six CApi.allan_curves dicts."""
+    from ._capi import ALLAN_CHANNELS, ALLAN_PARAMS
+    s0 = result["summary"][0]
+    doc = {"n_samples": float(s0["n_samples"]), "freq": float(s0["freq"]), "period": float(s0["period"]), "channels": {}}
+    for c, name in enumerate(ALLAN_CHANNELS):
+        cv, s = curves[c], result["summary"][c]
+        doc["channels"][name] = {
+            "factors": [float(v) for v in cv["factors"]], "tau": [float(v) for v in cv["tau"]], "sigma2": [float(v) for v in cv["sigma2"]],
+            "fit_deviation": [float(v) for v in cv["fit_deviation"]],
+            "params": {k: float(v) for k, v in zip(ALLAN_PARAMS, result["params"][c])},
+            "noise": {k: float(v) for k, v in result["noise"][c].items()},
+            "fit": {"points": float(s["n_fit_points"]), "iterations": float(s["iterations"]), "termination": float(s["termination"]),
+                    "initial_cost": float(s["initial_cost"]), "final_cost": float(s["final_cost"])},
+        }
+    return doc
+
+
+def write_allan_variance_json(path: str, result: dict, curves: list) -> None:
+    with open(path, "w") as f:
+        json.dump(allan_variance_document(result, curves), f, indent=1)

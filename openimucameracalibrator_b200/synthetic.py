@@ -313,3 +313,32 @@ def make_static_imu_sequence(rate_hz=200.0, seed=7, n_poses=36, init_s=15.0, pos
 def static_imu_full_size(seed=11) -> dict:
     """1 kHz, about ten minutes: 30 s still, 40 poses of 2-4 s joined by 8-12 s rotations."""
     return make_static_imu_sequence(rate_hz=1000.0, seed=seed, n_poses=40, init_s=30.0, pose_s=(2.0, 4.0), move_s=(8.0, 12.0))
+
+
+# ---- static IMU noise log (input of fit_allan_variance) --------------------------------------------------------------------------
+ALLAN_TRUTH = dict(acc_white=2.0e-3, acc_walk=4.0e-5, acc_bias=(0.05, -0.08, 9.81), gyr_white=1.5e-4, gyr_walk=2.0e-6, gyr_bias=(3e-3, -2e-3, 1e-3))
+
+
+def make_allan_log(rate_hz=200.0, duration_s=1200.0, seed=5, truth=ALLAN_TRUTH) -> dict:
+    """A static IMU log: per axis, white noise of density `*_white` (units/sqrt(Hz)), a bias random walk of strength `*_walk`
+    (units/s/sqrt(Hz)) and a constant bias.  In Allan terms the white noise gives sigma^2 = white^2 / tau (N = white) and the walk
+    sigma^2 = walk^2 tau / 3 (K = walk / sqrt(3)).  Accelerometer in m/s^2, gyroscope in rad/s."""
+    rng = np.random.default_rng(seed)
+    n = int(round(duration_s * rate_hz)); dt = 1.0 / rate_hz
+    t = np.arange(n) * dt
+    out = {"t_s": t, "rate_hz": rate_hz, "truth": dict(truth)}
+    for key in ("acc", "gyr"):
+        white = truth[key + "_white"] * np.sqrt(rate_hz) * rng.standard_normal((n, 3))
+        walk = np.cumsum(truth[key + "_walk"] * np.sqrt(dt) * rng.standard_normal((n, 3)), axis=0)
+        out["accel" if key == "acc" else "gyro"] = np.asarray(truth[key + "_bias"]) + walk + white
+    return out
+
+
+def allan_small(seed=5) -> dict:
+    """20 minutes at 200 Hz (240 000 samples)."""
+    return make_allan_log(200.0, 1200.0, seed)
+
+
+def allan_full_size(seed=6) -> dict:
+    """2 hours at 400 Hz (2.88 M samples)."""
+    return make_allan_log(400.0, 7200.0, seed)
