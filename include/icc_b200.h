@@ -208,7 +208,37 @@ icc_status icc_evaluate(icc_handle* h, int flags, double* cost, double* residual
 /* J^T J V for nvec caller vectors (canonical tangent order, one vector after the other) from the packed normal equations of the
  * current state: full-size parity of the reduced system without a dense Hessian (evaluation helper, like icc_evaluate). */
 icc_status icc_normal_matvec(icc_handle* h, int flags, int nvec, const double* V, double* HV);
+/* Elimination plan of the damped normal-equation solve (nested dissection of the knot band, see DESIGN.md §3.2).
+ * Level 0 cuts the nk knot columns into P chunks: chunk c owns len + (c < rem) interior columns, P - 1 separators of kd columns
+ * lie between them.  S[l] (l = 1..L+1) is the separator-block count of reduced system l; levels 1..L eliminate every other block. */
+typedef struct icc_solver_plan_info {
+  int32_t valid;               /* 0: no plan fits the shared-memory limits (the solve returns ICC_ERR_UNSUPPORTED) */
+  int32_t nk, kd, nb;          /* knot (band) columns, half bandwidth, border columns */
+  int32_t P, len, rem, L;
+  int32_t cl_global, cs_global;  /* level-0 local border block / root border block live in HBM instead of shared memory */
+  int32_t stage0;              /* level-0 back-substitution may stage its El rows in shared memory */
+  int32_t WS_A;                /* level-0 window slots (power of two) */
+  int32_t backsub0_staged;     /* level-0 chunks whose back-substitution is staged (interior <= 128 columns and stage0) */
+  int32_t max_leaf;            /* len + (rem > 0) */
+  int32_t S[16];
+  int64_t smem_bytes[5];       /* dynamic shared memory: eliminate, reduce, root, level-0 back-substitution, level >= 1 back-substitution */
+  int64_t workspace_doubles;   /* device workspace of the plan (0 when not valid) */
+} icc_solver_plan_info;
+/* The plan icc_solve_normal_equations would use under `flags` with `chunks` level-0 chunks (0 = the planner's choice).  Host
+ * only: also works on a host-only (device -1) handle. */
+icc_status icc_solver_plan(icc_handle* h, int flags, int chunks, icc_solver_plan_info* plan);
+/* One damped solve of the normal equations that the preceding icc_evaluate (with gradient or Hessian) or icc_normal_matvec left
+ * in the handle for the same `flags`; no evaluation, the state is not touched (ICC_ERR_STATE when those normal equations are not
+ * current).  Jacobi scale s = 1/(1+sqrt(H_ii)) (1 without jacobi_scaling), then (S H S + D) y = -S g with
+ * D = clamp(H_ii s_i^2, min_lm_diagonal, max_lm_diagonal) / radius, delta = S y: exactly the step of one LM iteration at that
+ * radius.  `chunks` as in icc_solver_plan; a plan that does not fit returns ICC_ERR_UNSUPPORTED before any launch.
+ * Outputs (canonical tangent order, any may be NULL): delta, scale, h_diag (diag(H) as the solver read it), the model cost change
+ * -(g^T delta + delta^T H delta / 2), step_ok (0 when a pivot was not positive: the delta output is then not written), plan. */
+icc_status icc_solve_normal_equations(icc_handle* h, int flags, double radius, int chunks, double* delta, double* scale, double* h_diag,
+                                      double* model_change, int32_t* step_ok, icc_solver_plan_info* plan);
 icc_status icc_lm_iterations(icc_handle* h, int n, int flags, icc_summary* summary);
+/* CUDA kernels this library has launched in this process, all handles together (tests: a refused call launches nothing). */
+int64_t icc_kernel_launch_count(void);
 /* Run `n` bare residual+Jacobian+normal-equation evaluations (the residual-eval kernels only); device ms per evaluation. */
 icc_status icc_time_evaluations(icc_handle* h, int n, int flags, int with_jacobian, double* ms_per_eval);
 /* The handle's cudaStream_t (so that callers can bracket calls with their own CUDA events on the launching stream). */

@@ -499,6 +499,48 @@ def _normal_matvec(self, flags, V):
 CApi.normal_matvec = _normal_matvec
 
 
+class SolverPlan(C.Structure):
+    """icc_solver_plan_info (include/icc_b200.h): the elimination plan of the damped normal-equation solve."""
+    _fields_ = [("valid", C.c_int32), ("nk", C.c_int32), ("kd", C.c_int32), ("nb", C.c_int32), ("P", C.c_int32), ("len", C.c_int32),
+                ("rem", C.c_int32), ("L", C.c_int32), ("cl_global", C.c_int32), ("cs_global", C.c_int32), ("stage0", C.c_int32),
+                ("WS_A", C.c_int32), ("backsub0_staged", C.c_int32), ("max_leaf", C.c_int32), ("S", C.c_int32 * 16),
+                ("smem_bytes", C.c_int64 * 5), ("workspace_doubles", C.c_int64)]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        d["S"] = list(self.S)[1:self.L + 2]
+        d["smem_bytes"] = list(self.smem_bytes)
+        return d
+
+
+def _solver_plan(self, flags, chunks=0) -> dict:
+    """The plan the solve would use under `flags` with `chunks` level-0 chunks (0 = the planner's choice); host only."""
+    p = SolverPlan()
+    self._call("solver_plan", [C.c_int, C.c_int, C.POINTER(SolverPlan)], int(flags), int(chunks), C.byref(p))
+    return p.as_dict()
+
+
+def _solve_normal_equations(self, flags, radius, chunks=0) -> dict:
+    """One damped solve of the normal equations left by the preceding evaluate / normal_matvec with the same flags
+    -> dict(delta, scale, h_diag, model_change, step_ok, plan), vectors in canonical tangent order."""
+    n = self.num_tangent(flags)
+    d, s, hd = np.full(n, np.nan), np.zeros(n), np.zeros(n)
+    mc, ok, p = C.c_double(), C.c_int32(), SolverPlan()
+    self._call("solve_normal_equations", [C.c_int, C.c_double, C.c_int, c_double_p, c_double_p, c_double_p, c_double_p, c_int32_p, C.POINTER(SolverPlan)],
+               int(flags), float(radius), int(chunks), _dp(d), _dp(s), _dp(hd), C.byref(mc), C.byref(ok), C.byref(p))
+    return dict(delta=d, scale=s, h_diag=hd, model_change=mc.value, step_ok=ok.value, plan=p.as_dict())
+
+
+def kernel_launch_count(lib) -> int:
+    """CUDA kernels the library has launched in this process (all handles)."""
+    f = lib.icc_kernel_launch_count; f.restype = C.c_int64; f.argtypes = []
+    return int(f())
+
+
+CApi.solver_plan = _solver_plan
+CApi.solve_normal_equations = _solve_normal_equations
+
+
 class Comm:
     """icc_comm: the library's own NCCL communicator (include/icc_b200.h).  `unique_id()` on one rank, `Comm(lib, id, rank, world,
     device)` on every rank (collective)."""

@@ -196,6 +196,7 @@ struct icc_handle {
   bool knots_dirty_host = false;   // only the spline knots are newer on the device (device-side initialisation): globals / biases on the host are current
   // ---- active set ------------------------------------------------------------------------------------------------
   int cur_flags = -1;
+  int ne_flags = -1;        // flags of the normal equations in d_ne that icc_evaluate / icc_normal_matvec left for icc_solve_normal_equations (-1: none)
   std::vector<int> so3_col, r3_col, ba_col, bg_col;   // solver index of first dim or -1
   int col_tic = -1, col_g = -1, col_ld = -1;
   int n_tan = 0;
@@ -292,6 +293,7 @@ cudaError_t upload_staged(icc_handle* h, DevBuf<T>& d, const std::vector<T>& v) 
 
 // board points of state `which`: homogeneous vectors up, de-homogenised copy + local Jacobians derived on the device
 icc_status upload_points(icc_handle* h, int which, bool staged) {
+  h->ne_flags = -1;                        // every state upload passes here: the normal equations no longer belong to the state
   StateBufs& s = h->st[which];
   const size_t np = h->points.size() / 4;
   if (!np) return ICC_OK;
@@ -377,6 +379,9 @@ icc_status push_state_to_device(icc_handle* h) {
 icc_status configure(icc_handle* h, int flags) {
   if ((flags & ICC_FLAG_POINTS) && (flags & ICC_FLAG_CAM_INTRINSICS)) return fail(h, ICC_ERR_UNSUPPORTED, "POINTS together with CAM_INTRINSICS (an extension flag of this library) is not supported");
   if (h->cur_flags == flags) return ICC_OK;
+  // the host layout below is rewritten before the shape checks: until it is complete, no flags are configured, so that a refused
+  // shape cannot leave its layout behind under the previous flags (the device-side problem P keeps the previous layout, complete)
+  h->cur_flags = -1; h->ne_flags = -1;
   const int nso3 = (int)h->so3.size() / 4, nr3 = (int)h->r3.size() / 3, nba = (int)h->ba.size() / 3, nbg = (int)h->bg.size() / 3;
   const bool spline = flags & ICC_FLAG_SPLINE, tic = flags & ICC_FLAG_T_I_C, grav = flags & ICC_FLAG_GRAVITY_DIR;
   const bool ld = (flags & ICC_FLAG_CAM_LINE_DELAY) && h->ip.init_line_delay_s != 0.0;
@@ -448,7 +453,27 @@ icc_status configure(icc_handle* h, int flags) {
     }
   }
   if (kd > 255) return fail(h, ICC_ERR_UNSUPPORTED, "knot-spacing ratio produces a half bandwidth > 255");
-  h->cur_flags = flags;
+  {   // the knot band alone must fit an elimination plan; a border that does not fit is reported by the solve (evaluation works at any width)
+    DeviceProblem B; memset(&B, 0, sizeof B);
+    B.nk = nk; B.kd = kd; B.ldb = kd + 1;
+    icc_solver_plan_info pi; solver_plan_info(B, 0, &pi);
+    if (!pi.valid) {
+      // a band too wide for several chunks leaves one chunk, whose back-substitution holds every knot column in shared memory:
+      // find the longest sequence that one chunk of this band takes (none from a half bandwidth of 112: the level-0 window alone is too large)
+      int lo = 0, hi = nk;
+      while (lo < hi) { const int mid = lo + (hi - lo + 1) / 2; B.nk = mid; solver_plan_info(B, 1, &pi); if (pi.valid) lo = mid; else hi = mid - 1; }
+      char msg[400];
+      if (lo > 0)
+        snprintf(msg, sizeof msg, "the knot spacing (dt_so3 / dt_r3 ratio) gives a half bandwidth of %d columns over %d knot columns: no elimination "
+                 "plan of the solver fits in shared memory (a band this wide is solved as one chunk, which takes at most %d knot columns; "
+                 "use a knot-spacing ratio closer to 1 or a shorter sequence)", kd, nk, lo);
+      else
+        snprintf(msg, sizeof msg, "the knot spacing (dt_so3 / dt_r3 ratio) gives a half bandwidth of %d columns over %d knot columns: no elimination "
+                 "plan of the solver fits in shared memory at any sequence length (half bandwidths from 112 never fit; use a knot-spacing "
+                 "ratio closer to 1)", kd, nk);
+      return fail(h, ICC_ERR_UNSUPPORTED, msg);
+    }
+  }
   DeviceProblem& P = h->P;
   P.nk = nk; P.nb = nb; P.kd = kd; P.ldb = kd + 1;
   P.col_tic = h->col_tic; P.col_g = h->col_g; P.col_ld = h->col_ld; P.col_ai = col_ai; P.col_gi = col_gi; P.col_ci = col_ci; P.col_to = col_to; P.col_pts = col_pts; P.n_points = npts;
@@ -461,8 +486,9 @@ icc_status configure(icc_handle* h, int flags) {
     P.so3_col = h->d_so3_col.p; P.r3_col = h->d_r3_col.p; P.ba_col = h->d_ba_col.p; P.bg_col = h->d_bg_col.p;
     CU(h->d_ne.alloc((size_t)P.ne_size)); P.ne = h->d_ne.p;
     CU(h->d_scale.alloc((size_t)std::max(1, nk + nb))); CU(h->d_delta.alloc((size_t)std::max(1, nk + nb)));
-    CU(h->d_ws.alloc(solve_workspace_doubles(P)));
+    CU(h->d_ws.alloc(solve_workspace_doubles(P, 0)));
   }
+  h->cur_flags = flags;
   return ICC_OK;
 }
 
@@ -478,6 +504,7 @@ icc_status cross_rank_sum(icc_handle* h, double* dev, int64_t n) {
 
 // One Jacobian evaluation on the current state: zero the packed normal equations, run the kernels, cross-rank reduce.
 icc_status eval_jacobian(icc_handle* h, const DeviceState& S, double* residuals_dev) {
+  h->ne_flags = -1;
   CU(cudaMemsetAsync(h->P.ne, 0, (size_t)h->P.ne_size * sizeof(double), h->stream));
   if (launch_eval(h->P, S, true, nullptr, residuals_dev, nullptr, h->stream, h->aux_ok ? &h->aux : nullptr)) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
   if (h->P.col_pts >= 0 && h->P.rolling) launch_points_jac(h->P, S, S.pjac, h->P.col_pts, h->sm_count, h->stream);   // board-point columns (POINTS)
@@ -503,6 +530,14 @@ icc_status mean_reproj(icc_handle* h, double* out) {
   if (!(sc[SC_REPROJ_CNT] > 0.0)) { *out = 0.0; return ICC_OK; }
   *out = sc[SC_REPROJ_SUM] / sc[SC_REPROJ_CNT];
   return ICC_OK;
+}
+
+// configure() accepted the knot band, so a plan that does not fit is the border's doing
+std::string border_too_wide_message(const DeviceProblem& P) {
+  char msg[256];
+  snprintf(msg, sizeof msg, "the border of %d columns (globals, bias knots, board points) is too wide for the solver's shared-memory plans "
+           "(half bandwidth %d, %d knot columns)", P.nb, P.kd, P.nk);
+  return msg;
 }
 
 // Levenberg-Marquardt with Ceres TrustRegionMinimizer semantics (options: impl.h:254-266 + Ceres 2.1 defaults).
@@ -559,8 +594,8 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
     }
     SolveParams sp; sp.radius = T.radius; sp.min_diag = to.min_diagonal; sp.max_diag = to.max_diagonal; sp.jacobi_scaling = h->opt.jacobi_scaling;
     const int a = mark();
-    { const int se = launch_solve(P, h->d_scale.p, sp, h->d_ws.p, h->d_delta.p, h->d_scal.p, h->stream);
-      if (se == 1) return fail(h, ICC_ERR_UNSUPPORTED, "the border (bias knots + globals) is too wide for the solver's shared-memory plans");
+    { const int se = launch_solve(P, h->d_scale.p, sp, h->d_ws.p, h->d_delta.p, h->d_scal.p, h->stream, 0);
+      if (se == 1) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(P));
       if (se) return fail(h, ICC_ERR_CUDA, std::string("solver launch: ") + cudaGetErrorString(cudaGetLastError())); }
     const int b = mark(); lin_spans.push_back({a, b});
     const int cand = 1 - h->cur;
@@ -1047,7 +1082,7 @@ icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
   P.w_acc = 1.0 / ipp->std_r3; P.w_gyr = 1.0 / ipp->std_so3;
   P.n_so3 = nso3; P.n_r3 = nr3; P.n_ba = nba; P.n_bg = nbg;
   P.n_res_vis = P.rolling ? 2 * P.n_corners : 0; P.n_res_acc = 3 * P.n_imu; P.n_res_gyr = 3 * P.n_imu;
-  h->cur_flags = -1; h->initialised = true; h->cur = 0; h->state_dirty_host = false; h->knots_dirty_host = false;
+  h->cur_flags = -1; h->ne_flags = -1; h->initialised = true; h->cur = 0; h->state_dirty_host = false; h->knots_dirty_host = false;
   if (h->device < 0) return ICC_OK;
   CU(cudaSetDevice(h->device));
   CU(cudaStreamSynchronize(h->stream));   // nothing may still read the staging arena of an earlier call
@@ -1337,6 +1372,7 @@ icc_status icc_evaluate(icc_handle* h, int flags, double* cost, double* residual
   CU(cudaMemcpyAsync(ne.data(), P.ne, ne.size() * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (residuals) CU(cudaMemcpyAsync(residuals, res_dev, (size_t)nres * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU(cudaStreamSynchronize(h->stream));
+  h->ne_flags = flags;
   if (cost) *cost = ne[P.ne_off_cost];
   if (gradient) for (int i = 0; i < n; ++i) gradient[i] = ne[P.ne_off_g + h->perm[i]];
   if (hessian) {
@@ -1383,6 +1419,60 @@ icc_status icc_normal_matvec(icc_handle* h, int flags, int nvec, const double* V
     }
     for (int i = 0; i < n; ++i) HV[(size_t)v * n + i] = y[h->perm[i]];
   }
+  h->ne_flags = flags;
+  return ICC_OK;
+}
+
+int64_t icc_kernel_launch_count(void) { return kernel_launch_count(); }
+
+icc_status icc_solver_plan(icc_handle* h, int flags, int chunks, icc_solver_plan_info* plan) {
+  if (!h || !plan || chunks < 0) return ICC_ERR_INVALID_ARGUMENT;
+  if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
+  if (h->device >= 0) CU(cudaSetDevice(h->device));
+  icc_status s = configure(h, flags); if (s != ICC_OK) return s;
+  solver_plan_info(h->P, chunks, plan);
+  return ICC_OK;
+}
+
+// The linear solve of one LM iteration on the normal equations already in the handle: what run_lm launches between the Jacobian
+// and the update, with the plan's own workspace, so that a test can compare the step with a dense solve of exactly the H and g
+// that were factored.
+icc_status icc_solve_normal_equations(icc_handle* h, int flags, double radius, int chunks, double* delta, double* scale, double* h_diag,
+                                      double* model_change, int32_t* step_ok, icc_solver_plan_info* plan) {
+  if (!h || chunks < 0 || !(radius > 0.0)) return ICC_ERR_INVALID_ARGUMENT;
+  NEED_DEVICE();
+  if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
+  if (h->ne_flags != flags || h->cur_flags != flags)
+    return fail(h, ICC_ERR_STATE, "no current normal equations for these flags: call icc_evaluate (gradient or Hessian) or icc_normal_matvec first");
+  CU(cudaSetDevice(h->device));
+  const DeviceProblem& P = h->P;
+  const int n = P.nk + P.nb;
+  icc_solver_plan_info pi; solver_plan_info(P, chunks, &pi);
+  if (plan) *plan = pi;
+  if (!pi.valid) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(P));
+  if (n == 0) { if (model_change) *model_change = 0.0; if (step_ok) *step_ok = 1; return ICC_OK; }
+  DevBuf<double> ws; CU(ws.alloc((size_t)pi.workspace_doubles));
+  CU(cudaMemsetAsync(h->d_scal.p, 0, SC_COUNT * sizeof(double), h->stream));
+  launch_compute_scale(P, h->d_scale.p, h->opt.jacobi_scaling, h->d_scal.p, h->stream);
+  SolveParams sp; sp.radius = radius; sp.min_diag = h->opt.min_lm_diagonal; sp.max_diag = h->opt.max_lm_diagonal; sp.jacobi_scaling = h->opt.jacobi_scaling;
+  const int se = launch_solve(P, h->d_scale.p, sp, ws.p, h->d_delta.p, h->d_scal.p, h->stream, chunks);
+  if (se) return fail(h, ICC_ERR_CUDA, std::string("solver launch: ") + cudaGetErrorString(cudaGetLastError()));
+  std::vector<double> d(n), s(n), hd(n); double sc[SC_COUNT];
+  CU(cudaMemcpyAsync(d.data(), h->d_delta.p, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaMemcpyAsync(s.data(), h->d_scale.p, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (P.nk) CU(cudaMemcpy2DAsync(hd.data(), sizeof(double), P.ne, (size_t)P.ldb * sizeof(double), sizeof(double), P.nk, cudaMemcpyDeviceToHost, h->stream));
+  if (P.nb) CU(cudaMemcpy2DAsync(hd.data() + P.nk, sizeof(double), P.ne + P.ne_off_C, (size_t)(P.nb + 1) * sizeof(double), sizeof(double), P.nb, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaMemcpyAsync(sc, h->d_scal.p, sizeof sc, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  const bool ok = sc[SC_OK] == 1.0;
+  for (int i = 0; i < n; ++i) {
+    const int k = h->perm[i];
+    if (delta && ok) delta[i] = d[k];
+    if (scale) scale[i] = s[k];
+    if (h_diag) h_diag[i] = hd[k];
+  }
+  if (model_change) *model_change = sc[SC_MODEL_CHANGE];
+  if (step_ok) *step_ok = ok ? 1 : 0;
   return ICC_OK;
 }
 
@@ -1392,6 +1482,7 @@ icc_status icc_time_evaluations(icc_handle* h, int n, int flags, int with_jacobi
   if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
   CU(cudaSetDevice(h->device));
   icc_status s = configure(h, flags); if (s != ICC_OK) return s;
+  h->ne_flags = -1;                        // the single-family modes accumulate into the normal equations without zeroing them
   cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   CU(cudaMemsetAsync(h->d_scal.p, 0, SC_COUNT * sizeof(double), h->stream));
   CU(cudaEventRecord(e0, h->stream));

@@ -16,6 +16,7 @@
 //   root      one CTA factors the last block + the border (T_i_c, gravity, line delay, bias knots, ...) and solves them;
 // then the back-substitution walks the levels in reverse.  The sequential pivot chain is O(nk / P + kd log P) columns instead
 // of nk.  The last kernel forms the step and the model cost change.
+#include "../../include/icc_b200.h"
 #include "icc_device_math.cuh"
 #include "icc_kernels.h"
 
@@ -978,12 +979,12 @@ size_t smem_CR(const DeviceProblem& P, const SolvePlan& pl) {
 
 // Chunking of the knot columns: leaves cost their interior length in sequential column eliminations, every cyclic-reduction
 // level a dense w = kd column front plus two launches.
-// Wide borders (bias splines active) keep P = 1: the left-separator coupling would not fit the shared-memory window.
-int env_int(const char* name, int dflt) { const char* v = getenv(name); return v && *v ? atoi(v) : dflt; }
-SolvePlan make_plan(const DeviceProblem& P) {
+// A border too wide for shared memory first moves the dense border blocks to HBM and drops the level-0 staging; only if the plan
+// still does not fit, the chunk count is halved, down to P = 1 (see `fits` below).
+// forced_chunks > 0 replaces the planner's chunk count (clamped so that every leaf keeps >= kd + 1 columns).
+SolvePlan make_plan(const DeviceProblem& P, int forced_chunks) {
   SolvePlan pl; memset(&pl, 0, sizeof pl);
   const int nk = P.nk, kd = P.kd, nb = P.nb;
-  static const int forced_chunks = env_int("ICC_SOLVER_CHUNKS", 0), leaf_cols = env_int("ICC_SOLVER_LEAF", 0);
   int Pn = 1;
   if (nk > 0 && kd > 0) {
     // P = 2^k chunks give a complete elimination tree of k-1 reduction levels
@@ -995,7 +996,6 @@ SolvePlan make_plan(const DeviceProblem& P) {
       const double cost = 0.45 * len + 25.0 * std::max(0, k - 1) + (k > 0 ? 25.0 : 0.0);
       if (cost < best) { best = cost; Pn = Pc; }
     }
-    if (leaf_cols > 0) Pn = (nk + kd) / (leaf_cols + kd);
     if (forced_chunks > 0) Pn = forced_chunks;
     Pn = std::max(1, std::min(Pn, 1 << (MAX_LEVELS - 1)));
     while (Pn > 1 && (nk - (Pn - 1) * kd) / Pn < kd + 1) --Pn;
@@ -1035,10 +1035,25 @@ SolvePlan make_plan(const DeviceProblem& P) {
 
 }  // namespace
 
-size_t solve_workspace_doubles(const DeviceProblem& P) {
-  const SolvePlan pl = make_plan(P);
+size_t solve_workspace_doubles(const DeviceProblem& P, int forced_chunks) {
+  const SolvePlan pl = make_plan(P, forced_chunks);
   if (!pl.valid) return 16;
   return carve(nullptr, P.nk, P.nb, P.ldb, pl).total;
+}
+
+void solver_plan_info(const DeviceProblem& P, int forced_chunks, icc_solver_plan_info* out) {
+  const SolvePlan pl = make_plan(P, forced_chunks);
+  memset(out, 0, sizeof *out);
+  out->valid = pl.valid; out->nk = P.nk; out->kd = P.kd; out->nb = P.nb;
+  out->P = pl.P; out->len = pl.len; out->rem = pl.rem; out->L = pl.L;
+  out->cl_global = pl.cl_global; out->cs_global = pl.cs_global; out->stage0 = pl.stage0; out->WS_A = pl.WS_A;
+  out->max_leaf = pl.len + (pl.rem > 0 ? 1 : 0);
+  // backsub_kernel<true> stages chunk c when its interior (len + (c < rem) columns) fits the 128-column panel and stage0 is set
+  if (P.nk > 0 && pl.stage0) out->backsub0_staged = pl.len + 1 <= 128 ? pl.P : (pl.len <= 128 ? pl.P - pl.rem : 0);
+  for (int l = 1; l <= pl.L + 1 && l < 16; ++l) out->S[l] = pl.S[l];
+  out->smem_bytes[0] = (int64_t)smem_A(P, pl); out->smem_bytes[1] = (int64_t)smem_R(P, pl); out->smem_bytes[2] = (int64_t)smem_B(P, pl);
+  out->smem_bytes[3] = (int64_t)smem_C(P, pl); out->smem_bytes[4] = (int64_t)smem_CR(P, pl);
+  out->workspace_doubles = pl.valid ? (int64_t)carve(nullptr, P.nk, P.nb, P.ldb, pl).total : 0;
 }
 
 void launch_compute_scale(const DeviceProblem& P, double* scale, int jacobi, double* scal, cudaStream_t st) {
@@ -1048,8 +1063,8 @@ void launch_compute_scale(const DeviceProblem& P, double* scale, int jacobi, dou
   count_launch();
 }
 
-int launch_solve(const DeviceProblem& P, const double* scale, SolveParams sp, double* workspace, double* delta, double* scal, cudaStream_t st) {
-  const SolvePlan pl = make_plan(P);
+int launch_solve(const DeviceProblem& P, const double* scale, SolveParams sp, double* workspace, double* delta, double* scal, cudaStream_t st, int forced_chunks) {
+  const SolvePlan pl = make_plan(P, forced_chunks);
   if (!pl.valid) return 1;                       // border too wide / problem too small for any plan within the shared-memory limit
   const SolveWs ws = carve(workspace, P.nk, P.nb, P.ldb, pl);
   static size_t cfgA = 0, cfgR = 0, cfgB = 0, cfgC = 0, cfgCR = 0;
