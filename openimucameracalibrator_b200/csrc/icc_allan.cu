@@ -20,7 +20,7 @@
 //   The factor set, the accelerometer point filter and the initial values (a 5x5 least-squares problem) are host code.
 #include "../../include/icc_b200.h"
 #include "icc_allan_math.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
 
 #include <algorithm>
 #include <chrono>
@@ -30,8 +30,6 @@
 #include <vector>
 
 namespace icc {
-
-void count_launch();
 
 namespace {
 
@@ -43,13 +41,6 @@ constexpr int kGroupGrid = 1024;                               // grid.y: groups
 constexpr int kSmemDoubles = 3 * kTile + 3 * kSpan;
 constexpr int kFitSums = 21;                                   // 15 (upper triangle of J^T J) + 5 (J^T r) + r^T r
 constexpr int kFitOut = 10;                                    // x[5], initial cost, final cost, iterations, termination, successful
-
-template <class T>
-struct Buf {
-  T* p = nullptr;
-  ~Buf() { if (p) cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)); }
-};
 
 // the sample of channel c (0-2 accelerometer x, y, z as given; 3-5 gyroscope x, y, z pushed as rad/s, i.e. x * 57.3 * 3600)
 ICC_D double sample(const double* __restrict__ acc, const double* __restrict__ gyr, int c, size_t k) {
@@ -240,7 +231,7 @@ void default_allan_options(icc_allan_options* o) {
   o->n_clusters = 10000;   // AllanVarianceFitter(telemetry, 10000) (applications/fit_allan_variance.cc:41)
 }
 
-#define SCU(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e__); return ICC_ERR_CUDA; } } while (0)
+#define CU(call) ICC_CUDA_CHECK(call, err)
 
 icc_status allan_variance(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options& o,
                           double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6], allan::Curves& curves, std::string& err) {
@@ -267,28 +258,22 @@ icc_status allan_variance(cudaStream_t st, int n, const double* t, const double*
   for (int f = 0; f < F; ++f) { div[f] = allan::variance_divisor(period, m[f], n); curves.tau[f] = period * m[f]; }   // getTimes
   const int nslice = std::max(1, (n + kSlice - 1) / kSlice);
   // ---- theta and the variance of all six channels --------------------------------------------------------------------------------
-  Buf<double> d_acc, d_gyr, d_total, d_theta, d_partial, d_div, d_sigma2;
-  Buf<int> d_m, d_gfirst, d_gcount;
-  SCU(d_acc.alloc(3 * (size_t)n)); SCU(d_gyr.alloc(3 * (size_t)n));
-  SCU(d_total.alloc(6)); SCU(d_theta.alloc(6 * (size_t)n)); SCU(d_partial.alloc(6 * (size_t)F * nslice)); SCU(d_div.alloc(F));
-  SCU(d_sigma2.alloc(6 * (size_t)F)); SCU(d_m.alloc(F)); SCU(d_gfirst.alloc(G)); SCU(d_gcount.alloc(G));
-  SCU(cudaMemcpyAsync(d_acc.p, acc, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_gyr.p, gyr, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_m.p, m.data(), F * sizeof(int), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_gfirst.p, gfirst.data(), G * sizeof(int), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_gcount.p, gcount.data(), G * sizeof(int), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_div.p, div.data(), F * sizeof(double), cudaMemcpyHostToDevice, st));
+  DevBuf<double> d_acc, d_gyr, d_total, d_theta, d_partial, d_div, d_sigma2;
+  DevBuf<int> d_m, d_gfirst, d_gcount;
+  CU(d_acc.upload(acc, 3 * (size_t)n, st)); CU(d_gyr.upload(gyr, 3 * (size_t)n, st)); CU(d_m.upload(m.data(), F, st));
+  CU(d_gfirst.upload(gfirst.data(), G, st)); CU(d_gcount.upload(gcount.data(), G, st)); CU(d_div.upload(div.data(), F, st));
+  CU(d_total.alloc(6)); CU(d_theta.alloc(6 * (size_t)n)); CU(d_partial.alloc(6 * (size_t)F * nslice)); CU(d_sigma2.alloc(6 * (size_t)F));
   theta_kernel<<<6, 32, 0, st>>>(n, freq, d_acc.p, d_gyr.p, d_theta.p, d_total.p); count_launch();
   VarArgs V; V.theta = d_theta.p; V.m = d_m.p; V.gfirst = d_gfirst.p; V.gcount = d_gcount.p; V.partial = d_partial.p; V.n = n; V.F = F; V.G = G; V.nslice = nslice;
   const size_t smem = kSmemDoubles * sizeof(double);
-  SCU(cudaFuncSetAttribute(variance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU(cudaFuncSetAttribute(variance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   variance_kernel<<<dim3(nslice, std::min(G, kGroupGrid), 6), kThreads, smem, st>>>(V); count_launch();
   variance_finish_kernel<<<(6 * F + 255) / 256, 256, 0, st>>>(n, F, nslice, d_m.p, d_div.p, d_partial.p, d_sigma2.p); count_launch();
   std::vector<double> sig(6 * (size_t)F), total(6);
-  SCU(cudaMemcpyAsync(sig.data(), d_sigma2.p, sig.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  SCU(cudaMemcpyAsync(total.data(), d_total.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  SCU(cudaStreamSynchronize(st));
-  SCU(cudaGetLastError());
+  CU(cudaMemcpyAsync(sig.data(), d_sigma2.p, sig.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(total.data(), d_total.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
   // ---- fit points and initial values (host), the six fits (device) ------------------------------------------------------------
   FitArgs A; memset(&A, 0, sizeof A);
   std::vector<double> ptau, pl10;
@@ -304,16 +289,14 @@ icc_status allan_variance(cudaStream_t st, int n, const double* t, const double*
     for (size_t i = 0; i < s2.size(); ++i) { ptau.push_back(fit_tau[c][i]); pl10.push_back(std::log(s2[i]) / std::log(10.0)); }
   }
   A.off[6] = (int)ptau.size();
-  Buf<double> d_tau, d_l10, d_out;
-  SCU(d_tau.alloc(ptau.size())); SCU(d_l10.alloc(pl10.size())); SCU(d_out.alloc(6 * kFitOut));
-  SCU(cudaMemcpyAsync(d_tau.p, ptau.data(), ptau.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_l10.p, pl10.data(), pl10.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  DevBuf<double> d_tau, d_l10, d_out;
+  CU(d_tau.upload(ptau.data(), ptau.size(), st)); CU(d_l10.upload(pl10.data(), pl10.size(), st)); CU(d_out.alloc(6 * kFitOut));
   A.tau = d_tau.p; A.l10s = d_l10.p; A.out = d_out.p;
   fit_kernel<<<6, kThreads, 0, st>>>(A); count_launch();
   std::vector<double> out(6 * kFitOut);
-  SCU(cudaMemcpyAsync(out.data(), d_out.p, out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  SCU(cudaStreamSynchronize(st));
-  SCU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out.data(), d_out.p, out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
   // ---- derived quantities (RunFit and the FitAllan* constructors' output) -------------------------------------------------------
   const int launches = kernel_launch_count() - launches0;
   const double seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count();

@@ -10,7 +10,7 @@
 #include "../../include/icc_b200.h"
 #include "icc_allan_math.cuh"
 #include "icc_camera.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
 #include "icc_trust_region.cuh"
 
 #include <algorithm>
@@ -19,63 +19,17 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 using namespace icc;
 
-namespace icc {   // icc_static_imu.cu
-void default_static_imu_options(icc_static_imu_options* o);
-icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_static_imu_options& o,
-                                double acc_out[9], double gyr_out[9], double bias_out[3], icc_static_imu_summary& S, std::vector<int32_t>& intervals, std::string& err);
-// icc_allan.cu
-void default_allan_options(icc_allan_options* o);
-icc_status allan_variance(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options& o,
-                          double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6], allan::Curves& curves, std::string& err);
-}  // namespace icc
 
 namespace {
 
 constexpr double S_TO_NS = 1e9, NS_TO_S = 1e-9;
-
-// Process-wide caching allocator for device blocks: a calibration job allocates ~30 buffers and the CUDA driver's
-// cudaMalloc / cudaFree cost 0.1-1 ms each, which would dominate the whole-job wall clock of back-to-back jobs.
-// Freed blocks are kept (per device) and handed out again best-fit; icc_trim_device_cache() returns them to the driver.
-struct BlockCache {
-  std::mutex mu;
-  std::multimap<size_t, std::pair<int, void*>> free_blocks;   // bytes -> (device, ptr)
-  cudaError_t get(size_t bytes, void** out) {
-    int dev = 0; cudaGetDevice(&dev);
-    {
-      std::lock_guard<std::mutex> lk(mu);
-      for (auto it = free_blocks.lower_bound(bytes); it != free_blocks.end() && it->first <= 2 * bytes + 4096; ++it)
-        if (it->second.first == dev) { *out = it->second.second; free_blocks.erase(it); return cudaSuccess; }
-    }
-    return cudaMalloc(out, bytes);
-  }
-  void put(size_t bytes, void* p) { int dev = 0; cudaGetDevice(&dev); std::lock_guard<std::mutex> lk(mu); free_blocks.emplace(bytes, std::make_pair(dev, p)); }
-  void trim() { std::lock_guard<std::mutex> lk(mu); for (auto& kv : free_blocks) { cudaSetDevice(kv.second.first); cudaFree(kv.second.second); } free_blocks.clear(); }
-};
-BlockCache& block_cache() { static BlockCache* c = new BlockCache(); return *c; }   // intentionally leaked: outlives every handle
-
-template <class T>
-struct DevBuf {
-  T* p = nullptr; size_t n = 0, cap_bytes = 0;
-  ~DevBuf() { release(); }
-  void release() { if (p) block_cache().put(cap_bytes, p); p = nullptr; n = 0; cap_bytes = 0; }
-  cudaError_t alloc(size_t count) {
-    const size_t bytes = (count * sizeof(T) + 255) / 256 * 256;
-    if (p && cap_bytes >= bytes) { n = count; return cudaSuccess; }
-    release(); n = count; if (!count) return cudaSuccess;
-    void* q = nullptr; cudaError_t e = block_cache().get(bytes, &q); if (e != cudaSuccess) { n = 0; return e; }
-    p = static_cast<T*>(q); cap_bytes = bytes; return cudaSuccess;
-  }
-  cudaError_t upload(const std::vector<T>& v) { cudaError_t e = alloc(v.size()); if (e != cudaSuccess || v.empty()) return e; return cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice); }
-};
 
 // Host staging of the large measurement arrays (corners, IMU samples): page-locked blocks from a process-wide cache (the first
 // job pays cudaHostAlloc, later ones reuse), so that the uploads of BatchInitSpline are asynchronous DMA transfers that overlap the
@@ -220,8 +174,15 @@ struct PhaseTrace {
     t = std::chrono::steady_clock::now();
   }
 };
-#define CU(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return fail(h, ICC_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e__)); } while (0)
+#define CU(call) ICC_CUDA_CHECK(call, h->err)
 #define NEED_DEVICE() do { if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device bound to this handle (host-only handle): compute entry points are unavailable"); } while (0)
+// Runs an upstream tool's host driver (icc_host.h) on the handle's device; a failed driver's message becomes the handle's error.
+template <class F> icc_status drive(icc_handle* h, F driver) {
+  CU(cudaSetDevice(h->device));
+  std::string err;
+  const icc_status rc = driver(err);
+  return rc == ICC_OK ? rc : fail(h, rc, err);
+}
 
 Q4 qn(const double* q) { return qnormalized(q4(q[0], q[1], q[2], q[3])); }
 
@@ -234,17 +195,6 @@ bool calc_times(int64_t sensor_ns, int64_t start_ns, int64_t dt_ns, size_t nr_kn
   if (size_t(s + N) > nr_knots) return false;
   u = double(st % dt_ns) / double(dt_ns);
   return true;
-}
-
-// CSR by board point of the corners selected by `take(c)`: pt_off[np + 1], pt_obs[...] (counting sort, stable in corner order)
-template <class F>
-void build_point_adjacency(int np, int nc, const int32_t* ids, F take, std::vector<int>& pt_off, std::vector<int>& pt_obs) {
-  pt_off.assign(np + 1, 0);
-  for (int c = 0; c < nc; ++c) if (take(c)) ++pt_off[ids[c] + 1];
-  for (int p = 0; p < np; ++p) pt_off[p + 1] += pt_off[p];
-  pt_obs.resize(pt_off[np]);
-  std::vector<int> fill(pt_off.begin(), pt_off.end() - 1);
-  for (int c = 0; c < nc; ++c) if (take(c)) pt_obs[fill[ids[c]]++] = c;
 }
 
 size_t nearest_index(double t, const std::vector<double>& ts, double& dist_out) {   // utils.cc:194-212
@@ -1505,76 +1455,28 @@ icc_status icc_time_evaluations(icc_handle* h, int n, int flags, int with_jacobi
 }
 
 void* icc_get_stream(icc_handle* h) { return h ? (void*)h->stream : nullptr; }
-// ---- upstream row f1: per-view board poses ---------------------------------------------------------------------------
+// ---- upstream row f1: per-view board poses (icc_pose.cu) ----------------------------------------------------------------
 icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, double* xy_out, int32_t* ok) {
   if (!h || n < 0 || (n > 0 && (!uv || !xy_out))) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+  NEED_DEVICE();
   if (h->model < 0) return fail(h, ICC_ERR_STATE, "icc_set_camera must be called first");
   if (n == 0) return ICC_OK;
-  CU(cudaSetDevice(h->device));
-  DevBuf<double2> d_uv, d_xy; DevBuf<int> d_ok;
-  CU(d_uv.alloc(n)); CU(d_xy.alloc(n)); CU(d_ok.alloc(n));
-  CU(cudaMemcpyAsync(d_uv.p, uv, (size_t)n * sizeof(double2), cudaMemcpyHostToDevice, h->stream));
-  launch_unproject(h->model, h->intr, n, d_uv.p, d_xy.p, d_ok.p, h->stream);
-  CU(cudaMemcpyAsync(xy_out, d_xy.p, (size_t)n * sizeof(double2), cudaMemcpyDeviceToHost, h->stream));
-  std::vector<int> okh(ok ? n : 0);
-  if (ok) CU(cudaMemcpyAsync(okh.data(), d_ok.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  if (ok) for (int i = 0; i < n; ++i) ok[i] = okh[i];
-  return ICC_OK;
+  return drive(h, [&](std::string& err) { return pixels_to_normalized(h->stream, h->model, h->intr, n, uv, xy_out, ok, err); });
 }
 
-icc_status icc_estimate_board_poses(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points,
-                                    double* q_wc, double* p_wc, double* mean_err, int32_t* valid) {
+icc_status icc_estimate_board_poses(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points, double* q_wc, double* p_wc, double* mean_err, int32_t* valid) {
   if (!h || nf <= 0 || !off || !ids || !uv || !q_wc || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+  NEED_DEVICE();
   if (h->model < 0 || h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_camera and icc_set_board_points must be called first");
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
-  const int nc = off[nf] - off[0];
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
-  CU(cudaSetDevice(h->device));
-  const int np = (int)(h->points.size() / 4);
-  std::vector<double4> board(np);
-  for (int i = 0; i < np; ++i) board[i] = make_double4(h->points[4 * i], h->points[4 * i + 1], h->points[4 * i + 2], h->points[4 * i + 3]);
-  DevBuf<double4> d_board; DevBuf<int> d_off, d_pid, d_ok, d_valid; DevBuf<double2> d_uv, d_xy; DevBuf<unsigned char> d_use; DevBuf<double> d_q, d_p, d_e;
-  CU(d_board.upload(board));
-  CU(d_off.alloc(nf + 1)); CU(d_pid.alloc(std::max(1, nc))); CU(d_uv.alloc(std::max(1, nc))); CU(d_xy.alloc(std::max(1, nc))); CU(d_ok.alloc(std::max(1, nc))); CU(d_use.alloc(std::max(1, nc)));
-  CU(d_q.alloc(4 * (size_t)nf)); CU(d_p.alloc(3 * (size_t)nf)); CU(d_e.alloc(nf)); CU(d_valid.alloc(nf));
-  CU(cudaMemcpyAsync(d_off.p, off, (size_t)(nf + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  if (nc > 0) {
-    CU(cudaMemcpyAsync(d_pid.p, ids, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(d_uv.p, uv, (size_t)nc * sizeof(double2), cudaMemcpyHostToDevice, h->stream));
-  }
-  launch_unproject(h->model, h->intr, nc, d_uv.p, d_xy.p, d_ok.p, h->stream);
-  PoseProblem Q; memset(&Q, 0, sizeof Q);
-  Q.model = h->model; for (int i = 0; i < 10; ++i) Q.intr[i] = h->intr[i];
-  Q.n_frames = nf; Q.n_points = np; Q.min_points = min_points > 0 ? min_points : 8;
-  Q.board = d_board.p; Q.f_off = d_off.p; Q.pid = d_pid.p;
-  const double W = h->width, H = h->height;
-  const double max_px = max_reproj_error > 0.0 ? max_reproj_error : 0.004 * H;            // pose_estimator.cc:97
-  Q.thresh_sq = (W > 0 && H > 0) ? max_px / std::sqrt(W * W + H * H) : 1e-3;               // :101 (compared with a SQUARED error by theia's RANSAC)
-  Q.max_err = max_px;                                                                       // :181 (pixels against a normalised error, as in the reference)
-  launch_board_poses(Q, d_xy.p, d_ok.p, d_use.p, d_q.p, d_p.p, d_e.p, d_valid.p, h->stream);
-  std::vector<double> eh(nf); std::vector<int> vh(nf);
-  CU(cudaMemcpyAsync(q_wc, d_q.p, 4 * (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaMemcpyAsync(p_wc, d_p.p, 3 * (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaMemcpyAsync(eh.data(), d_e.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaMemcpyAsync(vh.data(), d_valid.p, (size_t)nf * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  if (cudaGetLastError() != cudaSuccess) return fail(h, ICC_ERR_CUDA, "pose kernels failed");
-  for (int i = 0; i < nf; ++i) { valid[i] = vh[i]; if (mean_err) mean_err[i] = eh[i]; }
-  return ICC_OK;
+  return drive(h, [&](std::string& err) { return estimate_board_poses(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
+                                q_wc, p_wc, mean_err, valid, err); });
 }
 
 icc_status icc_filter_bad_poses(icc_handle* h, int nv, const double* p_wc, int32_t* valid) {
   if (nv <= 0 || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
-  std::vector<double> z; for (int i = 0; i < nv; ++i) if (valid[i]) z.push_back(p_wc[3 * i + 2]);
-  if (z.empty()) return ICC_OK;
-  const size_t n = z.size(); double med;   // utils::MedianOfDoubleVec (src/utils/utils.cc:77-97)
-  if (n % 2 == 0) { std::nth_element(z.begin(), z.begin() + n / 2 - 1, z.end()); const double e1 = z[n / 2 - 1]; std::nth_element(z.begin(), z.begin() + n / 2, z.end()); med = (e1 + z[n / 2]) / 2; }
-  else { std::nth_element(z.begin(), z.begin() + n / 2, z.end()); med = z[n / 2]; }
-  for (int i = 0; i < nv; ++i) if (valid[i] && std::fabs(p_wc[3 * i + 2] - med) > std::fabs(med)) valid[i] = 0;
-  (void)h;
+  filter_bad_poses(nv, p_wc, valid);
   return ICC_OK;
 }
 
@@ -1589,558 +1491,61 @@ icc_status icc_get_board_points(const icc_handle* h, double* xyzw, int n) {
 icc_status icc_optimize_board_points(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points,
                                      int min_observations, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, double* board_out, int32_t* n_opt_out) {
   if (!h || nf <= 0 || !off || !ids || !uv || !q_wc || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+  NEED_DEVICE();
   if (h->model < 0 || h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_camera and icc_set_board_points must be called first");
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
-  const int nc = off[nf], np = (int)(h->points.size() / 4);
-  CU(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  std::vector<double4> board(np);
-  for (int i = 0; i < np; ++i) board[i] = make_double4(h->points[4 * i], h->points[4 * i + 1], h->points[4 * i + 2], h->points[4 * i + 3]);
-  std::vector<int> obs_view(std::max(1, nc));
-  for (int f = 0; f < nf; ++f) for (int c = off[f]; c < off[f + 1]; ++c) obs_view[c] = f;
-  DevBuf<double4> d_board, d_board2; DevBuf<int> d_off, d_pid, d_ok, d_valid, d_view, d_pt_off, d_pt_obs, d_opt; DevBuf<double2> d_uv, d_xy; DevBuf<unsigned char> d_use;
-  DevBuf<double> d_q, d_p, d_e, d_qcw, d_c;
-  CU(d_board.upload(board)); CU(d_board2.alloc(np)); CU(d_opt.alloc(np));
-  CU(d_off.alloc(nf + 1)); CU(d_pid.alloc(std::max(1, nc))); CU(d_uv.alloc(std::max(1, nc))); CU(d_xy.alloc(std::max(1, nc))); CU(d_ok.alloc(std::max(1, nc))); CU(d_use.alloc(std::max(1, nc)));
-  CU(d_q.alloc(4 * (size_t)nf)); CU(d_p.alloc(3 * (size_t)nf)); CU(d_e.alloc(nf)); CU(d_valid.alloc(nf)); CU(d_view.upload(obs_view));
-  CU(cudaMemcpyAsync(d_off.p, off, (size_t)(nf + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (nc > 0) {
-    CU(cudaMemcpyAsync(d_pid.p, ids, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_uv.p, uv, (size_t)nc * sizeof(double2), cudaMemcpyHostToDevice, st));
-  }
-  CU(cudaMemcpyAsync(d_q.p, q_wc, 4 * (size_t)nf * sizeof(double), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_p.p, p_wc, 3 * (size_t)nf * sizeof(double), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_valid.p, valid, (size_t)nf * sizeof(int), cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(d_e.p, 0, (size_t)nf * sizeof(double), st));   // views that are not valid keep a zero error
-  launch_unproject(h->model, h->intr, nc, d_uv.p, d_xy.p, d_ok.p, st);
-  PoseProblem Q; memset(&Q, 0, sizeof Q);
-  Q.model = h->model; for (int i = 0; i < 10; ++i) Q.intr[i] = h->intr[i];
-  Q.n_frames = nf; Q.n_points = np; Q.min_points = min_points > 0 ? min_points : 8;
-  Q.board = d_board.p; Q.f_off = d_off.p; Q.pid = d_pid.p; Q.refine_only = 1;
-  const double W = h->width, H = h->height;
-  const double max_px = max_reproj_error > 0.0 ? max_reproj_error : 0.004 * H;
-  Q.thresh_sq = (W > 0 && H > 0) ? max_px / std::sqrt(W * W + H * H) : 1e-3;
-  Q.max_err = max_px;
-  // 1. the stored poses and their inlier sets (what the pose dataset holds after EstimatePosesFromJson)
-  launch_board_poses(Q, d_xy.p, d_ok.p, d_use.p, d_q.p, d_p.p, d_e.p, d_valid.p, st);
-  std::vector<unsigned char> use(std::max(1, nc)); std::vector<int> vh(nf); std::vector<double> qh(4 * (size_t)nf), ph(3 * (size_t)nf);
-  CU(cudaMemcpyAsync(use.data(), d_use.p, (size_t)std::max(1, nc), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(vh.data(), d_valid.p, (size_t)nf * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(qh.data(), d_q.p, qh.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(ph.data(), d_p.p, ph.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  // 2. OptimizeBoardPoints: one warp per point over its inlier observations in valid views, cameras constant
-  std::vector<int> pt_off, pt_obs;
-  build_point_adjacency(np, nc, ids, [&](int c) { return use[c] && vh[obs_view[c]]; }, pt_off, pt_obs);
-  std::vector<double> qcw(4 * (size_t)nf);
-  for (int f = 0; f < nf; ++f) { qcw[4 * f] = -qh[4 * f]; qcw[4 * f + 1] = -qh[4 * f + 1]; qcw[4 * f + 2] = -qh[4 * f + 2]; qcw[4 * f + 3] = qh[4 * f + 3]; }
-  CU(d_qcw.upload(qcw)); CU(d_c.upload(ph)); CU(d_pt_off.upload(pt_off)); CU(d_pt_obs.alloc(std::max<size_t>(1, pt_obs.size())));
-  if (!pt_obs.empty()) CU(cudaMemcpy(d_pt_obs.p, pt_obs.data(), pt_obs.size() * sizeof(int), cudaMemcpyHostToDevice));
-  PointProblem PQ; memset(&PQ, 0, sizeof PQ);
-  PQ.model = h->model; for (int i = 0; i < 10; ++i) PQ.intr[i] = h->intr[i];
-  PQ.normalized = 1; PQ.n_points = np; PQ.min_obs = min_observations > 0 ? min_observations : 30; PQ.huber = 1.345;
-  PQ.board_in = d_board.p; PQ.pt_off = d_pt_off.p; PQ.pt_obs = d_pt_obs.p; PQ.obs_view = d_view.p; PQ.meas = d_xy.p; PQ.q_cw = d_qcw.p; PQ.cam_c = d_c.p;
-  launch_point_refine(PQ, d_board2.p, d_opt.p, st);
-  // 3. OptimizeAllPoses on the new points
-  Q.board = d_board2.p;
-  launch_board_poses(Q, d_xy.p, d_ok.p, d_use.p, d_q.p, d_p.p, d_e.p, d_valid.p, st);
-  std::vector<double> eh(nf); std::vector<int> opt(np);
-  CU(cudaMemcpyAsync(board.data(), d_board2.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(opt.data(), d_opt.p, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(q_wc, d_q.p, 4 * (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(p_wc, d_p.p, 3 * (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(eh.data(), d_e.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(vh.data(), d_valid.p, (size_t)nf * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  if (cudaGetLastError() != cudaSuccess) return fail(h, ICC_ERR_CUDA, "board point kernels failed");
-  int n_opt = 0;
-  for (int i = 0; i < np; ++i) { h->points[4 * i] = board[i].x; h->points[4 * i + 1] = board[i].y; h->points[4 * i + 2] = board[i].z; h->points[4 * i + 3] = board[i].w; n_opt += opt[i]; }
+  std::vector<double> points;
+  const icc_status rc = drive(h, [&](std::string& err) { return optimize_board_points(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
+                                 min_observations, q_wc, p_wc, mean_err, valid, points, n_opt_out, err); });
+  if (rc != ICC_OK) return rc;
+  h->points.swap(points);
   if (board_out) std::copy(h->points.begin(), h->points.end(), board_out);
-  if (n_opt_out) *n_opt_out = n_opt;
-  for (int i = 0; i < nf; ++i) { valid[i] = vh[i]; if (mean_err) mean_err[i] = eh[i]; }
   return ICC_OK;
 }
 
-// ---- upstream row f3: IMU-to-camera rotation + time offset initialiser ---------------------------------------------------
-namespace {
-double median_like_reference(std::vector<double> v) {   // utils::MedianOfDoubleVec (src/utils/utils.cc:77-97)
-  const size_t n = v.size();
-  if (n % 2 == 0) {
-    std::nth_element(v.begin(), v.begin() + n / 2 - 1, v.end()); const double e1 = v[n / 2 - 1];
-    std::nth_element(v.begin(), v.begin() + n / 2, v.end()); const double e2 = v[n / 2];
-    return (e1 + e2) / 2;
-  }
-  std::nth_element(v.begin(), v.begin() + n / 2, v.end());
-  return v[n / 2];
-}
-void quat_from_rowmajor(const double* R, double* q) {    // -> x, y, z, w
-  const double m00 = R[0], m01 = R[1], m02 = R[2], m10 = R[3], m11 = R[4], m12 = R[5], m20 = R[6], m21 = R[7], m22 = R[8], tr = m00 + m11 + m22;
-  double x, y, z, w;
-  if (tr > 0.0) { const double s = std::sqrt(tr + 1.0) * 2.0; w = 0.25 * s; x = (m21 - m12) / s; y = (m02 - m20) / s; z = (m10 - m01) / s; }
-  else if (m00 > m11 && m00 > m22) { const double s = std::sqrt(1.0 + m00 - m11 - m22) * 2.0; w = (m21 - m12) / s; x = 0.25 * s; y = (m01 + m10) / s; z = (m02 + m20) / s; }
-  else if (m11 > m22) { const double s = std::sqrt(1.0 + m11 - m00 - m22) * 2.0; w = (m02 - m20) / s; x = (m01 + m10) / s; y = 0.25 * s; z = (m12 + m21) / s; }
-  else { const double s = std::sqrt(1.0 + m22 - m00 - m11) * 2.0; w = (m10 - m01) / s; x = (m02 + m20) / s; y = (m12 + m21) / s; z = 0.25 * s; }
-  const double n = std::sqrt(x * x + y * y + z * z + w * w);
-  q[0] = x / n; q[1] = y / n; q[2] = z / n; q[3] = w / n;
-}
-}  // namespace
-
+// ---- upstream row f3: IMU-to-camera rotation + time offset initialiser (icc_rotinit.cu) --------------------------------------
 icc_status icc_estimate_imu_to_camera_rotation(icc_handle* h, int n_views, const double* view_t, const double* q_cw, int n_imu, const double* imu_t,
                                                const double* gyro, const double* bias_in, double* q_out, double* td_out, double* bias_out, double* err_out, int32_t* iters_out) {
   if (!h || n_views < 2 || !view_t || !q_cw || n_imu < 2 || !imu_t || !gyro || !q_out || !td_out) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
-  CU(cudaSetDevice(h->device));
-  // ---- host preparation (app :96-162): ordered maps, median frame interval, regular grid, common window ------------------
-  // std::map semantics of the reference (time ordered, a repeated timestamp keeps the LAST sample); already-sorted input -- the
-  // normal case -- skips the tree
-  auto ordered = [](const double* t, int n) { std::vector<std::pair<double, int>> o; o.reserve(n);
-    bool inc = true; for (int i = 1; i < n && inc; ++i) inc = t[i] > t[i - 1];
-    if (inc) { for (int i = 0; i < n; ++i) o.emplace_back(t[i], i); return o; }
-    std::map<double, int> m; for (int i = 0; i < n; ++i) m[t[i]] = i;
-    for (const auto& kv : m) o.emplace_back(kv.first, kv.second);
-    return o; };
-  const std::vector<std::pair<double, int>> vmap = ordered(view_t, n_views), gmap = ordered(imu_t, n_imu);
-  if (vmap.size() < 2 || gmap.size() < 2) return fail(h, ICC_ERR_INVALID_ARGUMENT, "need at least two distinct view and gyroscope timestamps");
-  double imu_dt = 0.0;
-  for (int i = 1; i < n_imu; ++i) imu_dt += imu_t[i] - imu_t[i - 1];                     // app :103-108 (file order)
-  imu_dt /= (double)(n_imu - 1);
-  std::vector<double> tv; std::vector<double4> qv;
-  for (const auto& kv : vmap) { tv.push_back(kv.first); const double* q = q_cw + 4 * (size_t)kv.second; qv.push_back(make_double4(q[0], q[1], q[2], q[3])); }
-  std::vector<double> diffs; for (size_t i = 1; i < tv.size(); ++i) diffs.push_back(tv[i] - tv[i - 1]);
-  const double cam_dt = median_like_reference(diffs);
-  if (!(cam_dt > 0.0)) return fail(h, ICC_ERR_INVALID_ARGUMENT, "non-positive median frame interval");
-  std::vector<double> grid; for (double t = tv.front(); t < tv.back(); t += cam_dt) grid.push_back(t);   // app :139-144
-  std::vector<double> tg, gg;    // gyroscope, time ordered, bias removed
-  for (const auto& kv : gmap) { tg.push_back(kv.first); for (int d = 0; d < 3; ++d) gg.push_back(gyro[3 * (size_t)kv.second + d] - (bias_in ? bias_in[d] : 0.0)); }
-  const double t0 = grid.front() >= tg.front() ? grid.front() : tg.front();               // :127-129
-  const double tend = grid.back() >= tg.back() ? grid.back() : tg.back();                 // (the LATER end, as in the reference)
-  std::vector<double> tI, wI; for (size_t i = 0; i < tg.size(); ++i) if (tg[i] >= t0 && tg[i] <= tend) { tI.push_back(tg[i] - t0); for (int d = 0; d < 3; ++d) wI.push_back(gg[3 * i + d]); }
-  size_t g0 = 0; while (g0 < grid.size() && grid[g0] < t0) ++g0;
-  std::vector<double> tV; for (size_t i = g0; i < grid.size(); ++i) if (grid[i] <= tend) tV.push_back(grid[i] - t0);
-  const int N = (int)tI.size(), Mc = (int)tV.size(), M = (int)grid.size(), nv = (int)tv.size();
-  if (N < 2 || Mc < 1) return fail(h, ICC_ERR_INVALID_ARGUMENT, "camera and gyroscope streams do not overlap");
-  // ---- device pipeline --------------------------------------------------------------------------------------------------
-  DevBuf<double> d_tv, d_grid, d_tV, d_tI, d_wI, d_wraw, d_wheld, d_wvis, d_wimu, d_shift; DevBuf<double4> d_qv, d_qgrid, d_qi; DevBuf<unsigned char> d_bad; DevBuf<RotInitState> d_state;
-  CU(d_tv.upload(tv)); CU(d_qv.upload(qv)); CU(d_grid.upload(grid)); CU(d_tV.upload(tV)); CU(d_tI.upload(tI)); CU(d_wI.upload(wI));
-  CU(d_qgrid.alloc(M)); CU(d_qi.alloc(N)); CU(d_wraw.alloc(3 * (size_t)N)); CU(d_wheld.alloc(3 * (size_t)N)); CU(d_wvis.alloc(3 * (size_t)N)); CU(d_wimu.alloc(3 * (size_t)N));
-  CU(d_shift.alloc(6 * (size_t)N)); CU(d_bad.alloc(N)); CU(d_state.alloc(1));
-  launch_interp_quat(nv, d_tv.p, d_qv.p, M, d_grid.p, d_qgrid.p, h->stream);              // views -> regular frame grid (app :150-156)
-  launch_interp_quat(Mc, d_tV.p, d_qgrid.p + g0, N, d_tI.p, d_qi.p, h->stream);           // grid -> IMU rate (:172-173)
-  launch_visual_angular_velocity(N, d_qi.p, imu_dt, d_wraw.p, d_bad.p, d_wheld.p, d_wvis.p, d_wI.p, d_wimu.p, h->stream);
-  RotInitProblem Q; memset(&Q, 0, sizeof Q);
-  Q.n = N; Q.t = d_tI.p; Q.vis = d_wvis.p; Q.imu = d_wimu.p; Q.vis_shift = d_shift.p; Q.state = d_state.p;
-  Q.estimate_bias = bias_in ? 0 : 1; Q.tolerance = 1e-4;
-  for (int d = 0; d < 3; ++d) Q.bias_in[d] = bias_in ? bias_in[d] : 0.0;
-  // the bracket shrinks by the golden ratio per step whatever the data says, so the step count is known up to rounding
-  int n_it = 0; { const double g = (1.0 + std::sqrt(5.0)) / 2.0; double a = -1.0, b = 1.0, c = b - (b - a) / g, d = a + (b - a) / g; while (std::fabs(c - d) > Q.tolerance && n_it < 200) { b = d; c = b - (b - a) / g; d = a + (b - a) / g; ++n_it; } }
-  launch_golden_section(Q, 1.0, n_it + 2, h->sm_count > 0 ? h->sm_count : 132, h->stream);
-  RotInitState S;
-  CU(cudaMemcpyAsync(&S, d_state.p, sizeof S, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  if (cudaGetLastError() != cudaSuccess) return fail(h, ICC_ERR_CUDA, "rotation initialiser kernels failed");
-  if (!S.done) return fail(h, ICC_ERR_NUMERIC, "golden-section search did not terminate");
-  quat_from_rowmajor(S.R_best, q_out);
-  *td_out = (S.b + S.a) / 2;                                                               // :259
-  if (bias_out) for (int d = 0; d < 3; ++d) bias_out[d] = S.bias_best[d];
-  if (err_out) *err_out = S.error;
-  if (iters_out) *iters_out = S.iterations;
-  return ICC_OK;
+  NEED_DEVICE();
+  return drive(h, [&](std::string& err) { return estimate_imu_to_camera_rotation(h->stream, h->sm_count, n_views, view_t, q_cw, n_imu, imu_t, gyro, bias_in, q_out, td_out, bias_out, err_out, iters_out, err); });
 }
 
-// ---- upstream row f2: spline error weighting -----------------------------------------------------------------------------
-namespace {
-// scipy.optimize.brentq (Brent 1973 as implemented in scipy/optimize/Zeros/brentq.c), xtol = 2e-12, rtol = 4 eps, 100 iterations
-double brentq(const std::function<double(double)>& f, double xa, double xb, bool& ok) {
-  const double xtol = 2e-12, rtol = 8.881784197001252e-16;
-  double xpre = xa, xcur = xb, xblk = 0.0, fpre = f(xpre), fcur = f(xcur), fblk = 0.0, spre = 0.0, scur = 0.0;
-  ok = true;
-  if (fpre == 0.0) return xpre;
-  if (fcur == 0.0) return xcur;
-  if ((fpre > 0) == (fcur > 0)) { ok = false; return xcur; }
-  for (int i = 0; i < 100; ++i) {
-    if (fpre != 0.0 && fcur != 0.0 && ((fpre > 0) != (fcur > 0))) { xblk = xpre; fblk = fpre; spre = scur = xcur - xpre; }
-    if (std::fabs(fblk) < std::fabs(fcur)) { xpre = xcur; xcur = xblk; xblk = xpre; fpre = fcur; fcur = fblk; fblk = fpre; }
-    const double delta = (xtol + rtol * std::fabs(xcur)) / 2, sbis = (xblk - xcur) / 2;
-    if (fcur == 0.0 || std::fabs(sbis) < delta) return xcur;
-    if (std::fabs(spre) > delta && std::fabs(fcur) < std::fabs(fpre)) {
-      double stry;
-      if (xpre == xblk) stry = -fcur * (xcur - xpre) / (fcur - fpre);                       // secant
-      else { const double dpre = (fpre - fcur) / (xpre - xcur), dblk = (fblk - fcur) / (xblk - xcur); stry = -fcur * (fblk * dblk - fpre * dpre) / (dblk * dpre * (fblk - fpre)); }   // inverse quadratic
-      if (2 * std::fabs(stry) < std::min(std::fabs(spre), 3 * std::fabs(sbis) - delta)) { spre = scur; scur = stry; }
-      else { spre = sbis; scur = sbis; }
-    } else { spre = sbis; scur = sbis; }
-    xpre = xcur; fpre = fcur;
-    if (std::fabs(scur) > delta) xcur += scur; else xcur += (sbis > 0 ? delta : -delta);
-    fcur = f(xcur);
-  }
-  ok = false;
-  return xcur;
-}
-}  // namespace
-
-icc_status icc_spline_error_weighting(icc_handle* h, int n, const double* times, const double* signal, double quality, double min_dt, double max_dt,
-                                      double* dt_out, double* var_out, double* spectrum) {
+// ---- upstream row f2: spline error weighting (icc_sew.cu) -----------------------------------------------------------------------
+icc_status icc_spline_error_weighting(icc_handle* h, int n, const double* times, const double* signal, double quality, double min_dt, double max_dt, double* dt_out, double* var_out, double* spectrum) {
   if (!h || n < 4 || !times || !signal || !dt_out || !var_out || !(quality > 0.0 && quality < 1.0)) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
-  CU(cudaSetDevice(h->device));
-  double mean_dt = 0.0; for (int i = 1; i < n; ++i) mean_dt += times[i] - times[i - 1]; mean_dt /= (double)(n - 1);
-  if (!(mean_dt > 0.0)) return fail(h, ICC_ERR_INVALID_ARGUMENT, "timestamps must increase on average");
-  const double sample_rate = 1.0 / mean_dt, d = 1.0 / sample_rate, fscale = 1.0 / ((double)n * d);   // np.fft.fftfreq(n, d): k * (1 / (n d))
-  if (!(min_dt > 0.0)) min_dt = 1.0 / sample_rate;                                                     // sew.py:156-160
-  if (!(max_dt > 0.0)) max_dt = ((double)n / 4.0) / sample_rate;
-  const int M = sew_fft_length(n);
-  DevBuf<double> d_sig, d_xhat, d_scr, d_acc;
-  CU(d_sig.alloc(3 * (size_t)n)); CU(d_xhat.alloc(n)); CU(d_scr.alloc(16 * (size_t)M)); CU(d_acc.alloc(2));
-  CU(cudaMemcpyAsync(d_sig.p, signal, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  launch_sew_spectrum(n, d_sig.p, d_xhat.p, d_acc.p, d_scr.p, h->stream);
-  double esum = 0.0;
-  CU(cudaMemcpyAsync(&esum, d_acc.p, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  if (spectrum) CU(cudaMemcpyAsync(spectrum, d_xhat.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  if (cudaGetLastError() != cudaSuccess) return fail(h, ICC_ERR_CUDA, "spectrum kernels failed");
-  const double max_remove = esum / (double)n * (1.0 - quality);                                        // signal_energy(Xhat) * (1 - quality)
-  bool cuda_ok = true;
-  auto removed = [&](double dt) -> double {      // signal_energy((1 - H) * Xhat)
-    double e = 0.0;
-    launch_sew_residual_energy(n, d_xhat.p, fscale, dt, d_acc.p + 1, h->sm_count > 0 ? h->sm_count : 132, h->stream);
-    if (cudaMemcpyAsync(&e, d_acc.p + 1, sizeof(double), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess || cudaStreamSynchronize(h->stream) != cudaSuccess) cuda_ok = false;
-    return e / (double)n;
-  };
-  auto quality_func = [&](double dt) { return max_remove / removed(dt); };
-  // find_max_quality_dt(quality_func, 1.0, min_dt, max_dt)   (sew.py:86-145)
-  double dt = max_dt, found = 0.0; bool have = false;
-  if (quality_func(dt) >= 1.0) { found = dt; have = true; }
-  else {
-    double step = max_dt * 0.5, max_quality = 0.0, max_quality_dt = dt; bool any = false;
-    while (!have) {
-      dt -= step; dt = std::max(dt, min_dt);
-      const double q = quality_func(dt);
-      if (q > 1.0) { bool ok; found = brentq([&](double x) { return quality_func(x) - 1.0; }, dt, max_dt, ok); if (!ok) return fail(h, ICC_ERR_NUMERIC, "Brent root search failed"); have = true; }
-      else {
-        step *= 0.5;
-        if (q > max_quality) { max_quality = q; max_quality_dt = dt; any = true; }
-        if (dt <= min_dt) { if (!any) return fail(h, ICC_ERR_NUMERIC, "no knot spacing satisfies the quality"); found = max_quality_dt; have = true; }
-      }
-      if (!cuda_ok) return fail(h, ICC_ERR_CUDA, "quality kernels failed");
-    }
-  }
-  *dt_out = found;
-  *var_out = removed(found) / (double)n;                                                               // dt_to_variance_spectrum (:196-199)
-  if (!cuda_ok) return fail(h, ICC_ERR_CUDA, "quality kernels failed");
-  return ICC_OK;
+  NEED_DEVICE();
+  return drive(h, [&](std::string& err) { return spline_error_weighting(h->stream, h->sm_count, n, times, signal, quality, min_dt, max_dt, dt_out, var_out, spectrum, err); });
 }
 
-// ---- upstream row f4: camera intrinsic calibration (CameraCalibrator, src/core/camera_calibrator.cc) ----------------------
-namespace {
-// theia::CameraIntrinsicsModel::GetSubsetFromOptimizeIntrinsicsType per model, as bit masks over Theia's parameter order
-struct IntrinsicSubsets { unsigned focal, aspect, principal, radial, tangential; };
-IntrinsicSubsets intrinsic_subsets(int model) {
-  auto bits = [](std::initializer_list<int> l) { unsigned m = 0; for (int i : l) m |= 1u << i; return m; };
-  switch (model) {
-    case CAM_PINHOLE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
-    case CAM_PINHOLE_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};
-    case CAM_FISHEYE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7, 8}), 0u};
-    case CAM_FOV: return {bits({0}), bits({1}), bits({2, 3}), bits({4}), 0u};
-    case CAM_DIVISION_UNDISTORTION: return {bits({0}), bits({1}), bits({2, 3}), bits({4}), 0u};
-    case CAM_DOUBLE_SPHERE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
-    case CAM_EXTENDED_UNIFIED: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
-    default: return {0u, 0u, 0u, 0u, 0u};
-  }
-}
-}  // namespace
-
+// ---- upstream row f4: camera intrinsic calibration (icc_camcal.cu) ------------------------------------------------------------
 icc_status icc_calibrate_camera(icc_handle* h, int model, int W, int H, int nv, const int32_t* off, const int32_t* ids, const double* uv,
                                 const double* q_init, const double* p_init, const int32_t* init_valid, double focal_init, double distortion_init,
-                                const icc_camcal_options* options, double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out,
-                                icc_camcal_summary* summary) {
-  using clk = std::chrono::steady_clock;
-  const auto t_start = clk::now();
+                                const icc_camcal_options* options, double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary* summary) {
   if (!h || nv <= 0 || !off || !ids || !uv || !intr_out || !q_out || !p_out || !used_out || W <= 0 || H <= 0) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
+  NEED_DEVICE();
   if (camera_num_params(model) < 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "unknown camera model");
   if (h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_board_points must be called first");
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
   for (int i = 0; i < nv; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
-  const int nc = off[nv], np = (int)(h->points.size() / 4);
-  for (int i = 0; i < nc; ++i) if (ids[i] < 0 || ids[i] >= np) return fail(h, ICC_ERR_INVALID_ARGUMENT, "point id outside the board");
-  icc_camcal_options o; memset(&o, 0, sizeof o); if (options) o = *options;
-  if (o.grid_size < 0.0) o.grid_size = 0.04;
-  if (o.min_num_views <= 0) o.min_num_views = 10;
-  if (o.max_num_iterations <= 0) o.max_num_iterations = 100;
-  if (!(o.function_tolerance > 0.0)) o.function_tolerance = 1e-6;
-  if (!(o.parameter_tolerance > 0.0)) o.parameter_tolerance = 1e-8;
-  if (!(o.gradient_tolerance > 0.0)) o.gradient_tolerance = 1e-10;
-  if (!(o.huber_width > 0.0)) o.huber_width = 1.345;
-  if (!(o.max_view_error_stage1_px > 0.0)) o.max_view_error_stage1_px = 5.0;
-  if (!(o.max_view_error_final_px > 0.0)) o.max_view_error_final_px = 2.0;
-  icc_camcal_summary S; memset(&S, 0, sizeof S);
-  const int launches0 = kernel_launch_count();
-  CU(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  // ---- inputs to the device ------------------------------------------------------------------------------------------------
-  std::vector<double4> board(np);
-  for (int i = 0; i < np; ++i) board[i] = make_double4(h->points[4 * i], h->points[4 * i + 1], h->points[4 * i + 2], h->points[4 * i + 3]);
-  DevBuf<double4> d_board; DevBuf<int> d_off, d_pid, d_active; DevBuf<double2> d_uv;
-  CU(d_board.upload(board));
-  CU(d_off.alloc(nv + 1)); CU(d_pid.alloc(std::max(1, nc))); CU(d_uv.alloc(std::max(1, nc))); CU(d_active.alloc(nv));
-  CU(cudaMemcpyAsync(d_off.p, off, (size_t)(nv + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (nc > 0) {
-    CU(cudaMemcpyAsync(d_pid.p, ids, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_uv.p, uv, (size_t)nc * sizeof(double2), cudaMemcpyHostToDevice, st));
-  }
-  const double cx0 = W / 2.0, cy0 = H / 2.0;                       // AddView (:99)
-  // ---- initial focal length and poses ----------------------------------------------------------------------------------------
-  std::vector<double> q0(4 * (size_t)nv), p0(3 * (size_t)nv); std::vector<int> ok0(nv, 1);
-  const bool need_focal = !(focal_init > 0.0), need_poses = !q_init || !p_init;
-  double f0 = focal_init;
-  if (need_focal || need_poses) {
-    PoseProblem PQ; memset(&PQ, 0, sizeof PQ);
-    PQ.model = CAM_PINHOLE; PQ.n_frames = nv; PQ.n_points = np; PQ.min_points = 6;
-    PQ.board = d_board.p; PQ.f_off = d_off.p; PQ.pid = d_pid.p; PQ.thresh_sq = 1e300; PQ.max_err = 1e300;   // every corner takes part
-    PQ.lm_rel_tol = 1e-6;                                                                                  // these poses only start the bundle adjustment
-    DevBuf<double2> d_xy; DevBuf<unsigned char> d_use; DevBuf<double> d_f2, d_q, d_p, d_e; DevBuf<int> d_ok, d_valid;
-    CU(d_xy.alloc(std::max(1, nc))); CU(d_use.alloc(std::max(1, nc))); CU(d_ok.alloc(std::max(1, nc)));
-    if (need_focal) {
-      CU(d_f2.alloc(nv));
-      launch_board_focal(PQ, d_uv.p, cx0, cy0, d_xy.p, d_use.p, d_f2.p, st);
-      std::vector<double> f2(nv);
-      CU(cudaMemcpyAsync(f2.data(), d_f2.p, (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      std::vector<double> fs; for (double v : f2) if (v > 0.0 && std::isfinite(v)) fs.push_back(std::sqrt(v));
-      if (fs.empty()) return fail(h, ICC_ERR_NUMERIC, "no view yields a focal length estimate (fronto-parallel or degenerate views only)");
-      f0 = median_like_reference(fs);
-    }
-    if (need_poses) {
-      CU(d_q.alloc(4 * (size_t)nv)); CU(d_p.alloc(3 * (size_t)nv)); CU(d_e.alloc(nv)); CU(d_valid.alloc(nv));
-      launch_pinhole_normalize(nc, d_uv.p, cx0, cy0, f0, d_xy.p, d_ok.p, st);
-      launch_board_poses(PQ, d_xy.p, d_ok.p, d_use.p, d_q.p, d_p.p, d_e.p, d_valid.p, st);
-      CU(cudaMemcpyAsync(q0.data(), d_q.p, 4 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(p0.data(), d_p.p, 3 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(ok0.data(), d_valid.p, (size_t)nv * sizeof(int), cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-    }
-  }
-  if (!need_poses) {
-    memcpy(q0.data(), q_init, 4 * (size_t)nv * sizeof(double)); memcpy(p0.data(), p_init, 3 * (size_t)nv * sizeof(double));
-    if (init_valid) for (int i = 0; i < nv; ++i) ok0[i] = init_valid[i] != 0;
-  }
-  // ---- state: R_cw = conj(q_wc), camera centre, shared intrinsics ---------------------------------------------------------------
-  std::vector<double> qs(4 * (size_t)nv), k0(10, 0.0);
-  for (int v = 0; v < nv; ++v) { const Q4 q = qn(&q0[4 * v]); qs[4 * v] = -q.x; qs[4 * v + 1] = -q.y; qs[4 * v + 2] = -q.z; qs[4 * v + 3] = q.w; }
-  // the internal initialiser refines (focal length, division distortion, poses) jointly before the target model takes over -- the
-  // role of utils::initialize_radial_undistortion_camera (:283-306), which hands the reference a focal length and a division-model
-  // distortion for every non-pinhole model
-  const bool prestage = need_poses && need_focal && model != CAM_PINHOLE && model != CAM_PINHOLE_RADTAN;
-  std::vector<int> active;
-  for (int v = 0; v < nv; ++v) if (ok0[v]) active.push_back(v);
-  S.n_views_initialized = (int)active.size();
-  if (prestage) { k0[0] = f0; k0[1] = 1.0; k0[2] = cx0; k0[3] = cy0; k0[4] = -1e-2 / ((double)W * W + (double)H * H); }
-  DevBuf<double> d_q[2], d_c[2], d_k[2], d_blocks, d_Y, d_scale, d_sys, d_red, d_dk, d_scal, d_verr;
-  for (int i = 0; i < 2; ++i) { CU(d_q[i].upload(qs)); CU(d_c[i].upload(p0)); CU(d_k[i].upload(k0)); }
-  const size_t na0 = std::max<size_t>(1, active.size());
-  CU(d_blocks.alloc(na0 * CC_PACK)); CU(d_Y.alloc(na0 * CC_Y)); CU(d_scale.alloc(6 * na0 + 10)); CU(d_sys.alloc(CC_PACK + 1)); CU(d_red.alloc(66));
-  CU(d_dk.alloc(10)); CU(d_scal.alloc(CC_SCAL_COUNT)); CU(d_verr.alloc(nv));
-  int cur = 0;
-  CamCalProblem Q; memset(&Q, 0, sizeof Q);
-  Q.model = model; Q.n_points = np; Q.huber = o.huber_width; Q.board = d_board.p; Q.f_off = d_off.p; Q.pid = d_pid.p; Q.uv = d_uv.p; Q.active = d_active.p;
-  auto state = [&](int i) { CamCalState s; s.q = d_q[i].p; s.c = d_c[i].p; s.k = d_k[i].p; return s; };
-  auto set_active = [&]() -> icc_status {
-    Q.n_active = (int)active.size();
-    if (!active.empty()) CU(cudaMemcpyAsync(d_active.p, active.data(), active.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    CU(cudaStreamSynchronize(st));   // `active` may be modified by the caller right after
-    return ICC_OK;
-  };
-  std::vector<double> verr(nv, 0.0);
-  // GetReprojErrorOfView for every active view at the current state
-  auto view_errors = [&]() -> icc_status {
-    CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
-    launch_camcal_accumulate(Q, state(cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, d_verr.p, st);
-    CU(cudaMemcpyAsync(verr.data(), d_verr.p, (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    return ICC_OK;
-  };
-  // RemoveViewsReprojError (:59-76)
-  auto remove_views = [&](double max_err) -> icc_status {
-    icc_status r = view_errors(); if (r != ICC_OK) return r;
-    std::vector<int> keep; for (int v : active) if (!(verr[v] > max_err)) keep.push_back(v);
-    active.swap(keep);
-    return set_active();
-  };
-  // theia::BundleAdjustViews: Levenberg-Marquardt with Ceres' trust-region logic; one device->host read-back per iteration
-  auto bundle_adjust = [&](unsigned mask, bool pose_free, int stage) -> icc_status {
-    Q.intr_mask = mask; Q.pose_free = pose_free ? 1 : 0;
-    if (Q.n_active == 0 || (mask == 0u && !pose_free)) { if (stage >= 0) S.termination[stage] = 3; return ICC_OK; }
-    TrOptions to = ceres_default_options();   // theia::BundleAdjustmentOptions: the Ceres defaults but for these
-    to.function_tolerance = o.function_tolerance; to.parameter_tolerance = o.parameter_tolerance; to.gradient_tolerance = o.gradient_tolerance;
-    to.max_iterations = o.max_num_iterations;
-    TrustRegion T = tr_start(to);
-    double sc[CC_SCAL_COUNT];
-    while (tr_continue(T)) {
-      const bool fresh = T.jacobian_stale != 0;
-      if (fresh) {
-        CU(cudaMemsetAsync(d_sys.p, 0, (CC_PACK + 1) * sizeof(double), st));
-        launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, st);
-      }
-      CU(cudaMemsetAsync(d_red.p, 0, 66 * sizeof(double), st));
-      CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
-      launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, T.iterations == 0 ? 1 : 0, T.radius, to.min_diagonal, to.max_diagonal, d_dk.p, d_scal.p, st);
-      launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, st);
-      CU(cudaMemcpyAsync(sc, d_scal.p, sizeof sc, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      if (fresh) {
-        if (T.iterations == 0 && !std::isfinite(sc[CC_X_COST])) return fail(h, ICC_ERR_NUMERIC, "non-finite initial cost");
-        if (!tr_jacobian(T, sc[CC_X_COST], sc[CC_GRAD_MAX])) break;
-      }
-      if (tr_step(T, sc[CC_FAIL] == 0.0, 0.5 * (sc[CC_D_DELTA] - sc[CC_G_DELTA]), std::sqrt(sc[CC_STEP_SQ]), std::sqrt(sc[CC_X_SQ])) && tr_candidate(T, sc[CC_CAND_COST]))
-        cur = 1 - cur;
-    }
-    // both state copies must agree on everything outside the last step (inactive views never move; the intrinsics / poses of
-    // a rejected candidate are stale): bring the spare copy back to the current state
-    CU(cudaMemcpyAsync(d_q[1 - cur].p, d_q[cur].p, 4 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(d_c[1 - cur].p, d_c[cur].p, 3 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(d_k[1 - cur].p, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (stage == 0) S.initial_cost = T.initial_cost;
-    if (stage >= 0) { S.final_cost[stage] = T.cost; S.iterations[stage] = T.iterations; S.termination[stage] = T.termination; } else S.init_iterations = T.iterations;
-    return ICC_OK;
-  };
-  auto finish = [&](bool success) -> icc_status {
-    icc_status r = view_errors(); if (r != ICC_OK) return r;
-    std::vector<double> qh(4 * (size_t)nv), ch(3 * (size_t)nv), kh(10);
-    CU(cudaMemcpy(qh.data(), d_q[cur].p, qh.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(ch.data(), d_c[cur].p, ch.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(kh.data(), d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
-    for (int v = 0; v < nv; ++v) {
-      q_out[4 * v] = -qh[4 * v]; q_out[4 * v + 1] = -qh[4 * v + 1]; q_out[4 * v + 2] = -qh[4 * v + 2]; q_out[4 * v + 3] = qh[4 * v + 3];
-      for (int d = 0; d < 3; ++d) p_out[3 * v + d] = ch[3 * v + d];
-      used_out[v] = 0; if (err_out) err_out[v] = 0.0;
-    }
-    double tot = 0.0;
-    for (int v : active) { used_out[v] = 1; if (err_out) err_out[v] = verr[v]; tot += verr[v]; }
-    for (int i = 0; i < 10; ++i) intr_out[i] = kh[i];
-    S.success = success ? 1 : 0; S.n_views_used = (int)active.size();
-    S.final_reproj_error = active.empty() ? 0.0 : tot / (double)active.size();                 // :352-366
-    S.gpu_launches = kernel_launch_count() - launches0;
-    S.seconds_total = std::chrono::duration<double>(clk::now() - t_start).count();
-    if (summary) *summary = S;
-    if (!success) h->err = "Not enough views for proper calibration";
-    return ICC_OK;
-  };
-  icc_status rc = set_active(); if (rc != ICC_OK) return rc;
-  if (prestage) {
-    Q.model = CAM_DIVISION_UNDISTORTION;
-    rc = bundle_adjust((1u << 0) | (1u << 4), true, -1); if (rc != ICC_OK) return rc;
-    Q.model = model;
-    double kd[10];
-    CU(cudaMemcpy(kd, d_k[cur].p, sizeof kd, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(p0.data(), d_c[cur].p, p0.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    if (kd[0] > 0.0 && std::isfinite(kd[0])) { f0 = kd[0]; if (model == CAM_DIVISION_UNDISTORTION) distortion_init = kd[4]; }
-  }
-  S.focal_length_init = f0;
-  // ---- grid filter in file order (:313-325): a view is taken iff no accepted camera position lies within grid_size ---------------
-  // (the reference scans all accepted positions; a hash grid with cells of grid_size visits only the 27 cells that can hold one
-  // -- same decisions, linear time)
-  if (o.grid_size > 0.0) {
-    std::vector<int> sel;
-    std::unordered_map<uint64_t, std::vector<int>> cells;
-    const double inv = 1.0 / o.grid_size;
-    bool hashable = true;
-    for (int v : active) for (int d = 0; d < 3; ++d) if (!(std::fabs(p0[3 * v + d] * inv) < 1e6)) hashable = false;   // 21 bits per axis
-    auto key = [](int64_t x, int64_t y, int64_t z) { return (uint64_t)((x + (1 << 20)) & 0x1fffff) << 42 | (uint64_t)((y + (1 << 20)) & 0x1fffff) << 21 | (uint64_t)((z + (1 << 20)) & 0x1fffff); };
-    auto close_to = [&](int v, int a) { const double dx = p0[3 * v] - p0[3 * a], dy = p0[3 * v + 1] - p0[3 * a + 1], dz = p0[3 * v + 2] - p0[3 * a + 2]; return std::sqrt(dx * dx + dy * dy + dz * dz) < o.grid_size; };
-    for (int v : active) {
-      bool take = true;
-      if (hashable) {
-        const int64_t cx = (int64_t)std::floor(p0[3 * v] * inv), cy = (int64_t)std::floor(p0[3 * v + 1] * inv), cz = (int64_t)std::floor(p0[3 * v + 2] * inv);
-        for (int64_t x = cx - 1; x <= cx + 1 && take; ++x) for (int64_t y = cy - 1; y <= cy + 1 && take; ++y) for (int64_t z = cz - 1; z <= cz + 1 && take; ++z) {
-          auto it = cells.find(key(x, y, z));
-          if (it != cells.end()) for (int a : it->second) if (close_to(v, a)) { take = false; break; }
-        }
-        if (take) cells[key(cx, cy, cz)].push_back(v);
-      } else {
-        for (int a : sel) if (close_to(v, a)) { take = false; break; }
-      }
-      if (take) sel.push_back(v);
-    }
-    active.swap(sel);
-  }
-  S.n_views_selected = (int)active.size();
-  rc = set_active(); if (rc != ICC_OK) return rc;
-  // ---- initial intrinsics of the target model (AddView :84-129) --------------------------------------------------------------------
-  std::fill(k0.begin(), k0.end(), 0.0);
-  k0[0] = f0; k0[1] = 1.0;
-  switch (model) {
-    case CAM_FOV: case CAM_DIVISION_UNDISTORTION: k0[2] = cx0; k0[3] = cy0; break;
-    default: k0[3] = cx0; k0[4] = cy0; break;
-  }
-  if (model == CAM_DIVISION_UNDISTORTION) k0[4] = distortion_init;
-  if (model == CAM_FOV) k0[4] = distortion_init != 0.0 ? distortion_init : 1e-3;   // theia's FOV model has no gradient at omega = 0
-  if (model == CAM_DOUBLE_SPHERE) { k0[5] = -0.25; k0[6] = 0.5; }
-  if (model == CAM_EXTENDED_UNIFIED) { k0[5] = 0.5; k0[6] = 1.0; }
-  for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), 10 * sizeof(double), cudaMemcpyHostToDevice));
-  if ((int)active.size() < o.min_num_views) return finish(false);                               // :132-135
-  const IntrinsicSubsets sub = intrinsic_subsets(model);
-  // 1. focal length and radial distortion, principal point fixed (:146-160)
-  rc = bundle_adjust(sub.focal | (model != CAM_PINHOLE ? sub.radial : 0u), true, 0); if (rc != ICC_OK) return rc;
-  rc = remove_views(o.max_view_error_stage1_px); if (rc != ICC_OK) return rc;                    // :162
-  // 2. principal point, everything else fixed (:164-174)
-  rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
-  if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
-  // 3. full optimisation (:181-198)
-  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN ? sub.tangential : 0u);
-  rc = bundle_adjust(stage3_mask, true, 2);
+  const int np = (int)(h->points.size() / 4);
+  for (int i = 0; i < off[nv]; ++i) if (ids[i] < 0 || ids[i] >= np) return fail(h, ICC_ERR_INVALID_ARGUMENT, "point id outside the board");
+  std::vector<double> points; icc_camcal_summary S;
+  const icc_status rc = drive(h, [&](std::string& err) { return calibrate_camera(h->stream, model, W, H, np, h->points.data(), nv, off, ids, uv, q_init, p_init, init_valid, focal_init, distortion_init, options,
+                            intr_out, q_out, p_out, err_out, used_out, S, points, err); });
+  if (!points.empty()) h->points.swap(points);   // the board was refined, even if the final bundle adjustment then failed
   if (rc != ICC_OK) return rc;
-  rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200
-  if ((int)active.size() < o.min_num_views) return finish(false);                                // :202-205
-  if (o.optimize_board_points) {                                                                 // :207-216
-    // BundleAdjustTracks: every camera constant, one warp per board point over its observations in the remaining views ...
-    std::vector<int> obs_view(std::max(1, nc), -1), pt_off, pt_obs;
-    for (int v : active) for (int c = off[v]; c < off[v + 1]; ++c) obs_view[c] = v;
-    build_point_adjacency(np, nc, ids, [&](int c) { return obs_view[c] >= 0; }, pt_off, pt_obs);
-    DevBuf<int> d_view, d_pt_off, d_pt_obs, d_opt; DevBuf<double4> d_board2;
-    CU(d_view.upload(obs_view)); CU(d_pt_off.upload(pt_off)); CU(d_pt_obs.alloc(std::max<size_t>(1, pt_obs.size()))); CU(d_opt.alloc(np)); CU(d_board2.alloc(np));
-    if (!pt_obs.empty()) CU(cudaMemcpy(d_pt_obs.p, pt_obs.data(), pt_obs.size() * sizeof(int), cudaMemcpyHostToDevice));
-    PointProblem PQ; memset(&PQ, 0, sizeof PQ);
-    PQ.model = model; CU(cudaMemcpy(PQ.intr, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
-    PQ.normalized = 0; PQ.n_points = np; PQ.min_obs = 1; PQ.huber = o.huber_width;
-    PQ.board_in = d_board.p; PQ.pt_off = d_pt_off.p; PQ.pt_obs = d_pt_obs.p; PQ.obs_view = d_view.p; PQ.meas = d_uv.p; PQ.q_cw = d_q[cur].p; PQ.cam_c = d_c[cur].p;
-    launch_point_refine(PQ, d_board2.p, d_opt.p, st);
-    std::vector<int> opt(np);
-    CU(cudaMemcpyAsync(d_board.p, d_board2.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(board.data(), d_board2.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(opt.data(), d_opt.p, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    for (int i = 0; i < np; ++i) { h->points[4 * i] = board[i].x; h->points[4 * i + 1] = board[i].y; h->points[4 * i + 2] = board[i].z; h->points[4 * i + 3] = board[i].w; S.n_points_optimized += opt[i]; }
-    // ... then BundleAdjustViews once more with the options of stage 3
-    const int it3 = S.iterations[2];
-    rc = bundle_adjust(stage3_mask, true, 2); if (rc != ICC_OK) return rc;
-    S.iterations[2] += it3;
-  }
-  return finish(true);
+  if (summary) *summary = S;
+  if (!S.success) h->err = "Not enough views for proper calibration";   // camera_calibrator.cc:132-135, :176-179, :202-205
+  return ICC_OK;
 }
 
-// ---- upstream: static IMU biases (python/get_imu_biases.py:36-53) -------------------------------------------------------------------
+// ---- upstream: static IMU biases (icc_sew.cu) ---------------------------------------------------------------------------------------
 icc_status icc_estimate_imu_biases(icc_handle* h, int n, const double* acc, const double* gyr, double gravity_const, double accl_bias[3], double gyro_bias[3]) {
   if (!h || n <= 0 || !acc || !gyr || !accl_bias || !gyro_bias) return ICC_ERR_INVALID_ARGUMENT;
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
-  CU(cudaSetDevice(h->device));
-  DevBuf<double> d_a, d_g, d_s;
-  CU(d_a.alloc(3 * (size_t)n)); CU(d_g.alloc(3 * (size_t)n)); CU(d_s.alloc(6));
-  CU(cudaMemcpyAsync(d_a.p, acc, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CU(cudaMemcpyAsync(d_g.p, gyr, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  launch_imu_sums(n, d_a.p, d_g.p, d_s.p, h->sm_count, h->stream);
-  double s[6];
-  CU(cudaMemcpyAsync(s, d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
-  CU(cudaStreamSynchronize(h->stream));
-  if (cudaGetLastError() != cudaSuccess) return fail(h, ICC_ERR_CUDA, "bias kernel failed");
-  double mean_a[3], mean_g[3];
-  for (int d = 0; d < 3; ++d) { mean_a[d] = s[d] / n; mean_g[d] = s[3 + d] / n; }
-  int ax = 0; for (int d = 1; d < 3; ++d) if (std::fabs(mean_a[d]) > std::fabs(mean_a[ax])) ax = d;          // :39-41 (first maximum)
-  const double sgn = mean_a[ax] > 0.0 ? 1.0 : (mean_a[ax] < 0.0 ? -1.0 : 0.0);
-  const double grav = (double)(float)(gravity_const * sgn);                                                     // float32 array (:43-44)
-  for (int d = 0; d < 3; ++d) { accl_bias[d] = mean_a[d] - (d == ax ? grav : 0.0); gyro_bias[d] = mean_g[d]; }   // :46, :49-50
-  return ICC_OK;
+  NEED_DEVICE();
+  return drive(h, [&](std::string& err) { return imu_biases(h->stream, h->sm_count, n, acc, gyr, gravity_const, accl_bias, gyro_bias, err); });
 }
 
 // ---- upstream: static multi-pose IMU intrinsics (icc_static_imu.cu) ---------------------------------------------------------------
@@ -2149,15 +1554,13 @@ void icc_default_static_imu_options(icc_static_imu_options* o) { if (o) default_
 icc_status icc_static_imu_calibration(icc_handle* h, int n, const double* t, const double* acc, const double* gyr, const icc_static_imu_options* opt,
                                       double acc_params[9], double gyr_params[9], double gyr_bias[3], icc_static_imu_summary* summary) {
   if (!h || n < 3 || !t || !acc || !gyr || !acc_params || !gyr_params || !gyr_bias) return ICC_ERR_INVALID_ARGUMENT;   // InitialInterval needs 3 samples
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
-  CU(cudaSetDevice(h->device));
+  NEED_DEVICE();
   icc_static_imu_options o; default_static_imu_options(&o);
   if (opt) o = *opt;
-  icc_static_imu_summary S; std::string err;
-  const icc_status rc = static_imu_calibrate(h->stream, n, t, acc, gyr, o, acc_params, gyr_params, gyr_bias, S, h->static_imu_intervals, err);
-  if (rc != ICC_OK) return fail(h, rc, err);
-  if (summary) *summary = S;
-  return ICC_OK;
+  icc_static_imu_summary S;
+  const icc_status rc = drive(h, [&](std::string& err) { return static_imu_calibrate(h->stream, n, t, acc, gyr, o, acc_params, gyr_params, gyr_bias, S, h->static_imu_intervals, err); });
+  if (rc == ICC_OK && summary) *summary = S;
+  return rc;
 }
 
 icc_status icc_get_static_imu_intervals(const icc_handle* h, int32_t* buf, int32_t* len) {
@@ -2173,19 +1576,16 @@ icc_status icc_get_static_imu_intervals(const icc_handle* h, int32_t* buf, int32
 // ---- upstream: Allan variance noise characterisation (icc_allan.cu) -----------------------------------------------------------------
 void icc_default_allan_options(icc_allan_options* o) { if (o) default_allan_options(o); }
 
-icc_status icc_allan_variance(icc_handle* h, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options* opt,
-                              double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6]) {
+icc_status icc_allan_variance(icc_handle* h, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options* opt, double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6]) {
   if (!h || !t || !acc || !gyr || !params || !noise || !summary) return ICC_ERR_INVALID_ARGUMENT;
   icc_allan_options o; default_allan_options(&o);
   if (opt) o = *opt;
   if (n < 3 || o.n_clusters < 2) return fail(h, ICC_ERR_INVALID_ARGUMENT, "icc_allan_variance needs n >= 3 samples and n_clusters >= 2");
-  if (h->device < 0) return fail(h, ICC_ERR_NO_DEVICE, "no CUDA device: this library has no CPU fallback");
-  CU(cudaSetDevice(h->device));
-  h->allan_curves = allan::Curves();
-  std::string err;
-  const icc_status rc = allan_variance(h->stream, n, t, acc, gyr, o, params, noise, summary, h->allan_curves, err);
-  if (rc != ICC_OK) { h->allan_curves = allan::Curves(); return fail(h, rc, err); }
-  return ICC_OK;
+  NEED_DEVICE();
+  const icc_status rc = drive(h, [&](std::string& err) { h->allan_curves = allan::Curves();
+    return allan_variance(h->stream, n, t, acc, gyr, o, params, noise, summary, h->allan_curves, err); });
+  if (rc != ICC_OK) h->allan_curves = allan::Curves();
+  return rc;
 }
 
 icc_status icc_get_allan_curves(const icc_handle* h, int channel, int32_t* factors, double* tau, double* sigma2, double* fit_deviation, int32_t* len) {

@@ -16,15 +16,28 @@
 //       onto the intrinsics, summed over the CTA through shared memory and added to the reduced 10x10 system.
 //   camcal_solve_kernel      : the reduced system (<= 10 unknowns) by Cholesky, intrinsics step, candidate intrinsics.
 //   camcal_update_kernel     : back-substitution of every view's pose step, candidate poses, step / model-decrease sums.
-// The host only sequences these launches and applies Ceres' trust-region logic to eight scalars per iteration (icc_api.cu).
+// The host only sequences these launches and applies Ceres' trust-region logic to eight scalars per iteration (calibrate_camera below).
 #include "icc_camera.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
+#include "icc_trust_region.cuh"
 
+#include <chrono>
 #include <cmath>
+#include <unordered_map>
 
 namespace icc {
 
-void count_launch();
+// Column order of a view's [J | r] rows: 0-2 rotation increment, 3-5 camera centre, 6-15 intrinsics (Theia order), 16 residual.
+constexpr int CC_COLS = 17, CC_PACK = CC_COLS * (CC_COLS + 1) / 2, CC_Y = 66;   // packed upper triangle; Y = A^-1 [H_pk | g_p] (6 x 11)
+enum { CC_CAND_COST = 0, CC_G_DELTA = 1, CC_D_DELTA = 2, CC_STEP_SQ = 3, CC_X_SQ = 4, CC_FAIL = 5, CC_GRAD_MAX = 6, CC_X_COST = 7, CC_SCAL_COUNT = 8 };
+struct CamCalProblem {
+  int model, n_points, n_active, pose_free;
+  unsigned intr_mask;          // bit i set = intrinsic i is optimised in this stage
+  double huber;                // loss width (camera_calibrator.cc:143)
+  const double4* board; const int* f_off; const int* pid; const double2* uv;
+  const int* active;           // indices of the views that take part (n_active)
+};
+struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) per view, camera centre per view, 10 intrinsics
 
 namespace {
 
@@ -354,8 +367,26 @@ __global__ void __launch_bounds__(128) camcal_update_kernel(CamCalProblem Q, Cam
   if (lane == 0) { atomicAdd(&scal[CC_G_DELTA], gd); atomicAdd(&scal[CC_D_DELTA], dd); atomicAdd(&scal[CC_STEP_SQ], st); atomicAdd(&scal[CC_X_SQ], xs); }
 }
 
+// theia::CameraIntrinsicsModel::GetSubsetFromOptimizeIntrinsicsType per model, as bit masks over Theia's parameter order
+struct IntrinsicSubsets { unsigned focal, aspect, principal, radial, tangential; };
+IntrinsicSubsets intrinsic_subsets(int model) {
+  auto bits = [](std::initializer_list<int> l) { unsigned m = 0; for (int i : l) m |= 1u << i; return m; };
+  switch (model) {
+    case CAM_PINHOLE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
+    case CAM_PINHOLE_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};
+    case CAM_FISHEYE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7, 8}), 0u};
+    case CAM_FOV: return {bits({0}), bits({1}), bits({2, 3}), bits({4}), 0u};
+    case CAM_DIVISION_UNDISTORTION: return {bits({0}), bits({1}), bits({2, 3}), bits({4}), 0u};
+    case CAM_DOUBLE_SPHERE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
+    case CAM_EXTENDED_UNIFIED: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
+    default: return {0u, 0u, 0u, 0u, 0u};
+  }
+}
+
 }  // namespace
 
+// with_jacobian: per-view packed blocks (n_active x CC_PACK) + the intrinsics part and the cost summed into sys[CC_PACK + 1];
+// otherwise cost only into *cost_out and (optional) the per-view mean reprojection error [px] into view_err (indexed by view)
 void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool with_jacobian, double* blocks, double* sys, double* cost_out, double* view_err, cudaStream_t st) {
   if (Q.n_active <= 0) return;
   const int grid = (Q.n_active + 3) / 4;
@@ -364,8 +395,9 @@ void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool
   count_launch();
 }
 
-void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const CamCalState& cand, const double* blocks, const double* sys, double* red, double* Y,
-                        double* scale, int compute_scale, double radius, double min_diag, double max_diag, double* dk, double* scal, cudaStream_t st) {
+// one damped step: per-view Schur elimination, reduced intrinsics system, back-substitution into the candidate state
+void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const CamCalState& cand, const double* blocks, const double* sys, double* red /* 66 */, double* Y,
+                        double* scale /* 6 n_active + 10 */, int compute_scale, double radius, double min_diag, double max_diag, double* dk /* 10 */, double* scal, cudaStream_t st) {
   if (Q.n_active <= 0) return;
   const int grid = (Q.n_active + 127) / 128;
   camcal_reduce_kernel<<<(Q.n_active + RED_THREADS - 1) / RED_THREADS, RED_THREADS, 0, st>>>(Q, blocks, red, Y, scale, compute_scale, radius, min_diag, max_diag, scal);
@@ -374,6 +406,247 @@ void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const Ca
   count_launch();
   camcal_update_kernel<<<grid, 128, 0, st>>>(Q, cur, cand, blocks, Y, dk, scale, radius, min_diag, max_diag, scal);
   count_launch();
+}
+
+// ---- host driver of row f4 (icc_calibrate_camera): CameraCalibrator, src/core/camera_calibrator.cc ------------------------------
+#define CU(call) ICC_CUDA_CHECK(call, err)
+
+icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, const double* points, int nv, const int32_t* off, const int32_t* ids, const double* uv,
+                            const double* q_init, const double* p_init, const int32_t* init_valid, double focal_init, double distortion_init, const icc_camcal_options* options,
+                            double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary& S, std::vector<double>& points_out, std::string& err) {
+  using clk = std::chrono::steady_clock;
+  const auto t_start = clk::now();
+  memset(&S, 0, sizeof S);
+  const int launches0 = kernel_launch_count();
+  // ---- inputs to the device ------------------------------------------------------------------------------------------------
+  BoardViews B;
+  icc_status rc = upload_board_views(st, np, points, nv, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
+  const int nc = B.nc;
+  icc_camcal_options o; memset(&o, 0, sizeof o); if (options) o = *options;
+  if (o.grid_size < 0.0) o.grid_size = 0.04;
+  if (o.min_num_views <= 0) o.min_num_views = 10;
+  if (o.max_num_iterations <= 0) o.max_num_iterations = 100;
+  if (!(o.function_tolerance > 0.0)) o.function_tolerance = 1e-6;
+  if (!(o.parameter_tolerance > 0.0)) o.parameter_tolerance = 1e-8;
+  if (!(o.gradient_tolerance > 0.0)) o.gradient_tolerance = 1e-10;
+  if (!(o.huber_width > 0.0)) o.huber_width = 1.345;
+  if (!(o.max_view_error_stage1_px > 0.0)) o.max_view_error_stage1_px = 5.0;
+  if (!(o.max_view_error_final_px > 0.0)) o.max_view_error_final_px = 2.0;
+  DevBuf<int> d_active; CU(d_active.alloc(nv));
+  const double cx0 = W / 2.0, cy0 = H / 2.0;                       // AddView (:99)
+  // ---- initial focal length and poses ----------------------------------------------------------------------------------------
+  std::vector<double> q0(4 * (size_t)nv), p0(3 * (size_t)nv); std::vector<int> ok0(nv, 1);
+  const bool need_focal = !(focal_init > 0.0), need_poses = !q_init || !p_init;
+  double f0 = focal_init;
+  if (need_focal || need_poses) {
+    PoseProblem PQ; memset(&PQ, 0, sizeof PQ);
+    PQ.model = CAM_PINHOLE; PQ.n_frames = nv; PQ.n_points = np; PQ.min_points = 6;
+    PQ.board = B.board.p; PQ.f_off = B.off.p; PQ.pid = B.pid.p; PQ.thresh_sq = 1e300; PQ.max_err = 1e300;   // every corner takes part
+    PQ.lm_rel_tol = 1e-6;                                                                                  // these poses only start the bundle adjustment
+    if (need_focal) {
+      DevBuf<double> d_f2; CU(d_f2.alloc(nv));
+      launch_board_focal(PQ, B.uv.p, cx0, cy0, B.xy.p, B.use.p, d_f2.p, st);
+      std::vector<double> f2(nv);
+      CU(cudaMemcpyAsync(f2.data(), d_f2.p, (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      std::vector<double> fs; for (double v : f2) if (v > 0.0 && std::isfinite(v)) fs.push_back(std::sqrt(v));
+      if (fs.empty()) { err = "no view yields a focal length estimate (fronto-parallel or degenerate views only)"; return ICC_ERR_NUMERIC; }
+      f0 = median_like_reference(fs);
+    }
+    if (need_poses) {
+      launch_pinhole_normalize(nc, B.uv.p, cx0, cy0, f0, B.xy.p, B.ok.p, st);
+      launch_board_poses(PQ, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+      rc = read_poses(st, B, q0.data(), p0.data(), nullptr, ok0.data(), err); if (rc != ICC_OK) return rc;
+    }
+  }
+  if (!need_poses) {
+    memcpy(q0.data(), q_init, 4 * (size_t)nv * sizeof(double)); memcpy(p0.data(), p_init, 3 * (size_t)nv * sizeof(double));
+    if (init_valid) for (int i = 0; i < nv; ++i) ok0[i] = init_valid[i] != 0;
+  }
+  // ---- state: R_cw = conj(q_wc), camera centre, shared intrinsics ---------------------------------------------------------------
+  std::vector<double> qs(4 * (size_t)nv), k0(10, 0.0);
+  for (int v = 0; v < nv; ++v) {
+    const Q4 q = qnormalized(q4(q0[4 * v], q0[4 * v + 1], q0[4 * v + 2], q0[4 * v + 3]));
+    qs[4 * v] = -q.x; qs[4 * v + 1] = -q.y; qs[4 * v + 2] = -q.z; qs[4 * v + 3] = q.w;
+  }
+  // the internal initialiser refines (focal length, division distortion, poses) jointly before the target model takes over -- the
+  // role of utils::initialize_radial_undistortion_camera (:283-306), which hands the reference a focal length and a division-model
+  // distortion for every non-pinhole model
+  const bool prestage = need_poses && need_focal && model != CAM_PINHOLE && model != CAM_PINHOLE_RADTAN;
+  std::vector<int> active;
+  for (int v = 0; v < nv; ++v) if (ok0[v]) active.push_back(v);
+  S.n_views_initialized = (int)active.size();
+  if (prestage) { k0[0] = f0; k0[1] = 1.0; k0[2] = cx0; k0[3] = cy0; k0[4] = -1e-2 / ((double)W * W + (double)H * H); }
+  DevBuf<double> d_q[2], d_c[2], d_k[2], d_blocks, d_Y, d_scale, d_sys, d_red, d_dk, d_scal, d_verr;
+  for (int i = 0; i < 2; ++i) { CU(d_q[i].upload(qs)); CU(d_c[i].upload(p0)); CU(d_k[i].upload(k0)); }
+  const size_t na0 = std::max<size_t>(1, active.size());
+  CU(d_blocks.alloc(na0 * CC_PACK)); CU(d_Y.alloc(na0 * CC_Y)); CU(d_scale.alloc(6 * na0 + 10)); CU(d_sys.alloc(CC_PACK + 1)); CU(d_red.alloc(66));
+  CU(d_dk.alloc(10)); CU(d_scal.alloc(CC_SCAL_COUNT)); CU(d_verr.alloc(nv));
+  int cur = 0;
+  CamCalProblem Q; memset(&Q, 0, sizeof Q);
+  Q.model = model; Q.n_points = np; Q.huber = o.huber_width; Q.board = B.board.p; Q.f_off = B.off.p; Q.pid = B.pid.p; Q.uv = B.uv.p; Q.active = d_active.p;
+  auto state = [&](int i) { CamCalState s; s.q = d_q[i].p; s.c = d_c[i].p; s.k = d_k[i].p; return s; };
+  auto set_active = [&]() -> icc_status {
+    Q.n_active = (int)active.size();
+    if (!active.empty()) CU(cudaMemcpyAsync(d_active.p, active.data(), active.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));   // `active` may be modified by the caller right after
+    return ICC_OK;
+  };
+  std::vector<double> verr(nv, 0.0);
+  // GetReprojErrorOfView for every active view at the current state
+  auto view_errors = [&]() -> icc_status {
+    CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
+    launch_camcal_accumulate(Q, state(cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, d_verr.p, st);
+    CU(cudaMemcpyAsync(verr.data(), d_verr.p, (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return ICC_OK;
+  };
+  // RemoveViewsReprojError (:59-76)
+  auto remove_views = [&](double max_err) -> icc_status {
+    icc_status r = view_errors(); if (r != ICC_OK) return r;
+    std::vector<int> keep; for (int v : active) if (!(verr[v] > max_err)) keep.push_back(v);
+    active.swap(keep);
+    return set_active();
+  };
+  // theia::BundleAdjustViews: Levenberg-Marquardt with Ceres' trust-region logic; one device->host read-back per iteration
+  auto bundle_adjust = [&](unsigned mask, bool pose_free, int stage) -> icc_status {
+    Q.intr_mask = mask; Q.pose_free = pose_free ? 1 : 0;
+    if (Q.n_active == 0 || (mask == 0u && !pose_free)) { if (stage >= 0) S.termination[stage] = 3; return ICC_OK; }
+    TrOptions to = ceres_default_options();   // theia::BundleAdjustmentOptions: the Ceres defaults but for these
+    to.function_tolerance = o.function_tolerance; to.parameter_tolerance = o.parameter_tolerance; to.gradient_tolerance = o.gradient_tolerance;
+    to.max_iterations = o.max_num_iterations;
+    TrustRegion T = tr_start(to);
+    double sc[CC_SCAL_COUNT];
+    while (tr_continue(T)) {
+      const bool fresh = T.jacobian_stale != 0;
+      if (fresh) {
+        CU(cudaMemsetAsync(d_sys.p, 0, (CC_PACK + 1) * sizeof(double), st));
+        launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, st);
+      }
+      CU(cudaMemsetAsync(d_red.p, 0, 66 * sizeof(double), st));
+      CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
+      launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, T.iterations == 0 ? 1 : 0, T.radius, to.min_diagonal, to.max_diagonal, d_dk.p, d_scal.p, st);
+      launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, st);
+      CU(cudaMemcpyAsync(sc, d_scal.p, sizeof sc, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      if (fresh) {
+        if (T.iterations == 0 && !std::isfinite(sc[CC_X_COST])) { err = "non-finite initial cost"; return ICC_ERR_NUMERIC; }
+        if (!tr_jacobian(T, sc[CC_X_COST], sc[CC_GRAD_MAX])) break;
+      }
+      if (tr_step(T, sc[CC_FAIL] == 0.0, 0.5 * (sc[CC_D_DELTA] - sc[CC_G_DELTA]), std::sqrt(sc[CC_STEP_SQ]), std::sqrt(sc[CC_X_SQ])) && tr_candidate(T, sc[CC_CAND_COST]))
+        cur = 1 - cur;
+    }
+    // both state copies must agree on everything outside the last step (inactive views never move; the intrinsics / poses of
+    // a rejected candidate are stale): bring the spare copy back to the current state
+    CU(cudaMemcpyAsync(d_q[1 - cur].p, d_q[cur].p, 4 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(d_c[1 - cur].p, d_c[cur].p, 3 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(d_k[1 - cur].p, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (stage == 0) S.initial_cost = T.initial_cost;
+    if (stage >= 0) { S.final_cost[stage] = T.cost; S.iterations[stage] = T.iterations; S.termination[stage] = T.termination; } else S.init_iterations = T.iterations;
+    return ICC_OK;
+  };
+  auto finish = [&](bool success) -> icc_status {
+    icc_status r = view_errors(); if (r != ICC_OK) return r;
+    std::vector<double> qh(4 * (size_t)nv), ch(3 * (size_t)nv), kh(10);
+    CU(cudaMemcpy(qh.data(), d_q[cur].p, qh.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(ch.data(), d_c[cur].p, ch.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(kh.data(), d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
+    for (int v = 0; v < nv; ++v) {
+      q_out[4 * v] = -qh[4 * v]; q_out[4 * v + 1] = -qh[4 * v + 1]; q_out[4 * v + 2] = -qh[4 * v + 2]; q_out[4 * v + 3] = qh[4 * v + 3];
+      for (int d = 0; d < 3; ++d) p_out[3 * v + d] = ch[3 * v + d];
+      used_out[v] = 0; if (err_out) err_out[v] = 0.0;
+    }
+    double tot = 0.0;
+    for (int v : active) { used_out[v] = 1; if (err_out) err_out[v] = verr[v]; tot += verr[v]; }
+    for (int i = 0; i < 10; ++i) intr_out[i] = kh[i];
+    S.success = success ? 1 : 0; S.n_views_used = (int)active.size();
+    S.final_reproj_error = active.empty() ? 0.0 : tot / (double)active.size();                 // :352-366
+    S.gpu_launches = kernel_launch_count() - launches0;
+    S.seconds_total = std::chrono::duration<double>(clk::now() - t_start).count();
+    return ICC_OK;
+  };
+  rc = set_active(); if (rc != ICC_OK) return rc;
+  if (prestage) {
+    Q.model = CAM_DIVISION_UNDISTORTION;
+    rc = bundle_adjust((1u << 0) | (1u << 4), true, -1); if (rc != ICC_OK) return rc;
+    Q.model = model;
+    double kd[10];
+    CU(cudaMemcpy(kd, d_k[cur].p, sizeof kd, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(p0.data(), d_c[cur].p, p0.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    if (kd[0] > 0.0 && std::isfinite(kd[0])) { f0 = kd[0]; if (model == CAM_DIVISION_UNDISTORTION) distortion_init = kd[4]; }
+  }
+  S.focal_length_init = f0;
+  // ---- grid filter in file order (:313-325): a view is taken iff no accepted camera position lies within grid_size ---------------
+  // (the reference scans all accepted positions; a hash grid with cells of grid_size visits only the 27 cells that can hold one
+  // -- same decisions, linear time)
+  if (o.grid_size > 0.0) {
+    std::vector<int> sel;
+    std::unordered_map<uint64_t, std::vector<int>> cells;
+    const double inv = 1.0 / o.grid_size;
+    bool hashable = true;
+    for (int v : active) for (int d = 0; d < 3; ++d) if (!(std::fabs(p0[3 * v + d] * inv) < 1e6)) hashable = false;   // 21 bits per axis
+    auto key = [](int64_t x, int64_t y, int64_t z) { return (uint64_t)((x + (1 << 20)) & 0x1fffff) << 42 | (uint64_t)((y + (1 << 20)) & 0x1fffff) << 21 | (uint64_t)((z + (1 << 20)) & 0x1fffff); };
+    auto close_to = [&](int v, int a) { const double dx = p0[3 * v] - p0[3 * a], dy = p0[3 * v + 1] - p0[3 * a + 1], dz = p0[3 * v + 2] - p0[3 * a + 2]; return std::sqrt(dx * dx + dy * dy + dz * dz) < o.grid_size; };
+    for (int v : active) {
+      bool take = true;
+      if (hashable) {
+        const int64_t cx = (int64_t)std::floor(p0[3 * v] * inv), cy = (int64_t)std::floor(p0[3 * v + 1] * inv), cz = (int64_t)std::floor(p0[3 * v + 2] * inv);
+        for (int64_t x = cx - 1; x <= cx + 1 && take; ++x) for (int64_t y = cy - 1; y <= cy + 1 && take; ++y) for (int64_t z = cz - 1; z <= cz + 1 && take; ++z) {
+          auto it = cells.find(key(x, y, z));
+          if (it != cells.end()) for (int a : it->second) if (close_to(v, a)) { take = false; break; }
+        }
+        if (take) cells[key(cx, cy, cz)].push_back(v);
+      } else {
+        for (int a : sel) if (close_to(v, a)) { take = false; break; }
+      }
+      if (take) sel.push_back(v);
+    }
+    active.swap(sel);
+  }
+  S.n_views_selected = (int)active.size();
+  rc = set_active(); if (rc != ICC_OK) return rc;
+  // ---- initial intrinsics of the target model (AddView :84-129) --------------------------------------------------------------------
+  std::fill(k0.begin(), k0.end(), 0.0);
+  k0[0] = f0; k0[1] = 1.0;
+  switch (model) {
+    case CAM_FOV: case CAM_DIVISION_UNDISTORTION: k0[2] = cx0; k0[3] = cy0; break;
+    default: k0[3] = cx0; k0[4] = cy0; break;
+  }
+  if (model == CAM_DIVISION_UNDISTORTION) k0[4] = distortion_init;
+  if (model == CAM_FOV) k0[4] = distortion_init != 0.0 ? distortion_init : 1e-3;   // theia's FOV model has no gradient at omega = 0
+  if (model == CAM_DOUBLE_SPHERE) { k0[5] = -0.25; k0[6] = 0.5; }
+  if (model == CAM_EXTENDED_UNIFIED) { k0[5] = 0.5; k0[6] = 1.0; }
+  for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), 10 * sizeof(double), cudaMemcpyHostToDevice));
+  if ((int)active.size() < o.min_num_views) return finish(false);                               // :132-135
+  const IntrinsicSubsets sub = intrinsic_subsets(model);
+  // 1. focal length and radial distortion, principal point fixed (:146-160)
+  rc = bundle_adjust(sub.focal | (model != CAM_PINHOLE ? sub.radial : 0u), true, 0); if (rc != ICC_OK) return rc;
+  rc = remove_views(o.max_view_error_stage1_px); if (rc != ICC_OK) return rc;                    // :162
+  // 2. principal point, everything else fixed (:164-174)
+  rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
+  if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
+  // 3. full optimisation (:181-198)
+  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN ? sub.tangential : 0u);
+  rc = bundle_adjust(stage3_mask, true, 2);
+  if (rc != ICC_OK) return rc;
+  rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200
+  if ((int)active.size() < o.min_num_views) return finish(false);                                // :202-205
+  if (o.optimize_board_points) {                                                                 // :207-216
+    // BundleAdjustTracks: every camera constant, one warp per board point over its observations in the remaining views ...
+    std::vector<int> obs_view(std::max(1, nc), -1);
+    for (int v : active) for (int c = off[v]; c < off[v + 1]; ++c) obs_view[c] = v;
+    PointProblem PQ; memset(&PQ, 0, sizeof PQ);
+    PQ.model = model; CU(cudaMemcpy(PQ.intr, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
+    PQ.normalized = 0; PQ.n_points = np; PQ.min_obs = 1; PQ.huber = o.huber_width;
+    PQ.board_in = B.board.p; PQ.meas = B.uv.p; PQ.q_cw = d_q[cur].p; PQ.cam_c = d_c[cur].p;
+    DevBuf<double4> d_board2; rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, S.n_points_optimized, err); if (rc != ICC_OK) return rc;
+    CU(cudaMemcpyAsync(B.board.p, d_board2.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToDevice, st));
+    // ... then BundleAdjustViews once more with the options of stage 3
+    const int it3 = S.iterations[2];
+    rc = bundle_adjust(stage3_mask, true, 2); if (rc != ICC_OK) return rc;
+    S.iterations[2] += it3;
+  }
+  return finish(true);
 }
 
 }  // namespace icc

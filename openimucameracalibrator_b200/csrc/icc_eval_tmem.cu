@@ -15,8 +15,6 @@
 
 namespace icc {
 
-void count_launch();
-
 namespace {
 
 // warps per CTA: per warp a 13.5 KB tile, a 21.3 KB park and its staging slot; six of them fill the 227 KB a block may use on sm_90a

@@ -12,8 +12,6 @@
 
 namespace icc {
 
-void count_launch();
-
 namespace {
 
 struct PoseD { Q4 q; V3 t; };

@@ -131,7 +131,6 @@ struct PoseProblem {
   double lm_rel_tol;           // relative cost decrease that ends the refinement (0 selects 1e-15: poses pinned to ~1e-9; an initialiser can stop far earlier)
   int refine_only;             // 1: start from the poses already in q_wc / p_wc (valid views only), no homography (OptimizeAllPoses, :226-236)
 };
-void launch_unproject(int model, const double* intr10, int n, const double2* uv, double2* xy, int* ok, cudaStream_t st);
 void launch_board_poses(const PoseProblem& Q, const double2* xy, const int* ok, unsigned char* use, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st);
 // board point refinement with constant cameras (theia::BundleAdjustTracks), one warp per point
 struct PointProblem {
@@ -145,56 +144,10 @@ struct PointProblem {
   const double2* meas;         // per corner: xy (normalised) or uv (pixels)
   const double* q_cw; const double* cam_c; // per view: R_cw as (x,y,z,w), camera centre
 };
-void launch_point_refine(const PointProblem& Q, double4* board_out, int* optimized, cudaStream_t st);
 // focal length per view from the board homography on centred pixels (f2[v] = f^2 or 0), pinhole normalisation of pixels
 void launch_board_focal(const PoseProblem& Q, const double2* uv, double cx, double cy, double2* xy, unsigned char* use, double* f2, cudaStream_t st);
 void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, double f, double2* xy, int* ok, cudaStream_t st);
-// ---- camera intrinsic calibration: bundle adjustment of view poses + shared intrinsics (icc_camcal.cu) ----------------------
-// Column order of a view's [J | r] rows: 0-2 rotation increment, 3-5 camera centre, 6-15 intrinsics (Theia order), 16 residual.
-constexpr int CC_COLS = 17, CC_PACK = CC_COLS * (CC_COLS + 1) / 2, CC_Y = 66;   // packed upper triangle; Y = A^-1 [H_pk | g_p] (6 x 11)
-enum { CC_CAND_COST = 0, CC_G_DELTA = 1, CC_D_DELTA = 2, CC_STEP_SQ = 3, CC_X_SQ = 4, CC_FAIL = 5, CC_GRAD_MAX = 6, CC_X_COST = 7, CC_SCAL_COUNT = 8 };
-struct CamCalProblem {
-  int model, n_points, n_active, pose_free;
-  unsigned intr_mask;          // bit i set = intrinsic i is optimised in this stage
-  double huber;                // loss width (camera_calibrator.cc:143)
-  const double4* board; const int* f_off; const int* pid; const double2* uv;
-  const int* active;           // indices of the views that take part (n_active)
-};
-struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) per view, camera centre per view, 10 intrinsics
-// with_jacobian: per-view packed blocks (n_active x CC_PACK) + the intrinsics part and the cost summed into sys[CC_PACK + 1];
-// otherwise cost only into *cost_out and (optional) the per-view mean reprojection error [px] into view_err (indexed by view)
-void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool with_jacobian, double* blocks, double* sys, double* cost_out, double* view_err, cudaStream_t st);
-// one damped step: per-view Schur elimination, reduced intrinsics system, back-substitution into the candidate state
-void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const CamCalState& cand, const double* blocks, const double* sys, double* red /* 66 */, double* Y,
-                        double* scale /* 6 n_active + 10 */, int compute_scale, double radius, double min_diag, double max_diag, double* dk /* 10 */, double* scal, cudaStream_t st);
-// ---- IMU-to-camera rotation + time offset initialiser (icc_rotinit.cu) -----------------------------------------------------
-struct RotInitState {
-  double a, b, c, d;          // golden-section bracket and its two interior candidates (time offsets, seconds)
-  double sums[2][16];         // per candidate: sum vis (3), sum imu (3), sum imu x vis (9), robust error
-  double R[2][9], bias[2][3]; // per candidate closed-form solution (row-major)
-  double R_best[9], bias_best[3], error;
-  int iterations, done;
-};
-struct RotInitProblem {
-  int n;                      // IMU samples inside the common time window
-  const double* t;            // their zero-based timestamps (sorted)
-  const double* vis;          // smoothed visual angular velocity at those times (3 per sample)
-  const double* imu;          // smoothed gyroscope rates (3 per sample)
-  double* vis_shift;          // scratch: 2 x 3n, the shifted + interpolated visual rates of both candidates
-  RotInitState* state;
-  int estimate_bias;
-  double tolerance;
-  double bias_in[3];
-};
-void launch_interp_quat(int n_old, const double* t_old, const double4* q_old, int n_new, const double* t_new, double4* q_new, cudaStream_t st);
-void launch_visual_angular_velocity(int n, const double4* q, double dt_imu, double* w_raw, unsigned char* bad, double* w_held, double* w_smooth, const double* imu, double* imu_smooth, cudaStream_t st);
-void launch_golden_section(const RotInitProblem& Q, double max_offset, int max_iterations, int sm_count, cudaStream_t st);
-// ---- spline error weighting (icc_sew.cu) ------------------------------------------------------------------------------------
-int sew_fft_length(int N);      // power-of-two length of the Bluestein convolution
-void launch_sew_spectrum(int N, const double* signal /* N x 3 */, double* xhat /* N */, double* energy_sum, double* scratch /* 16 * sew_fft_length(N) doubles */, cudaStream_t st);
-void launch_sew_residual_energy(int N, const double* xhat, double fscale, double dt, double* out, int sm_count, cudaStream_t st);
-// column sums of the accelerometer / gyroscope streams (static bias estimate, python/get_imu_biases.py)
-void launch_imu_sums(int n, const double* acc, const double* gyr, double* out6, int sm_count, cudaStream_t st);
-int kernel_launch_count();
+int kernel_launch_count();   // kernels launched so far in this process (icc_eval.cu)
+void count_launch();         // every launcher calls it once per kernel it enqueues
 
 }  // namespace icc

@@ -16,8 +16,6 @@
 
 namespace icc {
 
-void count_launch();
-
 namespace {
 
 // de-homogenised point + local Jacobian (row-major 4 x 3) of one board point (icc_points_math.cuh)

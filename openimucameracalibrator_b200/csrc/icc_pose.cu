@@ -14,14 +14,12 @@
 // reference's BundleAdjustView (normalised pinhole reprojection error, Huber 1.345) with Levenberg-Marquardt to a tighter
 // tolerance than Ceres' defaults, so both land on the same optimum.
 #include "icc_camera.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
 #include "icc_small_linalg.cuh"
 
 #include <cmath>
 
 namespace icc {
-
-void count_launch();
 
 namespace {
 
@@ -413,6 +411,120 @@ void launch_point_refine(const PointProblem& Q, double4* board_out, int* optimiz
   if (Q.n_points <= 0) return;
   point_refine_kernel<<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized);
   count_launch();
+}
+
+// ---- host drivers of row f1 (icc_pixels_to_normalized, icc_estimate_board_poses, icc_optimize_board_points, icc_filter_bad_poses) ----
+#define CU(call) ICC_CUDA_CHECK(call, err)
+
+icc_status upload_board_views(cudaStream_t st, int np, const double* points, int nf, const int32_t* off, const int32_t* ids, const double* uv, BoardViews& B, std::string& err) {
+  const int nc = off[nf];
+  B.nf = nf; B.nc = nc; B.np = np;
+  CU(B.board.upload(points, np, st)); CU(B.off.upload(off, nf + 1, st)); CU(B.pid.upload(ids, nc, st)); CU(B.uv.upload(uv, nc, st));
+  CU(B.xy.alloc(std::max(1, nc))); CU(B.ok.alloc(std::max(1, nc))); CU(B.use.alloc(std::max(1, nc)));
+  CU(B.q.alloc(4 * (size_t)nf)); CU(B.p.alloc(3 * (size_t)nf)); CU(B.e.alloc(nf)); CU(B.valid.alloc(nf));
+  return ICC_OK;
+}
+
+icc_status read_poses(cudaStream_t st, const BoardViews& B, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err) {
+  CU(cudaMemcpyAsync(q_wc, B.q.p, 4 * (size_t)B.nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(p_wc, B.p.p, 3 * (size_t)B.nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (mean_err) CU(cudaMemcpyAsync(mean_err, B.e.p, (size_t)B.nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(valid, B.valid.p, (size_t)B.nf * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return ICC_OK;
+}
+
+icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const int32_t* ids, const std::vector<int>& obs_view, DevBuf<double4>& d_out, std::vector<double>& points_out, int& n_opt, std::string& err) {
+  const int np = Q.n_points;
+  std::vector<int> pt_off, pt_obs;
+  build_point_adjacency(np, nc, ids, [&](int c) { return obs_view[c] >= 0; }, pt_off, pt_obs);
+  DevBuf<int> d_view, d_pt_off, d_pt_obs, d_opt;
+  CU(d_view.upload(obs_view)); CU(d_pt_off.upload(pt_off)); CU(d_pt_obs.alloc(std::max<size_t>(1, pt_obs.size()))); CU(d_opt.alloc(np)); CU(d_out.alloc(np));
+  if (!pt_obs.empty()) CU(cudaMemcpy(d_pt_obs.p, pt_obs.data(), pt_obs.size() * sizeof(int), cudaMemcpyHostToDevice));
+  Q.pt_off = d_pt_off.p; Q.pt_obs = d_pt_obs.p; Q.obs_view = d_view.p;
+  launch_point_refine(Q, d_out.p, d_opt.p, st);
+  std::vector<int> opt(np); points_out.resize(4 * (size_t)np);
+  CU(cudaMemcpyAsync(points_out.data(), d_out.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(opt.data(), d_opt.p, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  n_opt = 0; for (int o : opt) n_opt += o;
+  return ICC_OK;
+}
+
+// un-projection of every corner and the PoseProblem of EstimatePosesFromJson / OptimizeAllPoses for a W x H camera (pose_estimator.cc:97-101, :181)
+static PoseProblem unproject_corners(cudaStream_t st, int model, const double intr[10], int W, int H, const BoardViews& B, double max_reproj_error, int min_points) {
+  launch_unproject(model, intr, B.nc, B.uv.p, B.xy.p, B.ok.p, st);
+  PoseProblem Q; memset(&Q, 0, sizeof Q);
+  Q.model = model; for (int i = 0; i < 10; ++i) Q.intr[i] = intr[i];
+  Q.n_frames = B.nf; Q.n_points = B.np; Q.min_points = min_points > 0 ? min_points : 8;
+  Q.board = B.board.p; Q.f_off = B.off.p; Q.pid = B.pid.p;
+  const double max_px = max_reproj_error > 0.0 ? max_reproj_error : 0.004 * H;            // pose_estimator.cc:97
+  Q.thresh_sq = (W > 0 && H > 0) ? max_px / std::sqrt((double)W * W + (double)H * H) : 1e-3;   // :101 (compared with a SQUARED error by theia's RANSAC)
+  Q.max_err = max_px;                                                                       // :181 (pixels against a normalised error, as in the reference)
+  return Q;
+}
+
+icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err) {
+  DevBuf<double2> d_uv, d_xy; DevBuf<int> d_ok;
+  CU(d_uv.upload(uv, n, st)); CU(d_xy.alloc(n)); CU(d_ok.alloc(n));
+  launch_unproject(model, intr, n, d_uv.p, d_xy.p, d_ok.p, st);
+  CU(cudaMemcpyAsync(xy_out, d_xy.p, (size_t)n * sizeof(double2), cudaMemcpyDeviceToHost, st));
+  if (ok) CU(cudaMemcpyAsync(ok, d_ok.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return ICC_OK;
+}
+
+icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
+                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err) {
+  BoardViews B;
+  icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
+  launch_board_poses(unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points), B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
+  if (cudaGetLastError() != cudaSuccess) { err = "pose kernels failed"; return ICC_ERR_CUDA; }
+  return ICC_OK;
+}
+
+icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
+                                 const double* uv, double max_reproj_error, int min_points, int min_observations, double* q_wc, double* p_wc, double* mean_err, int32_t* valid,
+                                 std::vector<double>& points_out, int32_t* n_opt_out, std::string& err) {
+  BoardViews B;
+  icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
+  const int nc = B.nc;
+  CU(B.q.upload(q_wc, 4 * (size_t)nf, st)); CU(B.p.upload(p_wc, 3 * (size_t)nf, st)); CU(B.valid.upload(valid, nf, st));
+  CU(cudaMemsetAsync(B.e.p, 0, (size_t)nf * sizeof(double), st));   // views that are not valid keep a zero error
+  PoseProblem Q = unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points);
+  Q.refine_only = 1;
+  // 1. the stored poses and their inlier sets (what the pose dataset holds after EstimatePosesFromJson)
+  launch_board_poses(Q, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  std::vector<unsigned char> use(std::max(1, nc)); std::vector<int> vh(nf); std::vector<double> qh(4 * (size_t)nf), ph(3 * (size_t)nf);
+  CU(cudaMemcpyAsync(use.data(), B.use.p, (size_t)std::max(1, nc), cudaMemcpyDeviceToHost, st));
+  rc = read_poses(st, B, qh.data(), ph.data(), nullptr, vh.data(), err); if (rc != ICC_OK) return rc;
+  // 2. OptimizeBoardPoints: one warp per point over its inlier observations in valid views, cameras constant
+  std::vector<int> obs_view(std::max(1, nc), -1);
+  for (int f = 0; f < nf; ++f) if (vh[f]) for (int c = off[f]; c < off[f + 1]; ++c) if (use[c]) obs_view[c] = f;
+  for (int f = 0; f < nf; ++f) for (int d = 0; d < 3; ++d) qh[4 * f + d] = -qh[4 * f + d];   // R_cw = conj(q_wc)
+  DevBuf<double> d_qcw, d_c; DevBuf<double4> d_board2;
+  CU(d_qcw.upload(qh)); CU(d_c.upload(ph));
+  PointProblem PQ; memset(&PQ, 0, sizeof PQ);
+  PQ.model = model; for (int i = 0; i < 10; ++i) PQ.intr[i] = intr[i];
+  PQ.normalized = 1; PQ.n_points = np; PQ.min_obs = min_observations > 0 ? min_observations : 30; PQ.huber = 1.345;
+  PQ.board_in = B.board.p; PQ.meas = B.xy.p; PQ.q_cw = d_qcw.p; PQ.cam_c = d_c.p;
+  int n_opt = 0;
+  rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, n_opt, err); if (rc != ICC_OK) return rc;
+  // 3. OptimizeAllPoses on the new points
+  Q.board = d_board2.p;
+  launch_board_poses(Q, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
+  if (cudaGetLastError() != cudaSuccess) { err = "board point kernels failed"; return ICC_ERR_CUDA; }
+  if (n_opt_out) *n_opt_out = n_opt;
+  return ICC_OK;
+}
+
+void filter_bad_poses(int nv, const double* p_wc, int32_t* valid) {
+  std::vector<double> z; for (int i = 0; i < nv; ++i) if (valid[i]) z.push_back(p_wc[3 * i + 2]);
+  if (z.empty()) return;
+  const double med = median_like_reference(z);
+  for (int i = 0; i < nv; ++i) if (valid[i] && std::fabs(p_wc[3 * i + 2] - med) > std::fabs(med)) valid[i] = 0;
 }
 
 }  // namespace icc

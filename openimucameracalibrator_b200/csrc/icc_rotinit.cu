@@ -16,7 +16,7 @@
 // iteration are evaluated by the same launches and a one-thread kernel shrinks the bracket, so the host only enqueues launches
 // and reads the result once at the end.
 #include "icc_device_math.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
 
 #include "icc_rotinit_math.cuh"
 
@@ -24,7 +24,24 @@
 
 namespace icc {
 
-void count_launch();
+struct RotInitState {
+  double a, b, c, d;          // golden-section bracket and its two interior candidates (time offsets, seconds)
+  double sums[2][16];         // per candidate: sum vis (3), sum imu (3), sum imu x vis (9), robust error
+  double R[2][9], bias[2][3]; // per candidate closed-form solution (row-major)
+  double R_best[9], bias_best[3], error;
+  int iterations, done;
+};
+struct RotInitProblem {
+  int n;                      // IMU samples inside the common time window
+  const double* t;            // their zero-based timestamps (sorted)
+  const double* vis;          // smoothed visual angular velocity at those times (3 per sample)
+  const double* imu;          // smoothed gyroscope rates (3 per sample)
+  double* vis_shift;          // scratch: 2 x 3n, the shifted + interpolated visual rates of both candidates
+  RotInitState* state;
+  int estimate_bias;
+  double tolerance;
+  double bias_in[3];
+};
 
 namespace {
 
@@ -206,6 +223,17 @@ __global__ void init_state_kernel(RotInitProblem Q, double max_offset) {
   S->done = !(fabs(S->c - S->d) > Q.tolerance) ? 1 : 0;
 }
 
+void quat_from_rowmajor(const double* R, double* q) {    // -> x, y, z, w
+  const double m00 = R[0], m01 = R[1], m02 = R[2], m10 = R[3], m11 = R[4], m12 = R[5], m20 = R[6], m21 = R[7], m22 = R[8], tr = m00 + m11 + m22;
+  double x, y, z, w;
+  if (tr > 0.0) { const double s = std::sqrt(tr + 1.0) * 2.0; w = 0.25 * s; x = (m21 - m12) / s; y = (m02 - m20) / s; z = (m10 - m01) / s; }
+  else if (m00 > m11 && m00 > m22) { const double s = std::sqrt(1.0 + m00 - m11 - m22) * 2.0; w = (m21 - m12) / s; x = 0.25 * s; y = (m01 + m10) / s; z = (m02 + m20) / s; }
+  else if (m11 > m22) { const double s = std::sqrt(1.0 + m11 - m00 - m22) * 2.0; w = (m02 - m20) / s; x = (m01 + m10) / s; y = 0.25 * s; z = (m12 + m21) / s; }
+  else { const double s = std::sqrt(1.0 + m22 - m00 - m11) * 2.0; w = (m10 - m01) / s; x = (m02 + m20) / s; y = (m12 + m21) / s; z = 0.25 * s; }
+  const double n = std::sqrt(x * x + y * y + z * z + w * w);
+  q[0] = x / n; q[1] = y / n; q[2] = z / n; q[3] = w / n;
+}
+
 }  // namespace
 
 void launch_interp_quat(int n_old, const double* t_old, const double4* q_old, int n_new, const double* t_new, double4* q_new, cudaStream_t st) {
@@ -231,6 +259,69 @@ void launch_golden_section(const RotInitProblem& Q, double max_offset, int max_i
     error_kernel<<<dim3(gx, 2), 256, 0, st>>>(Q); count_launch();
     golden_kernel<<<1, 1, 0, st>>>(Q); count_launch();
   }
+}
+
+// ---- host driver of row f3 (icc_estimate_imu_to_camera_rotation) ----------------------------------------------------------
+#define CU(call) ICC_CUDA_CHECK(call, err)
+
+icc_status estimate_imu_to_camera_rotation(cudaStream_t st, int sm_count, int n_views, const double* view_t, const double* q_cw, int n_imu, const double* imu_t,
+                                           const double* gyro, const double* bias_in, double* q_out, double* td_out, double* bias_out, double* err_out,
+                                           int32_t* iters_out, std::string& err) {
+  // ---- host preparation (app :96-162): ordered maps, median frame interval, regular grid, common window ------------------
+  // std::map semantics of the reference (time ordered, a repeated timestamp keeps the LAST sample); already-sorted input -- the
+  // normal case -- skips the tree
+  auto ordered = [](const double* t, int n) { std::vector<std::pair<double, int>> o; o.reserve(n);
+    bool inc = true; for (int i = 1; i < n && inc; ++i) inc = t[i] > t[i - 1];
+    if (inc) { for (int i = 0; i < n; ++i) o.emplace_back(t[i], i); return o; }
+    std::map<double, int> m; for (int i = 0; i < n; ++i) m[t[i]] = i;
+    for (const auto& kv : m) o.emplace_back(kv.first, kv.second);
+    return o; };
+  const std::vector<std::pair<double, int>> vmap = ordered(view_t, n_views), gmap = ordered(imu_t, n_imu);
+  if (vmap.size() < 2 || gmap.size() < 2) { err = "need at least two distinct view and gyroscope timestamps"; return ICC_ERR_INVALID_ARGUMENT; }
+  double imu_dt = 0.0;
+  for (int i = 1; i < n_imu; ++i) imu_dt += imu_t[i] - imu_t[i - 1];                     // app :103-108 (file order)
+  imu_dt /= (double)(n_imu - 1);
+  std::vector<double> tv; std::vector<double4> qv;
+  for (const auto& kv : vmap) { tv.push_back(kv.first); const double* q = q_cw + 4 * (size_t)kv.second; qv.push_back(make_double4(q[0], q[1], q[2], q[3])); }
+  std::vector<double> diffs; for (size_t i = 1; i < tv.size(); ++i) diffs.push_back(tv[i] - tv[i - 1]);
+  const double cam_dt = median_like_reference(diffs);
+  if (!(cam_dt > 0.0)) { err = "non-positive median frame interval"; return ICC_ERR_INVALID_ARGUMENT; }
+  std::vector<double> grid; for (double t = tv.front(); t < tv.back(); t += cam_dt) grid.push_back(t);   // app :139-144
+  std::vector<double> tg, gg;    // gyroscope, time ordered, bias removed
+  for (const auto& kv : gmap) { tg.push_back(kv.first); for (int d = 0; d < 3; ++d) gg.push_back(gyro[3 * (size_t)kv.second + d] - (bias_in ? bias_in[d] : 0.0)); }
+  const double t0 = grid.front() >= tg.front() ? grid.front() : tg.front();               // :127-129
+  const double tend = grid.back() >= tg.back() ? grid.back() : tg.back();                 // (the LATER end, as in the reference)
+  std::vector<double> tI, wI; for (size_t i = 0; i < tg.size(); ++i) if (tg[i] >= t0 && tg[i] <= tend) { tI.push_back(tg[i] - t0); for (int d = 0; d < 3; ++d) wI.push_back(gg[3 * i + d]); }
+  size_t g0 = 0; while (g0 < grid.size() && grid[g0] < t0) ++g0;
+  std::vector<double> tV; for (size_t i = g0; i < grid.size(); ++i) if (grid[i] <= tend) tV.push_back(grid[i] - t0);
+  const int N = (int)tI.size(), Mc = (int)tV.size(), M = (int)grid.size(), nv = (int)tv.size();
+  if (N < 2 || Mc < 1) { err = "camera and gyroscope streams do not overlap"; return ICC_ERR_INVALID_ARGUMENT; }
+  // ---- device pipeline --------------------------------------------------------------------------------------------------
+  DevBuf<double> d_tv, d_grid, d_tV, d_tI, d_wI, d_wraw, d_wheld, d_wvis, d_wimu, d_shift; DevBuf<double4> d_qv, d_qgrid, d_qi; DevBuf<unsigned char> d_bad; DevBuf<RotInitState> d_state;
+  CU(d_tv.upload(tv)); CU(d_qv.upload(qv)); CU(d_grid.upload(grid)); CU(d_tV.upload(tV)); CU(d_tI.upload(tI)); CU(d_wI.upload(wI));
+  CU(d_qgrid.alloc(M)); CU(d_qi.alloc(N)); CU(d_wraw.alloc(3 * (size_t)N)); CU(d_wheld.alloc(3 * (size_t)N)); CU(d_wvis.alloc(3 * (size_t)N)); CU(d_wimu.alloc(3 * (size_t)N));
+  CU(d_shift.alloc(6 * (size_t)N)); CU(d_bad.alloc(N)); CU(d_state.alloc(1));
+  launch_interp_quat(nv, d_tv.p, d_qv.p, M, d_grid.p, d_qgrid.p, st);              // views -> regular frame grid (app :150-156)
+  launch_interp_quat(Mc, d_tV.p, d_qgrid.p + g0, N, d_tI.p, d_qi.p, st);           // grid -> IMU rate (:172-173)
+  launch_visual_angular_velocity(N, d_qi.p, imu_dt, d_wraw.p, d_bad.p, d_wheld.p, d_wvis.p, d_wI.p, d_wimu.p, st);
+  RotInitProblem Q; memset(&Q, 0, sizeof Q);
+  Q.n = N; Q.t = d_tI.p; Q.vis = d_wvis.p; Q.imu = d_wimu.p; Q.vis_shift = d_shift.p; Q.state = d_state.p;
+  Q.estimate_bias = bias_in ? 0 : 1; Q.tolerance = 1e-4;
+  for (int d = 0; d < 3; ++d) Q.bias_in[d] = bias_in ? bias_in[d] : 0.0;
+  // the bracket shrinks by the golden ratio per step whatever the data says, so the step count is known up to rounding
+  int n_it = 0; { const double g = (1.0 + std::sqrt(5.0)) / 2.0; double a = -1.0, b = 1.0, c = b - (b - a) / g, d = a + (b - a) / g; while (std::fabs(c - d) > Q.tolerance && n_it < 200) { b = d; c = b - (b - a) / g; d = a + (b - a) / g; ++n_it; } }
+  launch_golden_section(Q, 1.0, n_it + 2, sm_count > 0 ? sm_count : 132, st);
+  RotInitState S;
+  CU(cudaMemcpyAsync(&S, d_state.p, sizeof S, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (cudaGetLastError() != cudaSuccess) { err = "rotation initialiser kernels failed"; return ICC_ERR_CUDA; }
+  if (!S.done) { err = "golden-section search did not terminate"; return ICC_ERR_NUMERIC; }
+  quat_from_rowmajor(S.R_best, q_out);
+  *td_out = (S.b + S.a) / 2;                                                               // :259
+  if (bias_out) for (int d = 0; d < 3; ++d) bias_out[d] = S.bias_best[d];
+  if (err_out) *err_out = S.error;
+  if (iters_out) *iters_out = S.iterations;
+  return ICC_OK;
 }
 
 }  // namespace icc

@@ -12,13 +12,12 @@
 // power-of-two Stockham radix-2 passes written here (FP64, twiddles from sincospi, chirp phase reduced with exact integer
 // arithmetic n^2 mod 2N), batched over the three axes; the spectrum stays in HBM and each quality evaluation of the root search
 // is one fused response + energy reduction over the N bins.  The scalar root search (a dozen evaluations) runs on the host.
-#include "icc_kernels.h"
+#include "icc_host.h"
 
 #include <cmath>
+#include <functional>
 
 namespace icc {
-
-void count_launch();
 
 namespace {
 
@@ -105,6 +104,34 @@ __global__ void residual_energy_kernel(int N, const double* __restrict__ xhat, d
   if (threadIdx.x == 0) { double t = 0.0; for (int w2 = 0; w2 < (blockDim.x >> 5); ++w2) t += red[w2]; atomicAdd(out, t); }
 }
 
+// scipy.optimize.brentq (Brent 1973 as implemented in scipy/optimize/Zeros/brentq.c), xtol = 2e-12, rtol = 4 eps, 100 iterations
+double brentq(const std::function<double(double)>& f, double xa, double xb, bool& ok) {
+  const double xtol = 2e-12, rtol = 8.881784197001252e-16;
+  double xpre = xa, xcur = xb, xblk = 0.0, fpre = f(xpre), fcur = f(xcur), fblk = 0.0, spre = 0.0, scur = 0.0;
+  ok = true;
+  if (fpre == 0.0) return xpre;
+  if (fcur == 0.0) return xcur;
+  if ((fpre > 0) == (fcur > 0)) { ok = false; return xcur; }
+  for (int i = 0; i < 100; ++i) {
+    if (fpre != 0.0 && fcur != 0.0 && ((fpre > 0) != (fcur > 0))) { xblk = xpre; fblk = fpre; spre = scur = xcur - xpre; }
+    if (std::fabs(fblk) < std::fabs(fcur)) { xpre = xcur; xcur = xblk; xblk = xpre; fpre = fcur; fcur = fblk; fblk = fpre; }
+    const double delta = (xtol + rtol * std::fabs(xcur)) / 2, sbis = (xblk - xcur) / 2;
+    if (fcur == 0.0 || std::fabs(sbis) < delta) return xcur;
+    if (std::fabs(spre) > delta && std::fabs(fcur) < std::fabs(fpre)) {
+      double stry;
+      if (xpre == xblk) stry = -fcur * (xcur - xpre) / (fcur - fpre);                       // secant
+      else { const double dpre = (fpre - fcur) / (xpre - xcur), dblk = (fblk - fcur) / (xblk - xcur); stry = -fcur * (fblk * dblk - fpre * dpre) / (dblk * dpre * (fblk - fpre)); }   // inverse quadratic
+      if (2 * std::fabs(stry) < std::min(std::fabs(spre), 3 * std::fabs(sbis) - delta)) { spre = scur; scur = stry; }
+      else { spre = sbis; scur = sbis; }
+    } else { spre = sbis; scur = sbis; }
+    xpre = xcur; fpre = fcur;
+    if (std::fabs(scur) > delta) xcur += scur; else xcur += (sbis > 0 ? delta : -delta);
+    fcur = f(xcur);
+  }
+  ok = false;
+  return xcur;
+}
+
 }  // namespace
 
 int sew_fft_length(int N) { int M = 1; while (M < 2 * N - 1) M <<= 1; return M; }
@@ -157,6 +184,74 @@ void launch_imu_sums(int n, const double* acc, const double* gyr, double* out6, 
   if (n <= 0) return;
   int g = (n + 255) / 256; if (g > 4 * sm_count) g = 4 * sm_count;
   imu_sums_kernel<<<g, 256, 0, st>>>(n, acc, gyr, out6); count_launch();
+}
+
+// ---- host drivers: row f2 (icc_spline_error_weighting) and the static IMU biases (icc_estimate_imu_biases) -----------------------
+#define CU(call) ICC_CUDA_CHECK(call, err)
+
+icc_status spline_error_weighting(cudaStream_t st, int sm_count, int n, const double* times, const double* signal, double quality, double min_dt, double max_dt, double* dt_out, double* var_out, double* spectrum, std::string& err) {
+  double mean_dt = 0.0; for (int i = 1; i < n; ++i) mean_dt += times[i] - times[i - 1]; mean_dt /= (double)(n - 1);
+  if (!(mean_dt > 0.0)) { err = "timestamps must increase on average"; return ICC_ERR_INVALID_ARGUMENT; }
+  const double sample_rate = 1.0 / mean_dt, d = 1.0 / sample_rate, fscale = 1.0 / ((double)n * d);   // np.fft.fftfreq(n, d): k * (1 / (n d))
+  if (!(min_dt > 0.0)) min_dt = 1.0 / sample_rate;                                                     // sew.py:156-160
+  if (!(max_dt > 0.0)) max_dt = ((double)n / 4.0) / sample_rate;
+  const int M = sew_fft_length(n);
+  DevBuf<double> d_sig, d_xhat, d_scr, d_acc;
+  CU(d_sig.upload(signal, 3 * (size_t)n, st)); CU(d_xhat.alloc(n)); CU(d_scr.alloc(16 * (size_t)M)); CU(d_acc.alloc(2));
+  launch_sew_spectrum(n, d_sig.p, d_xhat.p, d_acc.p, d_scr.p, st);
+  double esum = 0.0;
+  CU(cudaMemcpyAsync(&esum, d_acc.p, sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (spectrum) CU(cudaMemcpyAsync(spectrum, d_xhat.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (cudaGetLastError() != cudaSuccess) { err = "spectrum kernels failed"; return ICC_ERR_CUDA; }
+  const double max_remove = esum / (double)n * (1.0 - quality);                                        // signal_energy(Xhat) * (1 - quality)
+  bool cuda_ok = true;
+  auto removed = [&](double dt) -> double {      // signal_energy((1 - H) * Xhat)
+    double e = 0.0;
+    launch_sew_residual_energy(n, d_xhat.p, fscale, dt, d_acc.p + 1, sm_count > 0 ? sm_count : 132, st);
+    if (cudaMemcpyAsync(&e, d_acc.p + 1, sizeof(double), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) cuda_ok = false;
+    return e / (double)n;
+  };
+  auto quality_func = [&](double dt) { return max_remove / removed(dt); };
+  // find_max_quality_dt(quality_func, 1.0, min_dt, max_dt)   (sew.py:86-145)
+  double dt = max_dt, found = 0.0; bool have = false;
+  if (quality_func(dt) >= 1.0) { found = dt; have = true; }
+  else {
+    double step = max_dt * 0.5, max_quality = 0.0, max_quality_dt = dt; bool any = false;
+    while (!have) {
+      dt -= step; dt = std::max(dt, min_dt);
+      const double q = quality_func(dt);
+      if (q > 1.0) { bool ok; found = brentq([&](double x) { return quality_func(x) - 1.0; }, dt, max_dt, ok); if (!ok) { err = "Brent root search failed"; return ICC_ERR_NUMERIC; } have = true; }
+      else {
+        step *= 0.5;
+        if (q > max_quality) { max_quality = q; max_quality_dt = dt; any = true; }
+        if (dt <= min_dt) { if (!any) { err = "no knot spacing satisfies the quality"; return ICC_ERR_NUMERIC; } found = max_quality_dt; have = true; }
+      }
+      if (!cuda_ok) { err = "quality kernels failed"; return ICC_ERR_CUDA; }
+    }
+  }
+  *dt_out = found;
+  *var_out = removed(found) / (double)n;                                                               // dt_to_variance_spectrum (:196-199)
+  if (!cuda_ok) { err = "quality kernels failed"; return ICC_ERR_CUDA; }
+  return ICC_OK;
+}
+
+// python/get_imu_biases.py:36-53
+icc_status imu_biases(cudaStream_t st, int sm_count, int n, const double* acc, const double* gyr, double gravity_const, double accl_bias[3], double gyro_bias[3], std::string& err) {
+  DevBuf<double> d_a, d_g, d_s;
+  CU(d_a.upload(acc, 3 * (size_t)n, st)); CU(d_g.upload(gyr, 3 * (size_t)n, st)); CU(d_s.alloc(6));
+  launch_imu_sums(n, d_a.p, d_g.p, d_s.p, sm_count, st);
+  double s[6];
+  CU(cudaMemcpyAsync(s, d_s.p, sizeof s, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (cudaGetLastError() != cudaSuccess) { err = "bias kernel failed"; return ICC_ERR_CUDA; }
+  double mean_a[3], mean_g[3];
+  for (int d = 0; d < 3; ++d) { mean_a[d] = s[d] / n; mean_g[d] = s[3 + d] / n; }
+  int ax = 0; for (int d = 1; d < 3; ++d) if (std::fabs(mean_a[d]) > std::fabs(mean_a[ax])) ax = d;          // :39-41 (first maximum)
+  const double sgn = mean_a[ax] > 0.0 ? 1.0 : (mean_a[ax] < 0.0 ? -1.0 : 0.0);
+  const double grav = (double)(float)(gravity_const * sgn);                                                     // float32 array (:43-44)
+  for (int d = 0; d < 3; ++d) { accl_bias[d] = mean_a[d] - (d == ax ? grav : 0.0); gyro_bias[d] = mean_g[d]; }   // :46, :49-50
+  return ICC_OK;
 }
 
 }  // namespace icc

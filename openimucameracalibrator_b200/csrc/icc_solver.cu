@@ -28,8 +28,6 @@
 
 namespace icc {
 
-void count_launch();
-
 namespace {
 
 constexpr int NT = 512;          // threads of the factorisation kernels

@@ -18,7 +18,7 @@
 //     The 9-12 unknown LM runs on the host with one small readback per iteration (like icc_camcal.cu's driver).
 #include "../../include/icc_b200.h"
 #include "icc_device_math.cuh"
-#include "icc_kernels.h"
+#include "icc_host.h"
 #include "icc_static_imu_math.cuh"
 
 #include <algorithm>
@@ -29,8 +29,6 @@
 #include <vector>
 
 namespace icc {
-
-void count_launch();
 
 namespace {
 
@@ -326,13 +324,6 @@ __global__ void __launch_bounds__(kChunks * kDirs) gyro_eval_kernel(GyroArgs G) 
   if (d < G.np) for (int k = 0; k < 3; ++k) o[3 + 12 * k + d] = r[k].d;
 }
 
-template <class T>
-struct Buf {
-  T* p = nullptr;
-  ~Buf() { if (p) cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)); }
-};
-
 // DataInterval::InitialInterval / TimeToIndex (imu_data_interval.h:104-118, :147-160): nearest-sample bisection, ties to the later index
 int initial_interval_end(int n, const double* t, double duration) {
   const double end_ts = t[0] + duration;
@@ -358,7 +349,7 @@ void default_static_imu_options(icc_static_imu_options* o) {
   o->init_gyr[6] = o->init_gyr[7] = o->init_gyr[8] = 1.0;
 }
 
-#define SCU(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e__); return ICC_ERR_CUDA; } } while (0)
+#define CU(call) ICC_CUDA_CHECK(call, err)
 
 icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_static_imu_options& o,
                                 double acc_out[9], double gyr_out[9], double bias_out[3], icc_static_imu_summary& S, std::vector<int32_t>& intervals, std::string& err) {
@@ -386,36 +377,33 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
   // ---- static detection, all ten multipliers ---------------------------------------------------------------------------------
   int win = o.win_size; if (win < 11) win = 11; if (!(win % 2)) win++;                        // :113-114
   const int h = win / 2;
-  Buf<double> d_t, d_acc, d_gyr; SCU(d_t.alloc(n)); SCU(d_acc.alloc(3 * (size_t)n)); SCU(d_gyr.alloc(3 * (size_t)n));
-  SCU(cudaMemcpyAsync(d_t.p, t, n * sizeof(double), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_acc.p, acc, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
-  SCU(cudaMemcpyAsync(d_gyr.p, gyr, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+  DevBuf<double> d_t, d_acc, d_gyr; CU(d_t.upload(t, n, st)); CU(d_acc.upload(acc, 3 * (size_t)n, st)); CU(d_gyr.upload(gyr, 3 * (size_t)n, st));
   std::vector<int> kept_n(kMult, 0);
   std::vector<std::vector<int2>> kept(kMult);
   if (win < n) {                                                                             // :118 (no intervals otherwise)
     const int nc = n - 2 * h, nb = (nc + kThreads - 1) / kThreads, cap = nc / 2 + 2;
-    Buf<double> d_norm; SCU(d_norm.alloc(n));
+    DevBuf<double> d_norm; CU(d_norm.alloc(n));
     const size_t smem = (size_t)(kThreads + 2 * h) * 3 * sizeof(double);
     const int stage = smem <= 48 * 1024 ? 1 : 0;
     window_norm_kernel<<<nb, kThreads, stage ? smem : 0, st>>>(n, h, d_acc.p, stage, d_norm.p); count_launch();
-    Buf<int> d_counts, d_offsets, d_totals, d_starts, d_ends, d_ks, d_ke, d_kn;
-    SCU(d_counts.alloc(2 * kMult * (size_t)nb)); SCU(d_offsets.alloc(2 * kMult * (size_t)nb)); SCU(d_totals.alloc(2 * kMult));
-    SCU(d_starts.alloc(kMult * (size_t)cap)); SCU(d_ends.alloc(kMult * (size_t)cap)); SCU(d_ks.alloc(kMult * (size_t)cap)); SCU(d_ke.alloc(kMult * (size_t)cap)); SCU(d_kn.alloc(kMult));
+    DevBuf<int> d_counts, d_offsets, d_totals, d_starts, d_ends, d_ks, d_ke, d_kn;
+    CU(d_counts.alloc(2 * kMult * (size_t)nb)); CU(d_offsets.alloc(2 * kMult * (size_t)nb)); CU(d_totals.alloc(2 * kMult));
+    CU(d_starts.alloc(kMult * (size_t)cap)); CU(d_ends.alloc(kMult * (size_t)cap)); CU(d_ks.alloc(kMult * (size_t)cap)); CU(d_ke.alloc(kMult * (size_t)cap)); CU(d_kn.alloc(kMult));
     RunArgs R; R.n = n; R.h = h; R.nb = nb; R.cap = cap; R.norm = d_norm.p; R.counts = d_counts.p; R.offsets = d_offsets.p; R.starts = d_starts.p; R.ends = d_ends.p;
     for (int m = 0; m < kMult; ++m) R.thr[m] = (double)(m + 1) * norm_th;                       // th_mult * norm_th (:95)
     runs_kernel<<<nb, kThreads, 0, st>>>(R, 0); count_launch();
     block_scan_kernel<<<2 * kMult, kThreads, 0, st>>>(nb, d_counts.p, d_offsets.p, d_totals.p); count_launch();
     runs_kernel<<<nb, kThreads, 0, st>>>(R, 1); count_launch();
     keep_kernel<<<kMult, kThreads, 0, st>>>(cap, o.interval_n_samples, d_totals.p, d_starts.p, d_ends.p, d_ks.p, d_ke.p, d_kn.p); count_launch();
-    SCU(cudaMemcpyAsync(kept_n.data(), d_kn.p, kMult * sizeof(int), cudaMemcpyDeviceToHost, st));
-    SCU(cudaStreamSynchronize(st));
+    CU(cudaMemcpyAsync(kept_n.data(), d_kn.p, kMult * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
     std::vector<int> ks, ke;
     for (int m = 0; m < kMult; ++m) {
       ks.resize(kept_n[m]); ke.resize(kept_n[m]);
       if (kept_n[m]) {
-        SCU(cudaMemcpyAsync(ks.data(), d_ks.p + (size_t)m * cap, kept_n[m] * sizeof(int), cudaMemcpyDeviceToHost, st));
-        SCU(cudaMemcpyAsync(ke.data(), d_ke.p + (size_t)m * cap, kept_n[m] * sizeof(int), cudaMemcpyDeviceToHost, st));
-        SCU(cudaStreamSynchronize(st));
+        CU(cudaMemcpyAsync(ks.data(), d_ks.p + (size_t)m * cap, kept_n[m] * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ke.data(), d_ke.p + (size_t)m * cap, kept_n[m] * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
       }
       for (int k = 0; k < kept_n[m]; ++k) kept[m].push_back(make_int2(ks[k], ke[k]));
     }
@@ -438,10 +426,9 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
   A.koff[kMult] = (int)all.size();
   int best = -1;
   std::vector<double> fit_out(kMult * kAccOut, 0.0);
-  Buf<int2> d_all; Buf<double> d_means, d_fit;
+  DevBuf<int2> d_all; DevBuf<double> d_means, d_fit;
   if (any) {
-    SCU(d_all.alloc(all.size())); SCU(d_means.alloc(3 * all.size())); SCU(d_fit.alloc(fit_out.size()));
-    SCU(cudaMemcpyAsync(d_all.p, all.data(), all.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+    CU(d_all.upload(all.data(), all.size(), st)); CU(d_means.alloc(3 * all.size())); CU(d_fit.alloc(fit_out.size()));
     if (o.acc_use_means) {
       AccTriad none; memset(&none, 0, sizeof none);
       interval_mean_kernel<<<((int)all.size() + 127) / 128, 128, 0, st>>>((int)all.size(), d_all.p, d_acc.p, 0, none, d_means.p); count_launch();
@@ -449,9 +436,9 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
     A.acc = d_acc.p; A.kept = d_all.p; A.means = d_means.p; A.ns = o.interval_n_samples; A.use_means = o.acc_use_means ? 1 : 0; A.g_mag = o.g_mag;
     memcpy(A.x0, x0, sizeof x0); A.o = ceres_default_options(); A.out = d_fit.p;
     acc_fit_kernel<<<kMult, kThreads, 0, st>>>(A); count_launch();
-    SCU(cudaMemcpyAsync(fit_out.data(), d_fit.p, fit_out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-    SCU(cudaStreamSynchronize(st));
-    SCU(cudaGetLastError());
+    CU(cudaMemcpyAsync(fit_out.data(), d_fit.p, fit_out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
     double min_cost = 1.7976931348623157e308;
     for (int m = 0; m < kMult; ++m) {
       if (!A.fit[m]) continue;
@@ -480,11 +467,11 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
   }
   std::vector<double> gm(3 * (size_t)npos);
   interval_mean_kernel<<<(npos + 127) / 128, 128, 0, st>>>(npos, d_all.p + A.koff[best], d_acc.p, 1, tri, d_means.p); count_launch();
-  SCU(cudaMemcpyAsync(gm.data(), d_means.p, gm.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(gm.data(), d_means.p, gm.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
   double gbias[3]; seq_mean(gyr, 0, initial_interval_end(n, t, o.init_interval_duration_s), gbias);   // :214-218
-  Buf<double> d_xg; SCU(d_xg.alloc(3 * (size_t)n));
+  DevBuf<double> d_xg; CU(d_xg.alloc(3 * (size_t)n));
   unbias_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, d_gyr.p, gbias[0], gbias[1], gbias[2], d_xg.p); count_launch();
-  SCU(cudaStreamSynchronize(st));
+  CU(cudaStreamSynchronize(st));
   // transitions (:245-297): gravity directions and the monotone scan, here a bisection on the sorted timestamps
   const int ntr = npos - 1;
   std::vector<int2> span(std::max(ntr, 0));
@@ -512,11 +499,9 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
   for (int p = 0; p < 9; ++p) x[p] = o.init_gyr[p];
   x[9] = x[10] = x[11] = 0.0;
   if (ntr > 0) {
-    Buf<int2> d_span; Buf<double> d_g01, d_out;
-    SCU(d_span.alloc(ntr)); SCU(d_g01.alloc(6 * (size_t)ntr)); SCU(d_out.alloc(kGyroOut * (size_t)ntr));
-    SCU(cudaMemcpyAsync(d_span.p, span.data(), ntr * sizeof(int2), cudaMemcpyHostToDevice, st));
-    SCU(cudaMemcpyAsync(d_g01.p, g01.data(), g01.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-    SCU(cudaMemsetAsync(d_out.p, 0, kGyroOut * (size_t)ntr * sizeof(double), st));
+    DevBuf<int2> d_span; DevBuf<double> d_g01, d_out;
+    CU(d_span.upload(span.data(), ntr, st)); CU(d_g01.upload(g01.data(), g01.size(), st)); CU(d_out.alloc(kGyroOut * (size_t)ntr));
+    CU(cudaMemsetAsync(d_out.p, 0, kGyroOut * (size_t)ntr * sizeof(double), st));
     GyroArgs G; memset(&G, 0, sizeof G);
     G.x = d_xg.p; G.t = d_t.p; G.span = d_span.p; G.g01 = d_g01.p; G.gyro_dt = o.gyro_dt; G.np = np; G.with_bias = o.optimize_gyro_bias ? 1 : 0; G.out = d_out.p;
     std::vector<double> out(kGyroOut * (size_t)ntr);
@@ -524,9 +509,9 @@ icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const d
     auto eval = [&](const double* xp) -> icc_status {
       for (int p = 0; p < 12; ++p) G.p[p] = xp[p];
       gyro_eval_kernel<<<ntr, kChunks * kDirs, 0, st>>>(G); count_launch();
-      SCU(cudaMemcpyAsync(out.data(), d_out.p, out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-      SCU(cudaStreamSynchronize(st));
-      SCU(cudaGetLastError());
+      CU(cudaMemcpyAsync(out.data(), d_out.p, out.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
       for (int p = 0; p < 12; ++p) { g[p] = 0.0; for (int q = 0; q < 12; ++q) H[p][q] = 0.0; }
       double c2 = 0.0;
       for (int i = 0; i < ntr; ++i) {

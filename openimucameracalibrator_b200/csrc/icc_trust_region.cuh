@@ -1,6 +1,6 @@
 // Ceres 2.1 TrustRegionMinimizer step control with the LevenbergMarquardtStrategy radius schedule: the one copy used by every LM
-// driver (spline LM and camera calibration in icc_api.cu, static IMU fits in icc_static_imu_math.cuh).  It sees only scalars; each
-// driver keeps its loop and may evaluate the candidate before tr_step or only when tr_step asks for it:
+// driver (spline LM in icc_api.cu, camera calibration in icc_camcal.cu, static IMU fits in icc_static_imu_math.cuh).  It sees
+// only scalars; each driver keeps its loop and may evaluate the candidate before tr_step or only when tr_step asks for it:
 //   TrustRegion T = tr_start(options);
 //   while (tr_continue(T)) {
 //     if (T.jacobian_stale) { evaluate J at x; if (!tr_jacobian(T, cost, max|g|)) break; }
