@@ -256,7 +256,10 @@ void* icc_get_stream(icc_handle* h);
  * so that the converged pose is the reference's BundleAdjustView optimum (RANSAC's random minimal samples are not reproduced:
  * the inlier set is taken with the same threshold around the refined pose).
  * Outputs (per view, caller-owned): q_wc (x,y,z,w) = R_cw^T and p_wc exactly as icc_set_frames consumes them, the mean
- * normalised reprojection error, valid (1 / 0).  max_reproj_error <= 0 selects 0.004 * image_height; min_points <= 0 selects 8. */
+ * normalised reprojection error, valid (1 / 0).  max_reproj_error <= 0 selects 0.004 * image_height; min_points <= 0 selects 8.
+ * Wide-angle lenses: the normalised plane cannot hold a ray 90 degrees or more off the axis, so such corners are lost (and views with them);
+ * icc_set_pose_error(h, ICC_POSE_ERROR_TANGENT) switches this call and icc_optimize_board_points to unit bearings (icc_pixels_to_bearings)
+ * and the local tangent reprojection error.  Then mean_reproj_error, the inlier threshold and max_reproj_error are in tangent units. */
 icc_status icc_estimate_board_poses(icc_handle* h, int n_frames, const int32_t* corner_offsets /* n_frames+1 */, const int32_t* point_ids,
                                     const double* uv, double max_reproj_error, int min_points,
                                     double* q_wc_xyzw, double* p_wc, double* mean_reproj_error, int32_t* valid);
@@ -280,6 +283,22 @@ icc_status icc_optimize_board_points(icc_handle* h, int n_frames, const int32_t*
 icc_status icc_get_board_points(const icc_handle* h, double* xyzw, int n);
 /* theia::Camera::PixelToNormalizedCoordinates / z for `n` pixels with the handle's camera: xy_out[2n], ok[n] (nullable). */
 icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, double* xy_out, int32_t* ok);
+/* Unit bearing vectors of `n` pixels with the handle's camera: xyz_out[3n], ok[n] (nullable; 0 where the ray reprojects more than 1e-6 px
+ * away).  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion give icc_pixels_to_normalized's ray normalised; Fisheye's ray
+ * stays in z > 0 (the model maps p and -p to one pixel); DoubleSphere and ExtendedUnified reach their whole domain, z <= 0 included. */
+icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double* xyz_out, int32_t* ok);
+
+/* Residual of the per-view pose refinement, the inlier test and the board-point refinement of icc_estimate_board_poses and
+ * icc_optimize_board_points (not of icc_calibrate_camera, which keeps the normalised start).
+ *   ICC_POSE_ERROR_NORMALIZED (default): the reference's normalised pinhole error of BundleAdjustView.
+ *   ICC_POSE_ERROR_TANGENT: corners are unit bearings b with a tangent basis (e1, e2); a predicted camera-frame point d scores
+ *     r = (e1.d, e2.d) / (b.d), with a 1e6 cost where b.d <= 0.  The start rotates a view's bearings so that their mean is the axis and
+ *     takes the homography of those within 80 degrees of it; the rules (min_points, >= 6 inliers, the squared-error threshold, the mean
+ *     error against max_reproj_error) are kept, on the tangent error.  mean_reproj_error is then in tangent units.
+ * Any other mode is ICC_ERR_INVALID_ARGUMENT.  Host state only: also accepted by a host-only handle. */
+#define ICC_POSE_ERROR_NORMALIZED 0
+#define ICC_POSE_ERROR_TANGENT 1
+icc_status icc_set_pose_error(icc_handle* h, int mode);
 
 /* ---- upstream row f3 (SURVEY.md §8(f)): IMU-to-camera rotation + time offset initialiser -----------------------------------
  * ImuToCameraRotationEstimator::EstimateCameraImuRotation (src/core/imu_to_camera_rotation_estimator.cc:116-274) together with

@@ -17,6 +17,8 @@ c_int64_p = C.POINTER(C.c_int64)
 FLAG_POINTS, FLAG_T_I_C, FLAG_IMU_BIASES, FLAG_IMU_INTRINSICS = 1, 2, 4, 8
 FLAG_GRAVITY_DIR, FLAG_CAM_LINE_DELAY, FLAG_SPLINE, FLAG_ACC_BIAS, FLAG_GYR_BIAS = 16, 32, 64, 128, 256
 FLAG_CAM_INTRINSICS, FLAG_TIME_OFFSET = 512, 1024     # north-star extensions (the reference keeps both fixed)
+POSE_ERROR_NORMALIZED, POSE_ERROR_TANGENT = 0, 1       # residual of the per-view pose step (icc_set_pose_error)
+POSE_ERRORS = {"normalized": POSE_ERROR_NORMALIZED, "tangent": POSE_ERROR_TANGENT}
 
 STATUS_NAMES = {0: "ICC_OK", 1: "ICC_ERR_INVALID_ARGUMENT", 2: "ICC_ERR_NO_DEVICE", 3: "ICC_ERR_CUDA", 4: "ICC_ERR_STATE",
                 5: "ICC_ERR_UNSUPPORTED", 6: "ICC_ERR_NUMERIC"}
@@ -246,6 +248,17 @@ class CApi:
         xy = np.zeros((n, 2)); ok = np.zeros(n, dtype=np.int32)
         self._call("pixels_to_normalized", [C.c_int, c_double_p, c_double_p, c_int32_p], n, _dp(uv), _dp(xy), ok.ctypes.data_as(c_int32_p))
         return xy, ok
+
+    def pixels_to_bearings(self, uv):
+        """Unit bearing vectors of an (n, 2) pixel array -> (xyz[n,3], ok[n]); rays past 90 degrees where the camera model has them."""
+        uv = _f64(uv).reshape(-1, 2); n = uv.shape[0]
+        xyz = np.zeros((n, 3)); ok = np.zeros(n, dtype=np.int32)
+        self._call("pixels_to_bearings", [C.c_int, c_double_p, c_double_p, c_int32_p], n, _dp(uv), _dp(xyz), ok.ctypes.data_as(c_int32_p))
+        return xyz, ok
+
+    def set_pose_error(self, mode):
+        """Residual of estimate_board_poses / optimize_board_points: POSE_ERROR_NORMALIZED (default), POSE_ERROR_TANGENT, or their names."""
+        self._call("set_pose_error", [C.c_int], POSE_ERRORS[mode] if isinstance(mode, str) else int(mode))
 
     # ---- upstream row f4: CameraCalibrator::CalibrateCameraFromJson / RunCalibration (src/core/camera_calibrator.cc:131-389) ----
     def calibrate_camera(self, model, image_width, image_height, corner_offsets, point_ids, uv, q_wc_init=None, p_wc_init=None, init_valid=None,

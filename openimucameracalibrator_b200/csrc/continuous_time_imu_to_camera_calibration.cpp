@@ -8,7 +8,9 @@
 // JSON:  {"views": {"<view name>": {"q_wc": [w,x,y,z], "p_wc": [x,y,z]}}, "tracks": {"<id>": [x,y,z,w]}}
 // where q_wc = R_cw^T and p_wc = camera position (what app :137-145 / impl.h:290-300 take from each theia::Camera).
 // When --input_pose_dataset is omitted, the per-view board poses are estimated in-process on the GPU from the corner file
-// (icc_estimate_board_poses = PoseEstimator::EstimatePosesFromJson, SURVEY.md §8(f) row f1), i.e. the corner file alone suffices.
+// (icc_estimate_board_poses = PoseEstimator::EstimatePosesFromJson, SURVEY.md §8(f) row f1), i.e. the corner file alone suffices;
+// --pose_error normalized|tangent (default normalized) selects that step's residual (icc_set_pose_error: tangent keeps the corners of
+// fisheye lenses beyond 90 degrees).
 // Extra flags (not in the reference): --device (CUDA ordinal, default 0), --parse_only (stop after parsing, print a summary),
 // --gpus N (residual blocks sharded by time slice over devices device..device+N-1 of this host: the binary spawns one rank process per
 // extra device -- hidden flags --shard_rank / --shard_world / --comm_id_hex -- each with the library's own NCCL communicator; one
@@ -37,7 +39,7 @@ icccli::Flags default_flags() {
   icccli::Flags f;
   f.str = {{"telemetry_json", ""}, {"input_pose_dataset", ""}, {"input_corners", ""}, {"camera_calibration_json", ""},
     {"gyro_to_cam_initial_calibration", ""}, {"imu_intrinsics", ""}, {"imu_bias_file", ""}, {"spline_error_weighting_json", ""}, {"output_path", ""},
-    {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}};
+    {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"}};
   f.boolean = {{"global_shutter", false}, {"calibrate_cam_line_delay", false}, {"reestimate_biases", false}, {"parse_only", false}, {"json_selftest", false}};
   f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0}};
   return f;
@@ -155,7 +157,8 @@ static int json_selftest() {
 
 int main(int argc, char** argv) {
   icccli::Flags F = default_flags();
-  try { icccli::parse_flags(argc, argv, F); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+  int pose_error = ICC_POSE_ERROR_NORMALIZED;
+  try { icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   const double S_TO_NS = 1e9, US_TO_S = 1e-6, S_TO_US = 1e6, NS_TO_S = 1e-9;
   if (F.boolean["json_selftest"]) return json_selftest();
   try {
@@ -224,6 +227,7 @@ int main(int argc, char** argv) {
       std::vector<double> q_all(4 * (size_t)nv), p_all(3 * (size_t)nv), err(nv); std::vector<int32_t> valid(nv);
       icc_status st = icc_set_camera(hp, model, intr.data(), (int)intr.size(), width, height);
       if (st == ICC_OK) st = icc_set_board_points(hp, max_id + 1, board.data());
+      if (st == ICC_OK) st = icc_set_pose_error(hp, pose_error);
       if (st == ICC_OK) st = icc_estimate_board_poses(hp, nv, sv.off.data(), sv.ids.data(), sv.uv.data(), 0.0, 0, q_all.data(), p_all.data(), err.data(), valid.data());
       if (st == ICC_OK) st = icc_filter_bad_poses(hp, nv, p_all.data(), valid.data());   // the pose app's last step (PoseEstimator::FilterBadPoses)
       if (st != ICC_OK) { std::cerr << "board pose estimation failed (" << st << "): " << icc_last_error(hp) << std::endl; return 2; }

@@ -8,7 +8,9 @@
 // "mean_reproj_error": e}}, "tracks": {"<id>": [x,y,z,w]}}), not as Theia's cereal-binary Reconstruction (unreadable without
 // Theia).  --optimize_board_points (app :61-65) runs icc_optimize_board_points (PoseEstimator::OptimizeBoardPoints + OptimizeAllPoses)
 // and writes the refined board points as the dataset's tracks; PoseEstimator::FilterBadPoses (app :66-67) is applied like in the
-// reference.  Extra flag: --device (CUDA ordinal, default 0).
+// reference.  Extra flags: --device (CUDA ordinal, default 0); --pose_error normalized|tangent (default normalized, the reference's
+// residual): tangent scores corners as unit bearings with the local tangent reprojection error, which keeps the corners and views of
+// fisheye lenses beyond 90 degrees (icc_set_pose_error); the written mean_reproj_error is then in tangent units.
 #include "../../include/icc_b200.h"
 #include "icc_cli_common.hpp"
 
@@ -20,10 +22,11 @@ using iccjson::Value;
 
 int main(int argc, char** argv) {
   icccli::Flags F;
-  F.str = {{"input_corners", ""}, {"camera_calibration_json", ""}, {"output_pose_dataset", ""}};
+  F.str = {{"input_corners", ""}, {"camera_calibration_json", ""}, {"output_pose_dataset", ""}, {"pose_error", "normalized"}};
   F.boolean = {{"optimize_board_points", false}};
   F.num = {{"device", 0.0}};
-  try { icccli::parse_flags(argc, argv, F); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+  int pose_error = ICC_POSE_ERROR_NORMALIZED;
+  try { icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   try {
     Value scene_json; icccli::SceneViews sv;
     try { scene_json = icccli::load_scene(F.str["input_corners"], sv); } catch (const std::exception& e) { std::cerr << "Check failed: Failed to load " << F.str["input_corners"] << ": " << e.what() << std::endl; return 1; }
@@ -41,6 +44,7 @@ int main(int argc, char** argv) {
     std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), err(nv); std::vector<int32_t> valid(nv);
     st = icc_set_camera(h, model, intr.data(), (int)intr.size(), width, height);
     if (st == ICC_OK) st = icc_set_board_points(h, np, board.data());
+    if (st == ICC_OK) st = icc_set_pose_error(h, pose_error);
     if (st == ICC_OK) st = icc_estimate_board_poses(h, nv, sv.off.data(), sv.ids.data(), sv.uv.data(), 0.0, 0, q.data(), p.data(), err.data(), valid.data());
     if (st != ICC_OK) { std::cerr << "board pose estimation failed (" << st << "): " << icc_last_error(h) << std::endl; return 2; }
     std::vector<double> board_out(board);
@@ -65,7 +69,7 @@ int main(int argc, char** argv) {
       ++kept; total += err[i];
     }
     for (int i = 0; i < np; ++i) { Value t = Value::array(); for (int d = 0; d < 4; ++d) t.push_back(Value(board_out[4 * i + d])); out["tracks"][std::to_string(i)] = t; }
-    std::cout << "Estimated " << kept << " of " << nv << " view poses, mean normalised reprojection error " << (kept ? total / kept : 0.0) << "\n";
+    std::cout << "Estimated " << kept << " of " << nv << " view poses, mean " << (pose_error == ICC_POSE_ERROR_TANGENT ? "tangent" : "normalised") << " reprojection error " << (kept ? total / kept : 0.0) << "\n";
     if (!F.str["output_pose_dataset"].empty()) {
       std::ofstream f(F.str["output_pose_dataset"]);
       if (!f.is_open()) { std::cerr << "could not write " << F.str["output_pose_dataset"] << std::endl; return 1; }

@@ -99,6 +99,7 @@ struct icc_handle {
   icc_solver_options opt;
   // ---- raw inputs -------------------------------------------------------------------------------------------
   int model = -1, n_intr = 0, width = 0, height = 0; double intr[10] = {0};
+  int pose_error = ICC_POSE_ERROR_NORMALIZED;   // residual of icc_estimate_board_poses / icc_optimize_board_points (icc_set_pose_error)
   std::vector<double> points;
   std::vector<double> frame_t; std::vector<int> corner_off; HostBuf<int> point_ids; HostBuf<double> uv; std::vector<double> q_wc, p_wc;
   HostBuf<double> imu_t, imu_acc, imu_gyr;
@@ -1464,6 +1465,21 @@ icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, doub
   return drive(h, [&](std::string& err) { return pixels_to_normalized(h->stream, h->model, h->intr, n, uv, xy_out, ok, err); });
 }
 
+icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double* xyz_out, int32_t* ok) {
+  if (!h || n < 0 || (n > 0 && (!uv || !xyz_out))) return ICC_ERR_INVALID_ARGUMENT;
+  NEED_DEVICE();
+  if (h->model < 0) return fail(h, ICC_ERR_STATE, "icc_set_camera must be called first");
+  if (n == 0) return ICC_OK;
+  return drive(h, [&](std::string& err) { return pixels_to_bearings(h->stream, h->model, h->intr, n, uv, xyz_out, ok, err); });
+}
+
+icc_status icc_set_pose_error(icc_handle* h, int mode) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (mode != ICC_POSE_ERROR_NORMALIZED && mode != ICC_POSE_ERROR_TANGENT) return fail(h, ICC_ERR_INVALID_ARGUMENT, "pose error must be ICC_POSE_ERROR_NORMALIZED (0) or ICC_POSE_ERROR_TANGENT (1)");
+  h->pose_error = mode;
+  return ICC_OK;
+}
+
 icc_status icc_estimate_board_poses(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points, double* q_wc, double* p_wc, double* mean_err, int32_t* valid) {
   if (!h || nf <= 0 || !off || !ids || !uv || !q_wc || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
   NEED_DEVICE();
@@ -1471,7 +1487,7 @@ icc_status icc_estimate_board_poses(icc_handle* h, int nf, const int32_t* off, c
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
   return drive(h, [&](std::string& err) { return estimate_board_poses(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
-                                q_wc, p_wc, mean_err, valid, err); });
+                                h->pose_error, q_wc, p_wc, mean_err, valid, err); });
 }
 
 icc_status icc_filter_bad_poses(icc_handle* h, int nv, const double* p_wc, int32_t* valid) {
@@ -1497,7 +1513,7 @@ icc_status icc_optimize_board_points(icc_handle* h, int nf, const int32_t* off, 
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
   std::vector<double> points;
   const icc_status rc = drive(h, [&](std::string& err) { return optimize_board_points(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
-                                 min_observations, q_wc, p_wc, mean_err, valid, points, n_opt_out, err); });
+                                 min_observations, h->pose_error, q_wc, p_wc, mean_err, valid, points, n_opt_out, err); });
   if (rc != ICC_OK) return rc;
   h->points.swap(points);
   if (board_out) std::copy(h->points.begin(), h->points.end(), board_out);

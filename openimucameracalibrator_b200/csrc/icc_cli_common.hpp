@@ -20,6 +20,13 @@ struct Flags {   // every tool fills in its own names and defaults
   std::map<std::string, double> num;
 };
 
+// --pose_error of the pose tools: the residual of the per-view pose step (icc_set_pose_error); any other value is a usage error
+inline int parse_pose_error(const std::string& v) {
+  if (v == "normalized") return ICC_POSE_ERROR_NORMALIZED;
+  if (v == "tangent") return ICC_POSE_ERROR_TANGENT;
+  throw std::runtime_error("flag --pose_error must be 'normalized' or 'tangent', not '" + v + "'");
+}
+
 inline bool parse_bool(const std::string& v) { return v == "true" || v == "1" || v == "t" || v == "yes" || v == "y" || v == "True"; }
 
 // gflags syntax: --name=value, --name value, -name..., --boolflag, --noboolflag

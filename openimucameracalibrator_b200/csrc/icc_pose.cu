@@ -13,11 +13,17 @@
 // planar, so the initial pose comes from the normalised DLT homography; the refinement minimises the same cost as the
 // reference's BundleAdjustView (normalised pinhole reprojection error, Huber 1.345) with Levenberg-Marquardt to a tighter
 // tolerance than Ceres' defaults, so both land on the same optimum.
+//
+// Opt-in wide-angle residual (ICC_POSE_ERROR_TANGENT): corners are unit bearings (icc_bearing_math.cuh) and the same kernels minimise the
+// local tangent reprojection error instead, so rays 90 degrees or more off the axis keep their views.  The residual is a template parameter
+// chosen by the measurement type (double2 = normalised point, double4 = bearing); the default kernels compile to the same code as before.
+#include "icc_bearing_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
 #include "icc_small_linalg.cuh"
 
 #include <cmath>
+#include <type_traits>
 
 namespace icc {
 
@@ -37,6 +43,15 @@ __global__ void unproject_kernel(int model, Intr K, int n, const double2* __rest
   double x = 0.0, y = 0.0;
   const bool good = unproject_gn(model, K.k, uv[i].x, uv[i].y, x, y);
   xy[i] = make_double2(x, y);
+  if (ok) ok[i] = good ? 1 : 0;
+}
+
+__global__ void bearing_kernel(int model, Intr K, int n, const double2* __restrict__ uv, double4* __restrict__ b, int* __restrict__ ok) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  V3 r;
+  const bool good = unproject_bearing(model, K.k, uv[i].x, uv[i].y, r);
+  b[i] = make_double4(r.x, r.y, r.z, 0.0);
   if (ok) ok[i] = good ? 1 : 0;
 }
 
@@ -85,8 +100,53 @@ ICC_D void pose_system(const PoseProblem& Q, const double2* xy, const unsigned c
   }
 }
 
+// The same system for the tangent residual against bearings (icc_bearing_math.cuh): r = (e1.d, e2.d) / (b.d), d = R X + t; 1e6 where b.d <= 0.
+// An overload rather than a shared body, so that the normalised system above keeps its code.
+ICC_D void pose_system(const PoseProblem& Q, const double4* bear, const unsigned char* use, int c0, int c1, double zref, Q4 q, V3 t, PoseSys& S, bool with_jacobian) {
+  const int lane = threadIdx.x & 31;
+  double H[21], g[6], cost = 0.0;
+#pragma unroll
+  for (int i = 0; i < 21; ++i) H[i] = 0.0;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) g[i] = 0.0;
+  const double hub = 1.345;
+  for (int c = c0 + lane; c < c1; c += 32) {
+    if (!use[c]) continue;
+    const double4 Xb = Q.board[Q.pid[c]];
+    const V3 X = v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref);
+    const V3 Pc = qrot(q, X) + t;
+    const TangentErr E(Pc, v3(bear[c].x, bear[c].y, bear[c].z));
+    const double r0 = E.r0, r1 = E.r1, rn = sqrt(r0 * r0 + r1 * r1);
+    const double w = rn <= hub ? 1.0 : hub / rn;
+    cost += rn <= hub ? 0.5 * rn * rn : hub * rn - 0.5 * hub * hub;
+    if (!with_jacobian || !E.front()) { if (!E.front()) cost += 1e6; continue; }
+    double J0[6], J1[6]; V3 P0, P1;
+    tangent_jacobians(E, q, X, J0, J1, P0, P1);
+    int idx = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+      g[i] += w * (J0[i] * r0 + J1[i] * r1);
+#pragma unroll
+      for (int j = 0; j <= i; ++j) { H[idx] += w * (J0[i] * J0[j] + J1[i] * J1[j]); ++idx; }
+    }
+  }
+  S.cost = wsum(cost);
+  if (!with_jacobian) return;
+  int idx = 0;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    S.g[i] = wsum(g[i]);
+#pragma unroll
+    for (int j = 0; j <= i; ++j) { const double v = wsum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
+  }
+}
+
+// the tangent error of one corner for the inlier and mean-error passes; false where b.d <= 0
+ICC_D bool tangent_err(V3 Pc, double4 m, double& r0, double& r1) { const TangentErr E(Pc, v3(m.x, m.y, m.z)); r0 = E.r0; r1 = E.r1; return E.front(); }
+
 // Levenberg-Marquardt on the 6 pose parameters (all lanes run the identical scalar logic on warp-reduced sums)
-ICC_D void pose_refine(const PoseProblem& Q, const double2* xy, const unsigned char* use, int c0, int c1, double zref, Q4& q, V3& t) {
+template <class M>
+ICC_D void pose_refine(const PoseProblem& Q, const M* xy, const unsigned char* use, int c0, int c1, double zref, Q4& q, V3& t) {
   PoseSys S;
   pose_system(Q, xy, use, c0, c1, zref, q, t, S, true);
   double lambda = 1e-4, cost = S.cost;
@@ -192,8 +252,61 @@ ICC_D bool board_homography(const PoseProblem& Q, const double2* __restrict__ xy
   return true;
 }
 
-__global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const double2* __restrict__ xy, const int* __restrict__ okc, unsigned char* __restrict__ use,
-                                                        double* q_out, double* p_out, double* __restrict__ err_out, int* valid_out) {
+// H ~ [r1 r2 t] (points on the plane z = zref, shifted to z = 0): scale, cheirality, Gram-Schmidt -> R_cw, t
+ICC_D void pose_from_homography(const double (&Hm)[9], Q4& q, V3& t) {
+  V3 h1 = v3(Hm[0], Hm[3], Hm[6]), h2 = v3(Hm[1], Hm[4], Hm[7]), h3 = v3(Hm[2], Hm[5], Hm[8]);
+  double s = 2.0 / (sqrt(dot(h1, h1)) + sqrt(dot(h2, h2)));
+  if (h3.z * s < 0.0) s = -s;
+  V3 r1 = s * h1, r2 = s * h2;
+  t = s * h3;
+  r1 = (1.0 / sqrt(dot(r1, r1))) * r1;
+  r2 = r2 - dot(r1, r2) * r1; r2 = (1.0 / sqrt(dot(r2, r2))) * r2;
+  const V3 r3 = cross(r1, r2);
+  q = quat_from_columns(r1, r2, r3);          // R_cw
+}
+
+// Start of a view from bearings: rotate them so that their normalised mean is +z (rows e1, e2, m of R_m), take the homography of those
+// within ~80 degrees of the mean on that frame's normalised plane (xy_h, ok_h: per-corner scratch), rotate the pose back.  Every usable
+// corner, those beyond 80 degrees included, is marked in use[] for the refinement.
+ICC_D bool bearing_start(const PoseProblem& Q, const double4* bear, const int* okc, unsigned char* use, double2* xy_h, int* ok_h, int c0, int c1, double& n, double& zref, Q4& q, V3& t) {
+  const int lane = threadIdx.x & 31;
+  V3 m = v3(0.0, 0.0, 0.0);
+  for (int c = c0 + lane; c < c1; c += 32) {
+    const int id = Q.pid[c];
+    if (okc[c] != 0 && id >= 0 && id < Q.n_points) m = m + v3(bear[c].x, bear[c].y, bear[c].z);
+  }
+  m = v3(wsum(m.x), wsum(m.y), wsum(m.z));
+  const double mn = sqrt(dot(m, m));
+  m = mn > 0.0 ? (1.0 / mn) * m : v3(0.0, 0.0, 1.0);
+  V3 e1, e2; tangent_basis(m, e1, e2);
+  const double cos_max = 0.17364817766693033;   // cos(80 degrees)
+  for (int c = c0 + lane; c < c1; c += 32) {
+    const V3 b = v3(bear[c].x, bear[c].y, bear[c].z), bm = v3(dot(e1, b), dot(e2, b), dot(m, b));
+    const bool near = bm.z > cos_max;
+    ok_h[c] = okc[c] != 0 && near ? 1 : 0;
+    xy_h[c] = near ? make_double2(bm.x / bm.z, bm.y / bm.z) : make_double2(0.0, 0.0);
+  }
+  __syncwarp();
+  double Hm[9];
+  if (!board_homography(Q, xy_h, ok_h, use, c0, c1, n, zref, Hm)) return false;
+  Q4 qm; V3 tm;
+  pose_from_homography(Hm, qm, tm);
+  const Q4 rm_t = quat_from_columns(e1, e2, m);   // R_m^T
+  q = qnormalized(qmul(rm_t, qm)); t = qrot(rm_t, tm);
+  for (int c = c0 + lane; c < c1; c += 32) {
+    const int id = Q.pid[c];
+    use[c] = okc[c] != 0 && id >= 0 && id < Q.n_points ? 1 : 0;
+  }
+  __syncwarp();
+  return true;
+}
+
+// M = double2: normalised points (the reference's residual); M = double4: bearings, the tangent residual (xy_h / ok_h: per-corner scratch of the
+// start).  The normalised branches keep their own text, so that board_pose_kernel<double2> compiles to the same code as the pre-template kernel.
+template <class M>
+__global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M* __restrict__ xy, const int* __restrict__ okc, unsigned char* __restrict__ use,
+                                                        double* q_out, double* p_out, double* __restrict__ err_out, int* valid_out, double2* __restrict__ xy_h, int* __restrict__ ok_h) {
+  constexpr bool kTangent = std::is_same<M, double4>::value;
   const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (f >= Q.n_frames) return;
   const int c0 = Q.f_off[f], c1 = Q.f_off[f + 1];
@@ -219,18 +332,22 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const do
     q = qconj(qw);
     t = -qrot(q, v3(p_out[3 * f], p_out[3 * f + 1], p_out[3 * f + 2]));
   } else {
-    double Hm[9];
-    if (!board_homography(Q, xy, okc, use, c0, c1, n, zref, Hm)) { fail(); return; }
-    // H ~ [r1 r2 t] (points on the plane z = zref, shifted to z = 0): scale, cheirality, Gram-Schmidt
-    V3 h1 = v3(Hm[0], Hm[3], Hm[6]), h2 = v3(Hm[1], Hm[4], Hm[7]), h3 = v3(Hm[2], Hm[5], Hm[8]);
-    double s = 2.0 / (sqrt(dot(h1, h1)) + sqrt(dot(h2, h2)));
-    if (h3.z * s < 0.0) s = -s;
-    V3 r1 = s * h1, r2 = s * h2;
-    t = s * h3;
-    r1 = (1.0 / sqrt(dot(r1, r1))) * r1;
-    r2 = r2 - dot(r1, r2) * r1; r2 = (1.0 / sqrt(dot(r2, r2))) * r2;
-    const V3 r3 = cross(r1, r2);
-    q = quat_from_columns(r1, r2, r3);          // R_cw
+    if constexpr (kTangent) {
+      if (!bearing_start(Q, xy, okc, use, xy_h, ok_h, c0, c1, n, zref, q, t)) { fail(); return; }
+    } else {
+      double Hm[9];
+      if (!board_homography(Q, xy, okc, use, c0, c1, n, zref, Hm)) { fail(); return; }
+      // H ~ [r1 r2 t] (points on the plane z = zref, shifted to z = 0): scale, cheirality, Gram-Schmidt
+      V3 h1 = v3(Hm[0], Hm[3], Hm[6]), h2 = v3(Hm[1], Hm[4], Hm[7]), h3 = v3(Hm[2], Hm[5], Hm[8]);
+      double s = 2.0 / (sqrt(dot(h1, h1)) + sqrt(dot(h2, h2)));
+      if (h3.z * s < 0.0) s = -s;
+      V3 r1 = s * h1, r2 = s * h2;
+      t = s * h3;
+      r1 = (1.0 / sqrt(dot(r1, r1))) * r1;
+      r2 = r2 - dot(r1, r2) * r1; r2 = (1.0 / sqrt(dot(r2, r2))) * r2;
+      const V3 r3 = cross(r1, r2);
+      q = quat_from_columns(r1, r2, r3);          // R_cw
+    }
   }
   // ---- refinement, inlier selection with the reference's squared normalised threshold, refinement on the inliers -------------
   pose_refine(Q, xy, use, c0, c1, zref, q, t);
@@ -239,8 +356,14 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const do
     if (!use[c]) continue;
     const double4 Xb = Q.board[Q.pid[c]];
     const V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
-    const double r0 = Pc.x / Pc.z - xy[c].x, r1e = Pc.y / Pc.z - xy[c].y;
-    const bool in = Pc.z > 0.0 && r0 * r0 + r1e * r1e < Q.thresh_sq;
+    bool in;
+    if constexpr (kTangent) {
+      double r0, r1e;
+      in = tangent_err(Pc, xy[c], r0, r1e) && r0 * r0 + r1e * r1e < Q.thresh_sq;
+    } else {
+      const double r0 = Pc.x / Pc.z - xy[c].x, r1e = Pc.y / Pc.z - xy[c].y;
+      in = Pc.z > 0.0 && r0 * r0 + r1e * r1e < Q.thresh_sq;
+    }
     if (in) n_in += 1.0; else { n_out += 1.0; use[c] = 0; }
   }
   n_in = wsum(n_in); n_out = wsum(n_out);
@@ -253,8 +376,14 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const do
     if (!use[c]) continue;
     const double4 Xb = Q.board[Q.pid[c]];
     const V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
-    const double r0 = Pc.x / Pc.z - xy[c].x, r1e = Pc.y / Pc.z - xy[c].y;
-    e += sqrt(r0 * r0 + r1e * r1e);
+    if constexpr (kTangent) {
+      double r0, r1e;
+      tangent_err(Pc, xy[c], r0, r1e);
+      e += sqrt(r0 * r0 + r1e * r1e);
+    } else {
+      const double r0 = Pc.x / Pc.z - xy[c].x, r1e = Pc.y / Pc.z - xy[c].y;
+      e += sqrt(r0 * r0 + r1e * r1e);
+    }
   }
   e = wsum(e) / n_in;
   if (lane == 0) {
@@ -268,7 +397,6 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const do
     err_out[f] = e; valid_out[f] = keep ? 1 : 0;
   }
 }
-
 
 // Focal length of a view from its board homography on principal-point-centred pixels (square pixels, zero skew):
 // H ~ K [r1 r2 t], K = diag(f, f, 1), r1 . r2 = 0 and |r1| = |r2| give two linear equations a_i + f^2 b_i = 0 (Zhang's
@@ -305,8 +433,10 @@ __global__ void pinhole_normalize_kernel(int n, const double2* __restrict__ uv, 
 // Levenberg-Marquardt system is warp-reduced and solved in registers by every lane.  Residual: Huber(1.345) on
 //   normalised == 1 :  (R_cw (X - c)).xy / z - x_n          (the pose estimator's unit-pinhole views with undistorted features)
 //   normalised == 0 :  CameraToPixelCoordinates(intr, R_cw (X - c)) - pixel     (the camera calibrator's views)
+//   TANGENT         :  the tangent error of R_cw (X - c) against the corner's bearing  (the pose estimator's views in tangent mode)
 struct PointSys { double H[3][3]; double g[3]; double cost; };
-ICC_D void point_system(const PointProblem& Q, int o0, int o1, V3 X, PointSys& S, bool with_jacobian) {
+template <bool TANGENT>
+ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear, int o0, int o1, V3 X, PointSys& S, bool with_jacobian) {
   const int lane = threadIdx.x & 31;
   double H[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0}, cost = 0.0;
   const double hub = Q.huber;
@@ -315,7 +445,12 @@ ICC_D void point_system(const PointProblem& Q, int o0, int o1, V3 X, PointSys& S
     const Q4 q = q4(Q.q_cw[4 * v], Q.q_cw[4 * v + 1], Q.q_cw[4 * v + 2], Q.q_cw[4 * v + 3]);
     const V3 pc = qrot(q, X - v3(Q.cam_c[3 * v], Q.cam_c[3 * v + 1], Q.cam_c[3 * v + 2]));
     double r0, r1; V3 a0, a1;
-    if (Q.normalized) {
+    if constexpr (TANGENT) {
+      const double4 m = bear[c];
+      const TangentErr E(pc, v3(m.x, m.y, m.z));
+      if (!E.front()) { cost += 1e6; continue; }
+      r0 = E.r0; r1 = E.r1; E.rows(a0, a1);
+    } else if (Q.normalized) {
       if (!(pc.z > 0.0)) { cost += 1e6; continue; }
       const double iz = 1.0 / pc.z, u = pc.x * iz, w = pc.y * iz;
       r0 = u - Q.meas[c].x; r1 = w - Q.meas[c].y;
@@ -342,7 +477,9 @@ ICC_D void point_system(const PointProblem& Q, int o0, int o1, V3 X, PointSys& S
   S.H[0][0] = h0; S.H[0][1] = h1; S.H[0][2] = h2; S.H[1][0] = h1; S.H[1][1] = h3; S.H[1][2] = h4; S.H[2][0] = h2; S.H[2][1] = h4; S.H[2][2] = h5;
 }
 
-__global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, double4* __restrict__ board_out, int* __restrict__ optimized) {
+// TANGENT: Q.meas is unused, the corners' bearings come in bear
+template <bool TANGENT>
+__global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, double4* __restrict__ board_out, int* __restrict__ optimized, const double4* __restrict__ bear) {
   const int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (p >= Q.n_points) return;
   const int o0 = Q.pt_off[p], o1 = Q.pt_off[p + 1];
@@ -350,7 +487,7 @@ __global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, doubl
   if (o1 - o0 <= Q.min_obs) { if (lane == 0) { board_out[p] = Xb; optimized[p] = 0; } return; }   // pose_estimator.cc:202-206
   V3 X = v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w);
   PointSys S;
-  point_system(Q, o0, o1, X, S, true);
+  point_system<TANGENT>(Q, bear, o0, o1, X, S, true);
   double lambda = 1e-4, cost = S.cost;
   for (int it = 0; it < 50; ++it) {
     double A[3][3], b[3];
@@ -364,13 +501,13 @@ __global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, doubl
     if (!chol_solve<3>(A, b)) { lambda *= 10.0; if (lambda > 1e12) break; continue; }
     const V3 Xn = X + v3(b[0], b[1], b[2]);
     PointSys Sn;
-    point_system(Q, o0, o1, Xn, Sn, false);
+    point_system<TANGENT>(Q, bear, o0, o1, Xn, Sn, false);
     const double step2 = b[0] * b[0] + b[1] * b[1] + b[2] * b[2];
     if (Sn.cost < cost) {
       const double dec = cost - Sn.cost;
       X = Xn; cost = Sn.cost; lambda = fmax(lambda * 0.1, 1e-12);
       if (dec <= 1e-15 * cost || step2 < 1e-30) break;
-      point_system(Q, o0, o1, X, S, true);
+      point_system<TANGENT>(Q, bear, o0, o1, X, S, true);
     } else {
       if (step2 < 1e-30) break;
       lambda *= 10.0;
@@ -389,9 +526,22 @@ void launch_unproject(int model, const double* intr10, int n, const double2* uv,
   count_launch();
 }
 
+void launch_bearings(int model, const double* intr10, int n, const double2* uv, double4* b, int* ok, cudaStream_t st) {
+  if (n <= 0) return;
+  Intr K; for (int i = 0; i < 10; ++i) K.k[i] = intr10[i];
+  bearing_kernel<<<(n + 127) / 128, 128, 0, st>>>(model, K, n, uv, b, ok);
+  count_launch();
+}
+
 void launch_board_poses(const PoseProblem& Q, const double2* xy, const int* ok, unsigned char* use, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st) {
   if (Q.n_frames <= 0) return;
-  board_pose_kernel<<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, xy, ok, use, q_wc, p_wc, err, valid);
+  board_pose_kernel<double2><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, xy, ok, use, q_wc, p_wc, err, valid, nullptr, nullptr);
+  count_launch();
+}
+
+void launch_board_poses_tangent(const PoseProblem& Q, const double4* bear, const int* ok, unsigned char* use, double2* xy_h, int* ok_h, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st) {
+  if (Q.n_frames <= 0) return;
+  board_pose_kernel<double4><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, bear, ok, use, q_wc, p_wc, err, valid, xy_h, ok_h);
   count_launch();
 }
 
@@ -407,13 +557,15 @@ void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, do
   count_launch();
 }
 
-void launch_point_refine(const PointProblem& Q, double4* board_out, int* optimized, cudaStream_t st) {
+void launch_point_refine(const PointProblem& Q, const double4* bear, double4* board_out, int* optimized, cudaStream_t st) {
   if (Q.n_points <= 0) return;
-  point_refine_kernel<<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized);
+  if (bear) point_refine_kernel<true><<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized, bear);
+  else point_refine_kernel<false><<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized, nullptr);
   count_launch();
 }
 
-// ---- host drivers of row f1 (icc_pixels_to_normalized, icc_estimate_board_poses, icc_optimize_board_points, icc_filter_bad_poses) ----
+// ---- host drivers of row f1 (icc_pixels_to_normalized, icc_pixels_to_bearings, icc_estimate_board_poses, icc_optimize_board_points,
+//      icc_filter_bad_poses) ----
 #define CU(call) ICC_CUDA_CHECK(call, err)
 
 icc_status upload_board_views(cudaStream_t st, int np, const double* points, int nf, const int32_t* off, const int32_t* ids, const double* uv, BoardViews& B, std::string& err) {
@@ -434,7 +586,8 @@ icc_status read_poses(cudaStream_t st, const BoardViews& B, double* q_wc, double
   return ICC_OK;
 }
 
-icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const int32_t* ids, const std::vector<int>& obs_view, DevBuf<double4>& d_out, std::vector<double>& points_out, int& n_opt, std::string& err) {
+icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const int32_t* ids, const std::vector<int>& obs_view, DevBuf<double4>& d_out, std::vector<double>& points_out, int& n_opt, std::string& err,
+                               const double4* bear) {
   const int np = Q.n_points;
   std::vector<int> pt_off, pt_obs;
   build_point_adjacency(np, nc, ids, [&](int c) { return obs_view[c] >= 0; }, pt_off, pt_obs);
@@ -442,7 +595,7 @@ icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const in
   CU(d_view.upload(obs_view)); CU(d_pt_off.upload(pt_off)); CU(d_pt_obs.alloc(std::max<size_t>(1, pt_obs.size()))); CU(d_opt.alloc(np)); CU(d_out.alloc(np));
   if (!pt_obs.empty()) CU(cudaMemcpy(d_pt_obs.p, pt_obs.data(), pt_obs.size() * sizeof(int), cudaMemcpyHostToDevice));
   Q.pt_off = d_pt_off.p; Q.pt_obs = d_pt_obs.p; Q.obs_view = d_view.p;
-  launch_point_refine(Q, d_out.p, d_opt.p, st);
+  launch_point_refine(Q, bear, d_out.p, d_opt.p, st);
   std::vector<int> opt(np); points_out.resize(4 * (size_t)np);
   CU(cudaMemcpyAsync(points_out.data(), d_out.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(opt.data(), d_opt.p, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -451,9 +604,11 @@ icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const in
   return ICC_OK;
 }
 
-// un-projection of every corner and the PoseProblem of EstimatePosesFromJson / OptimizeAllPoses for a W x H camera (pose_estimator.cc:97-101, :181)
-static PoseProblem unproject_corners(cudaStream_t st, int model, const double intr[10], int W, int H, const BoardViews& B, double max_reproj_error, int min_points) {
-  launch_unproject(model, intr, B.nc, B.uv.p, B.xy.p, B.ok.p, st);
+// un-projection of every corner and the PoseProblem of EstimatePosesFromJson / OptimizeAllPoses for a W x H camera (pose_estimator.cc:97-101, :181).
+// Tangent mode: bearings into B.bear (B.xy and B.okh are the start's scratch); the thresholds keep their values, now on the tangent error.
+static PoseProblem unproject_corners(cudaStream_t st, int model, const double intr[10], int W, int H, const BoardViews& B, double max_reproj_error, int min_points, int pose_error) {
+  if (pose_error == ICC_POSE_ERROR_TANGENT) launch_bearings(model, intr, B.nc, B.uv.p, B.bear.p, B.ok.p, st);
+  else launch_unproject(model, intr, B.nc, B.uv.p, B.xy.p, B.ok.p, st);
   PoseProblem Q; memset(&Q, 0, sizeof Q);
   Q.model = model; for (int i = 0; i < 10; ++i) Q.intr[i] = intr[i];
   Q.n_frames = B.nf; Q.n_points = B.np; Q.min_points = min_points > 0 ? min_points : 8;
@@ -474,28 +629,53 @@ icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10
   return ICC_OK;
 }
 
+icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err) {
+  DevBuf<double2> d_uv; DevBuf<double4> d_b; DevBuf<int> d_ok;
+  CU(d_uv.upload(uv, n, st)); CU(d_b.alloc(n)); CU(d_ok.alloc(n));
+  launch_bearings(model, intr, n, d_uv.p, d_b.p, d_ok.p, st);
+  std::vector<double4> b(n);
+  CU(cudaMemcpyAsync(b.data(), d_b.p, (size_t)n * sizeof(double4), cudaMemcpyDeviceToHost, st));
+  if (ok) CU(cudaMemcpyAsync(ok, d_ok.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) { xyz_out[3 * i] = b[i].x; xyz_out[3 * i + 1] = b[i].y; xyz_out[3 * i + 2] = b[i].z; }
+  return ICC_OK;
+}
+
+// the pose kernel of the selected residual on the views of B
+static void launch_views(const PoseProblem& Q, BoardViews& B, int pose_error, cudaStream_t st) {
+  if (pose_error == ICC_POSE_ERROR_TANGENT) launch_board_poses_tangent(Q, B.bear.p, B.ok.p, B.use.p, B.xy.p, B.okh.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  else launch_board_poses(Q, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+}
+
+static icc_status alloc_tangent(int pose_error, BoardViews& B, std::string& err) {
+  if (pose_error == ICC_POSE_ERROR_TANGENT) { CU(B.bear.alloc(std::max(1, B.nc))); CU(B.okh.alloc(std::max(1, B.nc))); }
+  return ICC_OK;
+}
+
 icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
-                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err) {
+                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err) {
   BoardViews B;
   icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
-  launch_board_poses(unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points), B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  rc = alloc_tangent(pose_error, B, err); if (rc != ICC_OK) return rc;
+  launch_views(unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points, pose_error), B, pose_error, st);
   rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
   if (cudaGetLastError() != cudaSuccess) { err = "pose kernels failed"; return ICC_ERR_CUDA; }
   return ICC_OK;
 }
 
 icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
-                                 const double* uv, double max_reproj_error, int min_points, int min_observations, double* q_wc, double* p_wc, double* mean_err, int32_t* valid,
+                                 const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid,
                                  std::vector<double>& points_out, int32_t* n_opt_out, std::string& err) {
   BoardViews B;
   icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
+  rc = alloc_tangent(pose_error, B, err); if (rc != ICC_OK) return rc;
   const int nc = B.nc;
   CU(B.q.upload(q_wc, 4 * (size_t)nf, st)); CU(B.p.upload(p_wc, 3 * (size_t)nf, st)); CU(B.valid.upload(valid, nf, st));
   CU(cudaMemsetAsync(B.e.p, 0, (size_t)nf * sizeof(double), st));   // views that are not valid keep a zero error
-  PoseProblem Q = unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points);
+  PoseProblem Q = unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points, pose_error);
   Q.refine_only = 1;
   // 1. the stored poses and their inlier sets (what the pose dataset holds after EstimatePosesFromJson)
-  launch_board_poses(Q, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  launch_views(Q, B, pose_error, st);
   std::vector<unsigned char> use(std::max(1, nc)); std::vector<int> vh(nf); std::vector<double> qh(4 * (size_t)nf), ph(3 * (size_t)nf);
   CU(cudaMemcpyAsync(use.data(), B.use.p, (size_t)std::max(1, nc), cudaMemcpyDeviceToHost, st));
   rc = read_poses(st, B, qh.data(), ph.data(), nullptr, vh.data(), err); if (rc != ICC_OK) return rc;
@@ -510,10 +690,10 @@ icc_status optimize_board_points(cudaStream_t st, int model, const double intr[1
   PQ.normalized = 1; PQ.n_points = np; PQ.min_obs = min_observations > 0 ? min_observations : 30; PQ.huber = 1.345;
   PQ.board_in = B.board.p; PQ.meas = B.xy.p; PQ.q_cw = d_qcw.p; PQ.cam_c = d_c.p;
   int n_opt = 0;
-  rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, n_opt, err); if (rc != ICC_OK) return rc;
+  rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, n_opt, err, pose_error == ICC_POSE_ERROR_TANGENT ? B.bear.p : nullptr); if (rc != ICC_OK) return rc;
   // 3. OptimizeAllPoses on the new points
   Q.board = d_board2.p;
-  launch_board_poses(Q, B.xy.p, B.ok.p, B.use.p, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  launch_views(Q, B, pose_error, st);
   rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
   if (cudaGetLastError() != cudaSuccess) { err = "board point kernels failed"; return ICC_ERR_CUDA; }
   if (n_opt_out) *n_opt_out = n_opt;
