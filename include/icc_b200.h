@@ -190,6 +190,13 @@ icc_status icc_get_imu_used(const icc_handle* h, double* t_s, double* accel_xyz,
  * s_so3, s_r3, s_acc_bias, s_gyr_bias, i_begin, i_end.  The evaluation kernels stage one knot window per cell. */
 icc_status icc_get_num_imu_cells(const icc_handle* h, int* n);
 icc_status icc_get_imu_cells(const icc_handle* h, int32_t* cells6);
+/* Schedule of the persistent Jacobian kernel (inspection / tests).  The corners of the non-empty frames and the samples of the IMU
+ * cells form two packed streams, each unit padded to a multiple of 4 positions; each stream is walked in chunks of up to 32
+ * positions from at most two consecutive units and cut into even per-warp runs.  counts4 = {vision chunks, IMU chunks, vision
+ * runs, IMU runs}; vitems3 / iitems3 (3 int32 per run, either may be NULL): first unit (index among the non-empty frames / cells),
+ * first stream position, end stream position.  ICC_ERR_STATE before icc_batch_init_spline.  The environment variable
+ * ICC_TMEM_RUNS=n, read by icc_batch_init_spline, caps the runs per stream at n (tests). */
+icc_status icc_get_eval_schedule(const icc_handle* h, int32_t counts4[4], int32_t* vitems3, int32_t* iitems3);
 /* GetAngularVelocity / GetAcceleration / GetGyroBias / GetAcclBias / GetPose evaluated on the GPU for n timestamps [ns];
  * valid[i] = 0 where CalcTimes rejects the timestamp (outputs left untouched there). Any output may be NULL. */
 icc_status icc_eval_trajectory(icc_handle* h, int n, const int64_t* t_ns, double* gyro_xyz, double* accel_xyz,

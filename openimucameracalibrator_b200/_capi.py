@@ -469,6 +469,15 @@ class CApi:
         self._call("get_imu_cells", [c_int32_p], c.ctypes.data_as(c_int32_p))
         return c
 
+    def eval_schedule(self):
+        """Per-warp runs of the persistent Jacobian kernel: dict with n_vchunks, n_ichunks and the vision / IMU runs as int32 rows
+        (first unit, pos_begin, pos_end) of the packed corner / sample streams."""
+        n = np.zeros(4, dtype=np.int32)
+        self._call("get_eval_schedule", [c_int32_p] * 3, n.ctypes.data_as(c_int32_p), None, None)
+        v, i = np.zeros((n[2], 3), dtype=np.int32), np.zeros((n[3], 3), dtype=np.int32)
+        self._call("get_eval_schedule", [c_int32_p] * 3, n.ctypes.data_as(c_int32_p), v.ctypes.data_as(c_int32_p), i.ctypes.data_as(c_int32_p))
+        return {"n_vchunks": int(n[0]), "n_ichunks": int(n[1]), "vitems": v, "iitems": i}
+
     def eval_trajectory(self, t_ns):
         t = np.ascontiguousarray(t_ns, dtype=np.int64); n = t.size
         out = dict(gyro=np.zeros((n, 3)), accel=np.zeros((n, 3)), gyro_bias=np.zeros((n, 3)), accel_bias=np.zeros((n, 3)),

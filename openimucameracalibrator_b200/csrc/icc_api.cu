@@ -141,6 +141,7 @@ struct icc_handle {
   DevBuf<double> d_view_t, d_view_q, d_view_p;   // per-view pose priors in time order (knot initialisation kernel)
   DevBuf<VisFrame> d_vframes; DevBuf<VisItem> d_vitems;
   DevBuf<ImuCellP> d_icells; DevBuf<VisItem> d_iitems;
+  std::vector<VisItem> vitems, iitems;   // host copies of the per-warp runs (icc_get_eval_schedule)
   DevBuf<double> d_imu_traw; DevBuf<VisionWork> d_vwork; DevBuf<int64_t> d_imu_t; DevBuf<double> d_imu_acc, d_imu_gyr; DevBuf<ImuCell> d_cells, d_iwork;
   DevBuf<int> d_so3_col, d_r3_col, d_ba_col, d_bg_col;
   DevBuf<double> d_ne, d_scale, d_ws, d_delta, d_scal, d_res;
@@ -1113,7 +1114,10 @@ icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
       ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0}); ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0});
       ipoff.push_back(poff); ipoff.push_back(poff);
       const Walk wv = walk(vpoff, nvf), wi = walk(ipoff, nic);
-      const int nVc = (int)wv.pos.size(), nIc = (int)wi.pos.size(), W = h->sm_count * eval_tmem_warps();
+      const int nVc = (int)wv.pos.size(), nIc = (int)wi.pos.size();
+      int W = h->sm_count * eval_tmem_warps();
+      // ICC_TMEM_RUNS=n caps the runs at n (tests: every warp then owns several chunks and carries its tile state between them)
+      if (const char* e = getenv("ICC_TMEM_RUNS")) { const int n = atoi(e); if (n > 0) W = std::min(W, n); }
       auto split = [W](const Walk& w) {      // even runs, one per warp
         const int nc = (int)w.pos.size(), n_items = std::min(W, nc);
         std::vector<VisItem> items((size_t)n_items);
@@ -1122,7 +1126,8 @@ icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
           items[(size_t)k] = {w.unit[a], w.pos[a], b < nc ? w.pos[b] : w.total, 0};
         }
         return items; };
-      const std::vector<VisItem> vi = split(wv), ii = split(wi);
+      h->vitems = split(wv); h->iitems = split(wi);
+      const std::vector<VisItem>& vi = h->vitems; const std::vector<VisItem>& ii = h->iitems;
       const int n_iit = (int)ii.size();
       P.n_vchunks = nVc; P.n_ichunks = nIc;
       CU(upload_staged(h, h->d_vframes, vf)); P.vframes = h->d_vframes.p; P.n_vframes = nvf;
@@ -1241,6 +1246,17 @@ icc_status icc_get_num_imu_cells(const icc_handle* h, int* n) { if (!h || !n) re
 icc_status icc_get_imu_cells(const icc_handle* h, int32_t* c6) {
   if (!h || !c6) return ICC_ERR_INVALID_ARGUMENT;
   for (size_t k = 0; k < h->cells.size(); ++k) { const ImuCell& c = h->cells[k]; int32_t* o = c6 + 6 * k; o[0] = c.s_so3; o[1] = c.s_r3; o[2] = c.s_ba; o[3] = c.s_bg; o[4] = c.i_begin; o[5] = c.i_end; }
+  return ICC_OK;
+}
+icc_status icc_get_eval_schedule(const icc_handle* h, int32_t counts4[4], int32_t* vitems3, int32_t* iitems3) {
+  if (!h || !counts4) return ICC_ERR_INVALID_ARGUMENT;
+  if (!h->initialised) return ICC_ERR_STATE;
+  counts4[0] = h->P.n_vchunks; counts4[1] = h->P.n_ichunks; counts4[2] = (int32_t)h->vitems.size(); counts4[3] = (int32_t)h->iitems.size();
+  for (int s = 0; s < 2; ++s) {
+    int32_t* o = s ? iitems3 : vitems3;
+    if (!o) continue;
+    for (const VisItem& it : s ? h->iitems : h->vitems) { o[0] = it.vf0; o[1] = it.pos_begin; o[2] = it.pos_end; o += 3; }
+  }
   return ICC_OK;
 }
 icc_status icc_get_num_imu_used(const icc_handle* h, int* n) { if (!h || !n) return ICC_ERR_INVALID_ARGUMENT; *n = (int)h->n_imu_used; return ICC_OK; }

@@ -38,7 +38,8 @@ def _assert_eval_parity(o, g, flags, hessian=True):
 def test_eval_parity_every_camera_model_all_blocks(oracle_factory, gpu_factory, k, eval_path):
     cfg = syn.config5(k); cfg.n_frames = 20
     o, g = _pair(oracle_factory, gpu_factory, syn.make_dataset(cfg), known_gravity=False)
-    for flags in (F_STAGE1, F_ALL, F_STAGE2, capi.FLAG_T_I_C, capi.FLAG_SPLINE | capi.FLAG_GYR_BIAS, capi.FLAG_GRAVITY_DIR | capi.FLAG_ACC_BIAS):
+    for flags in (F_STAGE1, F_ALL, F_STAGE2, capi.FLAG_T_I_C, capi.FLAG_SPLINE | capi.FLAG_GYR_BIAS, capi.FLAG_GRAVITY_DIR | capi.FLAG_ACC_BIAS,
+                  F_STAGE1 | capi.FLAG_GRAVITY_DIR):   # stage 1 with unknown gravity: the gravity columns on the persistent IMU items
         _assert_eval_parity(o, g, flags)
 
 
