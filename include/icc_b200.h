@@ -195,7 +195,8 @@ icc_status icc_get_imu_cells(const icc_handle* h, int32_t* cells6);
  * positions from at most two consecutive units and cut into even per-warp runs.  counts4 = {vision chunks, IMU chunks, vision
  * runs, IMU runs}; vitems3 / iitems3 (3 int32 per run, either may be NULL): first unit (index among the non-empty frames / cells),
  * first stream position, end stream position.  ICC_ERR_STATE before icc_batch_init_spline.  The environment variable
- * ICC_TMEM_RUNS=n, read by icc_batch_init_spline, caps the runs per stream at n (tests). */
+ * ICC_TMEM_RUNS=n, read by icc_batch_init_spline, caps the runs per stream at n (tests).  Host only: also works on a host-only
+ * (device -1) handle, whose run count assumes the 132 SMs of an H100 SXM. */
 icc_status icc_get_eval_schedule(const icc_handle* h, int32_t counts4[4], int32_t* vitems3, int32_t* iitems3);
 /* GetAngularVelocity / GetAcceleration / GetGyroBias / GetAcclBias / GetPose evaluated on the GPU for n timestamps [ns];
  * valid[i] = 0 where CalcTimes rejects the timestamp (outputs left untouched there). Any output may be NULL. */

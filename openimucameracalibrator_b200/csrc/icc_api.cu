@@ -11,6 +11,7 @@
 #include "icc_allan_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
+#include "icc_rotinit_math.cuh"
 #include "icc_trust_region.cuh"
 
 #include <algorithm>
@@ -29,7 +30,7 @@ using namespace icc;
 
 namespace {
 
-constexpr double S_TO_NS = 1e9, NS_TO_S = 1e-9;
+constexpr double S_TO_NS = 1e9;
 
 // Host staging of the large measurement arrays (corners, IMU samples): page-locked blocks from a process-wide cache (the first
 // job pays cudaHostAlloc, later ones reuse), so that the uploads of BatchInitSpline are asynchronous DMA transfers that overlap the
@@ -199,31 +200,6 @@ bool calc_times(int64_t sensor_ns, int64_t start_ns, int64_t dt_ns, size_t nr_kn
   return true;
 }
 
-size_t nearest_index(double t, const std::vector<double>& ts, double& dist_out) {   // utils.cc:194-212
-  // FindClosestTimestamp is a linear scan keeping the FIRST strict minimum of |t - ts[i]|; on the time-sorted, distinct
-  // view timestamps used here the same index is found by bisection + comparison of the two neighbours.
-  const size_t n = ts.size();
-  size_t hi = std::lower_bound(ts.begin(), ts.end(), t) - ts.begin();   // first ts >= t
-  size_t idx;
-  if (hi == 0) idx = 0;
-  else if (hi == n) idx = n - 1;
-  else idx = (std::fabs(t - ts[hi - 1]) <= std::fabs(t - ts[hi])) ? hi - 1 : hi;   // tie -> earlier index, like the scan
-  dist_out = std::fabs(t - ts[idx]);
-  return idx;
-}
-
-void quat_slerp(const double* a, const double* b, double t, double* o) {   // Eigen::Quaternion::slerp semantics (utils.cc:234)
-  const double thresh = 1.0 - 2.220446049250313e-16;
-  const double d = a[0] * b[0] + a[1] * b[1] + a[2] * b[2] + a[3] * b[3], ad = std::fabs(d);
-  double s0, s1;
-  if (ad >= thresh) { s0 = 1.0 - t; s1 = t; }
-  else { const double th = std::acos(ad), sth = std::sin(th); s0 = std::sin((1.0 - t) * th) / sth; s1 = std::sin(t * th) / sth; }
-  if (d < 0) s1 = -s1;
-  for (int i = 0; i < 4; ++i) o[i] = s0 * a[i] + s1 * b[i];
-}
-
-struct Pose { Q4 q; V3 t; };
-Pose pose_mul(const Pose& a, const Pose& b) { return {qnormalized(qmul(a.q, b.q)), a.t + qrot(a.q, b.t)}; }
 Pose pose_inv(const Pose& a) { const Q4 qi = qnormalized(qconj(a.q)); return {qi, qrot(qi, -a.t)}; }
 
 std::vector<double4> pad4(const std::vector<double>& v, int dim) {
@@ -588,6 +564,419 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
   return ICC_OK;
 }
 
+// ---- the steps of icc_batch_init_spline ------------------------------------------------------------------------------------------------
+
+struct KnotCounts { int so3, r3, ba, bg; };
+
+// T_i_c, IMU intrinsics, line delay (imu_camera_calibrator.cc:30-47), the spline time range and knot counts (imu_camera_calibrator.cc:49-72,
+// impl.h:37-51), and the bias splines: InitBiasSplines(bias, bias, 10 s, 10 s, 1.0, 0.1) (imu_camera_calibrator.cc:80-85, impl.h:53-90).
+// The SO(3) / R³ knots are only sized (zero) here.
+icc_status init_globals_and_knot_counts(icc_handle* h, KnotCounts& n) {
+  const icc_init_params& ip = h->ip;
+  { const Q4 q = qn(ip.T_i_c_init); h->glob[G_TIC + 0] = q.x; h->glob[G_TIC + 1] = q.y; h->glob[G_TIC + 2] = q.z; h->glob[G_TIC + 3] = q.w; for (int i = 4; i < 7; ++i) h->glob[G_TIC + i] = ip.T_i_c_init[i]; }
+  for (int i = 0; i < 6; ++i) h->glob[G_ACC_INTR + i] = ip.acc_intrinsics[i];
+  for (int i = 0; i < 9; ++i) h->glob[G_GYR_INTR + i] = ip.gyr_intrinsics[i];
+  h->glob[G_LD] = ip.init_line_delay_s;
+  for (int i = 0; i < 10; ++i) h->glob[G_CAM_INTR + i] = i < h->n_intr ? h->intr[i] : 0.0;
+  h->glob[G_TOFF] = 0.0;
+  const auto range = std::minmax_element(h->frame_t.begin(), h->frame_t.end());
+  h->t0_s = *range.first; h->tend_s = *range.second;
+  h->start_ns = (int64_t)(h->t0_s * S_TO_NS);
+  h->end_ns = (int64_t)(h->tend_s * S_TO_NS + 0.01 * S_TO_NS + ip.init_line_delay_s);
+  h->dt_so3_ns = (int64_t)(ip.dt_so3_s * S_TO_NS); h->dt_r3_ns = (int64_t)(ip.dt_r3_s * S_TO_NS);
+  if (h->dt_so3_ns <= 0 || h->dt_r3_ns <= 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "knot spacing must be positive");
+  h->dt_ba_ns = h->dt_bg_ns = (int64_t)(10 * 1e9); h->max_ba = 1.0; h->max_bg = 1e-1;
+  const int64_t duration = h->end_ns - h->start_ns;
+  n = {(int)(duration / h->dt_so3_ns) + SPLINE_N, (int)(duration / h->dt_r3_ns) + SPLINE_N, (int)(duration / h->dt_ba_ns) + BIAS_N, (int)(duration / h->dt_bg_ns) + BIAS_N};
+  h->so3.assign(4 * (size_t)n.so3, 0.0); h->r3.assign(3 * (size_t)n.r3, 0.0);
+  h->ba.resize(3 * (size_t)n.ba); h->bg.resize(3 * (size_t)n.bg);
+  for (int i = 0; i < n.ba; ++i) for (int d = 0; d < 3; ++d) h->ba[3 * i + d] = ip.acc_bias[d];
+  for (int i = 0; i < n.bg; ++i) for (int d = 0; d < 3; ++d) h->bg[3 * i + d] = ip.gyr_bias[d];
+  return ICC_OK;
+}
+
+// The per-view pose priors (raw q_wc, p_wc) in the order the reference walks its views: through a std::map keyed by timestamp (time order,
+// a repeated timestamp keeps the LAST view).  Strictly increasing timestamps -- the usual case -- give that order without the tree.
+struct ViewTable { std::vector<double> t, q, p; bool increasing = true; };
+ViewTable view_table(const icc_handle* h) {
+  const int nf = (int)h->frame_t.size();
+  ViewTable v;
+  for (int i = 1; i < nf && v.increasing; ++i) v.increasing = h->frame_t[i] > h->frame_t[i - 1];
+  std::vector<int> order;
+  if (v.increasing) { order.resize(nf); for (int i = 0; i < nf; ++i) order[i] = i; }
+  else { std::map<double, int> by_time; for (int i = 0; i < nf; ++i) by_time[h->frame_t[i]] = i; for (const auto& kv : by_time) order.push_back(kv.second); }
+  v.t.reserve(order.size()); v.q.reserve(4 * order.size()); v.p.reserve(3 * order.size());
+  for (const int i : order) { v.t.push_back(h->frame_t[i]); for (int d = 0; d < 4; ++d) v.q.push_back(h->q_wc[4 * i + d]); for (int d = 0; d < 3; ++d) v.p.push_back(h->p_wc[3 * i + d]); }
+  return v;
+}
+
+Pose T_c_i(const icc_handle* h) { return pose_inv({q4(h->glob[G_TIC + 0], h->glob[G_TIC + 1], h->glob[G_TIC + 2], h->glob[G_TIC + 3]), v3(h->glob[G_TIC + 4], h->glob[G_TIC + 5], h->glob[G_TIC + 6])}); }
+
+// BatchInitSO3R3VisPoses (impl.h:278-339) for the host-only handle: init_knots_kernel's per-knot functions, into the host mirror
+void init_knots_on_host(icc_handle* h, const ViewTable& v, const Pose& Tci) {
+  const int nv = (int)v.t.size(), nso3 = (int)h->so3.size() / 4, nr3 = (int)h->r3.size() / 3;
+  for (int i = 0; i < nso3; ++i) {
+    const double4 o = so3_knot(i, h->dt_so3_ns, nv, v.t.data(), v.q.data(), v.p.data(), Tci.q, Tci.t);
+    h->so3[4 * i] = o.x; h->so3[4 * i + 1] = o.y; h->so3[4 * i + 2] = o.z; h->so3[4 * i + 3] = o.w;
+  }
+  for (int j = 0; j < nr3; ++j) {
+    const double4 o = r3_knot(j, h->dt_r3_ns, nr3, nv, v.t.data(), v.q.data(), v.p.data(), Tci.q, Tci.t);
+    h->r3[3 * j] = o.x; h->r3[3 * j + 1] = o.y; h->r3[3 * j + 2] = o.z;
+  }
+}
+
+// CalcTimes of every frame (impl.h:541); `accepted` lists the frames both splines accept, in input order
+std::vector<FrameHost> frame_times(icc_handle* h, const KnotCounts& n, std::vector<int>& accepted) {
+  const int nf = (int)h->frame_t.size();
+  std::vector<FrameHost> frames(nf);
+  accepted.clear(); h->dropped_frames = 0;
+  for (int i = 0; i < nf; ++i) {
+    FrameHost& f = frames[i]; f.t_s = h->frame_t[i]; f.c0 = h->corner_off[i]; f.c1 = h->corner_off[i + 1];
+    const int64_t t_ns = (int64_t)(f.t_s * S_TO_NS);
+    int64_t s1 = 0, s2 = 0;
+    const bool ok = calc_times(t_ns, h->start_ns, h->dt_r3_ns, n.r3, SPLINE_N, f.u_r3, s1) && calc_times(t_ns, h->start_ns, h->dt_so3_ns, n.so3, SPLINE_N, f.u_so3, s2);
+    f.s_r3 = (int)s1; f.s_so3 = (int)s2;
+    if (ok) accepted.push_back(i); else ++h->dropped_frames;
+  }
+  return frames;
+}
+
+// Kept samples [ka, kb) of a sorted stream, used in place: the cells -- maximal runs of samples inside the same knot interval of all four
+// splines -- are found by galloping + bisection for the next interval boundary (CalcTimes' st is monotone in t), so the host touches
+// O(cells log run) time stamps instead of every sample.  The relative times st = int64((t + offset) 1e9) - start themselves are derived on
+// the device from the uploaded stamps (imu_times_kernel), bit for bit.
+void cells_by_bisection(icc_handle* h, size_t ka, size_t kb) {
+  const double* imu_t = h->imu_t.data(); const double toff = h->ip.time_offset_imu_to_cam_s;
+  auto st_of = [&](size_t i) { return (int64_t)((imu_t[i] + toff) * S_TO_NS) - h->start_ns; };
+  h->cells.clear(); h->imu_used_t.clear(); h->imu_used_st.clear();
+  size_t k = ka;
+  while (k < kb) {
+    const int64_t st = st_of(k);
+    const int64_t a = st / h->dt_r3_ns, b = st / h->dt_so3_ns, c = st / h->dt_ba_ns, d = st / h->dt_bg_ns;
+    const int64_t edge = std::min(std::min((a + 1) * h->dt_r3_ns, (b + 1) * h->dt_so3_ns), std::min((c + 1) * h->dt_ba_ns, (d + 1) * h->dt_bg_ns));
+    size_t prev = k, probe = k + 1, step = 1;                     // first index in (k, kb) with st >= edge: gallop, then bisect
+    while (probe < kb && st_of(probe) < edge) { prev = probe; probe += step; step *= 2; }
+    size_t lo = prev + 1, hi = std::min(probe, kb);                // st_of(prev) < edge <= st_of(probe) (or probe is past the end)
+    while (lo < hi) { const size_t m = (lo + hi) / 2; if (st_of(m) < edge) lo = m + 1; else hi = m; }
+    h->cells.push_back({(int)b, (int)a, (int)c, (int)d, (int)(k - ka), (int)(lo - ka)});
+    k = lo;
+  }
+  h->imu_lazy = true; h->n_imu_used = kb - ka; h->imu_contig = kb > ka; h->imu_src0 = kb > ka ? (int)ka : 0;
+}
+
+// Measurement selection of a time-sorted stream (the usual case; known from set_imu).  CalcTimes' validity tests are monotone in time, so
+// the kept samples are ONE index range [ia, ib) of imu_t, found by bisection.  The shard rule -- unit `mine` iff the scalar residuals of all
+// units before it in the time-merged order (frames before IMU samples on ties) fall in [lo, hi) -- is then evaluated on counts: frames are
+// break points found by bisection, and only the shard's own samples are walked, by cells_by_bisection.  O(frames log samples + cells log
+// run) instead of O(samples) per rank; same decisions as select_general (tests/test_capi_boundary.py, test_sharding_gloo.py).  One shard
+// keeps every accepted frame (the rule on counts would drop a corner-less frame after the last unit with residuals).  Declines (false) for
+// an unsorted stream, a stream without kept samples, and frames out of time order when there are several shards.
+bool select_sorted(icc_handle* h, const KnotCounts& n, const std::vector<FrameHost>& frames, const std::vector<int>& accepted, bool frames_increasing,
+                   std::vector<int>& frame_sel) {
+  if (!h->imu_sorted || (h->shard_world > 1 && !frames_increasing)) return false;
+  const size_t n_in = h->imu_t.size();
+  const double* imu_t = h->imu_t.data(); const double toff = h->ip.time_offset_imu_to_cam_s, t0 = h->t0_s, tend = h->tend_s;
+  auto bisect = [](size_t a, size_t b, auto pred) { while (a < b) { const size_t m = (a + b) / 2; if (pred(m)) a = m + 1; else b = m; } return a; };   // first index where pred is false
+  auto fits = [&](size_t i) {   // upper-side validity of CalcTimes for all four splines (monotone: true, then false)
+    const double t = imu_t[i] + toff;
+    if (t >= tend) return false;
+    const int64_t st = (int64_t)(t * S_TO_NS) - h->start_ns;
+    return size_t(st / h->dt_r3_ns + SPLINE_N) <= (size_t)n.r3 && size_t(st / h->dt_so3_ns + SPLINE_N) <= (size_t)n.so3 && size_t(st / h->dt_ba_ns + BIAS_N) <= (size_t)n.ba && size_t(st / h->dt_bg_ns + BIAS_N) <= (size_t)n.bg;
+  };
+  const size_t ia = bisect(0, n_in, [&](size_t i) { const double t = imu_t[i] + toff; return t < t0 || (int64_t)(t * S_TO_NS) - h->start_ns < 0; });
+  const size_t ib = bisect(ia, n_in, fits);
+  if (ib <= ia) return false;
+  const size_t in_window = bisect(ia, n_in, [&](size_t i) { return imu_t[i] + toff < tend; }) - ia;
+  h->dropped_imu = (int)(in_window - (ib - ia));
+  size_t ka = ia, kb = ib;                  // this shard's samples
+  if (h->shard_world == 1) frame_sel = accepted;
+  else {
+    long total = 6 * (long)(ib - ia);
+    for (int j : accepted) total += 2 * (frames[j].c1 - frames[j].c0);
+    const long lo = total * h->shard_rank / h->shard_world, hi = total * (h->shard_rank + 1) / h->shard_world;
+    auto ceil_div6 = [](long v) { return v <= 0 ? 0L : (v + 5) / 6; };
+    ka = ib; kb = ia;
+    size_t prev_p = ia;
+    long Rf = 0;                            // residuals of the accepted frames seen so far
+    auto take_imu = [&](size_t a, size_t b) {   // samples [a, b) lie between two frames: run_before(i) = Rf + 6 (i - ia)
+      const size_t first = std::max(a, ia + (size_t)ceil_div6(lo - Rf)), last = std::min(b, ia + (size_t)ceil_div6(hi - Rf));
+      if (first < last) { ka = std::min(ka, first); kb = std::max(kb, last); }
+    };
+    for (int j : accepted) {
+      const double tf = frames[j].t_s;
+      const size_t p = bisect(prev_p, ib, [&](size_t i) { return imu_t[i] + toff < tf; });   // samples strictly before the frame
+      take_imu(prev_p, p);
+      const long run = Rf + 6 * (long)(p - ia);
+      if (run >= lo && run < hi) frame_sel.push_back(j);
+      Rf += 2 * (frames[j].c1 - frames[j].c0);
+      prev_p = p;
+    }
+    take_imu(prev_p, ib);
+    if (ka > kb) ka = kb = ia;
+  }
+  cells_by_bisection(h, ka, kb);
+  return true;
+}
+
+// CalcTimes' segment index s = st / dt of a time-sorted stream only ever steps forward: track it with comparisons and fall back to the
+// division when a sample is not where the previous one left off (unsorted input); the results are identical
+struct SegTrack { int64_t dt, s = 0, lo = 0, hi = -1;   // [lo, hi) = time range of segment s; hi < lo until the first sample
+  int64_t seg(int64_t st) {
+    if (st >= lo && st < hi) return s;
+    if (hi > lo && st >= hi && st < hi + 63 * dt) { do { ++s; lo = hi; hi += dt; } while (st >= hi); return s; }
+    s = st / dt; lo = s * dt; hi = lo + dt; return s;
+  } };
+
+// Measurement selection of any stream: one pass collects the kept samples, frames and samples are merged in time order and cut by the
+// shard rule, and the shard's samples are copied (their readings gathered unless they are one contiguous run of the input).
+icc_status select_general(icc_handle* h, const KnotCounts& n, const std::vector<FrameHost>& frames, const std::vector<int>& accepted, std::vector<int>& frame_sel) {
+  struct ImuHost { double t_s; int64_t st; int s_so3, s_r3, s_ba, s_bg; int src; };
+  const size_t n_in = h->imu_t.size();
+  std::vector<ImuHost> kept; kept.reserve(n_in);
+  {
+    SegTrack tr_r3{h->dt_r3_ns}, tr_so3{h->dt_so3_ns}, tr_ba{h->dt_ba_ns}, tr_bg{h->dt_bg_ns};
+    h->dropped_imu = 0;
+    const double* imu_t = h->imu_t.data(); const double toff = h->ip.time_offset_imu_to_cam_s, t0 = h->t0_s, tend = h->tend_s;
+    for (size_t i = 0; i < n_in; ++i) {
+      const double t = imu_t[i] + toff;
+      if (t < t0 || t >= tend) continue;
+      const int64_t t_ns = (int64_t)(t * S_TO_NS), st = t_ns - h->start_ns;
+      bool ok = st >= 0;
+      int64_t a = 0, b = 0, c = 0, d = 0;
+      if (ok) { a = tr_r3.seg(st); b = tr_so3.seg(st); c = tr_ba.seg(st); d = tr_bg.seg(st);
+                ok = size_t(a + SPLINE_N) <= (size_t)n.r3 && size_t(b + SPLINE_N) <= (size_t)n.so3 && size_t(c + BIAS_N) <= (size_t)n.ba && size_t(d + BIAS_N) <= (size_t)n.bg; }
+      if (!ok) { ++h->dropped_imu; continue; }
+      kept.push_back({t, st, (int)b, (int)a, (int)c, (int)d, (int)i});
+    }
+  }
+  struct Unit { double t; int kind, idx, nres; };
+  std::vector<Unit> units; units.reserve(accepted.size() + kept.size());
+  for (int i : accepted) units.push_back({frames[i].t_s, 0, i, 2 * (frames[i].c1 - frames[i].c0)});
+  const size_t nfu = units.size();
+  for (size_t i = 0; i < kept.size(); ++i) units.push_back({kept[i].t_s, 1, (int)i, 6});
+  {   // time order with frames before IMU samples on ties (== stable sort of [frames..., imu...]); both streams are normally
+      // already sorted, so merge in O(n) and only fall back to sorting when they are not
+    auto lt = [](const Unit& x, const Unit& y) { return x.t < y.t; };
+    if (!std::is_sorted(units.begin(), units.begin() + nfu, lt)) std::stable_sort(units.begin(), units.begin() + nfu, lt);
+    if (!std::is_sorted(units.begin() + nfu, units.end(), lt)) std::stable_sort(units.begin() + nfu, units.end(), lt);
+    std::vector<Unit> merged(units.size());
+    std::merge(units.begin(), units.begin() + nfu, units.begin() + nfu, units.end(), merged.begin(), lt);
+    units.swap(merged);
+  }
+  long total = 0; for (const auto& u : units) total += u.nres;
+  const long lo = total * h->shard_rank / h->shard_world, hi = total * (h->shard_rank + 1) / h->shard_world;
+  long run = 0;
+  std::vector<int> imu_sel;
+  frame_sel.clear();
+  for (const auto& u : units) { const bool mine = run >= lo && run < hi; run += u.nres; if (!mine) continue; (u.kind == 0 ? frame_sel : imu_sel).push_back(u.idx); }
+  std::sort(frame_sel.begin(), frame_sel.end());
+  h->imu_lazy = false; h->n_imu_used = imu_sel.size();
+  h->imu_contig = !imu_sel.empty();
+  for (size_t k = 1; k < imu_sel.size() && h->imu_contig; ++k) h->imu_contig = kept[imu_sel[k]].src == kept[imu_sel[k - 1]].src + 1;
+  h->imu_src0 = imu_sel.empty() ? 0 : kept[imu_sel.front()].src;
+  h->imu_used_t.resize(imu_sel.size()); h->imu_used_st.resize(imu_sel.size(), h->device >= 0);
+  if (!h->imu_contig) { icc_status es = ensure_host_imu(h); if (es != ICC_OK) return es; }
+  if (!h->imu_contig) { h->imu_used_acc.resize(3 * imu_sel.size()); h->imu_used_gyr.resize(3 * imu_sel.size()); }
+  h->cells.clear();
+  for (size_t k = 0; k < imu_sel.size(); ++k) {
+    const ImuHost& m = kept[imu_sel[k]];
+    const int idx = (int)k;
+    h->imu_used_t[k] = m.t_s; h->imu_used_st[k] = m.st;
+    if (!h->imu_contig) { memcpy(&h->imu_used_acc[3 * k], &h->imu_acc[3 * (size_t)m.src], 3 * sizeof(double)); memcpy(&h->imu_used_gyr[3 * k], &h->imu_gyr[3 * (size_t)m.src], 3 * sizeof(double)); }
+    if (h->cells.empty() || h->cells.back().s_so3 != m.s_so3 || h->cells.back().s_r3 != m.s_r3 || h->cells.back().s_ba != m.s_ba || h->cells.back().s_bg != m.s_bg)
+      h->cells.push_back({m.s_so3, m.s_r3, m.s_ba, m.s_bg, idx, idx});
+    h->cells.back().i_end = idx + 1;
+  }
+  return ICC_OK;
+}
+
+// The corners of the selected frames: used in place when the frames are one contiguous run (the usual case: all frames, or one contiguous
+// shard), else gathered on the host
+icc_status gather_corners(icc_handle* h, const std::vector<FrameHost>& frames, const std::vector<int>& frame_sel) {
+  h->frames.clear(); h->used_uv.clear(); h->used_pid.clear();
+  h->frames.reserve(frame_sel.size());
+  bool consecutive = !frame_sel.empty();
+  for (size_t k = 1; k < frame_sel.size() && consecutive; ++k) consecutive = frame_sel[k] == frame_sel[k - 1] + 1;
+  h->used_contig = consecutive; h->used_c0 = 0; h->used_n = 0;
+  if (consecutive) {
+    const int cb = frames[frame_sel.front()].c0, ce = frames[frame_sel.back()].c1;
+    h->used_c0 = cb; h->used_n = ce - cb;
+    for (int fi : frame_sel) { FrameHost f = frames[fi]; f.c0 -= cb; f.c1 -= cb; h->frames.push_back(f); }
+  } else {
+    { icc_status es = ensure_host_corners(h); if (es != ICC_OK) return es; }
+    for (int fi : frame_sel) {
+      FrameHost f = frames[fi];
+      const int c0 = (int)h->used_pid.size();
+      for (int c = f.c0; c < f.c1; ++c) { h->used_pid.push_back(h->point_ids[c]); h->used_uv.push_back(h->uv[2 * c]); h->used_uv.push_back(h->uv[2 * c + 1]); }
+      f.c0 = c0; f.c1 = (int)h->used_pid.size();
+      h->frames.push_back(f);
+    }
+    h->used_n = (int)h->used_pid.size();
+  }
+  return ICC_OK;
+}
+
+// Gravity initialisation (imu_camera_calibrator.cc:130-161) incl. the integer-second truncation of the accelerometer time: the reference
+// visits the sorted camera timestamps; a repeated one names the same view (the map's) again and finds nothing new, so each view is
+// visited once, in time order
+icc_status init_gravity(icc_handle* h, const ViewTable& v, const Pose& Tci) {
+  bool ginit = false; double g0[3] = {0.0, 0.0, 9.81};   // GRAVITY_MAGN (spline_trajectory_estimator.h:29) when never initialised
+  for (size_t k = 0; k < v.t.size() && !ginit; ++k) {
+    const Pose Tai = view_T_w_i(v.q.data(), v.p.data(), (int)k, Tci.q, Tci.t);
+    for (size_t i = 0; i < h->imu_t.size(); ++i) {
+      const int64_t accl_t = (int64_t)h->imu_t[i];
+      if (std::fabs(double(accl_t) - v.t[k]) < 1. / 30.) {
+        double a3[3];
+        if (h->imu_dev && h->imu_acc.size() != 3 * h->n_imu_in) { CU(cudaMemcpy(a3, h->d_acc_all.p + 3 * i, sizeof a3, cudaMemcpyDeviceToHost)); }   // one reading
+        else { a3[0] = h->imu_acc[3 * i]; a3[1] = h->imu_acc[3 * i + 1]; a3[2] = h->imu_acc[3 * i + 2]; }
+        const V3 g = qrot(Tai.q, v3(a3[0], a3[1], a3[2])); g0[0] = g.x; g0[1] = g.y; g0[2] = g.z; ginit = true; break; }
+    }
+  }
+  for (int d = 0; d < 3; ++d) h->glob[G_GRAV + d] = g0[d];
+  return ICC_OK;
+}
+
+// Schedule of the persistent evaluation kernel (icc_eval_tmem.cu).  Both streams -- the corners of the non-empty frames and the samples of
+// the knot-interval cells, units padded to a multiple of 4 = one m8n8k4 k-step -- are walked with the kernel's own chunk rule (a chunk = up
+// to 32 stream positions from at most two consecutive units) and cut into even per-warp runs: h->vitems / h->iitems and the stream counts
+// of h->P.  Returns the unit tables the kernel reads.
+struct EvalStreams { std::vector<VisFrame> vf; std::vector<ImuCellP> ic; };
+EvalStreams eval_schedule(icc_handle* h) {
+  DeviceProblem& P = h->P;
+  struct Walk { std::vector<int> pos, unit; int total = 0; };
+  auto walk = [](const std::vector<int>& poff, int n_units) { Walk w; w.total = poff[n_units];
+    for (int pos = 0, u = 0; pos < w.total;) {
+      while (poff[u + 1] <= pos) ++u;
+      w.pos.push_back(pos); w.unit.push_back(u);
+      const int nA = std::min(32, poff[u + 1] - pos);
+      int n = nA;
+      if (nA < 32 && u + 1 < n_units) n += std::min(32 - nA, poff[u + 2] - poff[u + 1]);
+      pos += n;
+    }
+    return w; };
+  EvalStreams es;
+  std::vector<VisFrame>& vf = es.vf; vf.reserve(h->frames.size() + 2);
+  std::vector<int> vpoff;
+  int poff = 0;
+  if (P.rolling) for (const auto& f : h->frames) {
+    const int cn = f.c1 - f.c0;
+    if (cn <= 0) continue;
+    vf.push_back({poff, f.c0, cn, f.s_so3, f.s_r3, 0, f.u_so3, f.u_r3}); vpoff.push_back(poff);
+    poff += (cn + 3) / 4 * 4;
+  }
+  const int nvf = (int)vf.size();
+  vf.push_back({poff, 0, 0, 0, 0, 0, 0.0, 0.0}); vf.push_back({poff, 0, 0, 0, 0, 0, 0.0, 0.0});   // sentinels [n], [n+1]
+  vpoff.push_back(poff); vpoff.push_back(poff);
+  std::vector<ImuCellP>& ic = es.ic; ic.reserve(h->cells.size() + 2);
+  std::vector<int> ipoff;
+  poff = 0;
+  for (const auto& c : h->cells) {
+    const int n = c.i_end - c.i_begin;
+    if (n <= 0) continue;
+    ic.push_back({poff, c.i_begin, n, c.s_so3, c.s_r3, c.s_ba, c.s_bg, 0}); ipoff.push_back(poff);
+    poff += (n + 3) / 4 * 4;
+  }
+  const int nic = (int)ic.size();
+  ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0}); ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0});
+  ipoff.push_back(poff); ipoff.push_back(poff);
+  const Walk wv = walk(vpoff, nvf), wi = walk(ipoff, nic);
+  int W = h->sm_count * eval_tmem_warps();
+  // ICC_TMEM_RUNS=n caps the runs at n (tests: every warp then owns several chunks and carries its tile state between them)
+  if (const char* e = getenv("ICC_TMEM_RUNS")) { const int n = atoi(e); if (n > 0) W = std::min(W, n); }
+  auto split = [W](const Walk& w) {      // even runs, one per warp
+    const int nc = (int)w.pos.size(), n_items = std::min(W, nc);
+    std::vector<VisItem> items((size_t)n_items);
+    for (int k = 0; k < n_items; ++k) {
+      const int a = (int)((int64_t)nc * k / n_items), b = (int)((int64_t)nc * (k + 1) / n_items);
+      items[(size_t)k] = {w.unit[a], w.pos[a], b < nc ? w.pos[b] : w.total, 0};
+    }
+    return items; };
+  h->vitems = split(wv); h->iitems = split(wi);
+  P.n_vchunks = (int)wv.pos.size(); P.n_ichunks = (int)wi.pos.size();
+  P.n_vframes = nvf; P.n_vitems = (int)h->vitems.size(); P.n_icells = nic; P.n_iitems = (int)h->iitems.size();
+  return es;
+}
+
+// Device upload: the problem arrays and work lists, both state copies, and the knots by init_knots_kernel from the view table.  The small
+// arrays are staged through the pinned arena: its size below must cover everything staged through it until the next batch_init (each
+// array takes a multiple of 256 bytes), else upload_staged falls back to blocking copies.
+icc_status upload_problem(icc_handle* h, const ViewTable& v, const Pose& Tci, const EvalStreams& es, PhaseTrace& trace) {
+  DeviceProblem& P = h->P;
+  const size_t nf = h->frame_t.size();
+  CU(cudaSetDevice(h->device));
+  CU(cudaStreamSynchronize(h->stream));   // nothing may still read the staging arena of an earlier call
+  trace.lap("batch_init: gravity init");
+  h->arena.reset((size_t)(1 << 17) + 64 * nf + 48 * (nf + 4) + 16 * (size_t)(h->sm_count * 16 + 16) + 48 * (nf + h->used_n / 32 + 64) + (96 + 40) * (h->cells.size() + (size_t)P.n_imu / 32 + 64)
+                 + 8 * 8 * (nf + 8) + 2 * 40 * (size_t)(P.n_so3 + P.n_r3 + P.n_ba + P.n_bg + 16) + 3 * (32 * (h->points.size() / 4 + 8) + 256) + 3 * (4 * (size_t)(P.n_so3 + P.n_r3 + P.n_ba + P.n_bg) + 1024), true);
+  trace.lap("batch_init: pinned arena");
+  {
+    std::vector<double4> board(h->points.size() / 4);
+    // hnormalized(T^-1 X_h) of the functor (residuals.h:357-362) == T^-1 (X / w): the division is done once here
+    for (size_t i = 0; i < board.size(); ++i) { const double iw = 1.0 / h->points[4 * i + 3]; board[i] = make_double4(h->points[4 * i] * iw, h->points[4 * i + 1] * iw, h->points[4 * i + 2] * iw, 1.0); }
+    CU(upload_staged(h, h->d_board, board)); P.board = h->d_board.p;   // (the evaluation kernels read the copy that belongs to the state: DeviceState::board)
+    std::vector<int> off, s1, s2; std::vector<double> u1, u2;
+    for (const auto& f : h->frames) { off.push_back(f.c0); s1.push_back(f.s_so3); s2.push_back(f.s_r3); u1.push_back(f.u_so3); u2.push_back(f.u_r3); }
+    off.push_back(P.n_corners);
+    CU(upload_staged(h, h->d_f_off, off)); CU(upload_staged(h, h->d_f_s_so3, s1)); CU(upload_staged(h, h->d_f_s_r3, s2)); CU(upload_staged(h, h->d_f_u_so3, u1)); CU(upload_staged(h, h->d_f_u_r3, u2));
+    P.f_off = h->d_f_off.p; P.f_s_so3 = h->d_f_s_so3.p; P.f_s_r3 = h->d_f_s_r3.p; P.f_u_so3 = h->d_f_u_so3.p; P.f_u_r3 = h->d_f_u_r3.p;
+    const bool corners_in_place = h->frames_dev && h->used_contig;   // already on the device (set_frames): used where they lie
+    if (corners_in_place) { P.uv = h->d_uv_all.p + h->used_c0; P.pid = h->d_pid_all.p + h->used_c0; }
+    else { CU(h->d_uv.alloc(P.n_corners)); CU(h->d_pid.alloc(P.n_corners)); P.uv = h->d_uv.p; P.pid = h->d_pid.p; }   // (u, v) pairs are already laid out as double2
+    if (P.n_corners > 0 && !corners_in_place) {
+      const double* uv_src = h->used_contig ? h->uv.data() + 2 * (size_t)h->used_c0 : h->used_uv.data();
+      const int* pid_src = h->used_contig ? h->point_ids.data() + h->used_c0 : h->used_pid.data();
+      // page-locked sources (HostBuf): the DMA transfers run behind the rest of this function; kernels follow on the same stream
+      CU(cudaMemcpyAsync(h->d_uv.p, uv_src, (size_t)P.n_corners * sizeof(double2), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_pid.p, pid_src, (size_t)P.n_corners * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    }
+    // work lists: one warp per item; items sized so that the grid fills the GPU but every item amortises its tile flush
+    const int target_items = h->sm_count * 8;
+    auto round32 = [](long v) { return (int)((v + 31) / 32 * 32); };
+    const int per_v = std::max(32, round32(P.n_corners / std::max(1, target_items)));
+    std::vector<VisionWork> vw;
+    for (int fi = 0; fi < P.n_frames; ++fi) for (int c = h->frames[fi].c0; c < h->frames[fi].c1; c += per_v) vw.push_back({fi, c, std::min(c + per_v, h->frames[fi].c1), 0});
+    CU(upload_staged(h, h->d_vwork, vw)); P.vwork = h->d_vwork.p; P.n_vwork = (int)vw.size();
+    const int per_i = std::max(32, round32(P.n_imu / std::max(1, target_items)));
+    std::vector<ImuCell> iw;
+    for (const auto& c : h->cells) for (int i = c.i_begin; i < c.i_end; i += per_i) { ImuCell s = c; s.i_begin = i; s.i_end = std::min(i + per_i, c.i_end); iw.push_back(s); }
+    CU(upload_staged(h, h->d_iwork, iw)); P.iwork = h->d_iwork.p; P.n_iwork = (int)iw.size();
+    CU(upload_staged(h, h->d_cells, h->cells)); P.cells = h->d_cells.p;
+    CU(upload_staged(h, h->d_vframes, es.vf)); P.vframes = h->d_vframes.p;
+    CU(upload_staged(h, h->d_vitems, h->vitems)); P.vitems = h->d_vitems.p;
+    CU(upload_staged(h, h->d_icells, es.ic)); P.icells = h->d_icells.p;
+    CU(upload_staged(h, h->d_iitems, h->iitems)); P.iitems = h->d_iitems.p;
+    CU(h->d_imu_t.alloc(h->n_imu_used));
+    if (h->imu_lazy && h->n_imu_used) {   // sorted stream: the raw stamps go up, the relative integer times are derived there
+      CU(h->d_imu_traw.alloc(h->n_imu_used));
+      CU(cudaMemcpyAsync(h->d_imu_traw.p, h->imu_t.data() + h->imu_src0, h->n_imu_used * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+      launch_imu_times((int)h->n_imu_used, h->d_imu_traw.p, h->ip.time_offset_imu_to_cam_s, h->start_ns, h->d_imu_t.p, h->stream);
+    } else if (h->n_imu_used) CU(cudaMemcpyAsync(h->d_imu_t.p, h->imu_used_st.data(), h->n_imu_used * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
+    const bool imu_in_place = h->imu_dev && h->imu_contig;   // already on the device (set_imu): used where they lie
+    if (imu_in_place) { P.imu_acc = h->d_acc_all.p + 3 * (size_t)h->imu_src0; P.imu_gyr = h->d_gyr_all.p + 3 * (size_t)h->imu_src0; }
+    else { CU(h->d_imu_acc.alloc(3 * (size_t)P.n_imu)); CU(h->d_imu_gyr.alloc(3 * (size_t)P.n_imu)); P.imu_acc = h->d_imu_acc.p; P.imu_gyr = h->d_imu_gyr.p; }
+    if (P.n_imu > 0 && !imu_in_place) {
+      const double* a_src = h->imu_contig ? h->imu_acc.data() + 3 * (size_t)h->imu_src0 : h->imu_used_acc.data();
+      const double* g_src = h->imu_contig ? h->imu_gyr.data() + 3 * (size_t)h->imu_src0 : h->imu_used_gyr.data();
+      CU(cudaMemcpyAsync(h->d_imu_acc.p, a_src, 3 * (size_t)P.n_imu * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+      CU(cudaMemcpyAsync(h->d_imu_gyr.p, g_src, 3 * (size_t)P.n_imu * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    }
+    P.imu_t_ns = h->d_imu_t.p;
+  }
+  trace.lap("batch_init: problem upload");
+  icc_status s = upload_state(h, 0, true); if (s != ICC_OK) return s;
+  s = upload_state(h, 1, true); if (s != ICC_OK) return s;
+  trace.lap("batch_init: state upload");
+  {   // knots: BatchInitSO3R3VisPoses on the device, written into both state copies (the zero knots uploaded above only sized them)
+    CU(upload_staged(h, h->d_view_t, v.t)); CU(upload_staged(h, h->d_view_q, v.q)); CU(upload_staged(h, h->d_view_p, v.p));
+    const double Tci7[7] = {Tci.q.x, Tci.q.y, Tci.q.z, Tci.q.w, Tci.t.x, Tci.t.y, Tci.t.z};
+    launch_init_knots((int)v.t.size(), h->d_view_t.p, h->d_view_q.p, h->d_view_p.p, Tci7, P.n_so3, h->dt_so3_ns, P.n_r3, h->dt_r3_ns,
+                      h->st[0].so3.p, h->st[1].so3.p, h->st[0].r3.p, h->st[1].r3.p, h->stream);
+    h->knots_dirty_host = true;     // the device holds the knots; the host mirror is refreshed on demand (getters / setters)
+  }
+  trace.lap("batch_init: knot init");
+  return ICC_OK;
+}
+
 }  // namespace
 
 // =================================================================================================================
@@ -722,452 +1111,36 @@ icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
   PhaseTrace trace(h->device >= 0 ? h->stream : nullptr);
   if (h->id_lo < 0 || (size_t)(h->id_hi + 1) > h->points.size() / 4) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner references an unknown board point");
   h->ip = *ipp;
-  const int nf = (int)h->frame_t.size();
   trace.lap("batch_init: id range check");
-  // T_i_c, IMU intrinsics, line delay (imu_camera_calibrator.cc:30-47)
-  { const Q4 q = qn(ipp->T_i_c_init); h->glob[G_TIC + 0] = q.x; h->glob[G_TIC + 1] = q.y; h->glob[G_TIC + 2] = q.z; h->glob[G_TIC + 3] = q.w; for (int i = 4; i < 7; ++i) h->glob[G_TIC + i] = ipp->T_i_c_init[i]; }
-  for (int i = 0; i < 6; ++i) h->glob[G_ACC_INTR + i] = ipp->acc_intrinsics[i];
-  for (int i = 0; i < 9; ++i) h->glob[G_GYR_INTR + i] = ipp->gyr_intrinsics[i];
-  h->glob[G_LD] = ipp->init_line_delay_s;
-  for (int i = 0; i < 10; ++i) h->glob[G_CAM_INTR + i] = i < h->n_intr ? h->intr[i] : 0.0;
-  h->glob[G_TOFF] = 0.0;
-  // spline time range and knot counts (imu_camera_calibrator.cc:49-72, impl.h:37-51)
-  std::vector<double> cam_ts(h->frame_t); std::sort(cam_ts.begin(), cam_ts.end());
-  h->t0_s = cam_ts.front(); h->tend_s = cam_ts.back();
-  h->start_ns = (int64_t)(h->t0_s * S_TO_NS);
-  h->end_ns = (int64_t)(h->tend_s * S_TO_NS + 0.01 * S_TO_NS + ipp->init_line_delay_s);
-  h->dt_so3_ns = (int64_t)(ipp->dt_so3_s * S_TO_NS); h->dt_r3_ns = (int64_t)(ipp->dt_r3_s * S_TO_NS);
-  if (h->dt_so3_ns <= 0 || h->dt_r3_ns <= 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "knot spacing must be positive");
-  const int64_t duration = h->end_ns - h->start_ns;
-  const int nso3 = (int)(duration / h->dt_so3_ns) + SPLINE_N, nr3 = (int)(duration / h->dt_r3_ns) + SPLINE_N;
-  // knot initialisation from the per-view pose priors (impl.h:278-339)
-  const Pose Tic{q4(h->glob[0], h->glob[1], h->glob[2], h->glob[3]), v3(h->glob[4], h->glob[5], h->glob[6])};
-  const Pose Tci = pose_inv(Tic);
-  // the reference walks its views through a std::map keyed by timestamp (time order, a repeated timestamp keeps the LAST view);
-  // strictly increasing timestamps -- the usual case -- give that order without the tree
-  bool increasing = true; for (int i = 1; i < nf && increasing; ++i) increasing = h->frame_t[i] > h->frame_t[i - 1];
-  std::vector<int> view_order;
-  if (increasing) { view_order.resize(nf); for (int i = 0; i < nf; ++i) view_order[i] = i; }
-  else { std::map<double, int> by_time; for (int i = 0; i < nf; ++i) by_time[h->frame_t[i]] = i; for (const auto& kv : by_time) view_order.push_back(kv.second); }
-  std::vector<double> t_vis, q_vis, p_vis;
-  t_vis.reserve(view_order.size()); q_vis.reserve(4 * view_order.size()); p_vis.reserve(3 * view_order.size());
-  for (const int i : view_order) {
-    const Pose Twc{qn(&h->q_wc[4 * i]), v3(h->p_wc[3 * i], h->p_wc[3 * i + 1], h->p_wc[3 * i + 2])};
-    const Pose Twi = pose_mul(Twc, Tci);
-    t_vis.push_back(h->frame_t[i]);
-    q_vis.push_back(Twi.q.x); q_vis.push_back(Twi.q.y); q_vis.push_back(Twi.q.z); q_vis.push_back(Twi.q.w);
-    p_vis.push_back(Twi.t.x); p_vis.push_back(Twi.t.y); p_vis.push_back(Twi.t.z);
-  }
-  const size_t nv = t_vis.size();
-  h->so3.assign(4 * (size_t)nso3, 0.0); h->r3.assign(3 * (size_t)nr3, 0.0);
-  // With a device the knots are initialised by init_knots_kernel (icc_init.cu) straight into both state copies, from the uploaded
-  // view poses; the host statement below serves the host-only handle (device -1: assembly checks against the oracle on CPU).
-  if (h->device < 0) {
-  for (int i = 0; i < nso3; ++i) {   // InterpolateQuaternions (utils.cc:221-241); knot times are zero based (SURVEY quirk q7)
-    const double t = double(i) * double(h->dt_so3_ns) * NS_TO_S;
-    double dist = 0; const size_t k = nearest_index(t, t_vis, dist);
-    double q[4];
-    if (k < nv - 1) quat_slerp(&q_vis[4 * k], &q_vis[4 * (k + 1)], dist / (t_vis[k + 1] - t_vis[k]), q); else memcpy(q, &q_vis[4 * k], sizeof q);
-    const Q4 r = qn(q);
-    h->so3[4 * i] = r.x; h->so3[4 * i + 1] = r.y; h->so3[4 * i + 2] = r.z; h->so3[4 * i + 3] = r.w;
-  }
-  for (int i = 0; i < nr3; ++i) {    // InterpolateVector3d (utils.cc:243-261) incl. its `nearest < t_new.size()` test; the reference's
-    const double t = double(i) * double(h->dt_r3_ns) * NS_TO_S;   // out-of-range read past the last view falls back to the nearest value
-    double dist = 0; const size_t k = nearest_index(t, t_vis, dist);
-    if (k < (size_t)nr3 && k + 1 < nv) { const double f = dist / (t_vis[k + 1] - t_vis[k]); for (int d = 0; d < 3; ++d) h->r3[3 * i + d] = (1.0 - f) * p_vis[3 * k + d] + f * p_vis[3 * (k + 1) + d]; }
-    else for (int d = 0; d < 3; ++d) h->r3[3 * i + d] = p_vis[3 * k + d];
-  }
-  }
-  // bias splines: InitBiasSplines(bias, bias, 10 s, 10 s, 1.0, 0.1) (imu_camera_calibrator.cc:80-85, impl.h:53-90)
-  h->dt_ba_ns = h->dt_bg_ns = (int64_t)(10 * 1e9); h->max_ba = 1.0; h->max_bg = 1e-1;
-  const int nba = (int)(duration / h->dt_ba_ns) + BIAS_N, nbg = (int)(duration / h->dt_bg_ns) + BIAS_N;
-  h->ba.resize(3 * (size_t)nba); h->bg.resize(3 * (size_t)nbg);
-  for (int i = 0; i < nba; ++i) for (int d = 0; d < 3; ++d) h->ba[3 * i + d] = ipp->acc_bias[d];
-  for (int i = 0; i < nbg; ++i) for (int d = 0; d < 3; ++d) h->bg[3 * i + d] = ipp->gyr_bias[d];
-
+  KnotCounts n;
+  icc_status s = init_globals_and_knot_counts(h, n); if (s != ICC_OK) return s;
+  const ViewTable views = view_table(h);
+  const Pose Tci = T_c_i(h);
+  if (h->device < 0) init_knots_on_host(h, views, Tci);   // with a device, init_knots_kernel writes them straight into both state copies
   trace.lap("batch_init: ranges, view order, bias knots");
   // ---- measurement wiring (imu_camera_calibrator.cc:87-120; Add*Measurement impl.h:341-613) ----------------------
-  const bool pin = h->device >= 0;
-  std::vector<FrameHost> all_frames(nf);
-  std::vector<char> frame_ok(nf);
-  h->dropped_frames = h->dropped_imu = 0;
-  for (int i = 0; i < nf; ++i) {
-    FrameHost& f = all_frames[i]; f.t_s = h->frame_t[i]; f.c0 = h->corner_off[i]; f.c1 = h->corner_off[i + 1];
-    const int64_t t_ns = (int64_t)(f.t_s * S_TO_NS);
-    int64_t s1 = 0, s2 = 0;
-    const bool ok = calc_times(t_ns, h->start_ns, h->dt_r3_ns, nr3, SPLINE_N, f.u_r3, s1) && calc_times(t_ns, h->start_ns, h->dt_so3_ns, nso3, SPLINE_N, f.u_so3, s2);
-    f.s_r3 = (int)s1; f.s_so3 = (int)s2;
-    frame_ok[i] = ok; if (!ok) ++h->dropped_frames;
-  }
-  struct ImuHost { double t_s; int64_t st; int s_so3, s_r3, s_ba, s_bg; int src; };
-  // CalcTimes' segment index s = st / dt of a time-sorted stream only ever steps forward: track it with comparisons and fall back
-  // to the division when a sample is not where the previous one left off (unsorted input); the results are identical
-  struct SegTrack { int64_t dt, s = 0, lo = 0, hi = -1;   // [lo, hi) = time range of segment s; hi < lo until the first sample
-    int64_t seg(int64_t st) {
-      if (st >= lo && st < hi) return s;
-      if (hi > lo && st >= hi && st < hi + 63 * dt) { do { ++s; lo = hi; hi += dt; } while (st >= hi); return s; }
-      s = st / dt; lo = s * dt; hi = lo + dt; return s;
-    } };
-  const size_t n_imu_in = h->imu_t.size();
-  h->imu_used_t.clear(); h->imu_used_acc.clear(); h->imu_used_gyr.clear(); h->cells.clear();
-  h->imu_used_st.resize(n_imu_in, pin);
-  std::vector<ImuHost> all_imu;
-  // One pass over the IMU stream.  `direct` (one shard): the kept samples go straight into the problem arrays in arrival order,
-  // which IS the time order as long as the stream is sorted -- the pass gives up (returns false) at the first sample that is not.
-  // Otherwise they are collected for the general path below (time merge with the frames, residual-count sharding).
-  auto imu_pass = [&](bool direct) -> bool {
-    SegTrack tr_r3{h->dt_r3_ns}, tr_so3{h->dt_so3_ns}, tr_ba{h->dt_ba_ns}, tr_bg{h->dt_bg_ns};
-    h->dropped_imu = 0; h->imu_used_t.clear(); h->cells.clear(); all_imu.clear();
-    if (direct) h->imu_used_t.resize(n_imu_in); else all_imu.reserve(n_imu_in);
-    double* t_out = h->imu_used_t.data();
-    int64_t* st_out = h->imu_used_st.data();
-    double last_t = -1.7976931348623157e308; int prev_src = -1; bool contig = true; size_t k = 0;
-    const double* imu_t = h->imu_t.data(); const double toff = ipp->time_offset_imu_to_cam_s, t0 = h->t0_s, tend = h->tend_s;
-    for (size_t i = 0; i < n_imu_in; ++i) {
-      const double t = imu_t[i] + toff;
-      if (t < t0 || t >= tend) continue;
-      const int64_t t_ns = (int64_t)(t * S_TO_NS), st = t_ns - h->start_ns;
-      bool ok = st >= 0;
-      int64_t a = 0, b = 0, c = 0, d = 0;
-      if (ok) { a = tr_r3.seg(st); b = tr_so3.seg(st); c = tr_ba.seg(st); d = tr_bg.seg(st);
-                ok = size_t(a + SPLINE_N) <= (size_t)nr3 && size_t(b + SPLINE_N) <= (size_t)nso3 && size_t(c + BIAS_N) <= (size_t)nba && size_t(d + BIAS_N) <= (size_t)nbg; }
-      if (!ok) { ++h->dropped_imu; continue; }
-      if (!direct) { all_imu.push_back({t, st, (int)b, (int)a, (int)c, (int)d, (int)i}); continue; }
-      if (t < last_t) { h->imu_used_t.clear(); return false; }
-      last_t = t;
-      if (prev_src >= 0 && (int)i != prev_src + 1) contig = false;
-      if (prev_src < 0) h->imu_src0 = (int)i;
-      prev_src = (int)i;
-      t_out[k] = t; st_out[k] = st;
-      if (h->cells.empty() || h->cells.back().s_so3 != (int)b || h->cells.back().s_r3 != (int)a || h->cells.back().s_ba != (int)c || h->cells.back().s_bg != (int)d)
-        h->cells.push_back({(int)b, (int)a, (int)c, (int)d, (int)k, (int)k});
-      h->cells.back().i_end = (int)k + 1;
-      ++k;
-    }
-    if (direct) { h->imu_contig = k > 0 && contig; if (k == 0) h->imu_src0 = 0; h->imu_used_st.n = k; h->imu_used_t.resize(k); }
-    return true;
-  };
-  // Sorted stream (the usual case; known from set_imu): the kept samples [ka, kb) of imu_t are used in place, and the cells -- maximal runs of
-  // samples inside the same knot interval of all four splines -- are found by galloping + bisection for the next interval boundary
-  // (CalcTimes' st is monotone in t), so the host touches O(cells log run) time stamps instead of every sample.  The relative times
-  // st = int64((t + offset) 1e9) - start themselves are derived on the device from the uploaded stamps (imu_times_kernel), bit for bit.
-  auto cells_by_bisection = [&](size_t ka, size_t kb) {
-    const double* imu_t = h->imu_t.data(); const double toff = ipp->time_offset_imu_to_cam_s;
-    auto st_of = [&](size_t i) { return (int64_t)((imu_t[i] + toff) * S_TO_NS) - h->start_ns; };
-    h->cells.clear(); h->imu_used_t.clear(); h->imu_used_st.n = 0;
-    size_t k = ka;
-    while (k < kb) {
-      const int64_t st = st_of(k);
-      const int64_t a = st / h->dt_r3_ns, b = st / h->dt_so3_ns, c = st / h->dt_ba_ns, d = st / h->dt_bg_ns;
-      const int64_t edge = std::min(std::min((a + 1) * h->dt_r3_ns, (b + 1) * h->dt_so3_ns), std::min((c + 1) * h->dt_ba_ns, (d + 1) * h->dt_bg_ns));
-      size_t prev = k, probe = k + 1, step = 1;                     // first index in (k, kb) with st >= edge: gallop, then bisect
-      while (probe < kb && st_of(probe) < edge) { prev = probe; probe += step; step *= 2; }
-      size_t lo = prev + 1, hi = std::min(probe, kb);                // st_of(prev) < edge <= st_of(probe) (or probe is past the end)
-      while (lo < hi) { const size_t m = (lo + hi) / 2; if (st_of(m) < edge) lo = m + 1; else hi = m; }
-      h->cells.push_back({(int)b, (int)a, (int)c, (int)d, (int)(k - ka), (int)(lo - ka)});
-      k = lo;
-    }
-    h->imu_lazy = true; h->n_imu_used = kb - ka; h->imu_contig = kb > ka; h->imu_src0 = kb > ka ? (int)ka : 0;
-  };
-  auto imu_sorted_pass = [&]() -> bool {
-    if (h->shard_world != 1 || !h->imu_sorted || n_imu_in == 0 || getenv("ICC_NO_BISECTION")) return false;   // (the switch forces the sample-by-sample pass: tests)
-    const double* imu_t = h->imu_t.data(); const double toff = ipp->time_offset_imu_to_cam_s, t0 = h->t0_s, tend = h->tend_s;
-    auto bisect = [&](size_t a, size_t b, auto pred) { while (a < b) { const size_t m = (a + b) / 2; if (pred(m)) a = m + 1; else b = m; } return a; };   // first index where pred is false
-    auto fits = [&](size_t i) {   // upper-side validity of CalcTimes for all four splines (monotone: true, then false)
-      const double t = imu_t[i] + toff;
-      if (t >= tend) return false;
-      const int64_t st = (int64_t)(t * S_TO_NS) - h->start_ns;
-      return size_t(st / h->dt_r3_ns + SPLINE_N) <= (size_t)nr3 && size_t(st / h->dt_so3_ns + SPLINE_N) <= (size_t)nso3 && size_t(st / h->dt_ba_ns + BIAS_N) <= (size_t)nba && size_t(st / h->dt_bg_ns + BIAS_N) <= (size_t)nbg;
-    };
-    const size_t ia = bisect(0, n_imu_in, [&](size_t i) { const double t = imu_t[i] + toff; return t < t0 || (int64_t)(t * S_TO_NS) - h->start_ns < 0; });
-    const size_t ib = bisect(ia, n_imu_in, fits);
-    if (ib <= ia) return false;                                     // nothing kept: the sequential pass reports it
-    const size_t in_window = bisect(ia, n_imu_in, [&](size_t i) { return imu_t[i] + toff < tend; }) - ia;
-    h->dropped_imu = (int)(in_window - (ib - ia));
-    cells_by_bisection(ia, ib);
-    return true;
-  };
-  std::vector<int> frame_sel;
-  // (a stream with holes inside the kept range -- samples dropped in the middle -- takes the general path, which gathers the readings)
+  std::vector<int> accepted, frame_sel;
+  const std::vector<FrameHost> frames = frame_times(h, n, accepted);
   trace.lap("batch_init: frame times");
-  h->imu_lazy = false; h->n_imu_used = 0;
-  const bool direct = imu_sorted_pass() || (h->shard_world == 1 && imu_pass(true) && h->imu_contig);
+  if (!select_sorted(h, n, frames, accepted, views.increasing, frame_sel)) { s = select_general(h, n, frames, accepted, frame_sel); if (s != ICC_OK) return s; }
   trace.lap("batch_init: imu pass");
-  if (direct) {
-    for (int i = 0; i < nf; ++i) if (frame_ok[i]) frame_sel.push_back(i);
-  } else if ([&]() -> bool {
-    // Sharded fast path (every stream in time order, the usual case): the shard rule -- unit `mine` iff the scalar residuals of all
-    // units before it in the time-merged order (frames before IMU samples on ties) fall in [lo, hi) -- is evaluated on counts only:
-    // kept IMU samples of a sorted stream are ONE index range (the validity tests of CalcTimes are monotone in time), frames are
-    // break points found by bisection, and only the shard's own samples are then walked.  O(frames log samples + samples / world)
-    // instead of O(samples) per rank; same decisions as the general path below (tests/test_capi_boundary.py, test_sharding_gloo.py).
-    const double* imu_t = h->imu_t.data(); const double toff = ipp->time_offset_imu_to_cam_s, t0 = h->t0_s, tend = h->tend_s;
-    if (!increasing || !h->imu_sorted) return false;
-    auto fits = [&](size_t i) {   // upper-side validity (monotone: true, then false)
-      const double t = imu_t[i] + toff;
-      if (t >= tend) return false;
-      const int64_t st = (int64_t)(t * S_TO_NS) - h->start_ns;
-      return size_t(st / h->dt_r3_ns + SPLINE_N) <= (size_t)nr3 && size_t(st / h->dt_so3_ns + SPLINE_N) <= (size_t)nso3 && size_t(st / h->dt_ba_ns + BIAS_N) <= (size_t)nba && size_t(st / h->dt_bg_ns + BIAS_N) <= (size_t)nbg;
-    };
-    std::vector<size_t> idx(0);
-    struct It { size_t i; };   // bisection over indices
-    auto bisect = [&](size_t a, size_t b, auto pred) { while (a < b) { const size_t m = (a + b) / 2; if (pred(m)) a = m + 1; else b = m; } return a; };   // first index where pred is false
-    const size_t ia = bisect(0, n_imu_in, [&](size_t i) { const double t = imu_t[i] + toff; return t < t0 || (int64_t)(t * S_TO_NS) - h->start_ns < 0; });
-    const size_t ib = bisect(ia, n_imu_in, fits);
-    const size_t in_window = bisect(ia, n_imu_in, [&](size_t i) { return imu_t[i] + toff < tend; }) - ia;
-    h->dropped_imu = (int)(in_window - (ib - ia));
-    std::vector<int> fk; fk.reserve(nf);
-    for (int i = 0; i < nf; ++i) if (frame_ok[i]) fk.push_back(i);
-    long total = 6 * (long)(ib - ia);
-    for (int j : fk) total += 2 * (all_frames[j].c1 - all_frames[j].c0);
-    const long lo = total * h->shard_rank / h->shard_world, hi = total * (h->shard_rank + 1) / h->shard_world;
-    auto ceil_div6 = [](long v) { return v <= 0 ? 0L : (v + 5) / 6; };
-    size_t ka = ib, kb = ia, prev_p = ia;   // this shard's sample range [ka, kb)
-    long Rf = 0;                            // residuals of the kept frames seen so far
-    auto take_imu = [&](size_t a, size_t b) {   // samples [a, b) lie between two frames: run_before(i) = Rf + 6 (i - ia)
-      const size_t first = std::max(a, ia + (size_t)ceil_div6(lo - Rf)), last = std::min(b, ia + (size_t)ceil_div6(hi - Rf));
-      if (first < last) { ka = std::min(ka, first); kb = std::max(kb, last); }
-    };
-    for (int j : fk) {
-      const double tf = all_frames[j].t_s;
-      const size_t p = bisect(prev_p, ib, [&](size_t i) { return imu_t[i] + toff < tf; });   // samples strictly before the frame
-      take_imu(prev_p, p);
-      const long run = Rf + 6 * (long)(p - ia);
-      if (run >= lo && run < hi) frame_sel.push_back(j);
-      Rf += 2 * (all_frames[j].c1 - all_frames[j].c0);
-      prev_p = p;
-    }
-    take_imu(prev_p, ib);
-    if (ka > kb) ka = kb = ia;
-    // the shard's own samples: cells by bisection, readings used in place
-    cells_by_bisection(ka, kb);
-
-    return true;
-  }()) {
-  } else {
-    frame_sel.clear();
-    imu_pass(false);
-    struct Unit { double t; int kind, idx, nres; };
-    std::vector<Unit> units; units.reserve(nf + all_imu.size());
-    for (int i = 0; i < nf; ++i) if (frame_ok[i]) units.push_back({all_frames[i].t_s, 0, i, 2 * (all_frames[i].c1 - all_frames[i].c0)});
-    const size_t nfu = units.size();
-    for (size_t i = 0; i < all_imu.size(); ++i) units.push_back({all_imu[i].t_s, 1, (int)i, 6});
-    {   // time order with frames before IMU samples on ties (== stable sort of [frames..., imu...]); both streams are normally
-        // already sorted, so merge in O(n) and only fall back to sorting when they are not
-      auto lt = [](const Unit& x, const Unit& y) { return x.t < y.t; };
-      if (!std::is_sorted(units.begin(), units.begin() + nfu, lt)) std::stable_sort(units.begin(), units.begin() + nfu, lt);
-      if (!std::is_sorted(units.begin() + nfu, units.end(), lt)) std::stable_sort(units.begin() + nfu, units.end(), lt);
-      std::vector<Unit> merged(units.size());
-      std::merge(units.begin(), units.begin() + nfu, units.begin() + nfu, units.end(), merged.begin(), lt);
-      units.swap(merged);
-    }
-    long total = 0; for (const auto& u : units) total += u.nres;
-    const long lo = total * h->shard_rank / h->shard_world, hi = total * (h->shard_rank + 1) / h->shard_world;
-    long run = 0;
-    std::vector<int> imu_sel;
-    for (const auto& u : units) { const bool mine = run >= lo && run < hi; run += u.nres; if (!mine) continue; (u.kind == 0 ? frame_sel : imu_sel).push_back(u.idx); }
-    std::sort(frame_sel.begin(), frame_sel.end());
-    h->imu_contig = !imu_sel.empty();
-    for (size_t k = 1; k < imu_sel.size() && h->imu_contig; ++k) h->imu_contig = all_imu[imu_sel[k]].src == all_imu[imu_sel[k - 1]].src + 1;
-    h->imu_src0 = imu_sel.empty() ? 0 : all_imu[imu_sel.front()].src;
-    h->imu_used_t.resize(imu_sel.size()); h->imu_used_st.n = imu_sel.size();
-    if (!h->imu_contig) { icc_status es = ensure_host_imu(h); if (es != ICC_OK) return es; }
-    if (!h->imu_contig) { h->imu_used_acc.resize(3 * imu_sel.size()); h->imu_used_gyr.resize(3 * imu_sel.size()); }
-    for (size_t k = 0; k < imu_sel.size(); ++k) {
-      const ImuHost& m = all_imu[imu_sel[k]];
-      const int idx = (int)k;
-      h->imu_used_t[k] = m.t_s; h->imu_used_st[k] = m.st;
-      if (!h->imu_contig) { memcpy(&h->imu_used_acc[3 * k], &h->imu_acc[3 * (size_t)m.src], 3 * sizeof(double)); memcpy(&h->imu_used_gyr[3 * k], &h->imu_gyr[3 * (size_t)m.src], 3 * sizeof(double)); }
-      if (h->cells.empty() || h->cells.back().s_so3 != m.s_so3 || h->cells.back().s_r3 != m.s_r3 || h->cells.back().s_ba != m.s_ba || h->cells.back().s_bg != m.s_bg)
-        h->cells.push_back({m.s_so3, m.s_r3, m.s_ba, m.s_bg, idx, idx});
-      h->cells.back().i_end = idx + 1;
-    }
-  }
-  h->frames.clear(); h->used_uv.clear(); h->used_pid.clear();
-  h->frames.reserve(frame_sel.size());
-  bool consecutive = !frame_sel.empty();
-  for (size_t k = 1; k < frame_sel.size() && consecutive; ++k) consecutive = frame_sel[k] == frame_sel[k - 1] + 1;
-  h->used_contig = consecutive; h->used_c0 = 0; h->used_n = 0;
-  if (consecutive) {   // the usual case (all frames, or one contiguous shard): the corners are used in place, no host copy
-    const int cb = all_frames[frame_sel.front()].c0, ce = all_frames[frame_sel.back()].c1;
-    h->used_c0 = cb; h->used_n = ce - cb;
-    for (int fi : frame_sel) { FrameHost f = all_frames[fi]; f.c0 -= cb; f.c1 -= cb; h->frames.push_back(f); }
-  } else {
-    { icc_status es = ensure_host_corners(h); if (es != ICC_OK) return es; }
-    for (int fi : frame_sel) {
-      FrameHost f = all_frames[fi];
-      const int c0 = (int)h->used_pid.size();
-      for (int c = f.c0; c < f.c1; ++c) { h->used_pid.push_back(h->point_ids[c]); h->used_uv.push_back(h->uv[2 * c]); h->used_uv.push_back(h->uv[2 * c + 1]); }
-      f.c0 = c0; f.c1 = (int)h->used_pid.size();
-      h->frames.push_back(f);
-    }
-    h->used_n = (int)h->used_pid.size();
-  }
+  s = gather_corners(h, frames, frame_sel); if (s != ICC_OK) return s;
   trace.lap("batch_init: host assembly");
-  // gravity initialisation (imu_camera_calibrator.cc:130-161) incl. the integer-second truncation of the accelerometer time
-  auto view_of_time = [&](double t) { const size_t k = std::lower_bound(t_vis.begin(), t_vis.end(), t) - t_vis.begin(); return view_order[std::min(k, view_order.size() - 1)]; };
-  bool ginit = false; double g0[3] = {0.0, 0.0, 9.81};   // GRAVITY_MAGN (spline_trajectory_estimator.h:29) when never initialised
-  for (size_t j = 0; j < cam_ts.size() && !ginit; ++j) {
-    const int vi = view_of_time(cam_ts[j]);
-    const Pose Twc{qn(&h->q_wc[4 * vi]), v3(h->p_wc[3 * vi], h->p_wc[3 * vi + 1], h->p_wc[3 * vi + 2])};
-    const Pose Tai = pose_mul(Twc, Tci);
-    for (size_t i = 0; i < h->imu_t.size(); ++i) {
-      const int64_t accl_t = (int64_t)h->imu_t[i];
-      if (std::fabs(double(accl_t) - cam_ts[j]) < 1. / 30.) {
-        double a3[3];
-        if (h->imu_dev && h->imu_acc.size() != 3 * h->n_imu_in) { CU(cudaMemcpy(a3, h->d_acc_all.p + 3 * i, sizeof a3, cudaMemcpyDeviceToHost)); }   // one reading
-        else { a3[0] = h->imu_acc[3 * i]; a3[1] = h->imu_acc[3 * i + 1]; a3[2] = h->imu_acc[3 * i + 2]; }
-        const V3 g = qrot(Tai.q, v3(a3[0], a3[1], a3[2])); g0[0] = g.x; g0[1] = g.y; g0[2] = g.z; ginit = true; break; }
-    }
-  }
-  for (int d = 0; d < 3; ++d) h->glob[G_GRAV + d] = g0[d];
-
-  // ---- device upload ----------------------------------------------------------------------------------------------
+  s = init_gravity(h, views, Tci); if (s != ICC_OK) return s;
   DeviceProblem& P = h->P;
   memset(&P, 0, sizeof P);
   P.model = h->model; P.dispatch_fov = ipp->dispatch_fov; P.n_intr = h->n_intr;
   P.n_frames = (int)h->frames.size(); P.n_corners = h->used_n; P.rolling = ipp->init_line_delay_s != 0.0 ? 1 : 0;
-  if (!h->imu_lazy) h->n_imu_used = h->imu_used_t.size();
   P.n_imu = (int)h->n_imu_used; P.n_cells = (int)h->cells.size();
   P.dt_so3_ns = h->dt_so3_ns; P.dt_r3_ns = h->dt_r3_ns; P.dt_ba_ns = h->dt_ba_ns; P.dt_bg_ns = h->dt_bg_ns;
   P.inv_so3_dt = S_TO_NS / double(h->dt_so3_ns); P.inv_r3_dt = S_TO_NS / double(h->dt_r3_ns);
   P.w_acc = 1.0 / ipp->std_r3; P.w_gyr = 1.0 / ipp->std_so3;
-  P.n_so3 = nso3; P.n_r3 = nr3; P.n_ba = nba; P.n_bg = nbg;
+  P.n_so3 = n.so3; P.n_r3 = n.r3; P.n_ba = n.ba; P.n_bg = n.bg;
   P.n_res_vis = P.rolling ? 2 * P.n_corners : 0; P.n_res_acc = 3 * P.n_imu; P.n_res_gyr = 3 * P.n_imu;
+  const EvalStreams streams = eval_schedule(h);
   h->cur_flags = -1; h->ne_flags = -1; h->initialised = true; h->cur = 0; h->state_dirty_host = false; h->knots_dirty_host = false;
   if (h->device < 0) return ICC_OK;
-  CU(cudaSetDevice(h->device));
-  CU(cudaStreamSynchronize(h->stream));   // nothing may still read the staging arena of an earlier call
-  trace.lap("batch_init: gravity init");
-  h->arena.reset((size_t)(1 << 17) + 64 * (size_t)nf + 48 * (size_t)(nf + 4) + 16 * (size_t)(h->sm_count * 16 + 16) + 48 * (size_t)(nf + h->used_n / 32 + 64) + (96 + 40) * (h->cells.size() + (size_t)P.n_imu / 32 + 64)
-                 + 8 * 8 * (size_t)(nf + 8) + 2 * 40 * (size_t)(nso3 + nr3 + nba + nbg + 16) + 3 * (32 * (h->points.size() / 4 + 8) + 256) + 3 * (4 * (size_t)(nso3 + nr3 + nba + nbg) + 1024), true);
-  trace.lap("batch_init: pinned arena");
-  {
-    std::vector<double4> board(h->points.size() / 4);
-    // hnormalized(T^-1 X_h) of the functor (residuals.h:357-362) == T^-1 (X / w): the division is done once here
-    for (size_t i = 0; i < board.size(); ++i) { const double iw = 1.0 / h->points[4 * i + 3]; board[i] = make_double4(h->points[4 * i] * iw, h->points[4 * i + 1] * iw, h->points[4 * i + 2] * iw, 1.0); }
-    CU(upload_staged(h, h->d_board, board)); P.board = h->d_board.p;   // (the evaluation kernels read the copy that belongs to the state: DeviceState::board)
-    std::vector<int> off, s1, s2; std::vector<double> u1, u2;
-    for (const auto& f : h->frames) { off.push_back(f.c0); s1.push_back(f.s_so3); s2.push_back(f.s_r3); u1.push_back(f.u_so3); u2.push_back(f.u_r3); }
-    off.push_back(P.n_corners);
-    CU(upload_staged(h, h->d_f_off, off)); CU(upload_staged(h, h->d_f_s_so3, s1)); CU(upload_staged(h, h->d_f_s_r3, s2)); CU(upload_staged(h, h->d_f_u_so3, u1)); CU(upload_staged(h, h->d_f_u_r3, u2));
-    P.f_off = h->d_f_off.p; P.f_s_so3 = h->d_f_s_so3.p; P.f_s_r3 = h->d_f_s_r3.p; P.f_u_so3 = h->d_f_u_so3.p; P.f_u_r3 = h->d_f_u_r3.p;
-    const bool corners_in_place = h->frames_dev && h->used_contig;   // already on the device (set_frames): used where they lie
-    if (corners_in_place) { P.uv = h->d_uv_all.p + h->used_c0; P.pid = h->d_pid_all.p + h->used_c0; }
-    else { CU(h->d_uv.alloc(P.n_corners)); CU(h->d_pid.alloc(P.n_corners)); P.uv = h->d_uv.p; P.pid = h->d_pid.p; }   // (u, v) pairs are already laid out as double2
-    if (P.n_corners > 0 && !corners_in_place) {
-      const double* uv_src = h->used_contig ? h->uv.data() + 2 * (size_t)h->used_c0 : h->used_uv.data();
-      const int* pid_src = h->used_contig ? h->point_ids.data() + h->used_c0 : h->used_pid.data();
-      // page-locked sources (HostBuf): the DMA transfers run behind the rest of this function; kernels follow on the same stream
-      CU(cudaMemcpyAsync(h->d_uv.p, uv_src, (size_t)P.n_corners * sizeof(double2), cudaMemcpyHostToDevice, h->stream));
-      CU(cudaMemcpyAsync(h->d_pid.p, pid_src, (size_t)P.n_corners * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    }
-    // work lists: one warp per item; items sized so that the grid fills the GPU but every item amortises its tile flush
-    const int target_items = h->sm_count * 8;
-    auto round32 = [](long v) { return (int)((v + 31) / 32 * 32); };
-    const int per_v = std::max(32, round32(P.n_corners / std::max(1, target_items)));
-    std::vector<VisionWork> vw;
-    for (int fi = 0; fi < P.n_frames; ++fi) for (int c = h->frames[fi].c0; c < h->frames[fi].c1; c += per_v) vw.push_back({fi, c, std::min(c + per_v, h->frames[fi].c1), 0});
-    CU(upload_staged(h, h->d_vwork, vw)); P.vwork = h->d_vwork.p; P.n_vwork = (int)vw.size();
-    const int per_i = std::max(32, round32(P.n_imu / std::max(1, target_items)));
-    std::vector<ImuCell> iw;
-    for (const auto& c : h->cells) for (int i = c.i_begin; i < c.i_end; i += per_i) { ImuCell s = c; s.i_begin = i; s.i_end = std::min(i + per_i, c.i_end); iw.push_back(s); }
-    CU(upload_staged(h, h->d_iwork, iw)); P.iwork = h->d_iwork.p; P.n_iwork = (int)iw.size();
-    CU(upload_staged(h, h->d_cells, h->cells)); P.cells = h->d_cells.p;
-    {
-      // Schedule of the persistent evaluation kernel (icc_eval_tmem.cu).  Both streams -- the corners of the non-empty frames and
-      // the samples of the knot-interval cells, units padded to a multiple of 4 = one m8n8k4 k-step -- are walked with the kernel's own
-      // chunk rule (a chunk = up to 32 stream positions from at most two consecutive units) and cut into even per-warp runs.
-      struct Walk { std::vector<int> pos, unit; int total = 0; };
-      auto walk = [](const std::vector<int>& poff, int n_units) { Walk w; w.total = poff[n_units];
-        for (int pos = 0, u = 0; pos < w.total;) {
-          while (poff[u + 1] <= pos) ++u;
-          w.pos.push_back(pos); w.unit.push_back(u);
-          const int nA = std::min(32, poff[u + 1] - pos);
-          int n = nA;
-          if (nA < 32 && u + 1 < n_units) n += std::min(32 - nA, poff[u + 2] - poff[u + 1]);
-          pos += n;
-        }
-        return w; };
-      std::vector<VisFrame> vf; vf.reserve(h->frames.size() + 2);
-      std::vector<int> vpoff;
-      int poff = 0;
-      if (P.rolling) for (const auto& f : h->frames) {
-        const int cn = f.c1 - f.c0;
-        if (cn <= 0) continue;
-        vf.push_back({poff, f.c0, cn, f.s_so3, f.s_r3, 0, f.u_so3, f.u_r3}); vpoff.push_back(poff);
-        poff += (cn + 3) / 4 * 4;
-      }
-      const int nvf = (int)vf.size();
-      vf.push_back({poff, 0, 0, 0, 0, 0, 0.0, 0.0}); vf.push_back({poff, 0, 0, 0, 0, 0, 0.0, 0.0});   // sentinels [n], [n+1]
-      vpoff.push_back(poff); vpoff.push_back(poff);
-      std::vector<ImuCellP> ic; ic.reserve(h->cells.size() + 2);
-      std::vector<int> ipoff;
-      poff = 0;
-      for (const auto& c : h->cells) {
-        const int n = c.i_end - c.i_begin;
-        if (n <= 0) continue;
-        ic.push_back({poff, c.i_begin, n, c.s_so3, c.s_r3, c.s_ba, c.s_bg, 0}); ipoff.push_back(poff);
-        poff += (n + 3) / 4 * 4;
-      }
-      const int nic = (int)ic.size();
-      ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0}); ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0});
-      ipoff.push_back(poff); ipoff.push_back(poff);
-      const Walk wv = walk(vpoff, nvf), wi = walk(ipoff, nic);
-      const int nVc = (int)wv.pos.size(), nIc = (int)wi.pos.size();
-      int W = h->sm_count * eval_tmem_warps();
-      // ICC_TMEM_RUNS=n caps the runs at n (tests: every warp then owns several chunks and carries its tile state between them)
-      if (const char* e = getenv("ICC_TMEM_RUNS")) { const int n = atoi(e); if (n > 0) W = std::min(W, n); }
-      auto split = [W](const Walk& w) {      // even runs, one per warp
-        const int nc = (int)w.pos.size(), n_items = std::min(W, nc);
-        std::vector<VisItem> items((size_t)n_items);
-        for (int k = 0; k < n_items; ++k) {
-          const int a = (int)((int64_t)nc * k / n_items), b = (int)((int64_t)nc * (k + 1) / n_items);
-          items[(size_t)k] = {w.unit[a], w.pos[a], b < nc ? w.pos[b] : w.total, 0};
-        }
-        return items; };
-      h->vitems = split(wv); h->iitems = split(wi);
-      const std::vector<VisItem>& vi = h->vitems; const std::vector<VisItem>& ii = h->iitems;
-      const int n_iit = (int)ii.size();
-      P.n_vchunks = nVc; P.n_ichunks = nIc;
-      CU(upload_staged(h, h->d_vframes, vf)); P.vframes = h->d_vframes.p; P.n_vframes = nvf;
-      CU(upload_staged(h, h->d_vitems, vi)); P.vitems = h->d_vitems.p; P.n_vitems = (int)vi.size();
-      CU(upload_staged(h, h->d_icells, ic)); P.icells = h->d_icells.p; P.n_icells = nic;
-      CU(upload_staged(h, h->d_iitems, ii)); P.iitems = h->d_iitems.p; P.n_iitems = n_iit;
-    }
-    CU(h->d_imu_t.alloc(h->n_imu_used));
-    if (h->imu_lazy && h->n_imu_used) {   // sorted fast path: the raw stamps go up, the relative integer times are derived there
-      CU(h->d_imu_traw.alloc(h->n_imu_used));
-      CU(cudaMemcpyAsync(h->d_imu_traw.p, h->imu_t.data() + h->imu_src0, h->n_imu_used * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-      launch_imu_times((int)h->n_imu_used, h->d_imu_traw.p, ipp->time_offset_imu_to_cam_s, h->start_ns, h->d_imu_t.p, h->stream);
-    } else if (h->n_imu_used) CU(cudaMemcpyAsync(h->d_imu_t.p, h->imu_used_st.data(), h->n_imu_used * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
-    const bool imu_in_place = h->imu_dev && h->imu_contig;   // already on the device (set_imu): used where they lie
-    if (imu_in_place) { P.imu_acc = h->d_acc_all.p + 3 * (size_t)h->imu_src0; P.imu_gyr = h->d_gyr_all.p + 3 * (size_t)h->imu_src0; }
-    else { CU(h->d_imu_acc.alloc(3 * (size_t)P.n_imu)); CU(h->d_imu_gyr.alloc(3 * (size_t)P.n_imu)); P.imu_acc = h->d_imu_acc.p; P.imu_gyr = h->d_imu_gyr.p; }
-    if (P.n_imu > 0 && !imu_in_place) {
-      const double* a_src = h->imu_contig ? h->imu_acc.data() + 3 * (size_t)h->imu_src0 : h->imu_used_acc.data();
-      const double* g_src = h->imu_contig ? h->imu_gyr.data() + 3 * (size_t)h->imu_src0 : h->imu_used_gyr.data();
-      CU(cudaMemcpyAsync(h->d_imu_acc.p, a_src, 3 * (size_t)P.n_imu * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-      CU(cudaMemcpyAsync(h->d_imu_gyr.p, g_src, 3 * (size_t)P.n_imu * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    }
-    P.imu_t_ns = h->d_imu_t.p;
-  }
-  trace.lap("batch_init: problem upload");
-  icc_status s = upload_state(h, 0, true); if (s != ICC_OK) return s;
-  s = upload_state(h, 1, true); if (s != ICC_OK) return s;
-  trace.lap("batch_init: state upload");
-  {   // knots: BatchInitSO3R3VisPoses on the device, written into both state copies (the zero knots uploaded above only sized them)
-    std::vector<double> tv, qv, pv;
-    tv.reserve(view_order.size()); qv.reserve(4 * view_order.size()); pv.reserve(3 * view_order.size());
-    for (const int i : view_order) { tv.push_back(h->frame_t[i]); for (int d = 0; d < 4; ++d) qv.push_back(h->q_wc[4 * i + d]); for (int d = 0; d < 3; ++d) pv.push_back(h->p_wc[3 * i + d]); }
-    CU(upload_staged(h, h->d_view_t, tv)); CU(upload_staged(h, h->d_view_q, qv)); CU(upload_staged(h, h->d_view_p, pv));
-    const double Tci7[7] = {Tci.q.x, Tci.q.y, Tci.q.z, Tci.q.w, Tci.t.x, Tci.t.y, Tci.t.z};
-    launch_init_knots((int)tv.size(), h->d_view_t.p, h->d_view_q.p, h->d_view_p.p, Tci7, nso3, h->dt_so3_ns, nr3, h->dt_r3_ns,
-                      h->st[0].so3.p, h->st[1].so3.p, h->st[0].r3.p, h->st[1].r3.p, h->stream);
-    h->knots_dirty_host = true;     // the device holds the knots; the host mirror is refreshed on demand (getters / setters)
-  }
-  trace.lap("batch_init: knot init");
-  return ICC_OK;
+  return upload_problem(h, views, Tci, streams, trace);
 }
 
 icc_status icc_set_known_gravity_dir(icc_handle* h, const double g[3]) {

@@ -126,11 +126,22 @@ def test_host_assembly_general_paths_match_oracle(oracle_factory, case):
     assert np.allclose(o.get_gravity(), h.get_gravity(), rtol=0, atol=1e-14)
 
 
-@pytest.mark.parametrize("dts", [(0.05, 0.05), (0.04, 0.07), (0.09, 0.05)])
-def test_imu_cells_by_bisection_equal_the_sample_by_sample_pass(dts, monkeypatch):
-    """BatchInitSpline finds the knot-interval cells of a time-sorted IMU stream by galloping + bisection for the next interval boundary;
-    the sample-by-sample pass (forced with ICC_NO_BISECTION) is the reference statement: same cells, same kept samples -- for irregular
-    stamps, stamps exactly on knot boundaries of either spline and repeated stamps."""
+def calc_times_cells(ds, t_used):
+    """NumPy statement of CalcTimes' knot-interval cells (impl.h:763-788) of the kept samples t_used (offset-corrected, as imu_used()
+    returns them): st = int64((t + offset) 1e9) - int64(min(frame_t) 1e9), the segment indices st // dt of the SO(3), R^3 and both bias
+    splines (bias knots every 10 s), and cells = maximal runs of equal index tuples -> rows (s_so3, s_r3, s_acc_bias, s_gyr_bias, i_begin, i_end)."""
+    st = (np.asarray(t_used) * 1e9).astype(np.int64) - np.int64(np.min(ds["frame_t"]) * 1e9)
+    dts = (np.int64(ds["dt_so3_s"] * 1e9), np.int64(ds["dt_r3_s"] * 1e9), np.int64(10 * 10**9), np.int64(10 * 10**9))
+    seg = np.stack([st // dt for dt in dts], axis=1).reshape(-1, 4)
+    if len(seg) == 0:
+        return np.zeros((0, 6), dtype=np.int32)
+    bounds = np.concatenate([[0], np.flatnonzero(np.any(seg[1:] != seg[:-1], axis=1)) + 1, [len(seg)]])
+    return np.column_stack([seg[bounds[:-1]], bounds[:-1], bounds[1:]]).astype(np.int32)
+
+
+def _irregular_sorted_stream(dts):
+    """A time-sorted IMU stream at four times the rate with irregular stamps, stamps exactly on knot boundaries of either spline and
+    repeated stamps, reaching 0.2 s past the frames on both sides."""
     ds = dict(syn.make_dataset(syn.tiny_config(n_frames=40, dt_so3_s=dts[0], dt_r3_s=dts[1])))
     rng = np.random.default_rng(int(1000 * dts[0]))
     t0 = float(ds["frame_t"][0]) - ds["time_offset_imu_to_cam_s"]
@@ -140,15 +151,60 @@ def test_imu_cells_by_bisection_equal_the_sample_by_sample_pass(dts, monkeypatch
     k = np.arange(3, n, 11); t[k] = t0 + dts[1] * np.round((t[k] - t0) / dts[1])
     t = np.sort(t); t[5::13] = t[4::13][: len(t[5::13])]; t = np.sort(t)
     ds["imu_t"] = t; ds["accel"] = rng.normal(size=(n, 3)); ds["gyro"] = rng.normal(size=(n, 3))
-    out = {}
-    for mode in ("bisection", "sequential"):
-        if mode == "sequential": monkeypatch.setenv("ICC_NO_BISECTION", "1")
-        else: monkeypatch.delenv("ICC_NO_BISECTION", raising=False)
-        h = capi.CApi(calibrator.load_library(), "icc_", -1); capi.load_dataset(h, ds, known_gravity=False)
-        out[mode] = (h.imu_cells(), h.imu_used(), h.num_residuals()); h.close()
-    cb, ub, rb = out["bisection"]; cs, us, rs = out["sequential"]
-    assert rb == rs and len(cb) > 10
-    assert np.array_equal(cb, cs)
-    for a, b in zip(ub, us):
-        assert np.array_equal(a, b)
-    assert cb[0, 4] == 0 and cb[-1, 5] == len(ub[0]) and np.array_equal(cb[1:, 4], cb[:-1, 5])     # the cells tile the kept samples
+    return ds
+
+
+def _unsorted_copy(ds):
+    """The same stream with one more sample, far before the window, appended at its end: no longer sorted (the general selection),
+    same kept samples, still one contiguous run of the input."""
+    ds = dict(ds)
+    ds["imu_t"] = np.append(ds["imu_t"], ds["imu_t"][0] - 100.0)
+    ds["accel"] = np.vstack([ds["accel"], ds["accel"][:1]]); ds["gyro"] = np.vstack([ds["gyro"], ds["gyro"][:1]])
+    return ds
+
+
+def _host_assembly(ds, shard=None):
+    h = capi.CApi(calibrator.load_library(), "icc_", -1); capi.load_dataset(h, ds, known_gravity=False, shard=shard)
+    s = h.eval_schedule()
+    out = dict(used=h.imu_used(), cells=h.imu_cells(), res=h.num_residuals(),
+               schedule=(s["n_vchunks"], s["n_ichunks"], s["vitems"].tolist(), s["iitems"].tolist()))
+    h.close()
+    return out
+
+
+def _assert_same_assembly(a, b):
+    assert a["res"] == b["res"] and a["schedule"] == b["schedule"]
+    assert np.array_equal(a["cells"], b["cells"])
+    for x, y in zip(a["used"], b["used"]):
+        assert np.array_equal(x, y)
+
+
+@pytest.mark.parametrize("dts", [(0.05, 0.05), (0.04, 0.07), (0.09, 0.05)])
+def test_imu_cells_by_bisection_equal_calc_times_cells(dts):
+    """BatchInitSpline finds the knot-interval cells of a time-sorted IMU stream by galloping + bisection for the next interval boundary:
+    they are CalcTimes' cells of the kept samples, and the sample-by-sample selection of an unsorted copy keeps the same samples in the same
+    cells -- for irregular stamps, stamps exactly on knot boundaries of either spline and repeated stamps."""
+    ds = _irregular_sorted_stream(dts)
+    a, b = _host_assembly(ds), _host_assembly(_unsorted_copy(ds))
+    _assert_same_assembly(a, b)
+    cells, t_used = a["cells"], a["used"][0]
+    assert len(cells) > 10
+    assert np.array_equal(cells, calc_times_cells(ds, t_used))
+    assert cells[0, 4] == 0 and cells[-1, 5] == len(t_used) and np.array_equal(cells[1:, 4], cells[:-1, 5])     # the cells tile the kept samples
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 4])
+def test_sorted_and_general_selection_agree_on_every_shard(world):
+    """Every shard of a time-sorted stream (selected on counts) equals the same shard of the unsorted copy (time merge + shard rule):
+    kept samples, cells, residual counts and the persistent kernel's schedule; its cells are CalcTimes', and the shards tile the
+    one-shard selection."""
+    ds = _irregular_sorted_stream((0.04, 0.07))
+    full = _host_assembly(ds)
+    t_parts, res = [], np.zeros(3, dtype=int)
+    for rank in range(world):
+        a = _host_assembly(ds, shard=(rank, world))
+        _assert_same_assembly(a, _host_assembly(_unsorted_copy(ds), shard=(rank, world)))
+        assert np.array_equal(a["cells"], calc_times_cells(ds, a["used"][0]))
+        t_parts.append(a["used"][0]); res += np.array(a["res"])
+    assert np.array_equal(np.concatenate(t_parts), full["used"][0])
+    assert tuple(res) == full["res"]

@@ -7,8 +7,9 @@ re-stage when a unit ends exactly on a chunk boundary, runs that start or end in
 runs shorter than the longest.  The small parity cases give every warp one chunk, so ICC_TMEM_RUNS=n (read by batch_init) caps the
 run count here to put every one of those states on the path, and icc_get_eval_schedule shows which ones a case contains.
 
-  * CPU: a NumPy statement of the host walk + split and of the kernel's run loop, checked for consistency on ragged unit sizes;
-  * GPU: the library's schedule equals the statement; cost, residuals, J^T r and J^T J agree with the oracle for every camera model
+  * CPU: a NumPy statement of the host walk + split and of the kernel's run loop, checked for consistency on ragged unit sizes; the
+    library's schedule, which batch_init computes on a host-only handle too, equals the statement;
+  * GPU: the same on GPU handles; cost, residuals, J^T r and J^T J agree with the oracle for every camera model
     and the column sets of both stages -- including SPLINE | T_I_C | GRAVITY_DIR, the hot CLI's stage 1 with unknown gravity, whose
     gravity columns only the persistent IMU items carry -- on ragged frames, irregular IMU streams and at config-2 size."""
 import numpy as np
@@ -273,12 +274,29 @@ def _parity(oracle_factory, gpu_factory, tmem_runs, ds, caps, flag_sets, **kw):
 MATRIX_FLAGS = (F_STAGE1, F_GRAV1, capi.FLAG_SPLINE | capi.FLAG_GRAVITY_DIR, F_STAGE2, F_ALL, capi.FLAG_T_I_C)
 
 
+SCHEDULE_CAPS = (None, 1, 5, 6, 7, 13, 96)
+
+
+def _schedule_cases():
+    return [syn.make_dataset(syn.tiny_config(n_frames=30, dt_so3_s=0.04, dt_r3_s=0.07)), syn.make_dataset(syn.tiny_config(imu_rate_hz=1000.0, n_frames=20)),
+            _ragged_dataset()]
+
+
+def test_host_only_schedule_matches_the_statement(tmem_runs):
+    """The schedule is host logic: a host-only handle (whose default run count assumes 132 SMs) computes it without a GPU."""
+    from openimucameracalibrator_b200 import calibrator
+    for ds in _schedule_cases():
+        for cap in SCHEDULE_CAPS:
+            tmem_runs(cap)
+            h = capi.CApi(calibrator.load_library(), "icc_", -1); capi.load_dataset(h, ds)
+            checked_schedule(h, ds, cap)
+            h.close()
+
+
 @pytest.mark.gpu
 def test_schedule_matches_the_statement(gpu_factory, tmem_runs):
-    cases = [syn.make_dataset(syn.tiny_config(n_frames=30, dt_so3_s=0.04, dt_r3_s=0.07)), syn.make_dataset(syn.tiny_config(imu_rate_hz=1000.0, n_frames=20)),
-             _ragged_dataset()]
-    for ds in cases:
-        for cap in (None, 1, 5, 6, 7, 13, 96):
+    for ds in _schedule_cases():
+        for cap in SCHEDULE_CAPS:
             tmem_runs(cap)
             g = gpu_factory(); capi.load_dataset(g, ds)
             checked_schedule(g, ds, cap)
