@@ -21,6 +21,7 @@
 #include "../../include/icc_b200.h"
 #include "icc_allan_math.cuh"
 #include "icc_host.h"
+#include "icc_reduce.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -39,7 +40,7 @@ constexpr int kTile = 2048, kSpan = 1024, kGroup = 16;         // variance: k-va
 constexpr int kTilesPerSlice = 8, kSlice = kTile * kTilesPerSlice;
 constexpr int kGroupGrid = 1024;                               // grid.y: groups beyond it are a grid-stride loop
 constexpr int kSmemDoubles = 3 * kTile + 3 * kSpan;
-constexpr int kFitSums = 21;                                   // 15 (upper triangle of J^T J) + 5 (J^T r) + r^T r
+constexpr int kFitSums = normal_equation_sums(5);
 constexpr int kFitOut = 10;                                    // x[5], initial cost, final cost, iterations, termination, successful
 
 // the sample of channel c (0-2 accelerometer x, y, z as given; 3-5 gyroscope x, y, z pushed as rad/s, i.e. x * 57.3 * 3600)
@@ -119,8 +120,7 @@ __global__ void __launch_bounds__(kThreads) variance_kernel(VarArgs A) {
         if (k < e2) { const double w = (W2[i + 2 * d2] - 2 * W1[i + d2]) + a0; acc2 += w * w; }
       }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { acc1 += __shfl_down_sync(0xffffffffu, acc1, o); acc2 += __shfl_down_sync(0xffffffffu, acc2, o); }
+    acc1 = warp_sum(acc1); acc2 = warp_sum(acc2);
     if (lane == 0) {
       if (has1) A.partial[((size_t)c * A.F + f0 + warp) * A.nslice + s] = acc1;
       if (has2) A.partial[((size_t)c * A.F + f0 + warp + 8) * A.nslice + s] = acc2;
@@ -157,33 +157,9 @@ ICC_D void fit_normal_equations(const FitArgs& A, int c, const double* x, double
   for (int j = A.off[c] + threadIdx.x; j < A.off[c + 1]; j += blockDim.x) {
     double J[5];
     const double r = allan::residual(x, A.tau[j], A.l10s[j], J);
-    int q = 0;
-#pragma unroll
-    for (int a = 0; a < 5; ++a)
-#pragma unroll
-      for (int b = a; b < 5; ++b) s[q++] += J[a] * J[b];
-#pragma unroll
-    for (int a = 0; a < 5; ++a) s[15 + a] += J[a] * r;
-    s[20] += r * r;
+    normal_equation_row<5>(s, J, r);
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kFitSums; ++k) {
-    double v = s[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0) red[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < kFitSums) { double v = 0.0; for (int w = 0; w < nw; ++w) v += red[w][threadIdx.x]; tot[threadIdx.x] = v; }
-  __syncthreads();
-}
-
-ICC_D void unpack(const double* tot, double H[5][5], double b[5], double& cost) {
-  int q = 0;
-  for (int a = 0; a < 5; ++a) for (int c = a; c < 5; ++c) { H[a][c] = tot[q]; H[c][a] = tot[q]; ++q; }
-  for (int a = 0; a < 5; ++a) b[a] = tot[15 + a];
-  cost = 0.5 * tot[20];
+  block_sums<kFitSums>(s, red, tot);
 }
 
 // one CTA per channel: the reference's ceres::Solve (fitallan_gyr.cc:21-40) entirely on the device.  Thread 0 owns the minimiser
@@ -198,13 +174,13 @@ __global__ void __launch_bounds__(kThreads) fit_kernel(FitArgs A) {
   if (threadIdx.x < 5) x[threadIdx.x] = A.x0[c][threadIdx.x];
   __syncthreads();
   fit_normal_equations(A, c, x, red, tot);
-  if (threadIdx.x == 0) { double H[5][5], b[5], cost; unpack(tot, H, b, cost); allan::fit_start(F, A.x0[c], cost, H, b); }
+  if (threadIdx.x == 0) { double H[5][5], b[5], cost; unpack_normal_equations<5, 5>(tot, H, b, cost); allan::fit_start(F, A.x0[c], cost, H, b); }
   for (;;) {
     if (threadIdx.x == 0) { go = allan::fit_propose(F) ? 1 : 0; for (int p = 0; p < 5; ++p) x[p] = F.xc[p]; }
     __syncthreads();
     if (!go) break;
     fit_normal_equations(A, c, x, red, tot);
-    if (threadIdx.x == 0) { double H[5][5], b[5], cost; unpack(tot, H, b, cost); allan::fit_consider(F, cost, H, b); }
+    if (threadIdx.x == 0) { double H[5][5], b[5], cost; unpack_normal_equations<5, 5>(tot, H, b, cost); allan::fit_consider(F, cost, H, b); }
     __syncthreads();
   }
   if (threadIdx.x == 0) {

@@ -104,6 +104,8 @@ inline void init_value(const std::vector<double>& sigma2, const std::vector<doub
 }
 
 // Gauss-Newton system of the dogleg: (Hs + mu diag(d^2)) y = bs by Cholesky; false on a non-positive pivot or a non-finite y
+// Not chol_solve<5> (icc_small_linalg.cuh), which multiplies by the reciprocal pivot where this divides: the five-parameter fit is so
+// ill-conditioned that the last bit of the factor moves a parameter of a run that ends at the iteration limit by up to 1e-4 relative.
 ICC_HD bool gn_solve(const double Hs[5][5], const double bs[5], const double d[5], double mu, double y[5]) {
   double L[5][5];
   for (int j = 0; j < 5; ++j) {

@@ -19,6 +19,8 @@
 // The host only sequences these launches and applies Ceres' trust-region logic to eight scalars per iteration (calibrate_camera below).
 #include "icc_camera.cuh"
 #include "icc_host.h"
+#include "icc_reduce.cuh"
+#include "icc_small_linalg.cuh"
 #include "icc_trust_region.cuh"
 
 #include <chrono>
@@ -41,11 +43,6 @@ struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) 
 
 namespace {
 
-ICC_D double wsum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 ICC_HD int pk(int i, int j) { return i * CC_COLS - i * (i - 1) / 2 + (j - i); }   // packed upper triangle of the 17x17 block, i <= j
 ICC_HD int pk10(int a, int b) { return a * 10 - a * (a - 1) / 2 + (b - a); }       // packed upper triangle of the 10x10 reduced system
 
@@ -149,7 +146,7 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
       __syncwarp();
     }
   }
-  cost = wsum(cost); esum = wsum(esum);
+  cost = warp_sum(cost); esum = warp_sum(esum);
   if (JAC) {
     // fragment (bi, bj) of lane l holds entries (I, J), (I, J + 1) with I = 8 bi + l / 4, J = 8 bj + 2 (l % 4): keep the upper triangle
     int idx = 0;
@@ -187,12 +184,12 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
                                                            double* __restrict__ scale, int compute_scale, double radius, double mind, double maxd, double* __restrict__ scal) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
   const bool live = slot < Q.n_active && Q.pose_free;
-  double Yl[6][11];
+  double Yl[11][6];   // Yl[c] = column c of Y = A^-1 [H_pk | g_p]: one right-hand side of the 6x6 system each
   double Hpk[6][10];
 #pragma unroll
   for (int i = 0; i < 6; ++i) {
 #pragma unroll
-    for (int c = 0; c < 11; ++c) Yl[i][c] = 0.0;
+    for (int c = 0; c < 11; ++c) Yl[c][i] = 0.0;
 #pragma unroll
     for (int c = 0; c < 10; ++c) Hpk[i][c] = 0.0;
   }
@@ -205,58 +202,25 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
 #pragma unroll
       for (int j = 0; j < 6; ++j) if (j >= i) { A[j][i] = B[pk(i, j)]; }
 #pragma unroll
-      for (int c = 0; c < 10; ++c) { Hpk[i][c] = B[pk(i, 6 + c)]; Yl[i][c] = Hpk[i][c]; }
-      Yl[i][10] = B[pk(i, 16)];
-      gmax = fmax(gmax, fabs(Yl[i][10]));
+      for (int c = 0; c < 10; ++c) { Hpk[i][c] = B[pk(i, 6 + c)]; Yl[c][i] = Hpk[i][c]; }
+      Yl[10][i] = B[pk(i, 16)];
+      gmax = fmax(gmax, fabs(Yl[10][i]));
     }
-    bool ok = true;
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
       double s = compute_scale ? 1.0 / (1.0 + sqrt(A[i][i])) : scale[6 * slot + i];
       if (compute_scale) scale[6 * slot + i] = s;
       A[i][i] += lm_damping(A[i][i], s, radius, mind, maxd);
     }
-    // in-place Cholesky (lower), then forward / backward substitution of the 11 right-hand sides
+    const bool ok = chol_factor<6>(A);
 #pragma unroll
-    for (int j = 0; j < 6; ++j) {
-      double dj = A[j][j];
-#pragma unroll
-      for (int m = 0; m < 6; ++m) if (m < j) dj -= A[j][m] * A[j][m];
-      if (!(dj > 0.0)) { ok = false; dj = 1.0; }
-      const double l = sqrt(dj), il = 1.0 / l;
-      A[j][j] = l;
-#pragma unroll
-      for (int i = 0; i < 6; ++i) if (i > j) {
-        double s = A[i][j];
-#pragma unroll
-        for (int m = 0; m < 6; ++m) if (m < j) s -= A[i][m] * A[j][m];
-        A[i][j] = s * il;
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < 11; ++c) {
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        double s = Yl[i][c];
-#pragma unroll
-        for (int m = 0; m < 6; ++m) if (m < i) s -= A[i][m] * Yl[m][c];
-        Yl[i][c] = s / A[i][i];
-      }
-#pragma unroll
-      for (int ii = 0; ii < 6; ++ii) {
-        const int i = 5 - ii;
-        double s = Yl[i][c];
-#pragma unroll
-        for (int m = 0; m < 6; ++m) if (m > i) s -= A[m][i] * Yl[m][c];
-        Yl[i][c] = s / A[i][i];
-      }
-    }
+    for (int c = 0; c < 11; ++c) chol_substitute<6>(A, Yl[c]);
     if (!ok) atomicAdd(&scal[CC_FAIL], 1.0);
     double* Yo = Y + (size_t)slot * CC_Y;
 #pragma unroll
     for (int i = 0; i < 6; ++i)
 #pragma unroll
-      for (int c = 0; c < 11; ++c) Yo[i * 11 + c] = Yl[i][c];
+      for (int c = 0; c < 11; ++c) Yo[i * 11 + c] = Yl[c][i];
   } else if (slot < Q.n_active) {
     double* Yo = Y + (size_t)slot * CC_Y;
     for (int i = 0; i < CC_Y; ++i) Yo[i] = 0.0;
@@ -272,7 +236,7 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
       for (int b = 0; b < 11; ++b) if (b >= a) {
         double sacc = 0.0;
 #pragma unroll
-        for (int i = 0; i < 6; ++i) sacc -= Hpk[i][a] * Yl[i][b];
+        for (int i = 0; i < 6; ++i) sacc -= Hpk[i][a] * Yl[b][i];
         part[o][threadIdx.x] = sacc;
         ++o;
       }
@@ -287,8 +251,7 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
     const int b = a + r;
     if (sacc != 0.0) atomicAdd(&red[b < 10 ? pk10(a, b) : 55 + a], sacc);
   }
-  gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, 16)); gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, 8));
-  gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, 4)); gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, 2)); gmax = fmax(gmax, __shfl_xor_sync(0xffffffffu, gmax, 1));
+  gmax = warp_max(gmax);
   if (lane == 0 && gmax > 0.0) atomic_max_nonneg(&scal[CC_GRAD_MAX], gmax);
 }
 
@@ -296,7 +259,6 @@ __global__ void camcal_solve_kernel(CamCalProblem Q, CamCalState cur, CamCalStat
                                     double* __restrict__ scale_k, int compute_scale, double radius, double mind, double maxd, double* __restrict__ dk, double* __restrict__ scal) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   double A[10][10], b[10], D[10], g[10];
-  bool ok = true;
   double gmax = 0.0;
   for (int a = 0; a < 10; ++a) {
     const bool act = (Q.intr_mask >> a) & 1u;
@@ -313,16 +275,7 @@ __global__ void camcal_solve_kernel(CamCalProblem Q, CamCalState cur, CamCalStat
     } else { D[a] = 0.0; b[a] = 0.0; }
   }
   for (int a = 0; a < 10; ++a) if (!((Q.intr_mask >> a) & 1u)) { for (int c = 0; c < 10; ++c) { A[a][c] = 0.0; A[c][a] = 0.0; } A[a][a] = 1.0; }
-  for (int j = 0; j < 10; ++j) {
-    double dj = A[j][j];
-    for (int m = 0; m < j; ++m) dj -= A[j][m] * A[j][m];
-    if (!(dj > 0.0)) { ok = false; dj = 1.0; }
-    const double l = sqrt(dj);
-    A[j][j] = l;
-    for (int i = j + 1; i < 10; ++i) { double s = A[i][j]; for (int m = 0; m < j; ++m) s -= A[i][m] * A[j][m]; A[i][j] = s / l; }
-  }
-  for (int i = 0; i < 10; ++i) { double s = b[i]; for (int m = 0; m < i; ++m) s -= A[i][m] * b[m]; b[i] = s / A[i][i]; }
-  for (int i = 9; i >= 0; --i) { double s = b[i]; for (int m = i + 1; m < 10; ++m) s -= A[m][i] * b[m]; b[i] = s / A[i][i]; }
+  const bool ok = chol_solve<10>(A, b);
   double gd = 0.0, dd = 0.0, st = 0.0, xs = 0.0;
   for (int a = 0; a < 10; ++a) {
     dk[a] = b[a]; cand.k[a] = cur.k[a] + b[a];
@@ -363,7 +316,7 @@ __global__ void __launch_bounds__(128) camcal_update_kernel(CamCalProblem Q, Cam
     cand.c[3 * v] = c.x + dp[3]; cand.c[3 * v + 1] = c.y + dp[4]; cand.c[3 * v + 2] = c.z + dp[5];
     xs = 1.0 + dot(c, c);
   }
-  gd = wsum(gd); dd = wsum(dd); st = wsum(st); xs = wsum(xs);
+  gd = warp_sum(gd); dd = warp_sum(dd); st = warp_sum(st); xs = warp_sum(xs);
   if (lane == 0) { atomicAdd(&scal[CC_G_DELTA], gd); atomicAdd(&scal[CC_D_DELTA], dd); atomicAdd(&scal[CC_STEP_SQ], st); atomicAdd(&scal[CC_X_SQ], xs); }
 }
 

@@ -19,6 +19,7 @@
 // banded+bordered normal-equation buffer in HBM/L2.
 #include "icc_camera.cuh"
 #include "icc_kernels.h"
+#include "icc_reduce.cuh"
 #include "icc_spline_chain.cuh"
 
 #include <atomic>
@@ -91,12 +92,6 @@ ICC_D void flush_tile(const DeviceProblem& P, const int* gidx, int ncols, int re
       }
       ++idx;
     }
-}
-
-ICC_D double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
 }
 
 // Stage the SO(3) window (6 knots -> 5 log increments and their Jr^-1) for one work item.

@@ -20,6 +20,7 @@
 #include "icc_bearing_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
+#include "icc_reduce.cuh"
 #include "icc_small_linalg.cuh"
 
 #include <cmath>
@@ -28,12 +29,6 @@
 namespace icc {
 
 namespace {
-
-ICC_D double wsum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 struct Intr { double k[10]; };
 
@@ -89,14 +84,14 @@ ICC_D void pose_system(const PoseProblem& Q, const double2* xy, const unsigned c
       for (int j = 0; j <= i; ++j) { H[idx] += w * (J0[i] * J0[j] + J1[i] * J1[j]); ++idx; }
     }
   }
-  S.cost = wsum(cost);
+  S.cost = warp_sum(cost);
   if (!with_jacobian) return;
   int idx = 0;
 #pragma unroll
   for (int i = 0; i < 6; ++i) {
-    S.g[i] = wsum(g[i]);
+    S.g[i] = warp_sum(g[i]);
 #pragma unroll
-    for (int j = 0; j <= i; ++j) { const double v = wsum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
+    for (int j = 0; j <= i; ++j) { const double v = warp_sum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
   }
 }
 
@@ -130,14 +125,14 @@ ICC_D void pose_system(const PoseProblem& Q, const double4* bear, const unsigned
       for (int j = 0; j <= i; ++j) { H[idx] += w * (J0[i] * J0[j] + J1[i] * J1[j]); ++idx; }
     }
   }
-  S.cost = wsum(cost);
+  S.cost = warp_sum(cost);
   if (!with_jacobian) return;
   int idx = 0;
 #pragma unroll
   for (int i = 0; i < 6; ++i) {
-    S.g[i] = wsum(g[i]);
+    S.g[i] = warp_sum(g[i]);
 #pragma unroll
-    for (int j = 0; j <= i; ++j) { const double v = wsum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
+    for (int j = 0; j <= i; ++j) { const double v = warp_sum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
   }
 }
 
@@ -194,7 +189,7 @@ ICC_D bool board_homography(const PoseProblem& Q, const double2* __restrict__ xy
     const double4 Xb = Q.board[id];
     n += 1.0; sX += Xb.x / Xb.w; sY += Xb.y / Xb.w; sZ += Xb.z / Xb.w; sx += xy[c].x; sy += xy[c].y;
   }
-  n = wsum(n); sX = wsum(sX); sY = wsum(sY); sZ = wsum(sZ); sx = wsum(sx); sy = wsum(sy);
+  n = warp_sum(n); sX = warp_sum(sX); sY = warp_sum(sY); sZ = warp_sum(sZ); sx = warp_sum(sx); sy = warp_sum(sy);
   __syncwarp();
   n_out = n;
   if (c1 - c0 < Q.min_points || n < 6.0) return false;   // pose_estimator.cc:140 (all corners counted), :65
@@ -207,7 +202,7 @@ ICC_D bool board_homography(const PoseProblem& Q, const double2* __restrict__ xy
     const double X = Xb.x / Xb.w - mX, Y = Xb.y / Xb.w - mY, x = xy[c].x - mx, y = xy[c].y - my;
     dB += sqrt(X * X + Y * Y); dI += sqrt(x * x + y * y); dz = fmax(dz, fabs(Xb.z / Xb.w - zref));
   }
-  dB = wsum(dB) / n; dI = wsum(dI) / n;
+  dB = warp_sum(dB) / n; dI = warp_sum(dI) / n;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) dz = fmax(dz, __shfl_xor_sync(0xffffffffu, dz, o));
   if (!(dB > 0.0) || !(dI > 0.0) || dz > 0.05 * dB) return false;   // degenerate, or too far from a plane for the homography to start the refinement
@@ -237,9 +232,9 @@ ICC_D bool board_homography(const PoseProblem& Q, const double2* __restrict__ xy
     int idx = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      h[i] = wsum(v8[i]);
+      h[i] = warp_sum(v8[i]);
 #pragma unroll
-      for (int j = 0; j <= i; ++j) { const double v = wsum(M[idx]); A8[i][j] = v; A8[j][i] = v; ++idx; }
+      for (int j = 0; j <= i; ++j) { const double v = warp_sum(M[idx]); A8[i][j] = v; A8[j][i] = v; ++idx; }
     }
   }
   if (!chol_solve<8>(A8, h)) return false;
@@ -275,7 +270,7 @@ ICC_D bool bearing_start(const PoseProblem& Q, const double4* bear, const int* o
     const int id = Q.pid[c];
     if (okc[c] != 0 && id >= 0 && id < Q.n_points) m = m + v3(bear[c].x, bear[c].y, bear[c].z);
   }
-  m = v3(wsum(m.x), wsum(m.y), wsum(m.z));
+  m = v3(warp_sum(m.x), warp_sum(m.y), warp_sum(m.z));
   const double mn = sqrt(dot(m, m));
   m = mn > 0.0 ? (1.0 / mn) * m : v3(0.0, 0.0, 1.0);
   V3 e1, e2; tangent_basis(m, e1, e2);
@@ -325,7 +320,7 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
       use[c] = u ? 1 : 0;
       if (u) n += 1.0;
     }
-    n = wsum(n);
+    n = warp_sum(n);
     __syncwarp();
     if (c1 - c0 < Q.min_points || n < 6.0) { fail(); return; }
     const Q4 qw = qnormalized(q4(q_out[4 * f], q_out[4 * f + 1], q_out[4 * f + 2], q_out[4 * f + 3]));
@@ -366,7 +361,7 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
     }
     if (in) n_in += 1.0; else { n_out += 1.0; use[c] = 0; }
   }
-  n_in = wsum(n_in); n_out = wsum(n_out);
+  n_in = warp_sum(n_in); n_out = warp_sum(n_out);
   __syncwarp();
   if (n_in < 6.0) { fail(); return; }
   if (n_out > 0.0) pose_refine(Q, xy, use, c0, c1, zref, q, t);
@@ -385,7 +380,7 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
       e += sqrt(r0 * r0 + r1e * r1e);
     }
   }
-  e = wsum(e) / n_in;
+  e = warp_sum(e) / n_in;
   if (lane == 0) {
     // undo the plane shift: Pc = R (X - zref e_z) + t  =>  t_full = t - zref R e_z ; camera centre p_wc = -R^T t_full ; q_wc = q^*
     const V3 tf = t - zref * qrot(q, v3(0.0, 0.0, 1.0));
@@ -469,11 +464,11 @@ ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear,
     H[0] += wgt * (j0.x * j0.x + j1.x * j1.x); H[1] += wgt * (j0.x * j0.y + j1.x * j1.y); H[2] += wgt * (j0.x * j0.z + j1.x * j1.z);
     H[3] += wgt * (j0.y * j0.y + j1.y * j1.y); H[4] += wgt * (j0.y * j0.z + j1.y * j1.z); H[5] += wgt * (j0.z * j0.z + j1.z * j1.z);
   }
-  S.cost = wsum(cost);
+  S.cost = warp_sum(cost);
   if (!with_jacobian) return;
 #pragma unroll
-  for (int i = 0; i < 3; ++i) S.g[i] = wsum(g[i]);
-  const double h0 = wsum(H[0]), h1 = wsum(H[1]), h2 = wsum(H[2]), h3 = wsum(H[3]), h4 = wsum(H[4]), h5 = wsum(H[5]);
+  for (int i = 0; i < 3; ++i) S.g[i] = warp_sum(g[i]);
+  const double h0 = warp_sum(H[0]), h1 = warp_sum(H[1]), h2 = warp_sum(H[2]), h3 = warp_sum(H[3]), h4 = warp_sum(H[4]), h5 = warp_sum(H[5]);
   S.H[0][0] = h0; S.H[0][1] = h1; S.H[0][2] = h2; S.H[1][0] = h1; S.H[1][1] = h3; S.H[1][2] = h4; S.H[2][0] = h2; S.H[2][1] = h4; S.H[2][2] = h5;
 }
 

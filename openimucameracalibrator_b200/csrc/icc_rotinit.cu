@@ -17,6 +17,7 @@
 // and reads the result once at the end.
 #include "icc_device_math.cuh"
 #include "icc_host.h"
+#include "icc_reduce.cuh"
 
 #include "icc_rotinit_math.cuh"
 
@@ -99,14 +100,13 @@ __global__ void smooth_kernel(int n, const double* __restrict__ x, double* __res
 // ---- golden-section state on the device -------------------------------------------------------------------------------------
 // sums[c][0..2] = sum vis, [3..5] = sum imu, [6..14] = sum imu_a vis_b (row a, column b), [15] = robust error
 ICC_D double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   __syncthreads();
   if (lane == 0) red[warp] = v;
   __syncthreads();
   double t = 0.0;
-  if (warp == 0) { t = lane < nw ? red[lane] : 0.0; for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o); }
+  if (warp == 0) t = warp_sum(lane < nw ? red[lane] : 0.0);
   return t;                                        // valid in warp 0
 }
 

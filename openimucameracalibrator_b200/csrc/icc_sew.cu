@@ -13,6 +13,7 @@
 // arithmetic n^2 mod 2N), batched over the three axes; the spectrum stays in HBM and each quality evaluation of the root search
 // is one fused response + energy reduction over the N bins.  The scalar root search (a dozen evaluations) runs on the host.
 #include "icc_host.h"
+#include "icc_reduce.cuh"
 
 #include <cmath>
 #include <functional>
@@ -79,7 +80,7 @@ __global__ void spectrum_kernel(int N, int M, const cplx* __restrict__ c /* 3 x 
     const double xh = k == 0 ? 0.0 : sqrt(1.0 / 3.0) * sqrt(s2);
     xhat[k] = xh; e = xh * xh;
   }
-  for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+  e = warp_sum(e);   // one sum: thread 0 adds the warps in order behind a single barrier, where block_sums<1> would take two
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = e;
   __syncthreads();
   if (threadIdx.x == 0) { double t = 0.0; for (int w2 = 0; w2 < (blockDim.x >> 5); ++w2) t += red[w2]; atomicAdd(energy_sum, t); }
@@ -98,7 +99,7 @@ __global__ void residual_energy_kernel(int N, const double* __restrict__ xhat, d
     const double v = (1.0 - H) * xhat[k];
     e += v * v;
   }
-  for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+  e = warp_sum(e);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = e;
   __syncthreads();
   if (threadIdx.x == 0) { double t = 0.0; for (int w2 = 0; w2 < (blockDim.x >> 5); ++w2) t += red[w2]; atomicAdd(out, t); }
@@ -165,17 +166,9 @@ __global__ void __launch_bounds__(256) imu_sums_kernel(int n, const double* __re
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     s[0] += acc[3 * i]; s[1] += acc[3 * i + 1]; s[2] += acc[3 * i + 2]; s[3] += gyr[3 * i]; s[4] += gyr[3 * i + 1]; s[5] += gyr[3 * i + 2];
   }
-  __shared__ double sh[8][6];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    double v = s[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) sh[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) { double v = 0.0; for (int w = 0; w < 8; ++w) v += sh[w][threadIdx.x]; atomicAdd(&out[threadIdx.x], v); }
+  __shared__ double red[8][6], tot[6];
+  block_sums<6>(s, red, tot);
+  if (threadIdx.x < 6) atomicAdd(&out[threadIdx.x], tot[threadIdx.x]);
 }
 }  // namespace
 

@@ -1,13 +1,15 @@
-// Small dense linear algebra that runs per lane in the pose / board-point kernels (icc_pose.cu): kept __host__ __device__ in a header so that
+// Small dense linear algebra that runs per thread: the one Cholesky of the pose / board-point, camera calibration and static IMU
+// kernels, and the matrix-to-quaternion rule of the pose kernels.  Kept __host__ __device__ in a header so that
 // tests/test_host_device_math.py can compile exactly this code for the CPU.
 #pragma once
 #include "icc_device_math.cuh"
 
 namespace icc {
 
-// Cholesky solve of the symmetric positive definite N x N system (A lower triangle used), in registers; false if not SPD
+// In-place Cholesky factor (lower triangle) of the symmetric N x N matrix A, in registers.  A non-positive pivot is replaced by 1, the
+// factorisation runs to the end (finite entries) and false is returned: the matrix was not positive definite.
 template <int N>
-ICC_HD bool chol_solve(double (&A)[N][N], double (&b)[N]) {
+ICC_HD bool chol_factor(double (&A)[N][N]) {
   bool ok = true;
 #pragma unroll
   for (int j = 0; j < N; ++j) {
@@ -27,6 +29,12 @@ ICC_HD bool chol_solve(double (&A)[N][N], double (&b)[N]) {
       }
     }
   }
+  return ok;
+}
+
+// b <- A^-1 b by forward and backward substitution with the factor chol_factor left in A
+template <int N>
+ICC_HD void chol_substitute(const double (&A)[N][N], double (&b)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) {
     double s = b[i];
@@ -42,6 +50,13 @@ ICC_HD bool chol_solve(double (&A)[N][N], double (&b)[N]) {
     for (int k = 0; k < N; ++k) if (k > i) s -= A[k][i] * b[k];
     b[i] = s / A[i][i];
   }
+}
+
+// Cholesky solve of the symmetric positive definite N x N system (A lower triangle used); false if not SPD
+template <int N>
+ICC_HD bool chol_solve(double (&A)[N][N], double (&b)[N]) {
+  const bool ok = chol_factor<N>(A);
+  chol_substitute<N>(A, b);
   return ok;
 }
 

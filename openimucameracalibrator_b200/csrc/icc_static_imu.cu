@@ -19,6 +19,7 @@
 #include "../../include/icc_b200.h"
 #include "icc_device_math.cuh"
 #include "icc_host.h"
+#include "icc_reduce.cuh"
 #include "icc_static_imu_math.cuh"
 
 #include <algorithm>
@@ -206,7 +207,7 @@ struct AccFitArgs {
   TrOptions o;
   double* out;             // per multiplier: x[9], initial cost, final cost, iterations, termination, successful steps
 };
-constexpr int kAccOut = 14, kSums = 55;   // 45 (upper triangle of J^T J) + 9 (J^T r) + cost
+constexpr int kAccOut = 14, kSums = normal_equation_sums(9);
 
 // cost, J^T J, J^T r of one multiplier's problem at x, reduced over the block in a fixed order; valid in thread 0
 ICC_D void acc_normal_equations(const AccFitArgs& A, int m, const double* x, double (*red)[kSums], double* tot) {
@@ -221,33 +222,9 @@ ICC_D void acc_normal_equations(const AccFitArgs& A, int m, const double* x, dou
     else { const size_t q = (size_t)A.kept[k0 + j / A.ns].x + j % A.ns; a[0] = A.acc[3 * q]; a[1] = A.acc[3 * q + 1]; a[2] = A.acc[3 * q + 2]; }
     double J[9];
     const double r = simu::acc_residual(x, a, A.g_mag, J);
-    int c = 0;
-#pragma unroll
-    for (int p = 0; p < 9; ++p)
-#pragma unroll
-      for (int q = p; q < 9; ++q) s[c++] += J[p] * J[q];
-#pragma unroll
-    for (int p = 0; p < 9; ++p) s[45 + p] += J[p] * r;
-    s[54] += r * r;
+    normal_equation_row<9>(s, J, r);
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kSums; ++k) {
-    double v = s[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0) red[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < kSums) { double v = 0.0; for (int w = 0; w < nw; ++w) v += red[w][threadIdx.x]; tot[threadIdx.x] = v; }
-  __syncthreads();
-}
-
-ICC_D void unpack(const double* tot, double H[12][12], double g[12], double& cost) {
-  int c = 0;
-  for (int p = 0; p < 12; ++p) { g[p] = p < 9 ? tot[45 + p] : 0.0; for (int q = 0; q < 12; ++q) H[p][q] = 0.0; }
-  for (int p = 0; p < 9; ++p) for (int q = p; q < 9; ++q) { H[p][q] = tot[c]; H[q][p] = tot[c]; ++c; }
-  cost = 0.5 * tot[54];
+  block_sums<kSums>(s, red, tot);
 }
 
 // one CTA per threshold multiplier: CalibrateAcc's ceres::Solve (static_imu_calibrator.cc:113-130) entirely on the device
@@ -263,7 +240,7 @@ __global__ void __launch_bounds__(kThreads) acc_fit_kernel(AccFitArgs A) {
   __syncthreads();
   acc_normal_equations(A, m, x, red, tot);
   if (threadIdx.x == 0) {
-    double H[12][12], g[12], c; unpack(tot, H, g, c);
+    double H[12][12], g[12], c; unpack_normal_equations<9, 12>(tot, H, g, c);
     simu::lm_start(L, A.o, 9, x, c, H, g);
   }
   for (;;) {
@@ -271,7 +248,7 @@ __global__ void __launch_bounds__(kThreads) acc_fit_kernel(AccFitArgs A) {
     __syncthreads();
     if (!go) break;
     acc_normal_equations(A, m, x, red, tot);
-    if (threadIdx.x == 0) { double H[12][12], g[12], c; unpack(tot, H, g, c); simu::lm_consider(L, c, H, g); }
+    if (threadIdx.x == 0) { double H[12][12], g[12], c; unpack_normal_equations<9, 12>(tot, H, g, c); simu::lm_consider(L, c, H, g); }
     __syncthreads();
   }
   if (threadIdx.x == 0) {

@@ -15,6 +15,7 @@
 // multiplication.
 #pragma once
 #include "icc_device_math.cuh"
+#include "icc_small_linalg.cuh"
 #include "icc_trust_region.cuh"
 
 namespace icc {
@@ -196,19 +197,7 @@ ICC_HD bool lm_propose(LmState& L) {
     // LM diagonal, clamped; Ceres reuses it after a failed step, which is the same value: H and the scaling have not changed
     double M[12][12];
     for (int i = 0; i < 12; ++i) for (int j = 0; j < 12; ++j) M[i][j] = A[i][j] + ((i == j && i < n) ? fmin(fmax(A[i][i], T.o.min_diagonal), T.o.max_diagonal) / T.radius : 0.0);
-    bool ok = true;
-    {   // Cholesky solve M y = -gs
-      for (int j = 0; j < 12; ++j) {
-        double d = M[j][j];
-        for (int k = 0; k < j; ++k) d -= M[j][k] * M[j][k];
-        if (!(d > 0.0)) { ok = false; d = 1.0; }
-        const double l = ::sqrt(d);
-        M[j][j] = l;
-        for (int i = j + 1; i < 12; ++i) { double s = M[i][j]; for (int k = 0; k < j; ++k) s -= M[i][k] * M[j][k]; M[i][j] = s / l; }
-      }
-      for (int i = 0; i < 12; ++i) { double s = y[i]; for (int k = 0; k < i; ++k) s -= M[i][k] * y[k]; y[i] = s / M[i][i]; }
-      for (int i = 11; i >= 0; --i) { double s = y[i]; for (int k = i + 1; k < 12; ++k) s -= M[k][i] * y[k]; y[i] = s / M[i][i]; }
-    }
+    const bool ok = chol_solve<12>(M, y);   // M y = -gs
     double yg = 0.0, yHy = 0.0;
     for (int i = 0; i < n; ++i) { double s = 0.0; for (int j = 0; j < n; ++j) s += A[i][j] * y[j]; Hs_y[i] = s; }
     for (int i = 0; i < n; ++i) { yg += y[i] * gs[i]; yHy += y[i] * Hs_y[i]; }

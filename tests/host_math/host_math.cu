@@ -20,6 +20,18 @@ template <int N> static int chol_n(const double* A_in, double* b_io) {
   for (int i = 0; i < N; ++i) b_io[i] = b[i];
   return ok ? 1 : 0;
 }
+// one factorisation, nrhs right-hand sides (row-major nrhs x N), substituted one after the other
+template <int N> static int chol_multi_n(const double* A_in, int nrhs, double* B_io) {
+  double A[N][N], b[N];
+  for (int i = 0; i < N; ++i) for (int j = 0; j < N; ++j) A[i][j] = A_in[N * i + j];
+  const bool ok = chol_factor<N>(A);
+  for (int r = 0; r < nrhs; ++r) {
+    for (int i = 0; i < N; ++i) b[i] = B_io[N * r + i];
+    chol_substitute<N>(A, b);
+    for (int i = 0; i < N; ++i) B_io[N * r + i] = b[i];
+  }
+  return ok ? 1 : 0;
+}
 }  // namespace
 
 extern "C" {
@@ -122,8 +134,20 @@ void hm_eig4_max(const double* A16, double* q4out) {
   eig4_max(A, q);
   for (int i = 0; i < 4; ++i) q4out[i] = q[i];
 }
-// ---- small dense linear algebra of the pose / board-point kernels (icc_small_linalg.cuh) ----------------------------------------------
-int hm_chol_solve(int n, const double* A, double* b) { return n == 3 ? chol_n<3>(A, b) : n == 6 ? chol_n<6>(A, b) : n == 8 ? chol_n<8>(A, b) : -1; }
+// ---- small dense linear algebra of the upstream kernels (icc_small_linalg.cuh), at every size they instantiate -------------------------
+int hm_chol_solve(int n, const double* A, double* b) {
+  switch (n) {
+    case 3: return chol_n<3>(A, b); case 6: return chol_n<6>(A, b); case 8: return chol_n<8>(A, b);
+    case 10: return chol_n<10>(A, b); case 12: return chol_n<12>(A, b); default: return -1;
+  }
+}
+int hm_chol_factor_substitute(int n, const double* A, int nrhs, double* B) {
+  switch (n) {
+    case 3: return chol_multi_n<3>(A, nrhs, B); case 6: return chol_multi_n<6>(A, nrhs, B);
+    case 8: return chol_multi_n<8>(A, nrhs, B); case 10: return chol_multi_n<10>(A, nrhs, B); case 12: return chol_multi_n<12>(A, nrhs, B);
+    default: return -1;
+  }
+}
 void hm_quat_from_columns(const double* R9 /* row-major */, double* q) {
   const Q4 r = quat_from_columns(v3(R9[0], R9[3], R9[6]), v3(R9[1], R9[4], R9[7]), v3(R9[2], R9[5], R9[8]));
   q[0] = r.x; q[1] = r.y; q[2] = r.z; q[3] = r.w;

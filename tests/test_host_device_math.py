@@ -392,11 +392,14 @@ def test_device_dominant_eigenvector_of_horns_matrix(hm):
         assert abs(q @ N @ q - w[-1]) < 1e-10 * max(1.0, abs(w[-1]))
 
 
-# ---- small dense linear algebra of the pose / board-point kernels ---------------------------------------------------------------------
-@pytest.mark.parametrize("n", [3, 6, 8])
+# ---- small dense linear algebra of the upstream kernels -------------------------------------------------------------------------------
+CHOL_SIZES = [3, 6, 8, 10, 12]
+
+
+@pytest.mark.parametrize("n", CHOL_SIZES)
 def test_device_cholesky_solve(hm, n):
-    """chol_solve<N> (3x3 point systems, 6x6 pose systems, 8x8 homography normal equations) against numpy.linalg.solve; an indefinite
-    matrix is reported instead of producing NaNs."""
+    """chol_solve<N> (3x3 point systems, 6x6 pose systems, 8x8 homography normal equations, 10x10 reduced intrinsics
+    systems, 12x12 static IMU steps) against numpy.linalg.solve; an indefinite matrix is reported instead of producing NaNs."""
     rng = np.random.default_rng(20 + n)
     for trial in range(50):
         G = rng.normal(0, 1, (n + 3, n)); A = G.T @ G * 10.0 ** rng.uniform(-3, 3)
@@ -407,6 +410,28 @@ def test_device_cholesky_solve(hm, n):
     A = np.eye(n); A[n - 1, n - 1] = -1.0
     x = np.ones(n)
     assert hm.hm_chol_solve(ctypes.c_int(n), A.ctypes.data_as(DP), x.ctypes.data_as(DP)) == 0 and np.isfinite(x).all()
+
+
+@pytest.mark.parametrize("n", CHOL_SIZES)
+def test_device_cholesky_factor_once_substitute_many(hm, n):
+    """chol_factor<N> once, chol_substitute<N> per right-hand side (the camera calibration's 11 columns per view): every column
+    against numpy.linalg.solve and equal, bit for bit, to chol_solve<N> of that column alone; an indefinite matrix is reported with
+    finite output in every column."""
+    rng = np.random.default_rng(40 + n)
+    nrhs = 11
+    for trial in range(20):
+        G = rng.normal(0, 1, (n + 3, n)); A = np.ascontiguousarray(G.T @ G * 10.0 ** rng.uniform(-3, 3))
+        B = rng.normal(0, 1, (nrhs, n)); X = B.copy()
+        assert hm.hm_chol_factor_substitute(ctypes.c_int(n), A.ctypes.data_as(DP), ctypes.c_int(nrhs), X.ctypes.data_as(DP)) == 1
+        ref = np.linalg.solve(A, B.T).T
+        assert np.abs(X - ref).max() < 1e-9 * np.linalg.cond(A) * max(1e-12, np.abs(ref).max()) + 1e-300
+        for r in range(nrhs):
+            x = B[r].copy()
+            assert hm.hm_chol_solve(ctypes.c_int(n), A.ctypes.data_as(DP), x.ctypes.data_as(DP)) == 1
+            assert np.array_equal(x, X[r])
+    A = np.eye(n); A[n // 2, n // 2] = -1.0
+    X = np.ones((nrhs, n))
+    assert hm.hm_chol_factor_substitute(ctypes.c_int(n), A.ctypes.data_as(DP), ctypes.c_int(nrhs), X.ctypes.data_as(DP)) == 0 and np.isfinite(X).all()
 
 
 def test_device_quaternion_from_rotation_matrix(hm):
