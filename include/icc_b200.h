@@ -308,6 +308,27 @@ icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double
 #define ICC_POSE_ERROR_TANGENT 1
 icc_status icc_set_pose_error(icc_handle* h, int mode);
 
+/* Shutter of icc_estimate_board_poses and icc_optimize_board_points.  line_delay_s = 0 (the default) is the global shutter: one rigid pose per
+ * view, and frame_t_s may be NULL.  line_delay_s > 0 is a rolling shutter: pixel row v of a view is exposed v * line_delay_s after its frame
+ * time frame_t_s[i] (the rule of the reference's RS functor, feature.y() * line_delay), and the reported pose is the one at the frame time
+ * (row 0).  Over one readout the camera moves with constant camera-frame angular velocity w and linear velocity u, so a corner seen at
+ * tau = v * line_delay_s is predicted from P(tau) = exp(-tau [w]x) (R_cw X + t_cw - tau u) with either residual of icc_set_pose_error.
+ * The velocities are not free unknowns; they come from each view's neighbours in time.  The views are sorted by time; a view's neighbours are
+ * the nearest valid views before and after it whose time differs by more than 0 and by at most 2.5 x the median positive spacing of all
+ * view times.  With both neighbours p and n:  w = R_wc,f^T R_wc,p Log(R_wc,p^T R_wc,n) / (t_n - t_p),  u = R_wc,f^T (p_wc,n - p_wc,p) / (t_n - t_p);
+ * with one, the same between it and the view; with none, w = u = 0 and the view keeps the global-shutter model.
+ * icc_estimate_board_poses runs its global-shutter pass, then exactly two rolling-shutter passes.  Each pass computes the velocities from the
+ * current poses and refines every valid view from its pose as icc_optimize_board_points does (usable corners, refinement, inlier threshold,
+ * refinement, mean error, max_reproj_error); a view dropped by a pass stays dropped.  icc_optimize_board_points runs one such pass on the
+ * given poses, refines the board points with the corners at their row times and the velocities of the new poses, and one more pass.
+ * The next pose call must pass n_frames views (else ICC_ERR_INVALID_ARGUMENT).  A negative or non-finite delay or time, or n_frames <= 0 /
+ * frame_t_s NULL with a positive delay, is ICC_ERR_INVALID_ARGUMENT.  Host state only: also accepted by a host-only handle. */
+icc_status icc_set_pose_rolling_shutter(icc_handle* h, double line_delay_s, int32_t n_frames, const double* frame_t_s);
+/* The velocities of the last rolling-shutter pose call on this handle: w_u[6 * n_frames] = (w, u) per view at its frame time (zero for a view
+ * that was not valid before that call's last pass, or that had no neighbour), n_without_neighbours (nullable) = the number of valid views
+ * without a neighbour.  ICC_ERR_STATE before any such call; ICC_ERR_INVALID_ARGUMENT when n_frames differs from that call's. */
+icc_status icc_get_pose_velocities(const icc_handle* h, int32_t n_frames, double* w_u, int32_t* n_without_neighbours);
+
 /* ---- upstream row f3 (SURVEY.md §8(f)): IMU-to-camera rotation + time offset initialiser -----------------------------------
  * ImuToCameraRotationEstimator::EstimateCameraImuRotation (src/core/imu_to_camera_rotation_estimator.cc:116-274) together with
  * the preparation done by applications/estimate_imu_to_camera_rotation.cc:96-173: view rotations q_cw (quaternion of

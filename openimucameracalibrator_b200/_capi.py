@@ -260,6 +260,19 @@ class CApi:
         """Residual of estimate_board_poses / optimize_board_points: POSE_ERROR_NORMALIZED (default), POSE_ERROR_TANGENT, or their names."""
         self._call("set_pose_error", [C.c_int], POSE_ERRORS[mode] if isinstance(mode, str) else int(mode))
 
+    def set_pose_rolling_shutter(self, line_delay_s, frame_t_s=None):
+        """Shutter of estimate_board_poses / optimize_board_points: line_delay_s = 0 is the global shutter (the default); > 0 a rolling
+        shutter with the views' frame times frame_t_s (one per view of the next pose call)."""
+        t = None if frame_t_s is None else _f64(frame_t_s).ravel()
+        self._call("set_pose_rolling_shutter", [C.c_double, C.c_int32, c_double_p], float(line_delay_s), 0 if t is None else t.size, _dp(t))
+
+    def pose_velocities(self, n_frames):
+        """Velocities of the last rolling-shutter pose call -> (w[n,3] rad/s, u[n,3] m/s, both camera frame at the frame time,
+        number of valid views without a neighbour)."""
+        vel = np.zeros((int(n_frames), 6)); ns = C.c_int32()
+        self._call("get_pose_velocities", [C.c_int32, c_double_p, C.POINTER(C.c_int32)], int(n_frames), _dp(vel), C.byref(ns))
+        return vel[:, :3], vel[:, 3:], ns.value
+
     # ---- upstream row f4: CameraCalibrator::CalibrateCameraFromJson / RunCalibration (src/core/camera_calibrator.cc:131-389) ----
     def calibrate_camera(self, model, image_width, image_height, corner_offsets, point_ids, uv, q_wc_init=None, p_wc_init=None, init_valid=None,
                          focal_length_init=0.0, distortion_init=0.0, **options):

@@ -10,7 +10,9 @@
 // When --input_pose_dataset is omitted, the per-view board poses are estimated in-process on the GPU from the corner file
 // (icc_estimate_board_poses = PoseEstimator::EstimatePosesFromJson, SURVEY.md §8(f) row f1), i.e. the corner file alone suffices;
 // --pose_error normalized|tangent (default normalized) selects that step's residual (icc_set_pose_error: tangent keeps the corners of
-// fisheye lenses beyond 90 degrees).
+// fisheye lenses beyond 90 degrees); --pose_shutter global|rolling (default global) its shutter (icc_set_pose_rolling_shutter: rolling gives each
+// view's pose at its frame timestamp from row-timed corners, line delay 1 / fps / height).  --pose_shutter rolling with --global_shutter or
+// with --input_pose_dataset is a usage error: the first contradicts it, the second skips the pose step.
 // Extra flags (not in the reference): --device (CUDA ordinal, default 0), --parse_only (stop after parsing, print a summary),
 // --gpus N (residual blocks sharded by time slice over devices device..device+N-1 of this host: the binary spawns one rank process per
 // extra device -- hidden flags --shard_rank / --shard_world / --comm_id_hex -- each with the library's own NCCL communicator; one
@@ -39,7 +41,8 @@ icccli::Flags default_flags() {
   icccli::Flags f;
   f.str = {{"telemetry_json", ""}, {"input_pose_dataset", ""}, {"input_corners", ""}, {"camera_calibration_json", ""},
     {"gyro_to_cam_initial_calibration", ""}, {"imu_intrinsics", ""}, {"imu_bias_file", ""}, {"spline_error_weighting_json", ""}, {"output_path", ""},
-    {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"}};
+    {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"},
+    {"pose_shutter", "global"}};
   f.boolean = {{"global_shutter", false}, {"calibrate_cam_line_delay", false}, {"reestimate_biases", false}, {"parse_only", false}, {"json_selftest", false}};
   f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0}};
   return f;
@@ -158,7 +161,12 @@ static int json_selftest() {
 int main(int argc, char** argv) {
   icccli::Flags F = default_flags();
   int pose_error = ICC_POSE_ERROR_NORMALIZED;
-  try { icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+  bool pose_rolling = false;
+  try {
+    icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); pose_rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]);
+    if (pose_rolling && F.boolean["global_shutter"]) throw std::runtime_error("--pose_shutter rolling contradicts --global_shutter");
+    if (pose_rolling && !F.str["input_pose_dataset"].empty()) throw std::runtime_error("--pose_shutter rolling applies to the in-process pose step, which --input_pose_dataset skips");
+  } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   const double S_TO_NS = 1e9, US_TO_S = 1e-6, S_TO_US = 1e6, NS_TO_S = 1e-9;
   if (F.boolean["json_selftest"]) return json_selftest();
   try {
@@ -228,9 +236,21 @@ int main(int argc, char** argv) {
       icc_status st = icc_set_camera(hp, model, intr.data(), (int)intr.size(), width, height);
       if (st == ICC_OK) st = icc_set_board_points(hp, max_id + 1, board.data());
       if (st == ICC_OK) st = icc_set_pose_error(hp, pose_error);
+      std::vector<double> view_t(nv);
+      for (int i = 0; i < nv; ++i) view_t[i] = sv.timestamp_us[i] * US_TO_S + t_offset_cam_s;
+      if (st == ICC_OK && pose_rolling) {
+        double ld = 0.0;
+        try { ld = icccli::pose_line_delay(fps, height); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+        st = icc_set_pose_rolling_shutter(hp, ld, nv, view_t.data());
+      }
       if (st == ICC_OK) st = icc_estimate_board_poses(hp, nv, sv.off.data(), sv.ids.data(), sv.uv.data(), 0.0, 0, q_all.data(), p_all.data(), err.data(), valid.data());
       if (st == ICC_OK) st = icc_filter_bad_poses(hp, nv, p_all.data(), valid.data());   // the pose app's last step (PoseEstimator::FilterBadPoses)
       if (st != ICC_OK) { std::cerr << "board pose estimation failed (" << st << "): " << icc_last_error(hp) << std::endl; return 2; }
+      if (pose_rolling) {
+        std::vector<double> vel(6 * (size_t)nv); int32_t n_static = 0;
+        if (icc_get_pose_velocities(hp, nv, vel.data(), &n_static) == ICC_OK)
+          std::cout << "Rolling-shutter board poses: " << n_static << " valid views without a neighbour in time keep the global-shutter model\n";
+      }
       icc_destroy(hp);
       int kept = 0;
       for (int i = 0; i < nv; ++i) {

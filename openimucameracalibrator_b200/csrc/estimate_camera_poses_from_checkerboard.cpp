@@ -10,7 +10,9 @@
 // and writes the refined board points as the dataset's tracks; PoseEstimator::FilterBadPoses (app :66-67) is applied like in the
 // reference.  Extra flags: --device (CUDA ordinal, default 0); --pose_error normalized|tangent (default normalized, the reference's
 // residual): tangent scores corners as unit bearings with the local tangent reprojection error, which keeps the corners and views of
-// fisheye lenses beyond 90 degrees (icc_set_pose_error); the written mean_reproj_error is then in tangent units.
+// fisheye lenses beyond 90 degrees (icc_set_pose_error); the written mean_reproj_error is then in tangent units.  --pose_shutter global|rolling
+// (default global): rolling reports each view's pose at its frame timestamp from corners exposed row by row, line delay 1 / fps / height
+// of the camera calibration (icc_set_pose_rolling_shutter); the pose dataset keeps its format.
 #include "../../include/icc_b200.h"
 #include "icc_cli_common.hpp"
 
@@ -22,17 +24,21 @@ using iccjson::Value;
 
 int main(int argc, char** argv) {
   icccli::Flags F;
-  F.str = {{"input_corners", ""}, {"camera_calibration_json", ""}, {"output_pose_dataset", ""}, {"pose_error", "normalized"}};
+  F.str = {{"input_corners", ""}, {"camera_calibration_json", ""}, {"output_pose_dataset", ""}, {"pose_error", "normalized"}, {"pose_shutter", "global"}};
   F.boolean = {{"optimize_board_points", false}};
   F.num = {{"device", 0.0}};
   int pose_error = ICC_POSE_ERROR_NORMALIZED;
-  try { icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+  bool rolling = false;
+  try { icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]); }
+  catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   try {
     Value scene_json; icccli::SceneViews sv;
     try { scene_json = icccli::load_scene(F.str["input_corners"], sv); } catch (const std::exception& e) { std::cerr << "Check failed: Failed to load " << F.str["input_corners"] << ": " << e.what() << std::endl; return 1; }
     std::vector<double> intr; int width = 0, height = 0; double fps = 0; int model = -1;
     try { model = icccli::read_camera(iccjson::load_json(F.str["camera_calibration_json"]), intr, width, height, fps); }
     catch (const std::exception& e) { std::cerr << "Check failed: Could not read camera calibration: " << F.str["camera_calibration_json"] << ": " << e.what() << std::endl; return 1; }
+    double line_delay = 0.0;
+    if (rolling) { try { line_delay = icccli::pose_line_delay(fps, height); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; } }
     int np = 0;
     const std::vector<double> board = icccli::read_scene_points(scene_json, np);
     const int nv = (int)sv.timestamp_us.size();
@@ -45,8 +51,17 @@ int main(int argc, char** argv) {
     st = icc_set_camera(h, model, intr.data(), (int)intr.size(), width, height);
     if (st == ICC_OK) st = icc_set_board_points(h, np, board.data());
     if (st == ICC_OK) st = icc_set_pose_error(h, pose_error);
+    std::vector<double> frame_t(nv);
+    for (int i = 0; i < nv; ++i) frame_t[i] = sv.timestamp_us[i] * 1e-6;
+    if (st == ICC_OK && rolling) st = icc_set_pose_rolling_shutter(h, line_delay, nv, frame_t.data());
     if (st == ICC_OK) st = icc_estimate_board_poses(h, nv, sv.off.data(), sv.ids.data(), sv.uv.data(), 0.0, 0, q.data(), p.data(), err.data(), valid.data());
     if (st != ICC_OK) { std::cerr << "board pose estimation failed (" << st << "): " << icc_last_error(h) << std::endl; return 2; }
+    auto report_shutter = [&]() {
+      std::vector<double> vel(6 * (size_t)nv); int32_t n_static = 0;
+      if (icc_get_pose_velocities(h, nv, vel.data(), &n_static) == ICC_OK)
+        std::cout << "Rolling shutter: line delay " << line_delay << " s, " << n_static << " valid views without a neighbour in time keep the global-shutter model.\n";
+    };
+    if (rolling) report_shutter();
     std::vector<double> board_out(board);
     if (F.boolean["optimize_board_points"]) {                                  // app :61-65
       int32_t n_opt = 0;

@@ -101,6 +101,8 @@ struct icc_handle {
   // ---- raw inputs -------------------------------------------------------------------------------------------
   int model = -1, n_intr = 0, width = 0, height = 0; double intr[10] = {0};
   int pose_error = ICC_POSE_ERROR_NORMALIZED;   // residual of icc_estimate_board_poses / icc_optimize_board_points (icc_set_pose_error)
+  double pose_line_delay = 0.0; std::vector<double> pose_frame_t;   // their shutter (icc_set_pose_rolling_shutter; 0 = global)
+  std::vector<double> pose_vel; int32_t pose_n_static = 0;          // what their last rolling-shutter pass used (icc_get_pose_velocities)
   std::vector<double> points;
   std::vector<double> frame_t; std::vector<int> corner_off; HostBuf<int> point_ids; HostBuf<double> uv; std::vector<double> q_wc, p_wc;
   HostBuf<double> imu_t, imu_acc, imu_gyr;
@@ -1469,14 +1471,55 @@ icc_status icc_set_pose_error(icc_handle* h, int mode) {
   return ICC_OK;
 }
 
+icc_status icc_set_pose_rolling_shutter(icc_handle* h, double line_delay_s, int32_t n_frames, const double* frame_t_s) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (!std::isfinite(line_delay_s) || line_delay_s < 0.0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "line delay must be finite and >= 0");
+  if (line_delay_s == 0.0) { h->pose_line_delay = 0.0; h->pose_frame_t.clear(); return ICC_OK; }
+  if (n_frames <= 0 || !frame_t_s) return fail(h, ICC_ERR_INVALID_ARGUMENT, "a rolling shutter needs the n_frames > 0 view times");
+  for (int i = 0; i < n_frames; ++i)
+    if (!std::isfinite(frame_t_s[i]) || frame_t_s[i] < 0.0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "view times must be finite and >= 0");
+  h->pose_line_delay = line_delay_s;
+  h->pose_frame_t.assign(frame_t_s, frame_t_s + n_frames);
+  return ICC_OK;
+}
+
+icc_status icc_get_pose_velocities(const icc_handle* h, int32_t n_frames, double* w_u, int32_t* n_without_neighbours) {
+  if (!h || n_frames <= 0 || !w_u) return ICC_ERR_INVALID_ARGUMENT;
+  if (h->pose_vel.empty()) return fail(const_cast<icc_handle*>(h), ICC_ERR_STATE, "no rolling-shutter pose call has run on this handle");
+  if ((size_t)n_frames * 6 != h->pose_vel.size()) return fail(const_cast<icc_handle*>(h), ICC_ERR_INVALID_ARGUMENT, "n_frames differs from the last rolling-shutter pose call");
+  std::copy(h->pose_vel.begin(), h->pose_vel.end(), w_u);
+  if (n_without_neighbours) *n_without_neighbours = h->pose_n_static;
+  return ICC_OK;
+}
+
+// The shutter of the next pose call of nf views; its velocity outputs land in vel / n_static, which keep_velocities moves into the handle
+// once the call has succeeded (a failed call leaves icc_get_pose_velocities as it was).  false (with the error set) when the view times of
+// icc_set_pose_rolling_shutter are for another number of views.
+struct PoseCallShutter {
+  PoseShutter S; std::vector<double> vel; int32_t n_static = 0;
+  bool prepare(icc_handle* h, int nf) {
+    if (h->pose_line_delay <= 0.0) return true;
+    if ((int)h->pose_frame_t.size() != nf) { fail(h, ICC_ERR_INVALID_ARGUMENT, "n_frames differs from the view times of icc_set_pose_rolling_shutter"); return false; }
+    vel.assign(6 * (size_t)nf, 0.0);
+    S.line_delay = h->pose_line_delay; S.frame_t = h->pose_frame_t.data(); S.vel = vel.data(); S.n_static = &n_static;
+    return true;
+  }
+  icc_status keep_velocities(icc_handle* h, icc_status rc) {
+    if (rc == ICC_OK && S.line_delay > 0.0) { h->pose_vel.swap(vel); h->pose_n_static = n_static; }
+    return rc;
+  }
+};
+
 icc_status icc_estimate_board_poses(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points, double* q_wc, double* p_wc, double* mean_err, int32_t* valid) {
   if (!h || nf <= 0 || !off || !ids || !uv || !q_wc || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
+  PoseCallShutter R;
+  if (!R.prepare(h, nf)) return ICC_ERR_INVALID_ARGUMENT;
   NEED_DEVICE();
   if (h->model < 0 || h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_camera and icc_set_board_points must be called first");
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
-  return drive(h, [&](std::string& err) { return estimate_board_poses(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
-                                h->pose_error, q_wc, p_wc, mean_err, valid, err); });
+  return R.keep_velocities(h, drive(h, [&](std::string& err) { return estimate_board_poses(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv,
+                                max_reproj_error, min_points, h->pose_error, R.S, q_wc, p_wc, mean_err, valid, err); }));
 }
 
 icc_status icc_filter_bad_poses(icc_handle* h, int nv, const double* p_wc, int32_t* valid) {
@@ -1496,14 +1539,16 @@ icc_status icc_get_board_points(const icc_handle* h, double* xyzw, int n) {
 icc_status icc_optimize_board_points(icc_handle* h, int nf, const int32_t* off, const int32_t* ids, const double* uv, double max_reproj_error, int min_points,
                                      int min_observations, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, double* board_out, int32_t* n_opt_out) {
   if (!h || nf <= 0 || !off || !ids || !uv || !q_wc || !p_wc || !valid) return ICC_ERR_INVALID_ARGUMENT;
+  PoseCallShutter R;
+  if (!R.prepare(h, nf)) return ICC_ERR_INVALID_ARGUMENT;
   NEED_DEVICE();
   if (h->model < 0 || h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_camera and icc_set_board_points must be called first");
   if (off[0] != 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must start at 0");
   for (int i = 0; i < nf; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
   std::vector<double> points;
   const icc_status rc = drive(h, [&](std::string& err) { return optimize_board_points(h->stream, h->model, h->intr, h->width, h->height, (int)(h->points.size() / 4), h->points.data(), nf, off, ids, uv, max_reproj_error, min_points,
-                                 min_observations, h->pose_error, q_wc, p_wc, mean_err, valid, points, n_opt_out, err); });
-  if (rc != ICC_OK) return rc;
+                                 min_observations, h->pose_error, R.S, q_wc, p_wc, mean_err, valid, points, n_opt_out, err); });
+  if (R.keep_velocities(h, rc) != ICC_OK) return rc;
   h->points.swap(points);
   if (board_out) std::copy(h->points.begin(), h->points.end(), board_out);
   return ICC_OK;

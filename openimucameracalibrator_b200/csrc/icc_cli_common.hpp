@@ -27,6 +27,19 @@ inline int parse_pose_error(const std::string& v) {
   throw std::runtime_error("flag --pose_error must be 'normalized' or 'tangent', not '" + v + "'");
 }
 
+// --pose_shutter of the pose tools: true = rolling (icc_set_pose_rolling_shutter); any other value than global / rolling is a usage error
+inline bool parse_pose_shutter(const std::string& v) {
+  if (v == "global") return false;
+  if (v == "rolling") return true;
+  throw std::runtime_error("flag --pose_shutter must be 'global' or 'rolling', not '" + v + "'");
+}
+
+// the line delay of --pose_shutter rolling: one readout per frame interval, 1 / fps / image height (the hot CLI's initial line delay)
+inline double pose_line_delay(double fps, int height) {
+  if (!(fps > 0.0) || height <= 0) throw std::runtime_error("--pose_shutter rolling needs fps > 0 and an image height in the camera calibration");
+  return 1.0 / fps / height;
+}
+
 inline bool parse_bool(const std::string& v) { return v == "true" || v == "1" || v == "t" || v == "yes" || v == "y" || v == "True"; }
 
 // gflags syntax: --name=value, --name value, -name..., --boolflag, --noboolflag

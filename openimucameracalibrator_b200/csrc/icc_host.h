@@ -86,19 +86,23 @@ icc_status upload_board_views(cudaStream_t st, int np, const double* points, int
 icc_status read_poses(cudaStream_t st, const BoardViews& B, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err);
 // theia::BundleAdjustTracks with constant cameras: Q carries the camera, measurements, poses and board_in; corner c observes point ids[c]
 // from view obs_view[c] and takes part iff obs_view[c] >= 0.  Refined points -> d_out and points_out (4 doubles each).  With bear (the corners'
-// bearings) the residual is the tangent error and Q.meas is not read.
+// bearings) the residual is the tangent error and Q.meas is not read.  With rs every corner is seen at its row time (the pose step's rolling shutter).
 icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const int32_t* ids, const std::vector<int>& obs_view, DevBuf<double4>& d_out, std::vector<double>& points_out, int& n_opt, std::string& err,
-                               const double4* bear = nullptr);
+                               const double4* bear = nullptr, const RsPass* rs = nullptr);
 
 // ---- the upstream tools' host drivers, each in the .cu file of its kernels -----------------------------------------------------
 icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err);
 icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err);
 // pose_error: ICC_POSE_ERROR_NORMALIZED or ICC_POSE_ERROR_TANGENT (the residual of the per-view refinement and of the board points)
+// The shutter of the pose step (icc_set_pose_rolling_shutter): line_delay = 0 is the global shutter; otherwise frame_t holds the nf view times,
+// and vel (6 per view: w, u) and n_static (valid views without a neighbour in time) receive what the last rolling-shutter pass used.
+struct PoseShutter { double line_delay = 0.0; const double* frame_t = nullptr; double* vel = nullptr; int32_t* n_static = nullptr; };
 icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
-                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err);
+                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc, double* mean_err,
+                                int32_t* valid, std::string& err);
 icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
-                                 const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid,
-                                 std::vector<double>& points_out, int32_t* n_opt_out, std::string& err);
+                                 const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc,
+                                 double* mean_err, int32_t* valid, std::vector<double>& points_out, int32_t* n_opt_out, std::string& err);
 void filter_bad_poses(int nv, const double* p_wc, int32_t* valid);
 icc_status estimate_imu_to_camera_rotation(cudaStream_t st, int sm_count, int n_views, const double* view_t, const double* q_cw, int n_imu, const double* imu_t, const double* gyro,
                                            const double* bias_in, double* q_out, double* td_out, double* bias_out, double* err_out, int32_t* iters_out, std::string& err);

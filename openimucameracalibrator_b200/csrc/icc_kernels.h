@@ -144,6 +144,8 @@ struct PointProblem {
   const double2* meas;         // per corner: xy (normalised) or uv (pixels)
   const double* q_cw; const double* cam_c; // per view: R_cw as (x,y,z,w), camera centre
 };
+// rolling-shutter passes of the pose step: corner c is seen uv[c].y * line_delay after its frame; vel[6v..6v+5] = view v's camera-frame (w, u)
+struct RsPass { const double2* uv; const double* vel; double line_delay; };
 // focal length per view from the board homography on centred pixels (f2[v] = f^2 or 0), pinhole normalisation of pixels
 void launch_board_focal(const PoseProblem& Q, const double2* uv, double cx, double cy, double2* xy, unsigned char* use, double* f2, cudaStream_t st);
 void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, double f, double2* xy, int* ok, cudaStream_t st);

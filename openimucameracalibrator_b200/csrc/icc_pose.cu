@@ -17,13 +17,20 @@
 // Opt-in wide-angle residual (ICC_POSE_ERROR_TANGENT): corners are unit bearings (icc_bearing_math.cuh) and the same kernels minimise the
 // local tangent reprojection error instead, so rays 90 degrees or more off the axis keep their views.  The residual is a template parameter
 // chosen by the measurement type (double2 = normalised point, double4 = bearing); the default kernels compile to the same code as before.
+//
+// Opt-in rolling shutter (icc_set_pose_rolling_shutter): after the global-shutter pass, two more refinement-only passes score each corner
+// against the pose at its row time (icc_rolling_shutter_math.cuh), with each view's velocities taken from its neighbours in time by a small
+// kernel before each pass.  Rolling shutter is a template parameter of board_pose_kernel and point_refine_kernel; false is the code as before.
 #include "icc_bearing_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
 #include "icc_reduce.cuh"
+#include "icc_rolling_shutter_math.cuh"
 #include "icc_small_linalg.cuh"
 
+#include <algorithm>
 #include <cmath>
+#include <numeric>
 #include <type_traits>
 
 namespace icc {
@@ -139,11 +146,60 @@ ICC_D void pose_system(const PoseProblem& Q, const double4* bear, const unsigned
 // the tangent error of one corner for the inlier and mean-error passes; false where b.d <= 0
 ICC_D bool tangent_err(V3 Pc, double4 m, double& r0, double& r1) { const TangentErr E(Pc, v3(m.x, m.y, m.z)); r0 = E.r0; r1 = E.r1; return E.front(); }
 
-// Levenberg-Marquardt on the 6 pose parameters (all lanes run the identical scalar logic on warp-reduced sums)
+// Rolling shutter: the per-corner row times (uv[c].y * line_delay) and this view's velocities
+struct RsView { const double2* uv; double line_delay; RsMotion m; };
+
+// The system of either residual with every corner at its row time (rs_pose_residual); 1e6 where the point is behind the measurement
 template <class M>
-ICC_D void pose_refine(const PoseProblem& Q, const M* xy, const unsigned char* use, int c0, int c1, double zref, Q4& q, V3& t) {
+ICC_D void pose_system_rs(const PoseProblem& Q, const M* meas, const unsigned char* use, int c0, int c1, double zref, Q4 q, V3 t, const RsView& rs, PoseSys& S, bool with_jacobian) {
+  const int lane = threadIdx.x & 31;
+  double H[21], g[6], cost = 0.0;
+#pragma unroll
+  for (int i = 0; i < 21; ++i) H[i] = 0.0;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) g[i] = 0.0;
+  const double hub = 1.345;
+  for (int c = c0 + lane; c < c1; c += 32) {
+    if (!use[c]) continue;
+    const double4 Xb = Q.board[Q.pid[c]];
+    const V3 X = v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref);
+    double r0, r1, J0[6], J1[6];
+    const bool front = rs_pose_residual(meas[c], q, t, X, rs.m, rs.uv[c].y * rs.line_delay, r0, r1, J0, J1);
+    const double rn = sqrt(r0 * r0 + r1 * r1);
+    const double w = rn <= hub ? 1.0 : hub / rn;
+    cost += rn <= hub ? 0.5 * rn * rn : hub * rn - 0.5 * hub * hub;
+    if (!with_jacobian || !front) { if (!front) cost += 1e6; continue; }
+    int idx = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+      g[i] += w * (J0[i] * r0 + J1[i] * r1);
+#pragma unroll
+      for (int j = 0; j <= i; ++j) { H[idx] += w * (J0[i] * J0[j] + J1[i] * J1[j]); ++idx; }
+    }
+  }
+  S.cost = warp_sum(cost);
+  if (!with_jacobian) return;
+  int idx = 0;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    S.g[i] = warp_sum(g[i]);
+#pragma unroll
+    for (int j = 0; j <= i; ++j) { const double v = warp_sum(H[idx]); S.H[i][j] = v; S.H[j][i] = v; ++idx; }
+  }
+}
+
+// the system of the pose refinement: global shutter (pose_system) or rolling shutter (pose_system_rs)
+template <bool RS, class M>
+ICC_D void view_system(const PoseProblem& Q, const M* xy, const unsigned char* use, int c0, int c1, double zref, Q4 q, V3 t, const RsView& rs, PoseSys& S, bool with_jacobian) {
+  if constexpr (RS) pose_system_rs(Q, xy, use, c0, c1, zref, q, t, rs, S, with_jacobian);
+  else pose_system(Q, xy, use, c0, c1, zref, q, t, S, with_jacobian);
+}
+
+// Levenberg-Marquardt on the 6 pose parameters (all lanes run the identical scalar logic on warp-reduced sums)
+template <class M, bool RS = false>
+ICC_D void pose_refine(const PoseProblem& Q, const M* xy, const unsigned char* use, int c0, int c1, double zref, Q4& q, V3& t, const RsView& rs) {
   PoseSys S;
-  pose_system(Q, xy, use, c0, c1, zref, q, t, S, true);
+  view_system<RS>(Q, xy, use, c0, c1, zref, q, t, rs, S, true);
   double lambda = 1e-4, cost = S.cost;
   for (int it = 0; it < 50; ++it) {
     double A[6][6], b[6];
@@ -158,13 +214,13 @@ ICC_D void pose_refine(const PoseProblem& Q, const M* xy, const unsigned char* u
     const Q4 qn = qnormalized(qmul(q, so3_exp(v3(b[0], b[1], b[2]))));
     const V3 tn = t + v3(b[3], b[4], b[5]);
     PoseSys Sn;
-    pose_system(Q, xy, use, c0, c1, zref, qn, tn, Sn, false);
+    view_system<RS>(Q, xy, use, c0, c1, zref, qn, tn, rs, Sn, false);
     const double step2 = b[0] * b[0] + b[1] * b[1] + b[2] * b[2] + b[3] * b[3] + b[4] * b[4] + b[5] * b[5];
     if (Sn.cost < cost) {
       const double dec = cost - Sn.cost;
       q = qn; t = tn; cost = Sn.cost; lambda = fmax(lambda * 0.1, 1e-12);
       if (dec <= (Q.lm_rel_tol > 0.0 ? Q.lm_rel_tol : 1e-15) * cost || step2 < 1e-28) break;
-      pose_system(Q, xy, use, c0, c1, zref, q, t, S, true);
+      view_system<RS>(Q, xy, use, c0, c1, zref, q, t, rs, S, true);
     } else {
       if (step2 < 1e-28) break;
       lambda *= 10.0;
@@ -298,9 +354,11 @@ ICC_D bool bearing_start(const PoseProblem& Q, const double4* bear, const int* o
 
 // M = double2: normalised points (the reference's residual); M = double4: bearings, the tangent residual (xy_h / ok_h: per-corner scratch of the
 // start).  The normalised branches keep their own text, so that board_pose_kernel<double2> compiles to the same code as the pre-template kernel.
-template <class M>
+// RS (refinement-only passes): every corner at its row time uv[c].y * line_delay, with the view's velocities vel[6f..6f+5] = (w, u).
+template <class M, bool RS = false>
 __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M* __restrict__ xy, const int* __restrict__ okc, unsigned char* __restrict__ use,
-                                                        double* q_out, double* p_out, double* __restrict__ err_out, int* valid_out, double2* __restrict__ xy_h, int* __restrict__ ok_h) {
+                                                        double* q_out, double* p_out, double* __restrict__ err_out, int* valid_out, double2* __restrict__ xy_h, int* __restrict__ ok_h,
+                                                        RsPass rsp) {
   constexpr bool kTangent = std::is_same<M, double4>::value;
   const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (f >= Q.n_frames) return;
@@ -310,6 +368,11 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
   };
   double n = 0.0, zref = 0.0;
   Q4 q; V3 t;
+  RsView rs;
+  if constexpr (RS) {
+    const double* v = rsp.vel + 6 * f;
+    rs.uv = rsp.uv; rs.line_delay = rsp.line_delay; rs.m.w = v3(v[0], v[1], v[2]); rs.m.u = v3(v[3], v[4], v[5]);
+  }
   if (Q.refine_only) {
     // PoseEstimator::OptimizeAllPoses (pose_estimator.cc:226-236): BundleAdjustView again from the stored pose -- no homography, so the
     // board may have left its plane (optimised board points); views that were dropped stay dropped and keep their outputs
@@ -345,12 +408,13 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
     }
   }
   // ---- refinement, inlier selection with the reference's squared normalised threshold, refinement on the inliers -------------
-  pose_refine(Q, xy, use, c0, c1, zref, q, t);
+  pose_refine<M, RS>(Q, xy, use, c0, c1, zref, q, t, rs);
   double n_in = 0.0, n_out = 0.0;
   for (int c = c0 + lane; c < c1; c += 32) {
     if (!use[c]) continue;
     const double4 Xb = Q.board[Q.pid[c]];
-    const V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
+    V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
+    if constexpr (RS) { const double tau = rs.uv[c].y * rs.line_delay; Pc = rs_point(rs_rotation(rs.m, tau), rs.m, tau, Pc); }
     bool in;
     if constexpr (kTangent) {
       double r0, r1e;
@@ -364,13 +428,14 @@ __global__ void __launch_bounds__(128) board_pose_kernel(PoseProblem Q, const M*
   n_in = warp_sum(n_in); n_out = warp_sum(n_out);
   __syncwarp();
   if (n_in < 6.0) { fail(); return; }
-  if (n_out > 0.0) pose_refine(Q, xy, use, c0, c1, zref, q, t);
+  if (n_out > 0.0) pose_refine<M, RS>(Q, xy, use, c0, c1, zref, q, t, rs);
   // ---- mean reprojection error of the kept observations (:164-181; the view camera is the unit pinhole) ----------------------
   double e = 0.0;
   for (int c = c0 + lane; c < c1; c += 32) {
     if (!use[c]) continue;
     const double4 Xb = Q.board[Q.pid[c]];
-    const V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
+    V3 Pc = qrot(q, v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w - zref)) + t;
+    if constexpr (RS) { const double tau = rs.uv[c].y * rs.line_delay; Pc = rs_point(rs_rotation(rs.m, tau), rs.m, tau, Pc); }
     if constexpr (kTangent) {
       double r0, r1e;
       tangent_err(Pc, xy[c], r0, r1e);
@@ -429,16 +494,24 @@ __global__ void pinhole_normalize_kernel(int n, const double2* __restrict__ uv, 
 //   normalised == 1 :  (R_cw (X - c)).xy / z - x_n          (the pose estimator's unit-pinhole views with undistorted features)
 //   normalised == 0 :  CameraToPixelCoordinates(intr, R_cw (X - c)) - pixel     (the camera calibrator's views)
 //   TANGENT         :  the tangent error of R_cw (X - c) against the corner's bearing  (the pose estimator's views in tangent mode)
+//   RS (with normalised or TANGENT): the point at the corner's row time, exp(-tau [w]x) (R_cw (X - c) - tau u), rows A^T a as in pose_system_rs
 struct PointSys { double H[3][3]; double g[3]; double cost; };
-template <bool TANGENT>
-ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear, int o0, int o1, V3 X, PointSys& S, bool with_jacobian) {
+template <bool TANGENT, bool RS = false>
+ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear, int o0, int o1, V3 X, PointSys& S, bool with_jacobian, const RsPass& rsp) {
   const int lane = threadIdx.x & 31;
   double H[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0}, cost = 0.0;
   const double hub = Q.huber;
   for (int o = o0 + lane; o < o1; o += 32) {
     const int c = Q.pt_obs[o], v = Q.obs_view[c];
     const Q4 q = q4(Q.q_cw[4 * v], Q.q_cw[4 * v + 1], Q.q_cw[4 * v + 2], Q.q_cw[4 * v + 3]);
-    const V3 pc = qrot(q, X - v3(Q.cam_c[3 * v], Q.cam_c[3 * v + 1], Q.cam_c[3 * v + 2]));
+    V3 pc = qrot(q, X - v3(Q.cam_c[3 * v], Q.cam_c[3 * v + 1], Q.cam_c[3 * v + 2]));
+    [[maybe_unused]] Q4 A;
+    if constexpr (RS) {
+      const double* vel = rsp.vel + 6 * v;
+      RsMotion m; m.w = v3(vel[0], vel[1], vel[2]); m.u = v3(vel[3], vel[4], vel[5]);
+      const double tau = rsp.uv[c].y * rsp.line_delay;
+      A = rs_rotation(m, tau); pc = rs_point(A, m, tau, pc);
+    }
     double r0, r1; V3 a0, a1;
     if constexpr (TANGENT) {
       const double4 m = bear[c];
@@ -459,6 +532,7 @@ ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear,
     const double rn = sqrt(r0 * r0 + r1 * r1), wgt = rn <= hub ? 1.0 : hub / rn;
     cost += rn <= hub ? 0.5 * rn * rn : hub * rn - 0.5 * hub * hub;
     if (!with_jacobian) continue;
+    if constexpr (RS) { a0 = qrot_inv(A, a0); a1 = qrot_inv(A, a1); }
     const V3 j0 = qrot_inv(q, a0), j1 = qrot_inv(q, a1);   // rows of J_proj R_cw
     g[0] += wgt * (j0.x * r0 + j1.x * r1); g[1] += wgt * (j0.y * r0 + j1.y * r1); g[2] += wgt * (j0.z * r0 + j1.z * r1);
     H[0] += wgt * (j0.x * j0.x + j1.x * j1.x); H[1] += wgt * (j0.x * j0.y + j1.x * j1.y); H[2] += wgt * (j0.x * j0.z + j1.x * j1.z);
@@ -472,9 +546,9 @@ ICC_D void point_system(const PointProblem& Q, const double4* __restrict__ bear,
   S.H[0][0] = h0; S.H[0][1] = h1; S.H[0][2] = h2; S.H[1][0] = h1; S.H[1][1] = h3; S.H[1][2] = h4; S.H[2][0] = h2; S.H[2][1] = h4; S.H[2][2] = h5;
 }
 
-// TANGENT: Q.meas is unused, the corners' bearings come in bear
-template <bool TANGENT>
-__global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, double4* __restrict__ board_out, int* __restrict__ optimized, const double4* __restrict__ bear) {
+// TANGENT: Q.meas is unused, the corners' bearings come in bear.  RS: the views' velocities and the corners' row times come in rsp.
+template <bool TANGENT, bool RS = false>
+__global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, double4* __restrict__ board_out, int* __restrict__ optimized, const double4* __restrict__ bear, RsPass rsp) {
   const int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (p >= Q.n_points) return;
   const int o0 = Q.pt_off[p], o1 = Q.pt_off[p + 1];
@@ -482,7 +556,7 @@ __global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, doubl
   if (o1 - o0 <= Q.min_obs) { if (lane == 0) { board_out[p] = Xb; optimized[p] = 0; } return; }   // pose_estimator.cc:202-206
   V3 X = v3(Xb.x / Xb.w, Xb.y / Xb.w, Xb.z / Xb.w);
   PointSys S;
-  point_system<TANGENT>(Q, bear, o0, o1, X, S, true);
+  point_system<TANGENT, RS>(Q, bear, o0, o1, X, S, true, rsp);
   double lambda = 1e-4, cost = S.cost;
   for (int it = 0; it < 50; ++it) {
     double A[3][3], b[3];
@@ -496,13 +570,13 @@ __global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, doubl
     if (!chol_solve<3>(A, b)) { lambda *= 10.0; if (lambda > 1e12) break; continue; }
     const V3 Xn = X + v3(b[0], b[1], b[2]);
     PointSys Sn;
-    point_system<TANGENT>(Q, bear, o0, o1, Xn, Sn, false);
+    point_system<TANGENT, RS>(Q, bear, o0, o1, Xn, Sn, false, rsp);
     const double step2 = b[0] * b[0] + b[1] * b[1] + b[2] * b[2];
     if (Sn.cost < cost) {
       const double dec = cost - Sn.cost;
       X = Xn; cost = Sn.cost; lambda = fmax(lambda * 0.1, 1e-12);
       if (dec <= 1e-15 * cost || step2 < 1e-30) break;
-      point_system<TANGENT>(Q, bear, o0, o1, X, S, true);
+      point_system<TANGENT, RS>(Q, bear, o0, o1, X, S, true, rsp);
     } else {
       if (step2 < 1e-30) break;
       lambda *= 10.0;
@@ -510,6 +584,33 @@ __global__ void __launch_bounds__(128) point_refine_kernel(PointProblem Q, doubl
     }
   }
   if (lane == 0) { board_out[p] = make_double4(X.x, X.y, X.z, 1.0); optimized[p] = 1; }
+}
+
+// Velocities of every view from its neighbours in time, one thread per view over the time-sorted index order[] (times ts[], ascending).
+// The neighbours are the nearest valid views before and after it at a positive gap of at most max_gap; both: central difference, one:
+// one-sided between it and the view, none: w = u = 0 (the global-shutter model).  nbr[f] = number of neighbours used; -1 (and zero velocities)
+// for an invalid view.
+__global__ void view_velocity_kernel(int n, const int* __restrict__ order, const double* __restrict__ ts, double max_gap, const double* __restrict__ q_wc,
+                                     const double* __restrict__ p_wc, const int* __restrict__ valid, double* __restrict__ vel, int* __restrict__ nbr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int f = order[i];
+  const double tf = ts[i];
+  int a = -1, b = -1;
+  if (valid[f]) {
+    for (int j = i - 1; j >= 0 && tf - ts[j] <= max_gap; --j) if (tf - ts[j] > 0.0 && valid[order[j]]) { a = j; break; }
+    for (int j = i + 1; j < n && ts[j] - tf <= max_gap; ++j) if (ts[j] - tf > 0.0 && valid[order[j]]) { b = j; break; }
+  }
+  RsMotion m; m.w = v3(0.0, 0.0, 0.0); m.u = v3(0.0, 0.0, 0.0);
+  if (a >= 0 || b >= 0) {
+    const int fa = a >= 0 ? order[a] : f, fb = b >= 0 ? order[b] : f;
+    auto qv = [&](int v) { return qnormalized(q4(q_wc[4 * v], q_wc[4 * v + 1], q_wc[4 * v + 2], q_wc[4 * v + 3])); };
+    auto pv = [&](int v) { return v3(p_wc[3 * v], p_wc[3 * v + 1], p_wc[3 * v + 2]); };
+    m = rs_view_velocity(qv(fa), pv(fa), a >= 0 ? ts[a] : tf, qv(fb), pv(fb), b >= 0 ? ts[b] : tf, qv(f));
+  }
+  double* o = vel + 6 * f;
+  o[0] = m.w.x; o[1] = m.w.y; o[2] = m.w.z; o[3] = m.u.x; o[4] = m.u.y; o[5] = m.u.z;
+  nbr[f] = valid[f] ? (a >= 0) + (b >= 0) : -1;
 }
 
 }  // namespace
@@ -530,13 +631,27 @@ void launch_bearings(int model, const double* intr10, int n, const double2* uv, 
 
 void launch_board_poses(const PoseProblem& Q, const double2* xy, const int* ok, unsigned char* use, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st) {
   if (Q.n_frames <= 0) return;
-  board_pose_kernel<double2><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, xy, ok, use, q_wc, p_wc, err, valid, nullptr, nullptr);
+  board_pose_kernel<double2><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, xy, ok, use, q_wc, p_wc, err, valid, nullptr, nullptr, RsPass{});
   count_launch();
 }
 
 void launch_board_poses_tangent(const PoseProblem& Q, const double4* bear, const int* ok, unsigned char* use, double2* xy_h, int* ok_h, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st) {
   if (Q.n_frames <= 0) return;
-  board_pose_kernel<double4><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, bear, ok, use, q_wc, p_wc, err, valid, xy_h, ok_h);
+  board_pose_kernel<double4><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, bear, ok, use, q_wc, p_wc, err, valid, xy_h, ok_h, RsPass{});
+  count_launch();
+}
+
+// a rolling-shutter refinement-only pass (Q.refine_only = 1) over the views of either residual: meas = double2 normalised points or double4 bearings
+template <class M>
+static void launch_board_poses_rs(const PoseProblem& Q, const M* meas, const int* ok, unsigned char* use, const RsPass& rsp, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st) {
+  if (Q.n_frames <= 0) return;
+  board_pose_kernel<M, true><<<(Q.n_frames + 3) / 4, 128, 0, st>>>(Q, meas, ok, use, q_wc, p_wc, err, valid, nullptr, nullptr, rsp);
+  count_launch();
+}
+
+static void launch_view_velocities(int n, const int* order, const double* ts, double max_gap, const double* q_wc, const double* p_wc, const int* valid, double* vel, int* nbr, cudaStream_t st) {
+  if (n <= 0) return;
+  view_velocity_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, order, ts, max_gap, q_wc, p_wc, valid, vel, nbr);
   count_launch();
 }
 
@@ -552,10 +667,13 @@ void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, do
   count_launch();
 }
 
-void launch_point_refine(const PointProblem& Q, const double4* bear, double4* board_out, int* optimized, cudaStream_t st) {
+static void launch_point_refine(const PointProblem& Q, const double4* bear, double4* board_out, int* optimized, cudaStream_t st, const RsPass* rs) {
   if (Q.n_points <= 0) return;
-  if (bear) point_refine_kernel<true><<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized, bear);
-  else point_refine_kernel<false><<<(Q.n_points + 3) / 4, 128, 0, st>>>(Q, board_out, optimized, nullptr);
+  const dim3 grid((Q.n_points + 3) / 4);
+  if (rs && bear) point_refine_kernel<true, true><<<grid, 128, 0, st>>>(Q, board_out, optimized, bear, *rs);
+  else if (rs) point_refine_kernel<false, true><<<grid, 128, 0, st>>>(Q, board_out, optimized, nullptr, *rs);
+  else if (bear) point_refine_kernel<true><<<grid, 128, 0, st>>>(Q, board_out, optimized, bear, RsPass{});
+  else point_refine_kernel<false><<<grid, 128, 0, st>>>(Q, board_out, optimized, nullptr, RsPass{});
   count_launch();
 }
 
@@ -582,7 +700,7 @@ icc_status read_poses(cudaStream_t st, const BoardViews& B, double* q_wc, double
 }
 
 icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const int32_t* ids, const std::vector<int>& obs_view, DevBuf<double4>& d_out, std::vector<double>& points_out, int& n_opt, std::string& err,
-                               const double4* bear) {
+                               const double4* bear, const RsPass* rs) {
   const int np = Q.n_points;
   std::vector<int> pt_off, pt_obs;
   build_point_adjacency(np, nc, ids, [&](int c) { return obs_view[c] >= 0; }, pt_off, pt_obs);
@@ -590,7 +708,7 @@ icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const in
   CU(d_view.upload(obs_view)); CU(d_pt_off.upload(pt_off)); CU(d_pt_obs.alloc(std::max<size_t>(1, pt_obs.size()))); CU(d_opt.alloc(np)); CU(d_out.alloc(np));
   if (!pt_obs.empty()) CU(cudaMemcpy(d_pt_obs.p, pt_obs.data(), pt_obs.size() * sizeof(int), cudaMemcpyHostToDevice));
   Q.pt_off = d_pt_off.p; Q.pt_obs = d_pt_obs.p; Q.obs_view = d_view.p;
-  launch_point_refine(Q, bear, d_out.p, d_opt.p, st);
+  launch_point_refine(Q, bear, d_out.p, d_opt.p, st, rs);
   std::vector<int> opt(np); points_out.resize(4 * (size_t)np);
   CU(cudaMemcpyAsync(points_out.data(), d_out.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(opt.data(), d_opt.p, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -647,34 +765,91 @@ static icc_status alloc_tangent(int pose_error, BoardViews& B, std::string& err)
   return ICC_OK;
 }
 
+// Rolling shutter: the views' time order, the largest neighbour gap (2.5 x the median positive spacing of the view times; -1 when there is
+// none, so that no view has a neighbour) and the per-view velocities and neighbour counts of the rolling-shutter passes
+struct RsState { DevBuf<int> order, nbr; DevBuf<double> ts, vel; double max_gap = -1.0; };
+
+static icc_status rs_prepare(cudaStream_t st, int nf, const double* frame_t, RsState& R, std::string& err) {
+  std::vector<int> order(nf);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return frame_t[a] < frame_t[b]; });
+  std::vector<double> ts(nf), gaps;
+  for (int i = 0; i < nf; ++i) ts[i] = frame_t[order[i]];
+  for (int i = 1; i < nf; ++i) if (ts[i] - ts[i - 1] > 0.0) gaps.push_back(ts[i] - ts[i - 1]);
+  if (!gaps.empty()) {
+    std::sort(gaps.begin(), gaps.end());
+    const size_t m = gaps.size() / 2;
+    R.max_gap = 2.5 * (gaps.size() % 2 ? gaps[m] : 0.5 * (gaps[m - 1] + gaps[m]));
+  }
+  CU(R.order.upload(order.data(), nf, st)); CU(R.ts.upload(ts.data(), nf, st)); CU(R.vel.alloc(6 * (size_t)nf)); CU(R.nbr.alloc(nf));
+  return ICC_OK;
+}
+
+// the velocities of B's views from their current poses
+static void rs_velocities(BoardViews& B, RsState& R, cudaStream_t st) {
+  launch_view_velocities(B.nf, R.order.p, R.ts.p, R.max_gap, B.q.p, B.p.p, B.valid.p, R.vel.p, R.nbr.p, st);
+}
+
+// one rolling-shutter pass (Q.refine_only = 1): the velocities from the current poses, then the refinement of every valid view with them
+static void rs_pass(const PoseProblem& Q, BoardViews& B, int pose_error, RsState& R, double line_delay, cudaStream_t st) {
+  rs_velocities(B, R, st);
+  const RsPass rsp{B.uv.p, R.vel.p, line_delay};
+  if (pose_error == ICC_POSE_ERROR_TANGENT) launch_board_poses_rs(Q, B.bear.p, B.ok.p, B.use.p, rsp, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+  else launch_board_poses_rs(Q, B.xy.p, B.ok.p, B.use.p, rsp, B.q.p, B.p.p, B.e.p, B.valid.p, st);
+}
+
+// the velocities of the last pass and the number of valid views without a neighbour to the caller (both optional); waits for the stream
+static icc_status rs_read(cudaStream_t st, int nf, RsState& R, const PoseShutter& S, std::string& err) {
+  std::vector<int> nbr(nf);
+  if (S.vel) CU(cudaMemcpyAsync(S.vel, R.vel.p, 6 * (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(nbr.data(), R.nbr.p, (size_t)nf * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (S.n_static) *S.n_static = (int32_t)std::count(nbr.begin(), nbr.end(), 0);
+  return ICC_OK;
+}
+
 icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
-                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid, std::string& err) {
+                                const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc, double* mean_err,
+                                int32_t* valid, std::string& err) {
   BoardViews B;
   icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
   rc = alloc_tangent(pose_error, B, err); if (rc != ICC_OK) return rc;
-  launch_views(unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points, pose_error), B, pose_error, st);
+  PoseProblem Q = unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points, pose_error);
+  launch_views(Q, B, pose_error, st);
+  RsState R;
+  if (shutter.line_delay > 0.0) {             // two rolling-shutter passes from the global-shutter poses; a view dropped by a pass stays dropped
+    rc = rs_prepare(st, nf, shutter.frame_t, R, err); if (rc != ICC_OK) return rc;
+    Q.refine_only = 1;
+    for (int pass = 0; pass < 2; ++pass) rs_pass(Q, B, pose_error, R, shutter.line_delay, st);
+    rc = rs_read(st, nf, R, shutter, err); if (rc != ICC_OK) return rc;
+  }
   rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
   if (cudaGetLastError() != cudaSuccess) { err = "pose kernels failed"; return ICC_ERR_CUDA; }
   return ICC_OK;
 }
 
 icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
-                                 const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, double* q_wc, double* p_wc, double* mean_err, int32_t* valid,
-                                 std::vector<double>& points_out, int32_t* n_opt_out, std::string& err) {
+                                 const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc,
+                                 double* mean_err, int32_t* valid, std::vector<double>& points_out, int32_t* n_opt_out, std::string& err) {
   BoardViews B;
   icc_status rc = upload_board_views(st, np, points, nf, off, ids, uv, B, err); if (rc != ICC_OK) return rc;
   rc = alloc_tangent(pose_error, B, err); if (rc != ICC_OK) return rc;
   const int nc = B.nc;
+  const bool rolling = shutter.line_delay > 0.0;
+  RsState R;
+  if (rolling) { rc = rs_prepare(st, nf, shutter.frame_t, R, err); if (rc != ICC_OK) return rc; }
   CU(B.q.upload(q_wc, 4 * (size_t)nf, st)); CU(B.p.upload(p_wc, 3 * (size_t)nf, st)); CU(B.valid.upload(valid, nf, st));
   CU(cudaMemsetAsync(B.e.p, 0, (size_t)nf * sizeof(double), st));   // views that are not valid keep a zero error
   PoseProblem Q = unproject_corners(st, model, intr, W, H, B, max_reproj_error, min_points, pose_error);
   Q.refine_only = 1;
-  // 1. the stored poses and their inlier sets (what the pose dataset holds after EstimatePosesFromJson)
-  launch_views(Q, B, pose_error, st);
+  // 1. the stored poses and their inlier sets (what the pose dataset holds after EstimatePosesFromJson); rolling shutter: one pass
+  if (rolling) rs_pass(Q, B, pose_error, R, shutter.line_delay, st);
+  else launch_views(Q, B, pose_error, st);
   std::vector<unsigned char> use(std::max(1, nc)); std::vector<int> vh(nf); std::vector<double> qh(4 * (size_t)nf), ph(3 * (size_t)nf);
   CU(cudaMemcpyAsync(use.data(), B.use.p, (size_t)std::max(1, nc), cudaMemcpyDeviceToHost, st));
   rc = read_poses(st, B, qh.data(), ph.data(), nullptr, vh.data(), err); if (rc != ICC_OK) return rc;
-  // 2. OptimizeBoardPoints: one warp per point over its inlier observations in valid views, cameras constant
+  // 2. OptimizeBoardPoints: one warp per point over its inlier observations in valid views, cameras constant (rolling shutter: with the
+  //    velocities of the poses of step 1)
   std::vector<int> obs_view(std::max(1, nc), -1);
   for (int f = 0; f < nf; ++f) if (vh[f]) for (int c = off[f]; c < off[f + 1]; ++c) if (use[c]) obs_view[c] = f;
   for (int f = 0; f < nf; ++f) for (int d = 0; d < 3; ++d) qh[4 * f + d] = -qh[4 * f + d];   // R_cw = conj(q_wc)
@@ -685,10 +860,18 @@ icc_status optimize_board_points(cudaStream_t st, int model, const double intr[1
   PQ.normalized = 1; PQ.n_points = np; PQ.min_obs = min_observations > 0 ? min_observations : 30; PQ.huber = 1.345;
   PQ.board_in = B.board.p; PQ.meas = B.xy.p; PQ.q_cw = d_qcw.p; PQ.cam_c = d_c.p;
   int n_opt = 0;
-  rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, n_opt, err, pose_error == ICC_POSE_ERROR_TANGENT ? B.bear.p : nullptr); if (rc != ICC_OK) return rc;
-  // 3. OptimizeAllPoses on the new points
+  const RsPass rsp{B.uv.p, R.vel.p, shutter.line_delay};
+  if (rolling) rs_velocities(B, R, st);
+  rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, n_opt, err, pose_error == ICC_POSE_ERROR_TANGENT ? B.bear.p : nullptr, rolling ? &rsp : nullptr);
+  if (rc != ICC_OK) return rc;
+  // 3. OptimizeAllPoses on the new points (rolling shutter: one pass)
   Q.board = d_board2.p;
-  launch_views(Q, B, pose_error, st);
+  if (rolling) {
+    rs_pass(Q, B, pose_error, R, shutter.line_delay, st);
+    rc = rs_read(st, nf, R, shutter, err); if (rc != ICC_OK) return rc;
+  } else {
+    launch_views(Q, B, pose_error, st);
+  }
   rc = read_poses(st, B, q_wc, p_wc, mean_err, valid, err); if (rc != ICC_OK) return rc;
   if (cudaGetLastError() != cudaSuccess) { err = "board point kernels failed"; return ICC_ERR_CUDA; }
   if (n_opt_out) *n_opt_out = n_opt;
