@@ -16,6 +16,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -882,10 +883,11 @@ EvalStreams eval_schedule(icc_handle* h) {
   ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0}); ic.push_back({poff, 0, 0, 0, 0, 0, 0, 0});
   ipoff.push_back(poff); ipoff.push_back(poff);
   const Walk wv = walk(vpoff, nvf), wi = walk(ipoff, nic);
-  int W = h->sm_count * eval_tmem_warps();
-  // ICC_TMEM_RUNS=n caps the runs at n (tests: every warp then owns several chunks and carries its tile state between them)
-  if (const char* e = getenv("ICC_TMEM_RUNS")) { const int n = atoi(e); if (n > 0) W = std::min(W, n); }
-  auto split = [W](const Walk& w) {      // even runs, one per warp
+  // at most one run per warp of the item type's persistent launch (one CTA per SM)
+  int cap = INT_MAX;   // ICC_TMEM_RUNS=n caps the runs at n (tests: every warp then owns several chunks and carries its tile state between them)
+  if (const char* e = getenv("ICC_TMEM_RUNS")) { const int n = atoi(e); if (n > 0) cap = n; }
+  auto split = [h, cap](const Walk& w, bool imu) {      // even runs, one per warp
+    const int W = std::min(h->sm_count * eval_tmem_warps(imu), cap);
     const int nc = (int)w.pos.size(), n_items = std::min(W, nc);
     std::vector<VisItem> items((size_t)n_items);
     for (int k = 0; k < n_items; ++k) {
@@ -893,7 +895,7 @@ EvalStreams eval_schedule(icc_handle* h) {
       items[(size_t)k] = {w.unit[a], w.pos[a], b < nc ? w.pos[b] : w.total, 0};
     }
     return items; };
-  h->vitems = split(wv); h->iitems = split(wi);
+  h->vitems = split(wv, false); h->iitems = split(wi, true);
   P.n_vchunks = (int)wv.pos.size(); P.n_ichunks = (int)wi.pos.size();
   P.n_vframes = nvf; P.n_vitems = (int)h->vitems.size(); P.n_icells = nic; P.n_iitems = (int)h->iitems.size();
   return es;

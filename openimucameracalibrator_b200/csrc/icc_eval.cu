@@ -540,12 +540,12 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
   // Jacobian evaluations of the standard column sets run as items of the persistent shared-memory-parking kernel (icc_eval_tmem.cu), which owns
   // every SM (one CTA each); whatever is not eligible (camera intrinsics / bias knots / IMU intrinsics free) follows on the same stream.
   const bool legacy_vision = getenv("ICC_VISION_LEGACY") != nullptr;   // A/B switch for profiling only (read per call)
-  // size test: the persistent kernel pays off once every warp has a few chunks (BASELINE config 4: 7.6 vision / 1.8 IMU chunks per warp);
+  // size test: the persistent kernel pays off once every warp has a few chunks (BASELINE config 4: 5.7 vision / 1.8 IMU chunks per warp);
   // below that the one-warp-per-frame / per-cell kernels finish sooner and run side by side
-  const int tm_warps = sm_count * eval_tmem_warps();
-  const bool tmem_vision = with_jacobian && !P.cam_intr_active && P.n_vitems > 0 && P.rolling && !legacy_vision && (P.n_vchunks >= 3 * tm_warps || getenv("ICC_TMEM_ALWAYS"));
+  const int tm_vwarps = sm_count * eval_tmem_warps(false), tm_iwarps = sm_count * eval_tmem_warps(true);
+  const bool tmem_vision = with_jacobian && !P.cam_intr_active && P.n_vitems > 0 && P.rolling && !legacy_vision && (P.n_vchunks >= 3 * tm_vwarps || getenv("ICC_TMEM_ALWAYS"));
   const bool legacy_imu = getenv("ICC_IMU_LEGACY") != nullptr;
-  const bool tmem_imu = with_jacobian && !P.bias_active && !P.intr_active && P.n_iitems > 0 && P.n_iwork > 0 && !legacy_imu && (2 * P.n_ichunks >= 3 * tm_warps || getenv("ICC_TMEM_ALWAYS"));
+  const bool tmem_imu = with_jacobian && !P.bias_active && !P.intr_active && P.n_iitems > 0 && P.n_iwork > 0 && !legacy_imu && (2 * P.n_ichunks >= 3 * tm_iwarps || getenv("ICC_TMEM_ALWAYS"));
   const bool fork = aux && P.n_vwork > 0 && P.rolling && P.n_iwork > 0 && !tmem_vision && !tmem_imu;
   cudaStream_t st = st_main;
   if (fork) { cudaEventRecord(aux->fork, st_main); cudaStreamWaitEvent(aux->stream, aux->fork, 0); }

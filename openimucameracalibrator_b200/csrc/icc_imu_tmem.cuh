@@ -23,7 +23,8 @@ namespace tmi {
 constexpr int IW = 6;                        // warps per CTA
 constexpr int LDT = TILE_LD, TCOLS = TILE_COLS;
 constexpr int TM_ACCA = 0, TM_ACCG = 30, TM_PARK = 42;   // park offsets in doubles per lane
-static_assert(TM_PARK + ACC_PARK <= PARK_DOUBLES && TM_PARK + GYR_PARK <= PARK_DOUBLES, "park layout");
+constexpr int PARK_N = 85;                   // park doubles per lane: 30 + 12 accumulators + 43 deferred-row doubles
+static_assert(TM_PARK + ACC_PARK <= PARK_N && TM_PARK + GYR_PARK <= PARK_N, "park layout");
 
 struct ImuSlot {
   ImuWin win[2];
@@ -195,7 +196,7 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst
         accel_part(L, *K, tile, part ? nA >> 2 : 0, part ? n >> 2 : nA >> 2, part ? true : fresh, part ? lastB : lastA, slot->gidxA[part ? cur ^ 1 : cur], ta, lane);
       __syncwarp();
       // ---- gyroscope ------------------------------------------------------------------------------------------------------
-      if (lock) asm volatile("bar.sync %0, %1;" :: "r"(bar_id + 6), "r"(bar_n) : "memory");
+      if (lock) asm volatile("bar.sync %0, %1;" :: "r"(bar_id + IW), "r"(bar_n) : "memory");
       {
         double park[GYR_PARK];
         double* row0 = tile + lane;
@@ -224,7 +225,7 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst
       pos += n;
     }
   }
-  while (rounds-- > 0) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); asm volatile("bar.sync %0, %1;" :: "r"(bar_id + 6), "r"(bar_n) : "memory"); }
+  while (rounds-- > 0) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); asm volatile("bar.sync %0, %1;" :: "r"(bar_id + IW), "r"(bar_n) : "memory"); }
 }
 
 }  // namespace tmi

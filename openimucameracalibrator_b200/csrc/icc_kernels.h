@@ -95,7 +95,8 @@ struct EvalAux { cudaStream_t stream; cudaEvent_t fork, join; };
 // Persistent Jacobian evaluation, vision + IMU items in one launch (icc_eval_tmem.cu); non-zero on a launch error.
 // P.vitems[k] / P.iitems[k] is the run of global warp k; the two item types go out as two launches of the same kernel.
 int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st);
-int eval_tmem_warps();
+// warps per CTA of the persistent kernel's vision (imu_items = false) or IMU launch
+int eval_tmem_warps(bool imu_items);
 int launch_eval(const DeviceProblem& P, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, double* reproj_out, cudaStream_t st, const EvalAux* aux = nullptr);
 // scale[i] = 1/(1+sqrt(H_ii)) (Jacobi scaling, computed once per optimize) ; gradient inf-norm
 void launch_compute_scale(const DeviceProblem& P, double* scale, int jacobi, double* scal, cudaStream_t st);

@@ -5,8 +5,6 @@
 
 namespace icc {
 
-constexpr int PARK_DOUBLES = 85;       // per lane: the largest park layout (IMU items: 30 + 12 accumulators + 43 parked doubles)
-
 // p = warp park + lane + 32 * (first double)
 template <int N>
 __device__ __forceinline__ void park_st(double* __restrict__ p, const double (&v)[N]) {

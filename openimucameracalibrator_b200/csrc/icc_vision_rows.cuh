@@ -54,19 +54,24 @@ ICC_HD void sincos_small(double x, double* s, double* c) {
   }
 }
 
-// One corner.  xrow: entry c of the x row is written to xrow[c * ldx] (c = 0..43).  yr: the y row in the parked layout.
+// One corner.  xrow: entry c of the x row is written to xrow[c * ldx] (c = 0..43).  yr: entry j of the y row in the parked layout
+// is written to yr[j * ldy] as soon as it is known, so that the kernel can send it straight to its shared-memory park instead of
+// holding the whole row in registers until the end of the corner.
 // Failed projection (quirk q12): both residuals are the constant 1e10 with zero Jacobian rows.
 template <int MODEL>   // MODEL >= 0: that camera model only; -1: runtime dispatch on K.model (host tests)
-ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double (&yr)[YR_N], double& r0, double& r1) {
+ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double* __restrict__ yr, int ldy, double& r0, double& r1) {
   const double us = W.u_so3 + oy * K.ld, ur = W.u_r3 + oy * K.ld;   // residuals.h:344-346: row time added to the normalised u
-  double lam[5], dlam[5], sn[5], cs[5];
-  cum_coeffs6(us, lam, dlam);
+  double sn[5], cs[5];
   Q4 q = W.q0;
+  {
+    double lam[5], dlam[5];
+    cum_coeffs6(us, lam, dlam);
 #pragma unroll
-  for (int i = 0; i < 5; ++i) {
-    sincos_small(0.5 * lam[i] * W.th[i], &sn[i], &cs[i]);
-    const V3 ax = W.dh[i];
-    q = qmul(q, q4(sn[i] * ax.x, sn[i] * ax.y, sn[i] * ax.z, cs[i]));
+    for (int i = 0; i < 5; ++i) {
+      sincos_small(0.5 * lam[i] * W.th[i], &sn[i], &cs[i]);
+      const V3 ax = W.dh[i];
+      q = qmul(q, q4(sn[i] * ax.x, sn[i] * ax.y, sn[i] * ax.z, cs[i]));
+    }
   }
   double cc[6], dc[6];
   coeffs6(ur, cc, dc, nullptr);
@@ -83,21 +88,48 @@ ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, doubl
     for (int c = 0; c < VIS_RES_COL; ++c) xrow[c * ldx] = 0.0;
     xrow[VIS_RES_COL * ldx] = r0;
 #pragma unroll
-    for (int c = 0; c < YR_N; ++c) yr[c] = 0.0;
-    yr[YR_R] = r1;
+    for (int c = 0; c < YR_N; ++c) yr[c * ldy] = c == YR_R ? r1 : 0.0;
     return;
   }
   r0 = pr.u - ox; r1 = pr.v - oy;             // residuals.h:395-398, cov = I
-  V3 w[2], zn[2], mt[2], Dp[2];
-  double du[2];
+  // Everything but the SO(3) knot columns and the line delay is written before the knot recursion, so that the point, the
+  // projection Jacobian and the R^3 coefficients are dead while it runs.
+  V3 w[2], zn[2];
+  double du[2], mtd[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    Dp[r] = v3(pr.J[3 * r], pr.J[3 * r + 1], pr.J[3 * r + 2]);
-    const V3 mq = mul(K.Ric, Dp[r]);          // Dp R_ic^T as a covector
+    const V3 Dp = v3(pr.J[3 * r], pr.J[3 * r + 1], pr.J[3 * r + 2]);
+    const V3 mq = mul(K.Ric, Dp);             // Dp R_ic^T as a covector
     w[r] = cross(mq, qi);                     // d r / d theta (right increment of R_w_i)
-    mt[r] = mul(R, mq);                       // covector of the translation
+    const V3 mt = mul(R, mq);                 // covector of the translation
     zn[r] = v3(0, 0, 0); du[r] = 0.0;
+    mtd[r] = dot(mt, tdot);
+    const V3 om = cross(Dp, pc);
+    if (r == 0) {
+#pragma unroll
+      for (int j = 0; j < 6; ++j) { xrow[(18 + 3 * j + 0) * ldx] = -cc[j] * mt.x; xrow[(18 + 3 * j + 1) * ldx] = -cc[j] * mt.y; xrow[(18 + 3 * j + 2) * ldx] = -cc[j] * mt.z; }
+      xrow[36 * ldx] = -Dp.x; xrow[37 * ldx] = -Dp.y; xrow[38 * ldx] = -Dp.z;
+      xrow[39 * ldx] = om.x; xrow[40 * ldx] = om.y; xrow[41 * ldx] = om.z;
+      xrow[VIS_RES_COL * ldx] = r0;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 6; ++j) yr[(YR_CC + j) * ldy] = cc[j];
+      yr[YR_MT * ldy] = mt.x; yr[(YR_MT + 1) * ldy] = mt.y; yr[(YR_MT + 2) * ldy] = mt.z;
+      yr[YR_DP * ldy] = Dp.x; yr[(YR_DP + 1) * ldy] = Dp.y; yr[(YR_DP + 2) * ldy] = Dp.z;
+      yr[YR_OM * ldy] = om.x; yr[(YR_OM + 1) * ldy] = om.y; yr[(YR_OM + 2) * ldy] = om.z;
+      yr[YR_R * ldy] = r1;
+      yr[(YR_N - 1) * ldy] = 0.0;
+    }
   }
+  // lambda and its derivative again rather than kept through the projection: ten doubles fewer at the kernel's register peak (the
+  // persistent kernel holds its tensor-core accumulators next to this chain).  The empty asm keeps the compiler from merging the two
+  // evaluations back into one; the values are the same bits.
+  double us_again = us;
+#ifdef __CUDA_ARCH__
+  asm volatile("" : "+d"(us_again));
+#endif
+  double lam[5], dlam[5];
+  cum_coeffs6(us_again, lam, dlam);
 #pragma unroll
   for (int i = 4; i >= 0; --i) {              // increment i couples knots i and i+1
     const double sphi = 2.0 * sn[i] * cs[i], omc = 2.0 * sn[i] * sn[i];          // sin(phi), 1 - cos(phi), phi = lambda_i theta_i
@@ -112,30 +144,20 @@ ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, doubl
       zn[r] = mul(W.jri[i], z);                         // knot i:   -Jr^-1(d_i) z  (= -z Jl^-1)
       w[r] = v3(w[r].x - sphi * xd.x + omc * xdd.x, w[r].y - sphi * xd.y + omc * xdd.y, w[r].z - sphi * xd.z + omc * xdd.z);   // exp(lambda d) w
       if (r == 0) { xrow[(3 * (i + 1) + 0) * ldx] = up.x; xrow[(3 * (i + 1) + 1) * ldx] = up.y; xrow[(3 * (i + 1) + 2) * ldx] = up.z; }
-      else { yr[YR_SO3 + 3 * (i + 1) + 0] = up.x; yr[YR_SO3 + 3 * (i + 1) + 1] = up.y; yr[YR_SO3 + 3 * (i + 1) + 2] = up.z; }
+      else { yr[(YR_SO3 + 3 * (i + 1) + 0) * ldy] = up.x; yr[(YR_SO3 + 3 * (i + 1) + 1) * ldy] = up.y; yr[(YR_SO3 + 3 * (i + 1) + 2) * ldy] = up.z; }
     }
   }
   {
     const V3 k0 = w[0] - zn[0], k1 = w[1] - zn[1];
     xrow[0] = k0.x; xrow[ldx] = k0.y; xrow[2 * ldx] = k0.z;
-    yr[YR_SO3 + 0] = k1.x; yr[YR_SO3 + 1] = k1.y; yr[YR_SO3 + 2] = k1.z;
+    yr[(YR_SO3 + 0) * ldy] = k1.x; yr[(YR_SO3 + 1) * ldy] = k1.y; yr[(YR_SO3 + 2) * ldy] = k1.z;
   }
-#pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    xrow[(18 + 3 * j + 0) * ldx] = -cc[j] * mt[0].x; xrow[(18 + 3 * j + 1) * ldx] = -cc[j] * mt[0].y; xrow[(18 + 3 * j + 2) * ldx] = -cc[j] * mt[0].z;
-    yr[YR_CC + j] = cc[j];
-  }
-  const V3 om0 = cross(Dp[0], pc), om1 = cross(Dp[1], pc);
-  xrow[36 * ldx] = -Dp[0].x; xrow[37 * ldx] = -Dp[0].y; xrow[38 * ldx] = -Dp[0].z;
-  xrow[39 * ldx] = om0.x; xrow[40 * ldx] = om0.y; xrow[41 * ldx] = om0.z;
-  xrow[42 * ldx] = oy * (du[0] - dot(mt[0], tdot));
-  xrow[VIS_RES_COL * ldx] = r0;
-  yr[YR_MT] = mt[1].x; yr[YR_MT + 1] = mt[1].y; yr[YR_MT + 2] = mt[1].z;
-  yr[YR_DP] = Dp[1].x; yr[YR_DP + 1] = Dp[1].y; yr[YR_DP + 2] = Dp[1].z;
-  yr[YR_OM] = om1.x; yr[YR_OM + 1] = om1.y; yr[YR_OM + 2] = om1.z;
-  yr[YR_LD] = oy * (du[1] - dot(mt[1], tdot));
-  yr[YR_R] = r1;
-  yr[YR_N - 1] = 0.0;
+  xrow[42 * ldx] = oy * (du[0] - mtd[0]);
+  yr[YR_LD * ldy] = oy * (du[1] - mtd[1]);
+}
+template <int MODEL>
+ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double (&yr)[YR_N], double& r0, double& r1) {
+  vision_corner_rows<MODEL>(W, K, X, ox, oy, xrow, ldx, yr, 1, r0, r1);
 }
 
 // Expand a parked y row into tile entries (what the kernel does after the x rows have been consumed); also used by the CPU test.

@@ -3,12 +3,13 @@
 // Same arithmetic contract as vision_kernel<1> of icc_eval.cu (reference: RSReprojectionCostFunctorSplit<6>::operator(),
 // basalt_spline/ceres_calib_split_residuals.h:319-402, under Ceres autodiff + LieLocalParameterization), re-mapped to the machine:
 //
-//  * ONE persistent CTA per SM.  The 21 FP64 tensor-core accumulator fragments (42 doubles per lane, live for a whole frame)
-//    would otherwise co-exist with the per-corner spline chain; here they are PARKED in the warp's lane-private shared-memory
-//    park (icc_park.cuh) while the warp is in its SIMT phase, and only live in registers during the DMMA phases.
+//  * ONE persistent CTA of eight warps per SM (two per SM sub-partition).  The 21 FP64 tensor-core accumulator fragments (42 doubles
+//    per lane) stay in registers for the warp's whole run, next to the per-corner spline chain.
 //  * Both rows of a corner are evaluated in ONE pass (icc_vision_rows.cuh): the x row goes to the warp's shared-memory tile, the
-//    y row (36 doubles, R^3 block factored) is parked and expanded into the same tile after the x rows have been contracted.
-//    Nothing of the spline chain survives a tensor-core phase, so nothing spills.
+//    y row (36 doubles, R^3 block factored) goes entry by entry to the warp's lane-private shared-memory park (icc_park.cuh) and is
+//    expanded into the same tile after the x rows have been contracted.  Neither row is held in registers, so chain and
+//    accumulators fit in 255 registers together and nothing spills; the park is 36 instead of 78 doubles per lane, which is what
+//    lets eight warps' tiles and parks fit in one block's shared memory.
 //  * The corners of all frames form ONE packed stream (frames padded to a multiple of 4 = one m8n8k4 k-step) that is cut into
 //    equal runs of 32-lane chunks, one run per warp: no partial last wave, no half-empty chunk at the end of a 144-corner frame.
 //    A chunk may straddle two frames (two staged knot windows, lanes pick theirs); the k-steps of the first frame finish its
@@ -24,9 +25,9 @@
 namespace icc {
 namespace tmv {
 
-constexpr int VW = 6;                  // warps per CTA
+constexpr int VW = 8;                  // warps per CTA: two per SM sub-partition
 constexpr int LDT = TILE_LD, TCOLS = TILE_COLS;   // 44 tile columns used
-constexpr int TM_ACC = 0, TM_YROW = 42;          // park offsets in doubles per lane
+constexpr int PARK_N = YR_N;           // park doubles per lane: the y row
 constexpr int NBLK = 21;               // upper block triangle of 6 x 6 blocks of 8 columns
 
 struct WarpSlot {
@@ -62,29 +63,21 @@ __device__ __noinline__ void stage_frame(WarpSlot* slot, int w, VisFrame F, Stag
   __syncwarp();
 }
 
-// One tile part: rows [4 k0, 4 k1) of the chunk belong to one frame.
-//   first: the frame's tile starts here (accumulators zero) -- otherwise they are fetched from the park;
-//   last:  the frame's tile (or the item) ends here: scatter -- otherwise park the accumulators.
-ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool first, bool last, const int* __restrict__ gidx, double* ta, int lane) {
-  double acc[2 * NBLK];
-  if (first) {
-#pragma unroll
-    for (int i = 0; i < 2 * NBLK; ++i) acc[i] = 0.0;
-  } else {
-    park_ld(ta + 32 * TM_ACC, acc);
-  }
+// One tile part: rows [4 k0, 4 k1) of the chunk belong to one frame.  acc holds the frame's accumulators (zero when its tile starts
+// here); last: the frame's tile (or the item) ends here: scatter them and zero them for the next frame.
+ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k1, bool last, const int* __restrict__ gidx, double (&acc)[2 * NBLK], double* ta, int lane) {
   tile_syrk<6>(tile, k0, k1, acc);                       // x rows
   __syncwarp();
   {                                               // expand the parked y rows of this part into the tile (same rows)
     const bool mine = lane >= 4 * k0 && lane < 4 * k1;
     double* yrow = tile + lane;
     double h[18];
-    park_ld(ta + 32 * TM_YROW, h);
+    park_ld(ta, h);
     if (mine) {
 #pragma unroll
       for (int c = 0; c < 18; ++c) yrow[c * LDT] = h[c];
     }
-    park_ld(ta + 32 * (TM_YROW + 18), h);       // [m_t 0..2 | Dp 3..5 | om 6..8 | ld 9 | r 10 | cc 11..16 | pad]
+    park_ld(ta + 32 * 18, h);                   // [m_t 0..2 | Dp 3..5 | om 6..8 | ld 9 | r 10 | cc 11..16 | pad]
     if (mine) {
 #pragma unroll
       for (int j = 0; j < 6; ++j) {
@@ -101,8 +94,8 @@ ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
   __syncwarp();
   if (last) {
     tile_flush<6, 4>(L, gidx, acc);
-  } else {
-    park_st(ta + 32 * TM_ACC, acc);
+#pragma unroll
+    for (int i = 0; i < 2 * NBLK; ++i) acc[i] = 0.0;
   }
 }
 
@@ -120,18 +113,19 @@ ICC_D void init_const(VisConst* K, const DeviceProblem& P, const DeviceState& S,
 template <int MODEL>
 ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
   StageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_tic = P.col_tic; A.col_ld = P.col_ld;
+  double acc[2 * NBLK];                           // the current frame's tile accumulators, in registers for the whole run
+#pragma unroll
+  for (int i = 0; i < 2 * NBLK; ++i) acc[i] = 0.0;
   {
     int f = it.vf0, pos = it.pos_begin, cur = 0;
     stage_frame(slot, cur, P.vframes[f], A);
     int endF = min(P.vframes[f + 1].poff, it.pos_end);
-    bool fresh = true;
     while (pos < it.pos_end) {
       if (rounds > 0) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); --rounds; }   // loose lockstep of the warps of a group: instruction-cache locality (icc_eval_tmem.cu)
       if (pos == endF) {                          // the previous chunk finished its frame exactly at the chunk boundary
         ++f;
         stage_frame(slot, cur, P.vframes[f], A);
         endF = min(P.vframes[f + 1].poff, it.pos_end);
-        fresh = true;
       }
       const int nA = min(32, endF - pos);
       int nB = 0, endB = 0;
@@ -146,33 +140,30 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst
         const bool inA = lane < nA;
         const int w = inA ? cur : cur ^ 1;
         const int rel = inA ? pos + lane - slot->finfo[w][0] : lane - nA;
-        double yr[YR_N];
         double* xrow = tile + lane;
         if (lane < n && rel < slot->finfo[w][2]) {
           const int c = slot->finfo[w][1] + rel;
           const double2 ob = P.uv[c];
           const double4 X = P.board[P.pid[c]];
           double r0, r1;
-          vision_corner_rows<MODEL>(slot->win[w], *K, v3(X.x, X.y, X.z), ob.x, ob.y, xrow, LDT, yr, r0, r1);
+          vision_corner_rows<MODEL>(slot->win[w], *K, v3(X.x, X.y, X.z), ob.x, ob.y, xrow, LDT, ta, 32, r0, r1);   // y row straight to the park
           if (res_out) { res_out[2 * c] = r0; res_out[2 * c + 1] = r1; }
         } else {                                  // padding lane of a frame whose corner count is not a multiple of 4, or beyond the chunk
 #pragma unroll
           for (int c = 0; c <= VIS_RES_COL; ++c) xrow[c * LDT] = 0.0;
 #pragma unroll
-          for (int c = 0; c < YR_N; ++c) yr[c] = 0.0;
+          for (int c = 0; c < PARK_N; ++c) ta[32 * c] = 0.0;
         }
-        park_st(ta + 32 * TM_YROW, yr);
       }
       __syncwarp();
       // ---- tensor-core passes: the rows of the frame that ends first, then (straddling chunk) the rows of the next frame --------
+      // (a straddling chunk always ends the first frame in part 0, so part 1 starts from zeroed accumulators)
 #pragma unroll 1
       for (int part = 0; part < (nB ? 2 : 1); ++part) {
         const int k0 = part ? nA >> 2 : 0, k1 = part ? n >> 2 : nA >> 2;
-        const bool first = part ? true : fresh;
         const bool last = part ? endF + nB == endB : pos + nA == endF;
-        tile_part(L, tile, k0, k1, first, last, slot->gidx[part ? cur ^ 1 : cur], ta, lane);
+        tile_part(L, tile, k0, k1, last, slot->gidx[part ? cur ^ 1 : cur], acc, ta, lane);
       }
-      fresh = false;
       if (nB) { ++f; cur ^= 1; endF = endB; }
       pos += n;
     }
