@@ -540,7 +540,7 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
   // Jacobian evaluations of the standard column sets run as items of the persistent shared-memory-parking kernel (icc_eval_tmem.cu), which owns
   // every SM (one CTA each); whatever is not eligible (camera intrinsics / bias knots / IMU intrinsics free) follows on the same stream.
   const bool legacy_vision = getenv("ICC_VISION_LEGACY") != nullptr;   // A/B switch for profiling only (read per call)
-  // size test: the persistent kernel pays off once every warp has a few chunks (BASELINE config 4: 5.7 vision / 1.8 IMU chunks per warp);
+  // size test: the persistent kernel pays off once every warp has a few chunks (BASELINE config 4 on 132 SMs: 12.8 vision / 3.1 IMU chunks per warp);
   // below that the one-warp-per-frame / per-cell kernels finish sooner and run side by side
   const int tm_vwarps = sm_count * eval_tmem_warps(false), tm_iwarps = sm_count * eval_tmem_warps(true);
   const bool tmem_vision = with_jacobian && !P.cam_intr_active && P.n_vitems > 0 && P.rolling && !legacy_vision && (P.n_vchunks >= 3 * tm_vwarps || getenv("ICC_TMEM_ALWAYS"));

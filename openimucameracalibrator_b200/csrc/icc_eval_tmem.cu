@@ -1,6 +1,6 @@
 // Persistent Jacobian evaluation kernel (sm_90a): every warp runs one contiguous run of the packed corner stream (vision items,
-// icc_vision_tmem.cuh) or of the packed IMU sample stream (IMU items, icc_imu_tmem.cuh), parking its deferred rows (IMU items: and
-// its tensor-core accumulators) in a lane-private shared-memory park (icc_park.cuh) between the tensor-core and SIMT phases.
+// icc_vision_tmem.cuh) or of the packed IMU sample stream (IMU items, icc_imu_tmem.cuh), with its tensor-core accumulators in
+// registers and its deferred rows parked in a lane-private shared-memory park (icc_park.cuh) between the SIMT and tensor-core phases.
 //
 // TWO launches per evaluation (vision items, then IMU items), each an instantiation with its own CTA shape: the unrolled FP64
 // recursions make this kernel large, and a launch that only walks one item type keeps its instruction working set to that type.
@@ -21,7 +21,7 @@ constexpr int IMU_ITEMS = -1;          // the MODEL argument of the IMU-item ins
 
 // CTA shape per item type: per warp a 13.5 KB tile, a lane-private park and a staging slot, plus the item type's constants.
 //   vision items: 8 warps x (13.5 KB tile + 9 KB park of the y row + 2.1 KB slot);
-//   IMU items:    6 warps x (13.5 KB tile + 21.3 KB park of accumulators and deferred rows + 2.6 KB slot).
+//   IMU items:    8 warps x (13.5 KB tile + 10.8 KB park of the deferred rows 1 and 2 + 2.6 KB slot).
 template <int MODEL>
 struct Cta {
   static constexpr bool imu = MODEL == IMU_ITEMS;
@@ -53,13 +53,14 @@ __global__ void __launch_bounds__(Cta<MODEL>::warps * 32, 1) eval_tmem_kernel(De
 
   const int gw = warp * gridDim.x + blockIdx.x;           // global warp: consecutive runs land on different SMs
   // lockstep groups: the whole CTA (groups == 1) or `groups` equal sets of warps (warp % groups; groups divides the CTA's warps), each
-  // with its own named barriers and started `stagger_ns` apart, so that one group's tensor-core phase meets the others' SIMT phases
+  // with its own named barrier (id 1 + group) and started `stagger_ns` apart, so that one group's tensor-core phase meets the others'
+  // SIMT phases
+  static_assert(C::warps < 16, "one named barrier per lockstep group, ids 1..groups");
   const int grp = warp % groups, bar_id = 1 + grp, bar_n = C::warps * 32 / groups;
   if (groups > 1 && stagger_ns > 0) for (int g = 0; g < grp; ++g) __nanosleep(stagger_ns);
   if constexpr (C::imu) {
-    static_assert(2 * tmi::IW < 16, "two named barriers per lockstep group");
     if (gw < P.n_iitems) tmi::run_item(P, S, reinterpret_cast<const ImuConst*>(smem_raw), reinterpret_cast<tmi::ImuSlot*>(slots + warp * C::slot_bytes), tile, ta, L, P.iitems[gw], res_out, lane, rounds, bar_id, bar_n);
-    else for (int r = 0; r < rounds; ++r) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); asm volatile("bar.sync %0, %1;" :: "r"(bar_id + tmi::IW), "r"(bar_n) : "memory"); }
+    else for (int r = 0; r < rounds; ++r) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); }
   } else {
     if (gw < P.n_vitems) tmv::run_item<MODEL>(P, S, reinterpret_cast<const VisConst*>(smem_raw), reinterpret_cast<tmv::WarpSlot*>(slots + warp * C::slot_bytes), tile, ta, L, P.vitems[gw], res_out, lane, rounds, bar_id, bar_n);
     else for (int r = 0; r < rounds; ++r) asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory");
@@ -78,8 +79,8 @@ int launch_model(const DeviceProblem& P, const DeviceState& S, double* residuals
   const int grid = (n_items + C::warps - 1) / C::warps < sm_count ? (n_items + C::warps - 1) / C::warps : sm_count;
   // loose lockstep: warps start every chunk together (one named barrier per chunk), so that they walk the same unrolled code at the
   // same time (instruction-cache locality).  The whole CTA steps together by default (ICC_TMEM_GROUPS = g splits it into g groups
-  // for any g > 1 that divides the CTA's warps, ICC_TMEM_STAGGER_NS delays group g by g x ns, ICC_TMEM_NO_LOCKSTEP lets every warp
-  // run free).
+  // for any g > 1 that divides the CTA's warps: 2, 4 or 8 for both item types, each group on its own named barrier; ICC_TMEM_STAGGER_NS
+  // delays group g by g x ns, ICC_TMEM_NO_LOCKSTEP lets every warp run free).
   const int rounds = getenv("ICC_TMEM_NO_LOCKSTEP") ? 0 : (n_chunks + n_items - 1) / n_items;
   const char* eg = getenv("ICC_TMEM_GROUPS"); const char* es = getenv("ICC_TMEM_STAGGER_NS");
   const int gq = eg ? atoi(eg) : 1, groups = (gq > 1 && gq <= C::warps && C::warps % gq == 0) ? gq : 1, stagger_ns = es ? atoi(es) : 0;

@@ -26,6 +26,7 @@ struct ImuConst {
   double w_acc, w_gyr;    // 1 / std_r3, 1 / std_so3
   double idt2;            // inv_r3_dt^2
   double inv_so3_dt;
+  double du_so3, du_r3, du_ba, du_bg;   // time-offset terms of the normalised spline times (persistent kernel only)
 };
 
 // Tile columns.  accelerometer: [so3 0..17 | r3 18..35 | gravity 36..38 | residual 39] (5 blocks of 8, no padding);
@@ -45,8 +46,11 @@ ICC_HD void coeffs6_dd_only(double u, double ddc[6]) {
   ddc[5] = k * (20.0 * u3);
 }
 
-// accelerometer rows.  row0: entry c at row0[c * ld] (c = 0..39).  park: rows 1 and 2 in the parked layout.
-ICC_HD void imu_accel_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_r3, double u_ba, V3 a_meas, double* __restrict__ row0, int ld, double (&park)[ACC_PARK], double (&ra)[3]) {
+// accelerometer rows.  row0: entry c at row0[c * ld] (c = 0..39).  pk: entry j of rows 1 and 2 in the parked layout is written to
+// pk[j * ldp] as soon as it is known, so that the kernel can send it straight to its shared-memory park instead of holding both rows
+// in registers until the end of the sample.  Everything but the SO(3) knot columns is written before the knot recursion, so that R,
+// the R^3 coefficients and the quaternion are dead while it runs.
+ICC_HD void imu_accel_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_r3, double u_ba, V3 a_meas, double* __restrict__ row0, int ld, double* __restrict__ pk, int ldp, double (&ra)[3]) {
   const FrameWin& F = W.f;
   double lam[5], dlam[5], sn[5], cs[5];
   cum_coeffs6(u_so3, lam, dlam);
@@ -71,6 +75,19 @@ ICC_HD void imu_accel_rows(const ImuWin& W, const ImuConst& K, double u_so3, dou
   ra[0] = K.w_acc * (h.x - (K.Ma[0] * a_raw.x + K.Ma[1] * a_raw.y + K.Ma[2] * a_raw.z));
   ra[1] = K.w_acc * (h.y - (K.Ma[3] * a_raw.x + K.Ma[4] * a_raw.y + K.Ma[5] * a_raw.z));
   ra[2] = K.w_acc * (h.z - (K.Ma[6] * a_raw.x + K.Ma[7] * a_raw.y + K.Ma[8] * a_raw.z));
+  // row 0: R^3 knots, gravity, residual.  m_t = R e_0 = first column of R
+  {
+    const V3 mt = v3(R.m[0], R.m[3], R.m[6]);
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+      const double s = K.w_acc * ddc[j] * K.idt2;
+      row0[(18 + 3 * j + 0) * ld] = s * mt.x; row0[(18 + 3 * j + 1) * ld] = s * mt.y; row0[(18 + 3 * j + 2) * ld] = s * mt.z;
+    }
+    row0[36 * ld] = K.w_acc * mt.x; row0[37 * ld] = K.w_acc * mt.y; row0[38 * ld] = K.w_acc * mt.z;
+    row0[ACC_RES_COL * ld] = ra[0];
+  }
+  pk[36 * ldp] = q.x; pk[37 * ldp] = q.y; pk[38 * ldp] = q.z; pk[39 * ldp] = q.w;
+  pk[40 * ldp] = ra[1]; pk[41 * ldp] = ra[2]; pk[42 * ldp] = u_r3;
   // d r_k / d theta = w_acc (e_k x h)  (row covector, right increment of R_w_i)
   V3 w[3], zn[3];
   // cross(e_0, h) = (0, -h.z, h.y), cross(e_1, h) = (h.z, 0, -h.x), cross(e_2, h) = (-h.y, h.x, 0)
@@ -92,26 +109,19 @@ ICC_HD void imu_accel_rows(const ImuWin& W, const ImuConst& K, double u_so3, dou
       zn[r] = mul(F.jri[i], z);
       w[r] = v3(w[r].x - sphi * xd.x + omc * xdd.x, w[r].y - sphi * xd.y + omc * xdd.y, w[r].z - sphi * xd.z + omc * xdd.z);
       if (r == 0) { row0[(3 * (i + 1) + 0) * ld] = up.x; row0[(3 * (i + 1) + 1) * ld] = up.y; row0[(3 * (i + 1) + 2) * ld] = up.z; }
-      else { park[18 * (r - 1) + 3 * (i + 1) + 0] = up.x; park[18 * (r - 1) + 3 * (i + 1) + 1] = up.y; park[18 * (r - 1) + 3 * (i + 1) + 2] = up.z; }
+      else { pk[(18 * (r - 1) + 3 * (i + 1) + 0) * ldp] = up.x; pk[(18 * (r - 1) + 3 * (i + 1) + 1) * ldp] = up.y; pk[(18 * (r - 1) + 3 * (i + 1) + 2) * ldp] = up.z; }
     }
   }
   {
     const V3 k0 = w[0] - zn[0], k1 = w[1] - zn[1], k2 = w[2] - zn[2];
     row0[0] = k0.x; row0[ld] = k0.y; row0[2 * ld] = k0.z;
-    park[0] = k1.x; park[1] = k1.y; park[2] = k1.z;
-    park[18] = k2.x; park[19] = k2.y; park[20] = k2.z;
+    pk[0] = k1.x; pk[ldp] = k1.y; pk[2 * ldp] = k1.z;
+    pk[18 * ldp] = k2.x; pk[19 * ldp] = k2.y; pk[20 * ldp] = k2.z;
   }
-  // row 0: R^3 knots, gravity, residual.  m_t = R e_0 = first column of R
-  const V3 mt = v3(R.m[0], R.m[3], R.m[6]);
-#pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    const double s = K.w_acc * ddc[j] * K.idt2;
-    row0[(18 + 3 * j + 0) * ld] = s * mt.x; row0[(18 + 3 * j + 1) * ld] = s * mt.y; row0[(18 + 3 * j + 2) * ld] = s * mt.z;
-  }
-  row0[36 * ld] = K.w_acc * mt.x; row0[37 * ld] = K.w_acc * mt.y; row0[38 * ld] = K.w_acc * mt.z;
-  row0[ACC_RES_COL * ld] = ra[0];
-  park[36] = q.x; park[37] = q.y; park[38] = q.z; park[39] = q.w;
-  park[40] = ra[1]; park[41] = ra[2]; park[42] = u_r3;
+}
+// park: rows 1 and 2 in the parked layout (the CPU test and the host harness)
+ICC_HD void imu_accel_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_r3, double u_ba, V3 a_meas, double* __restrict__ row0, int ld, double (&park)[ACC_PARK], double (&ra)[3]) {
+  imu_accel_rows(W, K, u_so3, u_r3, u_ba, a_meas, row0, ld, park, 1, ra);
 }
 
 // expand one parked accelerometer row (k = 1 or 2) into tile entries: so3 = its 18 knot entries, then the shared tail of the
@@ -134,22 +144,28 @@ ICC_HD void imu_accel_row_expand(const double (&so3)[18], Q4 q, double res, doub
   row[ACC_RES_COL * ld] = res;
 }
 
-// gyroscope rows.  row0: entry c at row0[c * ld] (c = 0..23, 19..23 zero).  park: rows 1 and 2.
-ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_bg, V3 g_meas, double* __restrict__ row0, int ld, double (&park)[GYR_PARK], double (&rg)[3]) {
+// gyroscope rows.  row0: entry c at row0[c * ld] (c = 0..23, 19..23 zero).  pk: entry j of rows 1 and 2 in the parked layout at
+// pk[j * ldp], written as soon as it is known (the residuals before the knot recursion).
+ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_bg, V3 g_meas, double* __restrict__ row0, int ld, double* __restrict__ pk, int ldp, double (&rg)[3]) {
   const FrameWin& F = W.f;
   double lam[5], dlam[5], sn[5], cs[5], cbg[3];
   cum_coeffs6(u_so3, lam, dlam);
   coeffs3(u_bg, cbg);
-  // body velocity: omega <- A_i^T omega + lambda'_i d_i / dt   (ceres_spline_helper.h:159-164); s_i = A_i^T omega_{i-1}
-  V3 s[5], om = v3(0, 0, 0);
+  // body velocity: omega <- A_i^T omega + lambda'_i d_i / dt   (ceres_spline_helper.h:159-164); s_i = A_i^T omega_{i-1}.
+  // The Jacobian recursion needs s_i again, in reverse order.  Rather than holding all five through it (15 doubles at the kernel's
+  // register peak: the persistent kernel keeps its tensor-core accumulators next to this chain), s_i waits in the parked slots of
+  // row 1's knot i+1, which the recursion overwrites only after its last read of s_i.  The volatile read keeps the compiler from
+  // forwarding the stored registers; the values are the same bits.
+  V3 om = v3(0, 0, 0);
 #pragma unroll
   for (int i = 0; i < 5; ++i) {
     sincos_small(0.5 * lam[i] * F.th[i], &sn[i], &cs[i]);
     const double sphi = 2.0 * sn[i] * cs[i], omc = 2.0 * sn[i] * sn[i];
     const V3 dh = F.dh[i];
     const V3 xd = cross(om, dh), xdd = cross(xd, dh);
-    s[i] = v3(om.x + sphi * xd.x + omc * xdd.x, om.y + sphi * xd.y + omc * xdd.y, om.z + sphi * xd.z + omc * xdd.z);   // rotation by -phi about dh
-    om = fma3(dlam[i] * K.inv_so3_dt, F.d[i], s[i]);
+    const V3 si = v3(om.x + sphi * xd.x + omc * xdd.x, om.y + sphi * xd.y + omc * xdd.y, om.z + sphi * xd.z + omc * xdd.z);   // rotation by -phi about dh
+    pk[(3 * (i + 1) + 0) * ldp] = si.x; pk[(3 * (i + 1) + 1) * ldp] = si.y; pk[(3 * (i + 1) + 2) * ldp] = si.z;
+    om = fma3(dlam[i] * K.inv_so3_dt, F.d[i], si);
   }
   V3 bgyr = v3(0, 0, 0);
 #pragma unroll
@@ -158,6 +174,10 @@ ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, doub
   rg[0] = K.w_gyr * (om.x - (K.Mg[0] * g_raw.x + K.Mg[1] * g_raw.y + K.Mg[2] * g_raw.z));
   rg[1] = K.w_gyr * (om.y - (K.Mg[3] * g_raw.x + K.Mg[4] * g_raw.y + K.Mg[5] * g_raw.z));
   rg[2] = K.w_gyr * (om.z - (K.Mg[6] * g_raw.x + K.Mg[7] * g_raw.y + K.Mg[8] * g_raw.z));
+  row0[GYR_RES_COL * ld] = rg[0];
+#pragma unroll
+  for (int c = GYR_RES_COL + 1; c < 24; ++c) row0[c * ld] = 0.0;
+  pk[36 * ldp] = rg[1]; pk[37 * ldp] = rg[2];
   // d omega_k / d eps_j = y_j Jr^-1_j - Jr^-1_{j+1} y_{j+1},  y_i = lambda_i ((w_i x s_i) Jr(phi_i)) + lambda'_i w_i / dt   (w scaled by w_gyr)
   V3 w[3], zn[3];
   w[0] = v3(K.w_gyr, 0, 0); w[1] = v3(0, K.w_gyr, 0); w[2] = v3(0, 0, K.w_gyr);
@@ -168,9 +188,11 @@ ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, doub
     const double sphi = 2.0 * sn[i] * cs[i], omc = 2.0 * sn[i] * sn[i];
     const double c1 = omc * F.ith[i], c2 = lam[i] - sphi * F.ith[i], dl = dlam[i] * K.inv_so3_dt;
     const V3 dh = F.dh[i];
+    const volatile double* sv = pk + 3 * (i + 1) * ldp;
+    const V3 si = v3(sv[0], sv[ldp], sv[2 * ldp]);
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-      const V3 x = cross(w[r], s[i]);
+      const V3 x = cross(w[r], si);
       const V3 xd = cross(x, dh), xdd = cross(xd, dh);
       const V3 yv = v3(lam[i] * x.x - c1 * xd.x + c2 * xdd.x + dl * w[r].x, lam[i] * x.y - c1 * xd.y + c2 * xdd.y + dl * w[r].y, lam[i] * x.z - c1 * xd.z + c2 * xdd.z + dl * w[r].z);
       const V3 up = mulT(F.jri[i], yv) - zn[r];
@@ -178,16 +200,16 @@ ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, doub
       const V3 wd = cross(w[r], dh), wdd = cross(wd, dh);
       w[r] = v3(w[r].x - sphi * wd.x + omc * wdd.x, w[r].y - sphi * wd.y + omc * wdd.y, w[r].z - sphi * wd.z + omc * wdd.z);   // exp(lambda d) w
       if (r == 0) { row0[(3 * (i + 1) + 0) * ld] = up.x; row0[(3 * (i + 1) + 1) * ld] = up.y; row0[(3 * (i + 1) + 2) * ld] = up.z; }
-      else { park[18 * (r - 1) + 3 * (i + 1) + 0] = up.x; park[18 * (r - 1) + 3 * (i + 1) + 1] = up.y; park[18 * (r - 1) + 3 * (i + 1) + 2] = up.z; }
+      else { pk[(18 * (r - 1) + 3 * (i + 1) + 0) * ldp] = up.x; pk[(18 * (r - 1) + 3 * (i + 1) + 1) * ldp] = up.y; pk[(18 * (r - 1) + 3 * (i + 1) + 2) * ldp] = up.z; }
     }
   }
   row0[0] = -zn[0].x; row0[ld] = -zn[0].y; row0[2 * ld] = -zn[0].z;
-  park[0] = -zn[1].x; park[1] = -zn[1].y; park[2] = -zn[1].z;
-  park[18] = -zn[2].x; park[19] = -zn[2].y; park[20] = -zn[2].z;
-  row0[GYR_RES_COL * ld] = rg[0];
-#pragma unroll
-  for (int c = GYR_RES_COL + 1; c < 24; ++c) row0[c * ld] = 0.0;
-  park[36] = rg[1]; park[37] = rg[2];
+  pk[0] = -zn[1].x; pk[ldp] = -zn[1].y; pk[2 * ldp] = -zn[1].z;
+  pk[18 * ldp] = -zn[2].x; pk[19 * ldp] = -zn[2].y; pk[20 * ldp] = -zn[2].z;
+}
+// park: rows 1 and 2 in the parked layout (the CPU test and the host harness)
+ICC_HD void imu_gyro_rows(const ImuWin& W, const ImuConst& K, double u_so3, double u_bg, V3 g_meas, double* __restrict__ row0, int ld, double (&park)[GYR_PARK], double (&rg)[3]) {
+  imu_gyro_rows(W, K, u_so3, u_bg, g_meas, row0, ld, park, 1, rg);
 }
 
 ICC_HD void imu_gyro_row_expand(const double (&park)[GYR_PARK], int k, double* __restrict__ row, int ld) {
