@@ -35,7 +35,8 @@ constexpr int NT = 512;          // threads of the factorisation kernels
 // Programmatic dependent launch: every solver kernel is launched with programmatic stream serialisation, does the work that
 // does not depend on its predecessor (shared-memory set-up, zero fill) first, then waits for the predecessor's results.  The
 // "launch dependents" trigger is issued right AFTER the wait, so when a kernel starts, everything older than its direct
-// predecessor is already complete and visible.
+// predecessor is already complete and visible.  The one exception, the reduction levels' back-substitution, triggers at entry
+// (see backsub_kernel): for it and its successor only the kernels up to the root's predecessor are known to be complete.
 __device__ __forceinline__ void pdl_wait_then_trigger() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -792,6 +793,23 @@ __global__ void __launch_bounds__(NT) root_kernel(DeviceProblem P, SolvePlan pl,
   if (tid == 0) scal[SC_OK] = 1.0;
 }
 
+// Inverse M = U^{-1} of a staged block's upper-triangular factor (U_cc = D_c, U_cj = L_jc D_c for j > c; column c of the
+// factor at F + c * ldb, reciprocal pivots in ipv), row-major n x n; thread k forms column k by back-substitution of e_k.
+// Only the upper triangle (k >= c) is written.
+__device__ void block_inverse(const double* F, const double* ipv, double* M, int n, int ldb) {
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    M[(size_t)k * n + k] = ipv[k];
+    for (int c = k - 1; c >= 0; --c) {
+      const double* u = F + (size_t)c * ldb - c;                  // u[j] = U_cj
+      double s0 = 0.0, s1 = 0.0;
+      int j = c + 1;
+      for (; j < k; j += 2) { s0 = fma(u[j], M[(size_t)j * n + k], s0); s1 = fma(u[j + 1], M[(size_t)(j + 1) * n + k], s1); }
+      if (j == k) s0 = fma(u[j], M[(size_t)j * n + k], s0);
+      M[(size_t)c * n + k] = -(s0 + s1) * ipv[c];
+    }
+  }
+}
+
 // ---- back-substitution of one level (level 0: chunk interiors, level >= 1: the blocks eliminated at that level) -----
 template <bool LEVEL0>
 __global__ void __launch_bounds__(NT) backsub_kernel(DeviceProblem P, SolvePlan pl, int level, double* wsp, const double* scal) {
@@ -817,12 +835,23 @@ __global__ void __launch_bounds__(NT) backsub_kernel(DeviceProblem P, SolvePlan 
   double* tw = xr + ((w + 3) & ~3);        // t / x for columns [a, b)
   double* Bw = tw + ((b - a + 3) & ~3);    // (PB + kd) * ldb panel of L, then PB reciprocal pivots
   double* Els = Bw + (size_t)(PB + kd) * ldb + PB;   // staged rows of El
+  // Reduction levels: the staged block's inverse, formed before the wait (while the root runs), turns the one-warp recurrence
+  // into a product that every warp shares.  kd >= b - a (always: kd = 2w - 1 there) puts the whole triangle inside the band and
+  // leaves room for the n x n inverse behind the block's n staged columns, before the reciprocal pivots at (PB + kd) * ldb.
+  const bool inverse = !LEVEL0 && staged && kd >= b - a;
+  double* Mi = Bw + (size_t)(b - a) * ldb;
+  // The reduction levels launch their successor at once: every level kernel then starts while the root runs (the root triggers
+  // after its wait, so all elimination kernels are complete) and stages and inverts its block there.  What a level reads after
+  // its own wait (the separator values) the chain of waits still orders.  The chunk interiors keep the trigger behind the wait,
+  // so that the finish kernel does not occupy SMs while leaves still need them.
+  if (!LEVEL0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (staged) {   // written by the elimination kernels, i.e. older than the direct predecessor: safe before the wait
     backsub_stage(Lb, Bw, a, b, kd, ldb, PB);
     const double* src = El + (int64_t)a * nbl;
     for (int i = tid; i < (b - a) * nbl; i += nt) Els[i] = src[i];
   }
-  pdl_wait_then_trigger();
+  if (inverse) { __syncthreads(); block_inverse(Bw, Bw + (size_t)(PB + kd) * ldb, Mi, b - a, ldb); }
+  if (LEVEL0) pdl_wait_then_trigger(); else asm volatile("griddepcontrol.wait;" ::: "memory");
   if (scal[SC_OK] != 1.0) return;
   for (int i = tid; i < w + nb; i += nt) xl[i] = i < w ? (has_left ? ws.y[y_left + i] : 0.0) : ws.y[nk + i - w];
   for (int i = tid; i < w; i += nt) xr[i] = has_right ? ws.y[y_right + i] : 0.0;
@@ -839,6 +868,17 @@ __global__ void __launch_bounds__(NT) backsub_kernel(DeviceProblem P, SolvePlan 
     if (lane == 0) tw[j - a] = le[w + nb] - acc;
   }
   __syncthreads();
+  if (inverse) {   // x = M t: one warp per row
+    const int n = b - a;
+    for (int c = warp; c < n; c += nwarps) {
+      const double* m = Mi + (size_t)c * n;
+      double acc = 0.0;
+      for (int k = c + lane; k < n; k += 32) acc = fma(m[k], tw[k], acc);
+      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      if (lane == 0) ws.y[y_own + c] = acc;
+    }
+    return;
+  }
   backsub_dispatch(Lb, tw, Bw, a, b, b, kd, ldb, PB, staged);
   for (int j = a + tid; j < b; j += nt) ws.y[y_own + (j - a)] = tw[j - a];
 }
