@@ -308,6 +308,22 @@ icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double
 #define ICC_POSE_ERROR_TANGENT 1
 icc_status icc_set_pose_error(icc_handle* h, int mode);
 
+/* Vision residual of the spline solve (icc_optimize, icc_lm_iterations, icc_evaluate and the other entry points that take flags).
+ *   ICC_REPROJ_ERROR_PIXEL (default): the reference's pixel residual project(p_c) - (u, v).
+ *   ICC_REPROJ_ERROR_TANGENT: the local tangent reprojection error.  Each corner is its unit bearing b (icc_pixels_to_bearings, formed once
+ *     at icc_batch_init_spline with the intrinsics set then) with the tangent basis (e1, e2) of icc_set_pose_error, and the predicted
+ *     camera-frame point p_c scores r = s (e1.p_c, e2.p_c) / (b.p_c).  s = sqrt(|det J0|), J0 = d(u, v)/d(x, y) of the camera at the
+ *     principal ray, keeps r in pixels at the image centre, the scale the IMU weights assume.  A corner whose bearing cannot be formed is a
+ *     zero residual with zero Jacobian rows; b.p_c <= 0 gives the constant 1e10 with zero rows, like a failed projection of the pixel
+ *     residual.  No camera model is evaluated during the solve, so a corner only drops out when its prediction is 90 degrees or more off
+ *     its own ray.  Any call with ICC_FLAG_CAM_INTRINSICS is ICC_ERR_UNSUPPORTED (the bearings are fixed by the intrinsics) and changes
+ *     nothing.  icc_evaluate returns the scaled tangent residuals; summary.mean_reproj_error and icc_get_mean_reprojection_error stay
+ *     in pixels in either mode.
+ * ICC_ERR_STATE after icc_batch_init_spline; any other mode is ICC_ERR_INVALID_ARGUMENT.  Also accepted by a host-only handle. */
+#define ICC_REPROJ_ERROR_PIXEL 0
+#define ICC_REPROJ_ERROR_TANGENT 1
+icc_status icc_set_reprojection_error(icc_handle* h, int mode);
+
 /* Shutter of icc_estimate_board_poses and icc_optimize_board_points.  line_delay_s = 0 (the default) is the global shutter: one rigid pose per
  * view, and frame_t_s may be NULL.  line_delay_s > 0 is a rolling shutter: pixel row v of a view is exposed v * line_delay_s after its frame
  * time frame_t_s[i] (the rule of the reference's RS functor, feature.y() * line_delay), and the reported pose is the one at the frame time

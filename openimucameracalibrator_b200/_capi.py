@@ -19,6 +19,8 @@ FLAG_GRAVITY_DIR, FLAG_CAM_LINE_DELAY, FLAG_SPLINE, FLAG_ACC_BIAS, FLAG_GYR_BIAS
 FLAG_CAM_INTRINSICS, FLAG_TIME_OFFSET = 512, 1024     # north-star extensions (the reference keeps both fixed)
 POSE_ERROR_NORMALIZED, POSE_ERROR_TANGENT = 0, 1       # residual of the per-view pose step (icc_set_pose_error)
 POSE_ERRORS = {"normalized": POSE_ERROR_NORMALIZED, "tangent": POSE_ERROR_TANGENT}
+REPROJ_ERROR_PIXEL, REPROJ_ERROR_TANGENT = 0, 1         # vision residual of the spline solve (icc_set_reprojection_error)
+REPROJ_ERRORS = {"pixel": REPROJ_ERROR_PIXEL, "tangent": REPROJ_ERROR_TANGENT}
 
 STATUS_NAMES = {0: "ICC_OK", 1: "ICC_ERR_INVALID_ARGUMENT", 2: "ICC_ERR_NO_DEVICE", 3: "ICC_ERR_CUDA", 4: "ICC_ERR_STATE",
                 5: "ICC_ERR_UNSUPPORTED", 6: "ICC_ERR_NUMERIC"}
@@ -259,6 +261,11 @@ class CApi:
     def set_pose_error(self, mode):
         """Residual of estimate_board_poses / optimize_board_points: POSE_ERROR_NORMALIZED (default), POSE_ERROR_TANGENT, or their names."""
         self._call("set_pose_error", [C.c_int], POSE_ERRORS[mode] if isinstance(mode, str) else int(mode))
+
+    def set_reprojection_error(self, mode):
+        """Vision residual of the spline solve, before batch_init_spline: REPROJ_ERROR_PIXEL (default), REPROJ_ERROR_TANGENT (the local
+        tangent reprojection error on the corners' bearings), or their names "pixel" / "tangent"."""
+        self._call("set_reprojection_error", [C.c_int], REPROJ_ERRORS[mode] if isinstance(mode, str) else int(mode))
 
     def set_pose_rolling_shutter(self, line_delay_s, frame_t_s=None):
         """Shutter of estimate_board_poses / optimize_board_points: line_delay_s = 0 is the global shutter (the default); > 0 a rolling

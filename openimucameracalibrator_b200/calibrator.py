@@ -68,6 +68,10 @@ class ImuCameraCalibrator:
     def SetShard(self, rank: int, world: int):
         self.api.set_shard(rank, world)
 
+    def SetReprojectionError(self, mode: str):
+        """"pixel" (default, the reference's residual) or "tangent" (corners as unit bearings); before BatchInitSpline."""
+        self.api.set_reprojection_error(mode)
+
     # -- reference API ------------------------------------------------------------------------------------------------
     def BatchInitSpline(self, T_i_c_init, dt_so3, dt_r3, std_so3, std_r3, time_offset_imu_to_cam, initial_line_delay,
                         accl_intrinsics=(0, 0, 0, 1, 1, 1), gyro_intrinsics=(0, 0, 0, 0, 0, 0, 1, 1, 1), accl_bias=(0, 0, 0),

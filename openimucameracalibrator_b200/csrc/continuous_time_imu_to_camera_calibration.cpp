@@ -13,6 +13,9 @@
 // fisheye lenses beyond 90 degrees); --pose_shutter global|rolling (default global) its shutter (icc_set_pose_rolling_shutter: rolling gives each
 // view's pose at its frame timestamp from row-timed corners, line delay 1 / fps / height).  --pose_shutter rolling with --global_shutter or
 // with --input_pose_dataset is a usage error: the first contradicts it, the second skips the pose step.
+// --reprojection_error pixel|tangent (default pixel) selects the vision residual of the spline solve (icc_set_reprojection_error: tangent
+// scores every corner as its unit bearing, so that corners of wide lenses keep pulling wherever the camera model's projection would fail;
+// the reported reprojection errors stay in pixels).  The rank processes of --gpus N re-execute this command line and so get the same residual.
 // Extra flags (not in the reference): --device (CUDA ordinal, default 0), --parse_only (stop after parsing, print a summary),
 // --gpus N (residual blocks sharded by time slice over devices device..device+N-1 of this host: the binary spawns one rank process per
 // extra device -- hidden flags --shard_rank / --shard_world / --comm_id_hex -- each with the library's own NCCL communicator; one
@@ -42,7 +45,7 @@ icccli::Flags default_flags() {
   f.str = {{"telemetry_json", ""}, {"input_pose_dataset", ""}, {"input_corners", ""}, {"camera_calibration_json", ""},
     {"gyro_to_cam_initial_calibration", ""}, {"imu_intrinsics", ""}, {"imu_bias_file", ""}, {"spline_error_weighting_json", ""}, {"output_path", ""},
     {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"},
-    {"pose_shutter", "global"}};
+    {"pose_shutter", "global"}, {"reprojection_error", "pixel"}};
   f.boolean = {{"global_shutter", false}, {"calibrate_cam_line_delay", false}, {"reestimate_biases", false}, {"parse_only", false}, {"json_selftest", false}};
   f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0}};
   return f;
@@ -160,10 +163,11 @@ static int json_selftest() {
 
 int main(int argc, char** argv) {
   icccli::Flags F = default_flags();
-  int pose_error = ICC_POSE_ERROR_NORMALIZED;
+  int pose_error = ICC_POSE_ERROR_NORMALIZED, reproj_error = ICC_REPROJ_ERROR_PIXEL;
   bool pose_rolling = false;
   try {
     icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); pose_rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]);
+    reproj_error = icccli::parse_reprojection_error(F.str["reprojection_error"]);
     if (pose_rolling && F.boolean["global_shutter"]) throw std::runtime_error("--pose_shutter rolling contradicts --global_shutter");
     if (pose_rolling && !F.str["input_pose_dataset"].empty()) throw std::runtime_error("--pose_shutter rolling applies to the in-process pose step, which --input_pose_dataset skips");
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
@@ -329,6 +333,7 @@ int main(int argc, char** argv) {
     icc_handle* h = nullptr;
     { icc_status s = icc_create(&h, (int)F.num["device"]); if (s != ICC_OK) { std::cerr << "icc_create failed (" << s << "): " << icc_last_error(h) << std::endl; return 2; } }
     ICC(icc_set_camera(h, model, intr.data(), (int)intr.size(), width, height));
+    ICC(icc_set_reprojection_error(h, reproj_error));
     ICC(icc_set_board_points(h, max_id + 1, board.data()));
     ICC(icc_set_frames(h, (int)frame_t.size(), frame_t.data(), off.data(), ids.data(), uv.data(), q_wc.data(), p_wc.data()));
     ICC(icc_set_imu(h, (int)imu_t.size(), imu_t.data(), acc.data(), gyr.data()));

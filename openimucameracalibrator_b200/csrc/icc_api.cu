@@ -9,6 +9,7 @@
 // and applies the trust-region accept/reject logic to a few scalars read back per iteration.  There is no CPU fallback.
 #include "../../include/icc_b200.h"
 #include "icc_allan_math.cuh"
+#include "icc_bearing_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
 #include "icc_rotinit_math.cuh"
@@ -102,6 +103,7 @@ struct icc_handle {
   // ---- raw inputs -------------------------------------------------------------------------------------------
   int model = -1, n_intr = 0, width = 0, height = 0; double intr[10] = {0};
   int pose_error = ICC_POSE_ERROR_NORMALIZED;   // residual of icc_estimate_board_poses / icc_optimize_board_points (icc_set_pose_error)
+  int reproj_error = ICC_REPROJ_ERROR_PIXEL;     // vision residual of the spline solve (icc_set_reprojection_error), fixed at batch_init
   double pose_line_delay = 0.0; std::vector<double> pose_frame_t;   // their shutter (icc_set_pose_rolling_shutter; 0 = global)
   std::vector<double> pose_vel; int32_t pose_n_static = 0;          // what their last rolling-shutter pass used (icc_get_pose_velocities)
   std::vector<double> points;
@@ -144,6 +146,8 @@ struct icc_handle {
   DevBuf<double4> d_board; DevBuf<int> d_f_off, d_f_s_so3, d_f_s_r3, d_pid; DevBuf<double> d_f_u_so3, d_f_u_r3; DevBuf<double2> d_uv;
   DevBuf<double> d_view_t, d_view_q, d_view_p;   // per-view pose priors in time order (knot initialisation kernel)
   DevBuf<VisFrame> d_vframes; DevBuf<VisItem> d_vitems;
+  DevBuf<double4> d_bear; DevBuf<int> d_bear_ok;   // tangent mode: the used corners' bearings, in stream order next to P.uv
+  TangentMeas tan{nullptr, nullptr, 0.0};          // ... and what the evaluation kernels read of them (tangent_meas)
   DevBuf<ImuCellP> d_icells; DevBuf<VisItem> d_iitems;
   std::vector<VisItem> vitems, iitems;   // host copies of the per-warp runs (icc_get_eval_schedule)
   DevBuf<double> d_imu_traw; DevBuf<VisionWork> d_vwork; DevBuf<int64_t> d_imu_t; DevBuf<double> d_imu_acc, d_imu_gyr; DevBuf<ImuCell> d_cells, d_iwork;
@@ -309,6 +313,8 @@ icc_status push_state_to_device(icc_handle* h) {
 // R3 on ties) form the banded part; T_i_c, gravity, line delay and bias knots form the border.
 icc_status configure(icc_handle* h, int flags) {
   if ((flags & ICC_FLAG_POINTS) && (flags & ICC_FLAG_CAM_INTRINSICS)) return fail(h, ICC_ERR_UNSUPPORTED, "POINTS together with CAM_INTRINSICS (an extension flag of this library) is not supported");
+  if (h->reproj_error == ICC_REPROJ_ERROR_TANGENT && (flags & ICC_FLAG_CAM_INTRINSICS))
+    return fail(h, ICC_ERR_UNSUPPORTED, "CAM_INTRINSICS with the tangent reprojection error is not supported: the corners' bearings are fixed by the intrinsics at batch_init_spline");
   if (h->cur_flags == flags) return ICC_OK;
   // the host layout below is rewritten before the shape checks: until it is complete, no flags are configured, so that a refused
   // shape cannot leave its layout behind under the previous flags (the device-side problem P keeps the previous layout, complete)
@@ -433,16 +439,19 @@ icc_status cross_rank_sum(icc_handle* h, double* dev, int64_t n) {
   return ICC_OK;   // shards evaluated on their own (tests add them up on the host)
 }
 
+// the tangent measurements the evaluation kernels take in tangent mode; nullptr selects the pixel residual
+const TangentMeas* tangent_meas(const icc_handle* h) { return h->reproj_error == ICC_REPROJ_ERROR_TANGENT ? &h->tan : nullptr; }
+
 // One Jacobian evaluation on the current state: zero the packed normal equations, run the kernels, cross-rank reduce.
 icc_status eval_jacobian(icc_handle* h, const DeviceState& S, double* residuals_dev) {
   h->ne_flags = -1;
   CU(cudaMemsetAsync(h->P.ne, 0, (size_t)h->P.ne_size * sizeof(double), h->stream));
-  if (launch_eval(h->P, S, true, nullptr, residuals_dev, nullptr, h->stream, h->aux_ok ? &h->aux : nullptr)) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
-  if (h->P.col_pts >= 0 && h->P.rolling) launch_points_jac(h->P, S, S.pjac, h->P.col_pts, h->sm_count, h->stream);   // board-point columns (POINTS)
+  if (launch_eval(h->P, S, true, nullptr, residuals_dev, nullptr, h->stream, h->aux_ok ? &h->aux : nullptr, tangent_meas(h))) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
+  if (h->P.col_pts >= 0 && h->P.rolling) launch_points_jac(h->P, S, S.pjac, h->P.col_pts, h->sm_count, h->stream, tangent_meas(h));   // board-point columns (POINTS)
   return cross_rank_sum(h, h->P.ne, h->P.ne_size);
 }
 icc_status eval_cost(icc_handle* h, const DeviceState& S, double* cost_dev, double* residuals_dev, double* reproj_dev) {
-  if (launch_eval(h->P, S, false, cost_dev, residuals_dev, reproj_dev, h->stream, h->aux_ok ? &h->aux : nullptr)) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
+  if (launch_eval(h->P, S, false, cost_dev, residuals_dev, reproj_dev, h->stream, h->aux_ok ? &h->aux : nullptr, tangent_meas(h))) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
   return cost_dev ? cross_rank_sum(h, cost_dev, 1) : ICC_OK;
 }
 
@@ -451,7 +460,7 @@ icc_status mean_reproj(icc_handle* h, double* out) {
   if (h->P.n_vwork == 0 && h->shard_world <= 1) { *out = 0.0; return ICC_OK; }
   CU(cudaMemsetAsync(h->d_scal.p, 0, SC_COUNT * sizeof(double), h->stream));
   if (h->P.n_vwork > 0) {
-    DeviceProblem P = h->P; P.n_iwork = 0; P.rolling = 1;
+    DeviceProblem P = h->P; P.n_iwork = 0; P.rolling = 1;   // the pixel residual in either mode (no TangentMeas)
     if (launch_eval(P, h->st[h->cur].view(), false, h->d_scal.p + SC_CAND_COST, nullptr, h->d_scal.p + SC_REPROJ_SUM, h->stream)) return fail(h, ICC_ERR_CUDA, "eval launch failed");
   }
   { icc_status r = cross_rank_sum(h, h->d_scal.p + SC_REPROJ_SUM, 2); if (r != ICC_OK) return r; }   // a rank without vision work still enters the sum
@@ -932,6 +941,11 @@ icc_status upload_problem(icc_handle* h, const ViewTable& v, const Pose& Tci, co
       // page-locked sources (HostBuf): the DMA transfers run behind the rest of this function; kernels follow on the same stream
       CU(cudaMemcpyAsync(h->d_uv.p, uv_src, (size_t)P.n_corners * sizeof(double2), cudaMemcpyHostToDevice, h->stream));
       CU(cudaMemcpyAsync(h->d_pid.p, pid_src, (size_t)P.n_corners * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    }
+    if (h->reproj_error == ICC_REPROJ_ERROR_TANGENT) {   // bearings of this shard's corners under the intrinsics of the start, and the pixel scale of the tangent residuals
+      CU(h->d_bear.alloc(P.n_corners)); CU(h->d_bear_ok.alloc(P.n_corners));
+      launch_bearings(h->model, h->intr, P.n_corners, P.uv, h->d_bear.p, h->d_bear_ok.p, h->stream);
+      h->tan = TangentMeas{h->d_bear.p, h->d_bear_ok.p, tangent_scale(h->model, h->intr, P.dispatch_fov != 0)};
     }
     // work lists: one warp per item; items sized so that the grid fills the GPU but every item amortises its tile flush
     const int target_items = h->sm_count * 8;
@@ -1435,7 +1449,7 @@ icc_status icc_time_evaluations(icc_handle* h, int n, int flags, int with_jacobi
     else if (with_jacobian == 2 || with_jacobian == 3) {   // one kernel family only (2 = vision, 3 = imu), Jacobian mode, no memset
       DeviceProblem Q = h->P; if (with_jacobian == 2) Q.n_iwork = 0; else { Q.n_vwork = 0; Q.n_vitems = 0; }
       if (with_jacobian == 2) Q.n_iitems = 0;
-      s = launch_eval(Q, h->st[h->cur].view(), true, nullptr, nullptr, nullptr, h->stream) ? fail(h, ICC_ERR_CUDA, "eval launch failed") : ICC_OK;
+      s = launch_eval(Q, h->st[h->cur].view(), true, nullptr, nullptr, nullptr, h->stream, nullptr, tangent_meas(h)) ? fail(h, ICC_ERR_CUDA, "eval launch failed") : ICC_OK;
     }
     else { s = eval_cost(h, h->st[h->cur].view(), h->d_scal.p + SC_CAND_COST, nullptr, nullptr); }
     if (s != ICC_OK) return s;
@@ -1464,6 +1478,14 @@ icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double
   if (h->model < 0) return fail(h, ICC_ERR_STATE, "icc_set_camera must be called first");
   if (n == 0) return ICC_OK;
   return drive(h, [&](std::string& err) { return pixels_to_bearings(h->stream, h->model, h->intr, n, uv, xyz_out, ok, err); });
+}
+
+icc_status icc_set_reprojection_error(icc_handle* h, int mode) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (h->initialised) return fail(h, ICC_ERR_STATE, "the reprojection error must be chosen before icc_batch_init_spline");
+  if (mode != ICC_REPROJ_ERROR_PIXEL && mode != ICC_REPROJ_ERROR_TANGENT) return fail(h, ICC_ERR_INVALID_ARGUMENT, "reprojection error must be ICC_REPROJ_ERROR_PIXEL (0) or ICC_REPROJ_ERROR_TANGENT (1)");
+  h->reproj_error = mode;
+  return ICC_OK;
 }
 
 icc_status icc_set_pose_error(icc_handle* h, int mode) {

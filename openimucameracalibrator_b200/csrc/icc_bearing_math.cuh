@@ -45,6 +45,28 @@ ICC_HD void tangent_jacobians(const TangentErr& E, Q4 q, V3 X, double J0[6], dou
   J1[0] = b1.x; J1[1] = b1.y; J1[2] = b1.z; J1[3] = a1.x; J1[4] = a1.y; J1[5] = a1.z;
 }
 
+// The spline solve's local tangent reprojection error (ICC_REPROJ_ERROR_TANGENT) of a predicted camera-frame point pc against the corner's
+// bearing, in the shape of a projection: (u, v) = s (e1.pc, e2.pc) / (b.pc) and J = s d(u, v)/d pc, so that every Jacobian column the
+// evaluation kernels derive from the projection Jacobian stays as it is.  s = pixels per tangent unit at the image centre (tangent_scale);
+// ok = the bearing could be formed (b_ok) and b.pc > 0.
+ICC_HD Proj tangent_projection(double4 b4, bool b_ok, double s, V3 pc) {
+  const TangentErr E(pc, v3(b4.x, b4.y, b4.z));
+  V3 a0, a1; E.rows(a0, a1);
+  Proj p;
+  p.u = s * E.r0; p.v = s * E.r1;
+  p.J[0] = s * a0.x; p.J[1] = s * a0.y; p.J[2] = s * a0.z; p.J[3] = s * a1.x; p.J[4] = s * a1.y; p.J[5] = s * a1.z;
+  p.ok = b_ok && E.front();
+  return p;
+}
+
+// sqrt(|det J0|), J0 = d(u, v)/d(x, y) of the model's projection at the principal ray (0, 0, 1): pixels per tangent unit at the image centre.
+// It keeps the tangent residuals on the pixel scale that the IMU residuals' weights were tuned against (cov = I); 0 when the model
+// cannot project the principal ray.
+ICC_HD double tangent_scale(int model, const double* k, bool dispatch_fov) {
+  const Proj p = project(model, k, v3(0.0, 0.0, 1.0), dispatch_fov);
+  return p.ok ? sqrt(fabs(p.J[0] * p.J[4] - p.J[1] * p.J[3])) : 0.0;
+}
+
 // Unit ray b with project(b) within 1e-6 px of (px, py); false otherwise.  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion
 // cannot see past 90 degrees: their ray is unproject_gn's normalised-plane point, normalised.  Fisheye, DoubleSphere and ExtendedUnified run
 // damped Gauss-Newton on the sphere: the step lives in the tangent plane of the current b, its 2x2 Jacobian is the 2x3 projection Jacobian

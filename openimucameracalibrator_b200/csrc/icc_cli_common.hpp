@@ -27,6 +27,13 @@ inline int parse_pose_error(const std::string& v) {
   throw std::runtime_error("flag --pose_error must be 'normalized' or 'tangent', not '" + v + "'");
 }
 
+// --reprojection_error of the hot CLI: the vision residual of the spline solve (icc_set_reprojection_error); any other value is a usage error
+inline int parse_reprojection_error(const std::string& v) {
+  if (v == "pixel") return ICC_REPROJ_ERROR_PIXEL;
+  if (v == "tangent") return ICC_REPROJ_ERROR_TANGENT;
+  throw std::runtime_error("flag --reprojection_error must be 'pixel' or 'tangent', not '" + v + "'");
+}
+
 // --pose_shutter of the pose tools: true = rolling (icc_set_pose_rolling_shutter); any other value than global / rolling is a usage error
 inline bool parse_pose_shutter(const std::string& v) {
   if (v == "global") return false;

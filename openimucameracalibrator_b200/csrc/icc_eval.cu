@@ -21,6 +21,7 @@
 #include "icc_kernels.h"
 #include "icc_reduce.cuh"
 #include "icc_spline_chain.cuh"
+#include "icc_bearing_math.cuh"
 
 #include <atomic>
 #include <cstdlib>
@@ -105,9 +106,10 @@ ICC_D void stage_so3_window(WarpCtx* wc, const DeviceState& S, int s_so3, int la
 // ---------------------------------------------------------------------------------------------------------------
 // Vision: rolling-shutter reprojection residuals.  Tile columns: [so3 0..17 | r3 18..35 | T_i_c 36..41 | ld 42 | r 43];
 // JAC == 2 (CAM_INTRINSICS extension): [... | ld 42 | intrinsics 43..43+K-1 | r 43+K], K = parameter count of the model.
+// TAN (JAC 0 / 1 only): the local tangent reprojection error against the corners' bearings (tangent_projection, icc_vision_rows.cuh).
 // ---------------------------------------------------------------------------------------------------------------
-template <int JAC>
-__global__ void __launch_bounds__(WARPS * 32) vision_kernel(DeviceProblem P, DeviceState S, double* cost_out, double* res_out, double* reproj_out) {
+template <int JAC, bool TAN = false>
+__global__ void __launch_bounds__(WARPS * 32) vision_kernel(DeviceProblem P, DeviceState S, double* cost_out, double* res_out, double* reproj_out, TangentMeas T) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   WarpCtx* wc = reinterpret_cast<WarpCtx*>(smem_raw) + warp;
@@ -169,9 +171,16 @@ __global__ void __launch_bounds__(WARPS * 32) vision_kernel(DeviceProblem P, Dev
         const double4 X = P.board[P.pid[c]];
         qi = qrot_inv(ch.q, v3(X.x, X.y, X.z) - t);   // point in the IMU frame (board points are de-homogenised once, at upload)
         pc = qrot_inv(q_ic, qi - t_ic);                                // point in the camera frame
-        if (JAC == 2) pr = project_with_k(P.model, intr, pc, P.dispatch_fov != 0, &pk); else pr = project(P.model, intr, pc, P.dispatch_fov != 0);
-        ok = pr.ok;
-        if (ok) { r0 = pr.u - ob.x; r1 = pr.v - ob.y; } else { r0 = 1e10; r1 = 1e10; }   // residuals.h:391-398, cov = I
+        if constexpr (TAN) {
+          const bool b_ok = T.ok[c] != 0;
+          pr = tangent_projection(T.bear[c], b_ok, T.s, pc);
+          ok = pr.ok;
+          if (ok) { r0 = pr.u; r1 = pr.v; } else if (!b_ok) { r0 = 0.0; r1 = 0.0; } else { r0 = 1e10; r1 = 1e10; }   // no bearing: zero residual
+        } else {
+          if (JAC == 2) pr = project_with_k(P.model, intr, pc, P.dispatch_fov != 0, &pk); else pr = project(P.model, intr, pc, P.dispatch_fov != 0);
+          ok = pr.ok;
+          if (ok) { r0 = pr.u - ob.x; r1 = pr.v - ob.y; } else { r0 = 1e10; r1 = 1e10; }   // residuals.h:391-398, cov = I
+        }
         if (res_out) { res_out[2 * c] = r0; res_out[2 * c + 1] = r1; }
         if (!JAC) {
           cost_acc += 0.5 * (r0 * r0 + r1 * r1);
@@ -518,7 +527,7 @@ int grid_for(int n_items, int sm_count) { const int ctas = (n_items + WARPS - 1)
 
 }  // namespace
 
-int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, double* reproj_out, cudaStream_t st_main, const EvalAux* aux) {
+int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, double* reproj_out, cudaStream_t st_main, const EvalAux* aux, const TangentMeas* tan) {
   DeviceProblem P = P_in;
   if (S.board) P.board = S.board;   // the board points belong to the state (parameter blocks under SplineOptimFlags::POINTS)
   static int sm_count = 0;
@@ -532,6 +541,7 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
   if (!attr_done) {
     int e = 0;
     e |= set_smem(vision_kernel<1>, sm_vis); e |= set_smem(vision_kernel<0>, sm_vis); e |= set_smem(vision_kernel<2>, sm_vis_k);
+    e |= set_smem(vision_kernel<1, true>, sm_vis); e |= set_smem(vision_kernel<0, true>, sm_vis);
     e |= set_smem(imu_kernel<true, 0>, sm_imu_nb); e |= set_smem(imu_kernel<false, 0>, sm_imu_nb);
     e |= set_smem(imu_kernel<true, 1>, sm_imu_b); e |= set_smem(imu_kernel<false, 1>, sm_imu_b); e |= set_smem(imu_kernel<true, 2>, sm_imu_b);
     if (e) return 1;
@@ -553,14 +563,18 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
     DeviceProblem Q = P;
     if (!tmem_vision) Q.n_vitems = 0;
     if (!tmem_imu) Q.n_iitems = 0;
-    if (launch_eval_tmem(Q, S, residuals_out, sm_count, st)) return 1;
+    if (launch_eval_tmem(Q, S, residuals_out, sm_count, st, tan)) return 1;
   }
   if (tmem_vision) {
   } else if (P.n_vwork > 0 && P.rolling) {
     const int grid = grid_for(P.n_vwork, sm_count);
-    if (with_jacobian && P.cam_intr_active) vision_kernel<2><<<grid, WARPS * 32, sm_vis_k, st>>>(P, S, cost_out, residuals_out, reproj_out);
-    else if (with_jacobian) vision_kernel<1><<<grid, WARPS * 32, sm_vis, st>>>(P, S, cost_out, residuals_out, reproj_out);
-    else vision_kernel<0><<<grid, WARPS * 32, sm_cost, st>>>(P, S, cost_out, residuals_out, reproj_out);
+    const TangentMeas T = tan ? *tan : TangentMeas{nullptr, nullptr, 0.0};
+    if (tan) {   // (icc_api.cu refuses CAM_INTRINSICS in tangent mode)
+      if (with_jacobian) vision_kernel<1, true><<<grid, WARPS * 32, sm_vis, st>>>(P, S, cost_out, residuals_out, reproj_out, T);
+      else vision_kernel<0, true><<<grid, WARPS * 32, sm_cost, st>>>(P, S, cost_out, residuals_out, reproj_out, T);
+    } else if (with_jacobian && P.cam_intr_active) vision_kernel<2><<<grid, WARPS * 32, sm_vis_k, st>>>(P, S, cost_out, residuals_out, reproj_out, T);
+    else if (with_jacobian) vision_kernel<1><<<grid, WARPS * 32, sm_vis, st>>>(P, S, cost_out, residuals_out, reproj_out, T);
+    else vision_kernel<0><<<grid, WARPS * 32, sm_cost, st>>>(P, S, cost_out, residuals_out, reproj_out, T);
     count_launch();
   }
   if (tmem_imu) {

@@ -34,9 +34,9 @@ struct Cta {
 };
 
 // MODEL >= 0: vision items of that camera model (one instantiation per model: only that model's projection code is resident in the
-// instruction cache); IMU_ITEMS: IMU items.
+// instruction cache); VIS_TANGENT: vision items of the tangent reprojection error, whatever the model; IMU_ITEMS: IMU items.
 template <int MODEL>
-__global__ void __launch_bounds__(Cta<MODEL>::warps * 32, 1) eval_tmem_kernel(DeviceProblem P, DeviceState S, double* __restrict__ res_out, int rounds, int groups, int stagger_ns) {
+__global__ void __launch_bounds__(Cta<MODEL>::warps * 32, 1) eval_tmem_kernel(DeviceProblem P, DeviceState S, double* __restrict__ res_out, int rounds, int groups, int stagger_ns, TangentMeas T) {
   using C = Cta<MODEL>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned char* slots = smem_raw + C::const_bytes;
@@ -62,14 +62,14 @@ __global__ void __launch_bounds__(Cta<MODEL>::warps * 32, 1) eval_tmem_kernel(De
     if (gw < P.n_iitems) tmi::run_item(P, S, reinterpret_cast<const ImuConst*>(smem_raw), reinterpret_cast<tmi::ImuSlot*>(slots + warp * C::slot_bytes), tile, ta, L, P.iitems[gw], res_out, lane, rounds, bar_id, bar_n);
     else for (int r = 0; r < rounds; ++r) { asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory"); }
   } else {
-    if (gw < P.n_vitems) tmv::run_item<MODEL>(P, S, reinterpret_cast<const VisConst*>(smem_raw), reinterpret_cast<tmv::WarpSlot*>(slots + warp * C::slot_bytes), tile, ta, L, P.vitems[gw], res_out, lane, rounds, bar_id, bar_n);
+    if (gw < P.n_vitems) tmv::run_item<MODEL>(P, T, S, reinterpret_cast<const VisConst*>(smem_raw), reinterpret_cast<tmv::WarpSlot*>(slots + warp * C::slot_bytes), tile, ta, L, P.vitems[gw], res_out, lane, rounds, bar_id, bar_n);
     else for (int r = 0; r < rounds; ++r) asm volatile("bar.sync %0, %1;" :: "r"(bar_id), "r"(bar_n) : "memory");
   }
 }
 
 // n_items: the launch's runs (P.n_vitems or P.n_iitems), n_chunks: the chunks of its stream
 template <int MODEL>
-int launch_model(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int n_items, int n_chunks, int sm_count, cudaStream_t st) {
+int launch_model(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int n_items, int n_chunks, int sm_count, cudaStream_t st, TangentMeas T) {
   using C = Cta<MODEL>;
   static bool attr_done = false;
   if (!attr_done) {
@@ -84,7 +84,7 @@ int launch_model(const DeviceProblem& P, const DeviceState& S, double* residuals
   const int rounds = getenv("ICC_TMEM_NO_LOCKSTEP") ? 0 : (n_chunks + n_items - 1) / n_items;
   const char* eg = getenv("ICC_TMEM_GROUPS"); const char* es = getenv("ICC_TMEM_STAGGER_NS");
   const int gq = eg ? atoi(eg) : 1, groups = (gq > 1 && gq <= C::warps && C::warps % gq == 0) ? gq : 1, stagger_ns = es ? atoi(es) : 0;
-  eval_tmem_kernel<MODEL><<<grid, C::warps * 32, C::smem_bytes, st>>>(P, S, residuals_out, rounds, groups, stagger_ns);
+  eval_tmem_kernel<MODEL><<<grid, C::warps * 32, C::smem_bytes, st>>>(P, S, residuals_out, rounds, groups, stagger_ns, T);
   return 0;
 }
 
@@ -94,20 +94,22 @@ int eval_tmem_warps(bool imu_items) { return imu_items ? Cta<IMU_ITEMS>::warps :
 
 // P.vitems[k] / P.iitems[k] is the run of global warp k (icc_api.cu cuts each stream into at most sm_count * eval_tmem_warps(type) runs);
 // vision and IMU items go out as separate launches, each with its own CTA shape.
-int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st) {
+int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st, const TangentMeas* tan) {
+  const TangentMeas T = tan ? *tan : TangentMeas{nullptr, nullptr, 0.0};
   if (P.n_vitems > 0) {
     DeviceProblem Q = P;
     Q.n_iitems = 0;
     const int nv = P.n_vitems, nc = P.n_vchunks;
     int e = 1;
-    switch (P.model) {
-      case CAM_PINHOLE: e = launch_model<CAM_PINHOLE>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_PINHOLE_RADTAN: e = launch_model<CAM_PINHOLE_RADTAN>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_FISHEYE: e = launch_model<CAM_FISHEYE>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_FOV: e = launch_model<CAM_FOV>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_DIVISION_UNDISTORTION: e = launch_model<CAM_DIVISION_UNDISTORTION>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_DOUBLE_SPHERE: e = launch_model<CAM_DOUBLE_SPHERE>(Q, S, residuals_out, nv, nc, sm_count, st); break;
-      case CAM_EXTENDED_UNIFIED: e = launch_model<CAM_EXTENDED_UNIFIED>(Q, S, residuals_out, nv, nc, sm_count, st); break;
+    if (tan) e = launch_model<VIS_TANGENT>(Q, S, residuals_out, nv, nc, sm_count, st, T);
+    else switch (P.model) {
+      case CAM_PINHOLE: e = launch_model<CAM_PINHOLE>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_PINHOLE_RADTAN: e = launch_model<CAM_PINHOLE_RADTAN>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_FISHEYE: e = launch_model<CAM_FISHEYE>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_FOV: e = launch_model<CAM_FOV>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_DIVISION_UNDISTORTION: e = launch_model<CAM_DIVISION_UNDISTORTION>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_DOUBLE_SPHERE: e = launch_model<CAM_DOUBLE_SPHERE>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
+      case CAM_EXTENDED_UNIFIED: e = launch_model<CAM_EXTENDED_UNIFIED>(Q, S, residuals_out, nv, nc, sm_count, st, T); break;
       default: return 1;
     }
     if (e) return 1;
@@ -116,7 +118,7 @@ int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* resid
   if (P.n_iitems > 0) {
     DeviceProblem Q = P;
     Q.n_vitems = 0;
-    if (launch_model<IMU_ITEMS>(Q, S, residuals_out, P.n_iitems, P.n_ichunks, sm_count, st)) return 1;
+    if (launch_model<IMU_ITEMS>(Q, S, residuals_out, P.n_iitems, P.n_ichunks, sm_count, st, T)) return 1;
     count_launch();
   }
   return cudaGetLastError() == cudaSuccess ? 0 : 1;

@@ -79,6 +79,11 @@ struct DeviceProblem {
   int n_res_vis, n_res_acc, n_res_gyr;
 };
 
+// Measurements of the local tangent reprojection error (ICC_REPROJ_ERROR_TANGENT): per corner of the stream, next to DeviceProblem::uv, its
+// unit bearing (x, y, z, unused) and whether it could be formed (ok != 0); s = pixels per tangent unit at the image centre (tangent_scale,
+// icc_bearing_math.cuh).  A kernel argument of its own, after the others, so that the kernels of the pixel residual keep their argument layout.
+struct TangentMeas { const double4* bear; const int* ok; double s; };
+
 struct SolveParams {
   double radius, min_diag, max_diag;
   int jacobi_scaling;
@@ -94,10 +99,12 @@ enum { SC_MODEL_CHANGE = 0, SC_STEP_SQ = 1, SC_X_SQ = 2, SC_CAND_COST = 3, SC_OK
 struct EvalAux { cudaStream_t stream; cudaEvent_t fork, join; };
 // Persistent Jacobian evaluation, vision + IMU items in one launch (icc_eval_tmem.cu); non-zero on a launch error.
 // P.vitems[k] / P.iitems[k] is the run of global warp k; the two item types go out as two launches of the same kernel.
-int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st);
+// tan != nullptr: the vision items evaluate the tangent reprojection error against its bearings (one instantiation for every camera model)
+int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st, const TangentMeas* tan = nullptr);
 // warps per CTA of the persistent kernel's vision (imu_items = false) or IMU launch
 int eval_tmem_warps(bool imu_items);
-int launch_eval(const DeviceProblem& P, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, double* reproj_out, cudaStream_t st, const EvalAux* aux = nullptr);
+// tan != nullptr: vision residuals of the tangent reprojection error (not with P.cam_intr_active); reproj_out then sums tangent residuals
+int launch_eval(const DeviceProblem& P, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, double* reproj_out, cudaStream_t st, const EvalAux* aux = nullptr, const TangentMeas* tan = nullptr);
 // scale[i] = 1/(1+sqrt(H_ii)) (Jacobi scaling, computed once per optimize) ; gradient inf-norm
 void launch_compute_scale(const DeviceProblem& P, double* scale, int jacobi, double* scal, cudaStream_t st);
 // banded + bordered Cholesky solve of (S H S + D) y = -S g ; delta = S y (solver order) ; model cost change
@@ -118,7 +125,7 @@ void launch_imu_times(int n, const double* t_raw, double offset_s, int64_t start
 // board points as parameters (icc_points.cu)
 void launch_points_prepare(int n, const double4* pts, double4* board, double* jac, cudaStream_t st);
 void launch_points_update(int n, int col_pts, const double4* cur, double4* cand, double4* board, double* jac, const double* delta, double* scal, cudaStream_t st);
-void launch_points_jac(const DeviceProblem& P, const DeviceState& S, const double* pjac, int col_pts, int sm_count, cudaStream_t st);
+void launch_points_jac(const DeviceProblem& P, const DeviceState& S, const double* pjac, int col_pts, int sm_count, cudaStream_t st, const TangentMeas* tan = nullptr);
 // trajectory getters
 void launch_eval_trajectory(const DeviceProblem& P, const DeviceState& S, int n, const int64_t* t_ns, int64_t start_ns, double* gyro, double* accel,
                             double* bg, double* ba, double* pose_q, double* pose_p, int* valid, cudaStream_t st);
@@ -150,6 +157,8 @@ struct RsPass { const double2* uv; const double* vel; double line_delay; };
 // focal length per view from the board homography on centred pixels (f2[v] = f^2 or 0), pinhole normalisation of pixels
 void launch_board_focal(const PoseProblem& Q, const double2* uv, double cx, double cy, double2* xy, unsigned char* use, double* f2, cudaStream_t st);
 void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, double f, double2* xy, int* ok, cudaStream_t st);
+// unit bearings of pixels (icc_bearing_math.cuh); ok[i] = 1 when b[i] could be formed (icc_pose.cu)
+void launch_bearings(int model, const double* intr10, int n, const double2* uv, double4* b, int* ok, cudaStream_t st);
 int kernel_launch_count();   // kernels launched so far in this process (icc_eval.cu)
 void count_launch();         // every launcher calls it once per kernel it enqueues
 

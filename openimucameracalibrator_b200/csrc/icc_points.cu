@@ -63,8 +63,9 @@ ICC_D void ne_add_any(const NeLayout& L, int gi, int gj, double v) {
   atomicAdd(dst, v);
 }
 
-// one warp per frame: window staged once, one corner per lane
-__global__ void __launch_bounds__(128) points_jac_kernel(DeviceProblem P, DeviceState S, const double* __restrict__ pjac, int col_pts) {
+// one warp per frame: window staged once, one corner per lane; TAN: the rows of the tangent reprojection error
+template <bool TAN>
+__global__ void __launch_bounds__(128) points_jac_kernel(DeviceProblem P, DeviceState S, const double* __restrict__ pjac, int col_pts, TangentMeas T) {
   __shared__ FrameWin wins[4];
   __shared__ VisConst K;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -95,7 +96,8 @@ __global__ void __launch_bounds__(128) points_jac_kernel(DeviceProblem P, Device
       const double2 ob = P.uv[c];
       const double4 X = P.board[pid];                                   // de-homogenised (w = 1)
       double row[2][44], yr[YR_N], r0, r1;
-      vision_corner_rows<-1>(W, K, v3(X.x, X.y, X.z), ob.x, ob.y, row[0], 1, yr, r0, r1);
+      if constexpr (TAN) vision_corner_rows<VIS_TANGENT>(W, K, v3(X.x, X.y, X.z), ob.y, T.bear[c], T.ok[c] != 0, T.s, row[0], 1, yr, r0, r1);
+      else vision_corner_rows<-1>(W, K, v3(X.x, X.y, X.z), ob.x, ob.y, row[0], 1, yr, r0, r1);
       if (r0 == 1e10) continue;                                          // failed projection: zero Jacobian rows
       vision_yrow_expand(yr, row[1], 1);
       const double* J = pjac + 12 * pid;
@@ -139,11 +141,13 @@ void launch_points_update(int n, int col_pts, const double4* cur, double4* cand,
   if (n <= 0) return;
   points_update_kernel<<<(n + 127) / 128, 128, 0, st>>>(n, col_pts, cur, cand, board, jac, delta, scal); count_launch();
 }
-void launch_points_jac(const DeviceProblem& P_in, const DeviceState& S, const double* pjac, int col_pts, int sm_count, cudaStream_t st) {
+void launch_points_jac(const DeviceProblem& P_in, const DeviceState& S, const double* pjac, int col_pts, int sm_count, cudaStream_t st, const TangentMeas* tan) {
   if (P_in.n_frames <= 0 || col_pts < 0) return;
   DeviceProblem P = P_in; P.board = S.board;
   int grid = (P.n_frames + 3) / 4; if (grid > 8 * sm_count) grid = 8 * sm_count;
-  points_jac_kernel<<<grid, 128, 0, st>>>(P, S, pjac, col_pts); count_launch();
+  if (tan) points_jac_kernel<true><<<grid, 128, 0, st>>>(P, S, pjac, col_pts, *tan);
+  else points_jac_kernel<false><<<grid, 128, 0, st>>>(P, S, pjac, col_pts, TangentMeas{nullptr, nullptr, 0.0});
+  count_launch();
 }
 
 }  // namespace icc

@@ -15,6 +15,7 @@
 //  * only the per-increment (sin, cos) pair is kept (the unit axis is per frame), not the quaternions.
 #pragma once
 #include "icc_camera.cuh"
+#include "icc_bearing_math.cuh"
 
 namespace icc {
 
@@ -54,12 +55,17 @@ ICC_HD void sincos_small(double x, double* s, double* c) {
   }
 }
 
+// MODEL of the local tangent reprojection error (ICC_REPROJ_ERROR_TANGENT): the corner is its unit bearing b, no camera model is evaluated.
+constexpr int VIS_TANGENT = -2;
+
 // One corner.  xrow: entry c of the x row is written to xrow[c * ldx] (c = 0..43).  yr: entry j of the y row in the parked layout
 // is written to yr[j * ldy] as soon as it is known, so that the kernel can send it straight to its shared-memory park instead of
 // holding the whole row in registers until the end of the corner.
 // Failed projection (quirk q12): both residuals are the constant 1e10 with zero Jacobian rows.
-template <int MODEL>   // MODEL >= 0: that camera model only; -1: runtime dispatch on K.model (host tests)
-ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double* __restrict__ yr, int ldy, double& r0, double& r1) {
+// MODEL == VIS_TANGENT: the residual is tangent_projection of the corner's bearing b4 (b_ok: it could be formed) scaled by s, and ox is not
+// used; a corner without a bearing is a zero residual with zero rows, one predicted 90 degrees or more off its ray fails as above.
+template <int MODEL>   // MODEL >= 0: that camera model only; -1: runtime dispatch on K.model (host tests); VIS_TANGENT: bearings
+ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double4 b4, bool b_ok, double s, double* __restrict__ xrow, int ldx, double* __restrict__ yr, int ldy, double& r0, double& r1) {
   const double us = W.u_so3 + oy * K.ld, ur = W.u_r3 + oy * K.ld;   // residuals.h:344-346: row time added to the normalised u
   double sn[5], cs[5];
   Q4 q = W.q0;
@@ -81,9 +87,12 @@ ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, doubl
   const M3 R = qmat(q);                       // R_w_i
   const V3 qi = mulT(R, X - t);               // point in the IMU frame
   const V3 pc = mulT(K.Ric, qi - K.tic);      // point in the camera frame
-  const Proj pr = MODEL >= 0 ? project_model<(MODEL >= 0 ? MODEL : 0)>(K.intr, pc, K.fov != 0) : project(K.model, K.intr, pc, K.fov != 0);
+  Proj pr;
+  if constexpr (MODEL == VIS_TANGENT) pr = tangent_projection(b4, b_ok, s, pc);
+  else pr = MODEL >= 0 ? project_model<(MODEL >= 0 ? MODEL : 0)>(K.intr, pc, K.fov != 0) : project(K.model, K.intr, pc, K.fov != 0);
   if (!pr.ok) {
     r0 = 1e10; r1 = 1e10;                     // residuals.h:391-393
+    if constexpr (MODEL == VIS_TANGENT) { if (!b_ok) { r0 = 0.0; r1 = 0.0; } }
 #pragma unroll
     for (int c = 0; c < VIS_RES_COL; ++c) xrow[c * ldx] = 0.0;
     xrow[VIS_RES_COL * ldx] = r0;
@@ -91,7 +100,8 @@ ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, doubl
     for (int c = 0; c < YR_N; ++c) yr[c * ldy] = c == YR_R ? r1 : 0.0;
     return;
   }
-  r0 = pr.u - ox; r1 = pr.v - oy;             // residuals.h:395-398, cov = I
+  if constexpr (MODEL == VIS_TANGENT) { r0 = pr.u; r1 = pr.v; }
+  else { r0 = pr.u - ox; r1 = pr.v - oy; }    // residuals.h:395-398, cov = I
   // Everything but the SO(3) knot columns and the line delay is written before the knot recursion, so that the point, the
   // projection Jacobian and the R^3 coefficients are dead while it runs.
   V3 w[2], zn[2];
@@ -156,8 +166,16 @@ ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, doubl
   yr[YR_LD * ldy] = oy * (du[1] - mtd[1]);
 }
 template <int MODEL>
+ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double* __restrict__ yr, int ldy, double& r0, double& r1) {
+  vision_corner_rows<MODEL>(W, K, X, ox, oy, make_double4(0.0, 0.0, 0.0, 0.0), false, 0.0, xrow, ldx, yr, ldy, r0, r1);
+}
+template <int MODEL>
 ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double ox, double oy, double* __restrict__ xrow, int ldx, double (&yr)[YR_N], double& r0, double& r1) {
   vision_corner_rows<MODEL>(W, K, X, ox, oy, xrow, ldx, yr, 1, r0, r1);
+}
+template <int MODEL>
+ICC_HD void vision_corner_rows(const FrameWin& W, const VisConst& K, V3 X, double oy, double4 b4, bool b_ok, double s, double* __restrict__ xrow, int ldx, double (&yr)[YR_N], double& r0, double& r1) {
+  vision_corner_rows<MODEL>(W, K, X, 0.0, oy, b4, b_ok, s, xrow, ldx, yr, 1, r0, r1);
 }
 
 // Expand a parked y row into tile entries (what the kernel does after the x rows have been consumed); also used by the CPU test.

@@ -111,7 +111,7 @@ ICC_D void init_const(VisConst* K, const DeviceProblem& P, const DeviceState& S,
 
 // One item = one contiguous run of 32-lane chunks of the packed corner stream, processed by one warp.
 template <int MODEL>
-ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
+ICC_D void run_item(const DeviceProblem& P, const TangentMeas& T, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
   StageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_tic = P.col_tic; A.col_ld = P.col_ld;
   double acc[2 * NBLK];                           // the current frame's tile accumulators, in registers for the whole run
 #pragma unroll
@@ -146,7 +146,8 @@ ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const VisConst
           const double2 ob = P.uv[c];
           const double4 X = P.board[P.pid[c]];
           double r0, r1;
-          vision_corner_rows<MODEL>(slot->win[w], *K, v3(X.x, X.y, X.z), ob.x, ob.y, xrow, LDT, ta, 32, r0, r1);   // y row straight to the park
+          if constexpr (MODEL == VIS_TANGENT) vision_corner_rows<MODEL>(slot->win[w], *K, v3(X.x, X.y, X.z), ob.x, ob.y, T.bear[c], T.ok[c] != 0, T.s, xrow, LDT, ta, 32, r0, r1);
+          else vision_corner_rows<MODEL>(slot->win[w], *K, v3(X.x, X.y, X.z), ob.x, ob.y, xrow, LDT, ta, 32, r0, r1);   // y row straight to the park
           if (res_out) { res_out[2 * c] = r0; res_out[2 * c + 1] = r1; }
         } else {                                  // padding lane of a frame whose corner count is not a multiple of 4, or beyond the chunk
 #pragma unroll
