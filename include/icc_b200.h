@@ -432,6 +432,30 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int image_width, int i
                                 double focal_length_init, double distortion_init, const icc_camcal_options* options /* nullable */,
                                 double* intrinsics /* 10 */, double* q_wc_xyzw, double* p_wc, double* view_reproj_error_px, int32_t* view_used,
                                 icc_camcal_summary* summary /* nullable */);
+/* Shutter of icc_calibrate_camera.  line_delay_s = 0 (the default) is the global shutter and leaves the calibration exactly as above.
+ * line_delay_s > 0 is a rolling shutter with the model of icc_set_pose_rolling_shutter: corner c of view i is seen tau = uv_c.y * line_delay_s
+ * after the frame and predicted from P(tau) = exp(-tau [w_i]x) (R_cw (X - c_wc) - tau u_i), with the view's camera-frame velocities (w_i, u_i)
+ * at row 0 held fixed in every bundle adjustment (the internal initialiser's included).  The residual is project(K, P(tau)) - uv with the same
+ * Huber loss; the per-view errors and the 5 px / 2 px view filters use it, and the reported poses are those at the frame times.  With
+ * optimize_board_points the board points are refined with the corners at their row times.  The line delay itself is not estimated here.
+ *   w_u given (6 per view: w, u):    one calibration with these velocities (fixed mode); frame_t_s may be NULL.
+ *   w_u NULL, frame_t_s given:       automatic mode.  Round 0 is the global-shutter calibration; if it returns success = 0, that result is
+ *                                    returned.  Otherwise two rounds follow, each: the pose step (icc_estimate_board_poses' driver with the
+ *                                    handle's icc_set_pose_error, max_reproj_error = 0, min_points = 0) on all n_views views under the previous
+ *                                    round's intrinsics and a rolling shutter with these view times, then a calibration with the same inputs
+ *                                    and options and the velocities that pose step used.  A view the pose step could not place, or that had
+ *                                    no neighbour in time, gets w = u = 0 (the global-shutter model).  Every round reads the board points
+ *                                    the handle held when icc_calibrate_camera was called; the outputs, the summary and (optimize_board_points)
+ *                                    the refined board points are the last round's.
+ * A negative or non-finite delay, a negative or non-finite time, a non-finite velocity, or a positive delay with n_views <= 0 or with both
+ * arrays NULL is ICC_ERR_INVALID_ARGUMENT; so is a later icc_calibrate_camera with another n_views.  Host state only (a host-only handle
+ * accepts it); the handle's camera and its pose-step shutter are not changed, by this call or by the calibration. */
+icc_status icc_set_camcal_rolling_shutter(icc_handle* h, double line_delay_s, int32_t n_views, const double* frame_t_s /* nullable */,
+                                          const double* w_u /* 6 per view, nullable */);
+/* The velocities the last rolling-shutter icc_calibrate_camera on this handle used: w_u[6 * n_views] = (w, u) per view, and
+ * n_without_neighbours (nullable) = the valid views without a neighbour in its last pose step (0 in fixed mode).  ICC_ERR_STATE before any
+ * such call; ICC_ERR_INVALID_ARGUMENT when n_views differs from that call's. */
+icc_status icc_get_camcal_velocities(const icc_handle* h, int32_t n_views, double* w_u, int32_t* n_without_neighbours);
 
 /* ---- upstream: static IMU biases, the `--imu_bias_file` input of the hot CLI ------------------------------------------------------------
  * python/get_imu_biases.py:36-53: gyroscope bias = mean of the gyroscope stream; accelerometer bias = mean of the accelerometer stream

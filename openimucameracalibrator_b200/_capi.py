@@ -280,6 +280,23 @@ class CApi:
         self._call("get_pose_velocities", [C.c_int32, c_double_p, C.POINTER(C.c_int32)], int(n_frames), _dp(vel), C.byref(ns))
         return vel[:, :3], vel[:, 3:], ns.value
 
+    def set_camcal_rolling_shutter(self, line_delay_s, frame_t_s=None, w_u=None):
+        """Shutter of calibrate_camera: line_delay_s = 0 is the global shutter (the default); > 0 a rolling shutter, either with the views'
+        fixed camera-frame velocities w_u[n,6] = (w, u), or (w_u None) in automatic mode with the views' frame times frame_t_s."""
+        t = None if frame_t_s is None else _f64(frame_t_s).ravel()
+        v = None if w_u is None else _f64(w_u).reshape(-1, 6)
+        n = v.shape[0] if v is not None else (t.size if t is not None else 0)
+        if t is not None and v is not None and t.size != n:
+            raise ValueError("frame_t_s and w_u must describe the same number of views")
+        self._call("set_camcal_rolling_shutter", [C.c_double, C.c_int32, c_double_p, c_double_p], float(line_delay_s), n, _dp(t), _dp(v))
+
+    def camcal_velocities(self, n_views):
+        """Velocities of the last rolling-shutter calibrate_camera -> (w[n,3] rad/s, u[n,3] m/s, both camera frame at the frame time,
+        number of valid views without a neighbour in its last pose step)."""
+        vel = np.zeros((int(n_views), 6)); ns = C.c_int32()
+        self._call("get_camcal_velocities", [C.c_int32, c_double_p, C.POINTER(C.c_int32)], int(n_views), _dp(vel), C.byref(ns))
+        return vel[:, :3], vel[:, 3:], ns.value
+
     # ---- upstream row f4: CameraCalibrator::CalibrateCameraFromJson / RunCalibration (src/core/camera_calibrator.cc:131-389) ----
     def calibrate_camera(self, model, image_width, image_height, corner_offsets, point_ids, uv, q_wc_init=None, p_wc_init=None, init_valid=None,
                          focal_length_init=0.0, distortion_init=0.0, **options):

@@ -135,6 +135,7 @@ class CameraCalibrator:
         self.grid_size, self.verbose = 0.04, False
         self._views, self._obs = [], {}
         self._image_size = None
+        self._rolling, self._line_delay = False, 0.0
         self.result = None
 
     def SetGridSize(self, grid_size: float = 0.04):
@@ -142,6 +143,21 @@ class CameraCalibrator:
 
     def SetVerbose(self):
         self.verbose = True
+
+    def SetRollingShutter(self, line_delay_s=None):
+        """Rolling-shutter calibration (icc_set_camcal_rolling_shutter, automatic mode) with the view timestamps this object holds: the
+        AddView times, or the corner file's view times.  line_delay_s None takes one readout per frame interval from the corner file,
+        1 / camera_fps / image_height (CalibrateCameraFromJson only); 0 returns to the global shutter."""
+        if line_delay_s is None:
+            self._rolling, self._line_delay = True, None
+            return
+        ld = float(line_delay_s)
+        if not np.isfinite(ld) or ld < 0.0:
+            raise IccError(f"line delay must be finite and >= 0, not {line_delay_s!r}")
+        self._rolling, self._line_delay = ld > 0.0, ld
+
+    def _set_shutter(self, times_s, line_delay_s):
+        self.api.set_camcal_rolling_shutter(line_delay_s if self._rolling else 0.0, frame_t_s=times_s if self._rolling else None)
 
     def SetBoardPoints(self, xyzw):
         self.api.set_board_points(xyzw)
@@ -173,6 +189,9 @@ class CameraCalibrator:
             off.append(len(ids))
         last = self._views[-1]                                     # the shared intrinsics keep the values of the last AddView (:101-113)
         W, H = self._image_size
+        if self._rolling and self._line_delay is None:
+            raise IccError("RunCalibration needs SetRollingShutter(line_delay_s) with a number")
+        self._set_shutter([v["t"] for v in self._views], self._line_delay)
         self.result = self.api.calibrate_camera(self.model, W, H, off, ids, np.array(uv).reshape(-1, 2), q_wc_init=np.array([v["q_wc"] for v in self._views]),
                                                 p_wc_init=np.array([v["p_wc"] for v in self._views]), focal_length_init=last["f"], distortion_init=last["k"], grid_size=0.0,
                                                 optimize_board_points=int(self.optimize_board_pts))
@@ -196,6 +215,13 @@ class CameraCalibrator:
             for pid in sorted(ip):
                 ids.append(int(pid)); uv.append(ip[pid])
             off.append(len(ids)); self._timestamps_s.append(float(key) * 1e-6)
+        if self._rolling and self._line_delay is None:
+            fps = float(scene_json["camera_fps"])
+            if not (fps > 0.0 and H > 0):
+                raise IccError("a rolling shutter needs camera_fps > 0 and image_height > 0 in the corner file")
+            self._set_shutter(self._timestamps_s, 1.0 / fps / H)
+        else:
+            self._set_shutter(self._timestamps_s, self._line_delay)
         self.result = self.api.calibrate_camera(self.model, W, H, off, ids, np.array(uv, dtype=np.float64).reshape(-1, 2), grid_size=self.grid_size,
                                                 optimize_board_points=int(self.optimize_board_pts))
         s = self.result["summary"]

@@ -10,7 +10,9 @@
 // {"q_wc": [w,x,y,z], "p_wc": [...], "timestamp_s": t, "mean_reproj_error": e}}, "tracks": {...}}), not Theia's cereal binary
 // (unreadable without Theia); the *_ransac_poses.ply / *_final_poses.ply point clouds are not written.  --optimize_board_points
 // (camera_calibrator.cc:207-216) refines the board points on the GPU and writes them as the dataset's tracks.
-// Extra flag: --device (CUDA ordinal, default 0).
+// Extra flags: --device (CUDA ordinal, default 0); --pose_shutter global|rolling (default global): rolling calibrates with corners exposed row
+// by row, line delay 1 / camera_fps / image_height of the corner file and the view velocities from the rolling-shutter pose step
+// (icc_set_camcal_rolling_shutter, automatic mode).  The output files keep their layout.
 #include "../../include/icc_b200.h"
 #include "icc_cli_common.hpp"
 
@@ -35,10 +37,11 @@ int model_from_string(const std::string& s) {   // theia::StringToCameraIntrinsi
 
 int main(int argc, char** argv) {
   icccli::Flags F;
-  F.str = {{"input_corners", ""}, {"camera_model_to_calibrate", "DOUBLE_SPHERE"}, {"save_path_calib_dataset", ""}};
+  F.str = {{"input_corners", ""}, {"camera_model_to_calibrate", "DOUBLE_SPHERE"}, {"save_path_calib_dataset", ""}, {"pose_shutter", "global"}};
   F.boolean = {{"optimize_board_points", false}, {"verbose", false}};
   F.num = {{"grid_size", 0.04}, {"device", 0.0}};
-  try { icccli::parse_flags(argc, argv, F); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
+  bool rolling = false;
+  try { icccli::parse_flags(argc, argv, F); rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   try {
     Value scene_json; icccli::SceneViews sv;
     try { scene_json = icccli::load_scene(F.str["input_corners"], sv); } catch (const std::exception& e) { std::cerr << "Check failed: Failed to load " << F.str["input_corners"] << ": " << e.what() << std::endl; return 1; }
@@ -51,6 +54,8 @@ int main(int argc, char** argv) {
     const std::vector<double> board = icccli::read_scene_points(scene_json, np);
     const int nv = (int)sv.timestamp_us.size();
     if (nv == 0) { std::cerr << "Check failed: the corner file holds no views" << std::endl; return 1; }
+    double line_delay = 0.0;
+    if (rolling) { try { line_delay = icccli::pose_line_delay(fps, height); } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; } }
     icc_handle* h = nullptr;
     icc_status st = icc_create(&h, (int)F.num["device"]);
     if (st != ICC_OK) { std::cerr << "icc_create failed (" << st << "): " << icc_last_error(h) << std::endl; return 2; }
@@ -58,11 +63,19 @@ int main(int argc, char** argv) {
     icc_camcal_options opt{}; opt.grid_size = F.num["grid_size"]; opt.optimize_board_points = F.boolean["optimize_board_points"] ? 1 : 0;
     icc_camcal_summary S{};
     st = icc_set_board_points(h, np, board.data());
+    std::vector<double> frame_t(nv);
+    for (int i = 0; i < nv; ++i) frame_t[i] = sv.timestamp_us[i] * 1e-6;
+    if (st == ICC_OK && rolling) st = icc_set_camcal_rolling_shutter(h, line_delay, nv, frame_t.data(), nullptr);
     if (st == ICC_OK) st = icc_calibrate_camera(h, model, width, height, nv, sv.off.data(), sv.ids.data(), sv.uv.data(), nullptr, nullptr, nullptr, 0.0, 0.0, &opt,
                                                 intr.data(), q.data(), p.data(), err.data(), used.data(), &S);
     if (st != ICC_OK) { std::cerr << "camera calibration failed (" << st << "): " << icc_last_error(h) << std::endl; return 2; }
     std::vector<double> board_out(board);
     if (opt.optimize_board_points) icc_get_board_points(h, board_out.data(), np);
+    if (rolling) {
+      std::vector<double> vel(6 * (size_t)nv); int32_t n_static = 0;
+      if (icc_get_camcal_velocities(h, nv, vel.data(), &n_static) == ICC_OK)
+        std::cout << "Rolling shutter: line delay " << line_delay << " s, " << n_static << " valid views without a neighbour in time keep the global-shutter model.\n";
+    }
     icc_destroy(h);
     std::cout << "Using " << S.n_views_selected << " views for camera calibration.\n";
     if (F.boolean["verbose"]) for (int i = 0; i < nv; ++i) if (used[i]) std::cout << "View: " << icccli::pose_view_name(sv.timestamp_us[i]) << " RMSE reprojection error: " << err[i] << "\n";

@@ -106,6 +106,9 @@ struct icc_handle {
   int reproj_error = ICC_REPROJ_ERROR_PIXEL;     // vision residual of the spline solve (icc_set_reprojection_error), fixed at batch_init
   double pose_line_delay = 0.0; std::vector<double> pose_frame_t;   // their shutter (icc_set_pose_rolling_shutter; 0 = global)
   std::vector<double> pose_vel; int32_t pose_n_static = 0;          // what their last rolling-shutter pass used (icc_get_pose_velocities)
+  double camcal_line_delay = 0.0; std::vector<double> camcal_frame_t, camcal_w_u;   // shutter of icc_calibrate_camera (icc_set_camcal_rolling_shutter)
+  int32_t camcal_n_views = 0;
+  std::vector<double> camcal_vel; int32_t camcal_n_static = 0;      // what its last rolling-shutter calibration used (icc_get_camcal_velocities)
   std::vector<double> points;
   std::vector<double> frame_t; std::vector<int> corner_off; HostBuf<int> point_ids; HostBuf<double> uv; std::vector<double> q_wc, p_wc;
   HostBuf<double> imu_t, imu_acc, imu_gyr;
@@ -1598,6 +1601,7 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int W, int H, int nv, 
                                 const double* q_init, const double* p_init, const int32_t* init_valid, double focal_init, double distortion_init,
                                 const icc_camcal_options* options, double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary* summary) {
   if (!h || nv <= 0 || !off || !ids || !uv || !intr_out || !q_out || !p_out || !used_out || W <= 0 || H <= 0) return ICC_ERR_INVALID_ARGUMENT;
+  if (h->camcal_line_delay > 0.0 && nv != h->camcal_n_views) return fail(h, ICC_ERR_INVALID_ARGUMENT, "n_views differs from that of icc_set_camcal_rolling_shutter");
   NEED_DEVICE();
   if (camera_num_params(model) < 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "unknown camera model");
   if (h->points.empty()) return fail(h, ICC_ERR_STATE, "icc_set_board_points must be called first");
@@ -1605,13 +1609,62 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int W, int H, int nv, 
   for (int i = 0; i < nv; ++i) if (off[i + 1] < off[i]) return fail(h, ICC_ERR_INVALID_ARGUMENT, "corner offsets must be non-decreasing");
   const int np = (int)(h->points.size() / 4);
   for (int i = 0; i < off[nv]; ++i) if (ids[i] < 0 || ids[i] >= np) return fail(h, ICC_ERR_INVALID_ARGUMENT, "point id outside the board");
+  const bool rolling = h->camcal_line_delay > 0.0;
   std::vector<double> points; icc_camcal_summary S;
-  const icc_status rc = drive(h, [&](std::string& err) { return calibrate_camera(h->stream, model, W, H, np, h->points.data(), nv, off, ids, uv, q_init, p_init, init_valid, focal_init, distortion_init, options,
-                            intr_out, q_out, p_out, err_out, used_out, S, points, err); });
+  std::vector<double> vel; int32_t n_static = 0;
+  const icc_status rc = drive(h, [&](std::string& err) {
+    auto calibrate = [&](const CamCalShutter& shutter) {
+      points.clear();
+      return calibrate_camera(h->stream, model, W, H, np, h->points.data(), nv, off, ids, uv, q_init, p_init, init_valid, focal_init, distortion_init, options,
+                              intr_out, q_out, p_out, err_out, used_out, S, points, err, shutter);
+    };
+    if (!rolling) return calibrate(CamCalShutter{});
+    if (!h->camcal_w_u.empty()) { vel = h->camcal_w_u; return calibrate(CamCalShutter{h->camcal_line_delay, vel.data()}); }
+    // automatic mode: global-shutter round 0, then two rounds of (rolling-shutter pose step under the last intrinsics, calibration)
+    icc_status r = calibrate(CamCalShutter{}); if (r != ICC_OK || !S.success) return r;
+    std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), intr(10);
+    std::vector<int32_t> valid(nv);
+    vel.assign(6 * (size_t)nv, 0.0);
+    for (int round = 1; round <= 2; ++round) {
+      std::copy(intr_out, intr_out + 10, intr.begin());
+      const PoseShutter ps{h->camcal_line_delay, h->camcal_frame_t.data(), vel.data(), &n_static};
+      r = estimate_board_poses(h->stream, model, intr.data(), W, H, np, h->points.data(), nv, off, ids, uv, 0.0, 0, h->pose_error, ps, q.data(), p.data(), nullptr, valid.data(), err);
+      if (r != ICC_OK) return r;
+      for (int i = 0; i < nv; ++i) if (!valid[i]) std::fill(vel.begin() + 6 * (size_t)i, vel.begin() + 6 * (size_t)i + 6, 0.0);
+      r = calibrate(CamCalShutter{h->camcal_line_delay, vel.data()}); if (r != ICC_OK) return r;
+    }
+    return ICC_OK;
+  });
   if (!points.empty()) h->points.swap(points);   // the board was refined, even if the final bundle adjustment then failed
   if (rc != ICC_OK) return rc;
+  if (rolling && !vel.empty()) { h->camcal_vel.swap(vel); h->camcal_n_static = n_static; }
   if (summary) *summary = S;
   if (!S.success) h->err = "Not enough views for proper calibration";   // camera_calibrator.cc:132-135, :176-179, :202-205
+  return ICC_OK;
+}
+
+icc_status icc_set_camcal_rolling_shutter(icc_handle* h, double line_delay_s, int32_t n_views, const double* frame_t_s, const double* w_u) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (!std::isfinite(line_delay_s) || line_delay_s < 0.0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "line delay must be finite and >= 0");
+  if (line_delay_s == 0.0) { h->camcal_line_delay = 0.0; h->camcal_n_views = 0; h->camcal_frame_t.clear(); h->camcal_w_u.clear(); return ICC_OK; }
+  if (n_views <= 0 || (!frame_t_s && !w_u)) return fail(h, ICC_ERR_INVALID_ARGUMENT, "a rolling shutter needs n_views > 0 and the view times or the view velocities");
+  if (frame_t_s)
+    for (int i = 0; i < n_views; ++i)
+      if (!std::isfinite(frame_t_s[i]) || frame_t_s[i] < 0.0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "view times must be finite and >= 0");
+  if (w_u)
+    for (size_t i = 0; i < 6 * (size_t)n_views; ++i) if (!std::isfinite(w_u[i])) return fail(h, ICC_ERR_INVALID_ARGUMENT, "view velocities must be finite");
+  h->camcal_line_delay = line_delay_s; h->camcal_n_views = n_views;
+  if (frame_t_s) h->camcal_frame_t.assign(frame_t_s, frame_t_s + n_views); else h->camcal_frame_t.clear();
+  if (w_u) h->camcal_w_u.assign(w_u, w_u + 6 * (size_t)n_views); else h->camcal_w_u.clear();
+  return ICC_OK;
+}
+
+icc_status icc_get_camcal_velocities(const icc_handle* h, int32_t n_views, double* w_u, int32_t* n_without_neighbours) {
+  if (!h || n_views <= 0 || !w_u) return ICC_ERR_INVALID_ARGUMENT;
+  if (h->camcal_vel.empty()) return fail(const_cast<icc_handle*>(h), ICC_ERR_STATE, "no rolling-shutter camera calibration has run on this handle");
+  if ((size_t)n_views * 6 != h->camcal_vel.size()) return fail(const_cast<icc_handle*>(h), ICC_ERR_INVALID_ARGUMENT, "n_views differs from the last rolling-shutter camera calibration");
+  std::copy(h->camcal_vel.begin(), h->camcal_vel.end(), w_u);
+  if (n_without_neighbours) *n_without_neighbours = h->camcal_n_static;
   return ICC_OK;
 }
 

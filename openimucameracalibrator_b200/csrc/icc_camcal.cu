@@ -20,6 +20,7 @@
 #include "icc_camera.cuh"
 #include "icc_host.h"
 #include "icc_reduce.cuh"
+#include "icc_rolling_shutter_math.cuh"
 #include "icc_small_linalg.cuh"
 #include "icc_trust_region.cuh"
 
@@ -40,6 +41,7 @@ struct CamCalProblem {
   const int* active;           // indices of the views that take part (n_active)
 };
 struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) per view, camera centre per view, 10 intrinsics
+struct CamCalRs { const double* vel; double line_delay; };  // rolling shutter: (w, u) per view (6 doubles), line delay [s]; vel == nullptr: global
 
 namespace {
 
@@ -72,9 +74,11 @@ ICC_D void syrk_tile(const double* __restrict__ T, int nsteps, double (&acc)[CC_
   }
 }
 
-template <bool JAC>
+// RS: rolling shutter (icc_set_camcal_rolling_shutter): corner c is predicted at its row time uv[c].y * rs.line_delay from P(tau) with the
+// view's velocities rs.vel[6 v .. 6 v + 5] (rs_camera_residual); RS = false is the global-shutter kernel, and never reads rs.
+template <bool JAC, bool RS>
 __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q, CamCalState S, double* __restrict__ blocks, double* __restrict__ sys,
-                                                               double* __restrict__ cost_out, double* __restrict__ view_err) {
+                                                               double* __restrict__ cost_out, double* __restrict__ view_err, CamCalRs rs) {
   __shared__ double tile_all[JAC ? 4 * CC_TCOLS * LDT : 1];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slot = blockIdx.x * 4 + warp;
@@ -100,7 +104,32 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
 #pragma unroll
       for (int i = 0; i < CC_COLS; ++i) { rx[i] = 0.0; ry[i] = 0.0; }
     }
-    if (c < c1) {
+    if (RS && c < c1) {
+      const double4 Xb = Q.board[Q.pid[c]];
+      const double iw = 1.0 / Xb.w;
+      const double* vel = rs.vel + 6 * v;
+      RsMotion m; m.w = v3(vel[0], vel[1], vel[2]); m.u = v3(vel[3], vel[4], vel[5]);
+      const double2 uv = Q.uv[c];
+      double r0, r1, J0[6], J1[6], Jk0[10], Jk1[10];
+      const bool ok = rs_camera_residual(Q.model, k, q, cc, v3(Xb.x * iw, Xb.y * iw, Xb.z * iw), m, uv.y * rs.line_delay, uv, r0, r1,
+                                         JAC ? J0 : nullptr, JAC ? J1 : nullptr, JAC ? Jk0 : nullptr, JAC ? Jk1 : nullptr);
+      if (!ok) { cost += 1e10; esum += 1e10; }
+      else {
+        const double s = r0 * r0 + r1 * r1, rn = sqrt(s);
+        const bool in = rn <= Q.huber;
+        cost += in ? 0.5 * s : Q.huber * rn - 0.5 * Q.huber * Q.huber;
+        esum += rn;
+        if (JAC) {
+          const double sw = in ? 1.0 : sqrt(Q.huber / rn);
+          if (Q.pose_free)
+#pragma unroll
+            for (int i = 0; i < 6; ++i) { rx[i] = sw * J0[i]; ry[i] = sw * J1[i]; }
+#pragma unroll
+          for (int i = 0; i < 10; ++i) if ((Q.intr_mask >> i) & 1u) { rx[6 + i] = sw * Jk0[i]; ry[6 + i] = sw * Jk1[i]; }
+          rx[16] = sw * r0; ry[16] = sw * r1;
+        }
+      }
+    } else if (!RS && c < c1) {
       const double4 Xb = Q.board[Q.pid[c]];
       const double iw = 1.0 / Xb.w;
       const V3 d = v3(Xb.x * iw, Xb.y * iw, Xb.z * iw) - cc;
@@ -340,11 +369,18 @@ IntrinsicSubsets intrinsic_subsets(int model) {
 
 // with_jacobian: per-view packed blocks (n_active x CC_PACK) + the intrinsics part and the cost summed into sys[CC_PACK + 1];
 // otherwise cost only into *cost_out and (optional) the per-view mean reprojection error [px] into view_err (indexed by view)
-void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool with_jacobian, double* blocks, double* sys, double* cost_out, double* view_err, cudaStream_t st) {
+// rs.vel == nullptr: the global shutter
+void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool with_jacobian, double* blocks, double* sys, double* cost_out, double* view_err, const CamCalRs& rs,
+                              cudaStream_t st) {
   if (Q.n_active <= 0) return;
   const int grid = (Q.n_active + 3) / 4;
-  if (with_jacobian) camcal_accumulate_kernel<true><<<grid, 128, 0, st>>>(Q, S, blocks, sys, nullptr, nullptr);
-  else camcal_accumulate_kernel<false><<<grid, 128, 0, st>>>(Q, S, nullptr, nullptr, cost_out, view_err);
+  if (rs.vel) {
+    if (with_jacobian) camcal_accumulate_kernel<true, true><<<grid, 128, 0, st>>>(Q, S, blocks, sys, nullptr, nullptr, rs);
+    else camcal_accumulate_kernel<false, true><<<grid, 128, 0, st>>>(Q, S, nullptr, nullptr, cost_out, view_err, rs);
+  } else {
+    if (with_jacobian) camcal_accumulate_kernel<true, false><<<grid, 128, 0, st>>>(Q, S, blocks, sys, nullptr, nullptr, CamCalRs{});
+    else camcal_accumulate_kernel<false, false><<<grid, 128, 0, st>>>(Q, S, nullptr, nullptr, cost_out, view_err, CamCalRs{});
+  }
   count_launch();
 }
 
@@ -366,7 +402,8 @@ void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const Ca
 
 icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, const double* points, int nv, const int32_t* off, const int32_t* ids, const double* uv,
                             const double* q_init, const double* p_init, const int32_t* init_valid, double focal_init, double distortion_init, const icc_camcal_options* options,
-                            double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary& S, std::vector<double>& points_out, std::string& err) {
+                            double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary& S, std::vector<double>& points_out, std::string& err,
+                            const CamCalShutter& shutter) {
   using clk = std::chrono::steady_clock;
   const auto t_start = clk::now();
   memset(&S, 0, sizeof S);
@@ -386,6 +423,12 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   if (!(o.max_view_error_stage1_px > 0.0)) o.max_view_error_stage1_px = 5.0;
   if (!(o.max_view_error_final_px > 0.0)) o.max_view_error_final_px = 2.0;
   DevBuf<int> d_active; CU(d_active.alloc(nv));
+  // rolling shutter: the views' fixed velocities on the device; every bundle adjustment (the initialiser's included) and the board points see
+  // each corner at its row time
+  DevBuf<double> d_vel;
+  const bool rolling = shutter.line_delay > 0.0;
+  if (rolling) { CU(d_vel.alloc(6 * (size_t)nv)); CU(cudaMemcpyAsync(d_vel.p, shutter.vel, 6 * (size_t)nv * sizeof(double), cudaMemcpyHostToDevice, st)); }
+  const CamCalRs rs{rolling ? d_vel.p : nullptr, rolling ? shutter.line_delay : 0.0};
   const double cx0 = W / 2.0, cy0 = H / 2.0;                       // AddView (:99)
   // ---- initial focal length and poses ----------------------------------------------------------------------------------------
   std::vector<double> q0(4 * (size_t)nv), p0(3 * (size_t)nv); std::vector<int> ok0(nv, 1);
@@ -449,7 +492,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   // GetReprojErrorOfView for every active view at the current state
   auto view_errors = [&]() -> icc_status {
     CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
-    launch_camcal_accumulate(Q, state(cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, d_verr.p, st);
+    launch_camcal_accumulate(Q, state(cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, d_verr.p, rs, st);
     CU(cudaMemcpyAsync(verr.data(), d_verr.p, (size_t)nv * sizeof(double), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     return ICC_OK;
@@ -474,12 +517,12 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
       const bool fresh = T.jacobian_stale != 0;
       if (fresh) {
         CU(cudaMemsetAsync(d_sys.p, 0, (CC_PACK + 1) * sizeof(double), st));
-        launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, st);
+        launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, rs, st);
       }
       CU(cudaMemsetAsync(d_red.p, 0, 66 * sizeof(double), st));
       CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
       launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, T.iterations == 0 ? 1 : 0, T.radius, to.min_diagonal, to.max_diagonal, d_dk.p, d_scal.p, st);
-      launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, st);
+      launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, rs, st);
       CU(cudaMemcpyAsync(sc, d_scal.p, sizeof sc, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
       if (fresh) {
@@ -592,7 +635,9 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     PQ.model = model; CU(cudaMemcpy(PQ.intr, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
     PQ.normalized = 0; PQ.n_points = np; PQ.min_obs = 1; PQ.huber = o.huber_width;
     PQ.board_in = B.board.p; PQ.meas = B.uv.p; PQ.q_cw = d_q[cur].p; PQ.cam_c = d_c[cur].p;
-    DevBuf<double4> d_board2; rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, S.n_points_optimized, err); if (rc != ICC_OK) return rc;
+    const RsPass rsp{B.uv.p, d_vel.p, shutter.line_delay};
+    DevBuf<double4> d_board2; rc = refine_board_points(st, PQ, nc, ids, obs_view, d_board2, points_out, S.n_points_optimized, err, nullptr, rolling ? &rsp : nullptr);
+    if (rc != ICC_OK) return rc;
     CU(cudaMemcpyAsync(B.board.p, d_board2.p, (size_t)np * sizeof(double4), cudaMemcpyDeviceToDevice, st));
     // ... then BundleAdjustViews once more with the options of stage 3
     const int it3 = S.iterations[2];

@@ -108,10 +108,14 @@ icc_status estimate_imu_to_camera_rotation(cudaStream_t st, int sm_count, int n_
                                            const double* bias_in, double* q_out, double* td_out, double* bias_out, double* err_out, int32_t* iters_out, std::string& err);
 icc_status spline_error_weighting(cudaStream_t st, int sm_count, int n, const double* times, const double* signal, double quality, double min_dt, double max_dt, double* dt_out, double* var_out, double* spectrum, std::string& err);
 icc_status imu_biases(cudaStream_t st, int sm_count, int n, const double* acc, const double* gyr, double gravity_const, double accl_bias[3], double gyro_bias[3], std::string& err);
+// The shutter of the camera calibration (icc_set_camcal_rolling_shutter): line_delay = 0 is the global shutter; otherwise vel holds the fixed
+// camera-frame velocities (w, u) of the nv views, 6 doubles each, and corner c is seen uv[c].y * line_delay after its frame.
+struct CamCalShutter { double line_delay = 0.0; const double* vel = nullptr; };
 // S.success = 0 when too few views remain; with optimize_board_points the refined board comes back in points_out (empty otherwise)
 icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, const double* points, int nv, const int32_t* off, const int32_t* ids, const double* uv,
                             const double* q_init, const double* p_init, const int32_t* init_valid, double focal_init, double distortion_init, const icc_camcal_options* options,
-                            double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary& S, std::vector<double>& points_out, std::string& err);
+                            double* intr_out, double* q_out, double* p_out, double* err_out, int32_t* used_out, icc_camcal_summary& S, std::vector<double>& points_out, std::string& err,
+                            const CamCalShutter& shutter = CamCalShutter{});
 void default_static_imu_options(icc_static_imu_options* o);
 icc_status static_imu_calibrate(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_static_imu_options& o,
                                 double acc_out[9], double gyr_out[9], double bias_out[3], icc_static_imu_summary& S, std::vector<int32_t>& intervals, std::string& err);

@@ -40,6 +40,30 @@ ICC_HD bool rs_pose_residual(double4 b, Q4 q, V3 t, V3 X, const RsMotion& m, dou
   return E.front();
 }
 
+// Pixel residual of one corner of the camera calibration (icc_set_camcal_rolling_shutter) against P(tau), P0 = R_cw (X - c):
+//   r = project(model, k, P(tau)) - uv.
+// With J0 / J1 (nullable) the 2x6 rows for the right increment R_cw exp(delta) and the camera centre c, the columns of camcal_accumulate_kernel:
+// (d x (R_cw^T A^T a), -(R_cw^T A^T a)), with a0, a1 the rows of the projection's 2x3 Jacobian at P(tau) and d = X - c.  With Jk0 / Jk1
+// (nullable) the 2x10 intrinsic rows d(u,v)/dk in Theia's order (zero beyond the model's parameters).  Returns the projection's ok flag.
+ICC_HD bool rs_camera_residual(int model, const double* k, Q4 q, V3 c, V3 X, const RsMotion& m, double tau, double2 uv, double& r0, double& r1,
+                               double J0[6], double J1[6], double Jk0[10], double Jk1[10]) {
+  const Q4 A = rs_rotation(m, tau);
+  const V3 d = X - c;
+  const V3 P = rs_point(A, m, tau, qrot(q, d));
+  ProjK pk;
+  const Proj pr = Jk0 ? project_with_k(model, k, P, true, &pk) : project(model, k, P, true);
+  r0 = pr.u - uv.x; r1 = pr.v - uv.y;
+  if (J0) {
+    const V3 t0 = qrot_inv(q, qrot_inv(A, v3(pr.J[0], pr.J[1], pr.J[2]))), t1 = qrot_inv(q, qrot_inv(A, v3(pr.J[3], pr.J[4], pr.J[5])));
+    const V3 b0 = cross(d, t0), b1 = cross(d, t1);
+    J0[0] = b0.x; J0[1] = b0.y; J0[2] = b0.z; J0[3] = -t0.x; J0[4] = -t0.y; J0[5] = -t0.z;
+    J1[0] = b1.x; J1[1] = b1.y; J1[2] = b1.z; J1[3] = -t1.x; J1[4] = -t1.y; J1[5] = -t1.z;
+  }
+  if (Jk0)
+    for (int i = 0; i < 10; ++i) { Jk0[i] = pk.Jk[i]; Jk1[i] = pk.Jk[10 + i]; }
+  return pr.ok;
+}
+
 // Velocities of view f (pose R_f = R_wc(qf), camera centre pf) from two poses a (earlier, time ta) and b (later, tb) of the same camera:
 //   w = R_f^T R_a Log(R_a^T R_b) / (tb - ta),   u = R_f^T (p_b - p_a) / (tb - ta).
 // a and b are the previous and next neighbours (central difference), or one neighbour and f itself (one-sided).  Quaternions are q_wc.
