@@ -14,6 +14,7 @@
 #include "icc_host.h"
 #include "icc_rotinit_math.cuh"
 #include "icc_trust_region.cuh"
+#include "icc_vision_rows.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -155,6 +156,7 @@ struct icc_handle {
   std::vector<VisItem> vitems, iitems;   // host copies of the per-warp runs (icc_get_eval_schedule)
   DevBuf<double> d_imu_traw; DevBuf<VisionWork> d_vwork; DevBuf<int64_t> d_imu_t; DevBuf<double> d_imu_acc, d_imu_gyr; DevBuf<ImuCell> d_cells, d_iwork;
   DevBuf<int> d_so3_col, d_r3_col, d_ba_col, d_bg_col;
+  DevBuf<double> d_incr;     // SO(3) increment table of the persistent Jacobian evaluation (DeviceProblem::incr)
   DevBuf<double> d_ne, d_scale, d_ws, d_delta, d_scal, d_res;
   PinnedArena arena;        // staging of the small uploads of BatchInitSpline
   DeviceProblem P;
@@ -425,6 +427,7 @@ icc_status configure(icc_handle* h, int flags) {
     CU(upload_staged(h, h->d_so3_col, h->so3_col)); CU(upload_staged(h, h->d_r3_col, h->r3_col)); CU(upload_staged(h, h->d_ba_col, h->ba_col)); CU(upload_staged(h, h->d_bg_col, h->bg_col));
     P.so3_col = h->d_so3_col.p; P.r3_col = h->d_r3_col.p; P.ba_col = h->d_ba_col.p; P.bg_col = h->d_bg_col.p;
     CU(h->d_ne.alloc((size_t)P.ne_size)); P.ne = h->d_ne.p;
+    CU(h->d_incr.alloc((size_t)INCR_DOUBLES * std::max(1, P.n_so3 - 1))); P.incr = h->d_incr.p;
     CU(h->d_scale.alloc((size_t)std::max(1, nk + nb))); CU(h->d_delta.alloc((size_t)std::max(1, nk + nb)));
     CU(h->d_ws.alloc(solve_workspace_doubles(P, 0)));
   }

@@ -34,35 +34,52 @@ struct ImuSlot {
   int gidxG[2][24];
   int cinfo[2][8];                           // per staged cell: padded stream offset, first sample, sample count, s_so3, s_r3, s_ba, s_bg
 };
-struct ImuStageArgs { const double4* so3; const double4* r3; const double4* ba; const double4* bg; const int* so3_col; const int* r3_col; int col_g; };
+// incr / n_incr: the evaluated state's SO(3) increment table (incr_table_entry) and its entry count
+struct ImuStageArgs { const double* incr; const double4* so3; const double4* r3; const double4* ba; const double4* bg; const int* so3_col; const int* r3_col; int n_incr, col_g; };
 
+// Stage the knot windows of one cell: all lanes copy the five SO(3) increments from the increment table, lane 0 takes the first knot,
+// lanes 8..13 the R^3 knots, lanes 16..18 / 20..22 the bias knots, all lanes the column maps.  Every load is issued before the first
+// store (one L2 round trip, no arithmetic).
 // slot_sa: the slot's shared-window address.  A generic slot pointer would keep one more register live across the run loop's calls,
 // whose callee-saved range leaves the run loop none to spare next to its register accumulators.
 __device__ __noinline__ void stage_cell(unsigned slot_sa, int w, ImuCellP C, ImuStageArgs A) {
   ImuSlot* slot = static_cast<ImuSlot*>(__cvta_shared_to_generic(slot_sa));
   const int lane = threadIdx.x & 31;
+  double inc[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { const int e = lane + 32 * k; inc[k] = e < WIN_INCR_DOUBLES ? A.incr[incr_table_index(e, C.s_so3, A.n_incr)] : 0.0; }
+  double4 k4 = make_double4(0, 0, 0, 1);
+  if (lane == 0) k4 = A.so3[C.s_so3];
+  else if (lane >= 8 && lane < 14) k4 = A.r3[C.s_r3 + lane - 8];
+  else if (lane >= 16 && lane < 19) k4 = A.ba[C.s_ba + lane - 16];
+  else if (lane >= 20 && lane < 23) k4 = A.bg[C.s_bg + lane - 20];
+  int g[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int c = lane + 32 * j;
+    g[j] = -1;
+    if (c < 18) { const int b = A.so3_col[C.s_so3 + c / 3]; g[j] = b < 0 ? -1 : b + c % 3; }
+    else if (c < 36) { const int b = A.r3_col[C.s_r3 + (c - 18) / 3]; g[j] = b < 0 ? -1 : b + (c - 18) % 3; }
+    else if (c < 39) g[j] = A.col_g < 0 ? -1 : A.col_g + (c - 36);
+    else if (c == ACC_RES_COL) g[j] = -2;
+  }
   __syncwarp();
   ImuWin& W = slot->win[w];
-  double4 k = make_double4(0, 0, 0, 1);
-  if (lane < 6) k = A.so3[C.s_so3 + lane];
-  const Q4 qa = q4(k.x, k.y, k.z, k.w);
-  const Q4 qb = q4(__shfl_down_sync(0xffffffffu, k.x, 1), __shfl_down_sync(0xffffffffu, k.y, 1), __shfl_down_sync(0xffffffffu, k.z, 1), __shfl_down_sync(0xffffffffu, k.w, 1));
-  if (lane < 5) stage_frame_increment(W.f, lane, qa, qb);
+  double* wi = win_incr(W.f);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) if (lane + 32 * k < WIN_INCR_DOUBLES) wi[lane + 32 * k] = inc[k];
   if (lane == 0) {
-    W.f.q0 = qa; W.f.u_so3 = 0.0; W.f.u_r3 = 0.0;
+    W.f.q0 = q4(k4.x, k4.y, k4.z, k4.w); W.f.u_so3 = 0.0; W.f.u_r3 = 0.0;
     slot->cinfo[w][0] = C.poff; slot->cinfo[w][1] = C.i0; slot->cinfo[w][2] = C.n; slot->cinfo[w][3] = C.s_so3; slot->cinfo[w][4] = C.s_r3; slot->cinfo[w][5] = C.s_ba; slot->cinfo[w][6] = C.s_bg;
   }
-  if (lane >= 8 && lane < 14) { const double4 p = A.r3[C.s_r3 + lane - 8]; W.f.p[lane - 8] = v3(p.x, p.y, p.z); }
-  if (lane >= 16 && lane < 19) { const double4 b = A.ba[C.s_ba + lane - 16]; W.ba[lane - 16] = v3(b.x, b.y, b.z); }
-  if (lane >= 20 && lane < 23) { const double4 b = A.bg[C.s_bg + lane - 20]; W.bg[lane - 20] = v3(b.x, b.y, b.z); }
-  for (int c = lane; c < TCOLS; c += 32) {
-    int g = -1;
-    if (c < 18) { const int b = A.so3_col[C.s_so3 + c / 3]; g = b < 0 ? -1 : b + c % 3; }
-    else if (c < 36) { const int b = A.r3_col[C.s_r3 + (c - 18) / 3]; g = b < 0 ? -1 : b + (c - 18) % 3; }
-    else if (c < 39) g = A.col_g < 0 ? -1 : A.col_g + (c - 36);
-    else if (c == ACC_RES_COL) g = -2;
-    slot->gidxA[w][c] = g;
-    if (c < 24) slot->gidxG[w][c] = c < 18 ? g : (c == GYR_RES_COL ? -2 : -1);
+  if (lane >= 8 && lane < 14) W.f.p[lane - 8] = v3(k4.x, k4.y, k4.z);
+  if (lane >= 16 && lane < 19) W.ba[lane - 16] = v3(k4.x, k4.y, k4.z);
+  if (lane >= 20 && lane < 23) W.bg[lane - 20] = v3(k4.x, k4.y, k4.z);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int c = lane + 32 * j;
+    if (c < TCOLS) slot->gidxA[w][c] = g[j];
+    if (c < 24) slot->gidxG[w][c] = c < 18 ? g[j] : (c == GYR_RES_COL ? -2 : -1);
   }
   __syncwarp();
 }
@@ -142,7 +159,7 @@ ICC_D void init_const(ImuConst* K, const DeviceProblem& P, const DeviceState& S)
 ICC_D void run_item(const DeviceProblem& P, const DeviceState& S, const ImuConst* K, ImuSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
   const bool lock = rounds > 0;
   const unsigned slot_sa = (unsigned)__cvta_generic_to_shared(slot);
-  ImuStageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.ba = S.ba; A.bg = S.bg; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_g = P.col_g;
+  ImuStageArgs A; A.incr = P.incr; A.n_incr = P.n_so3 - 1; A.so3 = S.so3; A.r3 = S.r3; A.ba = S.ba; A.bg = S.bg; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_g = P.col_g;
   double accA[30], accG[12];                  // the current cell's tile accumulators, in registers for the whole run
 #pragma unroll
   for (int k = 0; k < 30; ++k) accA[k] = 0.0;

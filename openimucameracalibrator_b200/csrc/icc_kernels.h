@@ -77,6 +77,9 @@ struct DeviceProblem {
   int64_t ne_off_E, ne_off_C, ne_off_g, ne_off_cost, ne_size;
   // residual layout
   int n_res_vis, n_res_acc, n_res_gyr;
+  // SO(3) increment table (n_so3 - 1 entries, incr_table_entry in icc_vision_rows.cuh): rebuilt from the evaluated state at the head
+  // of every persistent Jacobian evaluation (launch_eval_tmem), whose staging copies windows out of it
+  double* incr;
 };
 
 // Measurements of the local tangent reprojection error (ICC_REPROJ_ERROR_TANGENT): per corner of the stream, next to DeviceProblem::uv, its
@@ -98,7 +101,8 @@ enum { SC_MODEL_CHANGE = 0, SC_STEP_SQ = 1, SC_X_SQ = 2, SC_CAND_COST = 3, SC_OK
 // around the pair on `st`), which fills the partial last wave of either kernel.
 struct EvalAux { cudaStream_t stream; cudaEvent_t fork, join; };
 // Persistent Jacobian evaluation, vision + IMU items in one launch (icc_eval_tmem.cu); non-zero on a launch error.
-// P.vitems[k] / P.iitems[k] is the run of global warp k; the two item types go out as two launches of the same kernel.
+// P.vitems[k] / P.iitems[k] is the run of global warp k; the two item types go out as two launches of the same kernel, after one
+// launch that forms S's SO(3) increment table in P.incr.
 // tan != nullptr: the vision items evaluate the tangent reprojection error against its bearings (one instantiation for every camera model)
 int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* residuals_out, int sm_count, cudaStream_t st, const TangentMeas* tan = nullptr);
 // warps per CTA of the persistent kernel's vision (imu_items = false) or IMU launch

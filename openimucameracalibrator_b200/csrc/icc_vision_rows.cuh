@@ -14,6 +14,7 @@
 //    range reduction (library sincos beyond that);
 //  * only the per-increment (sin, cos) pair is kept (the unit axis is per frame), not the quaternions.
 #pragma once
+#include <cstddef>
 #include "icc_camera.cuh"
 #include "icc_bearing_math.cuh"
 
@@ -192,13 +193,48 @@ ICC_HD void vision_yrow_expand(const double (&yr)[YR_N], double* __restrict__ yr
   yrow[VIS_RES_COL * ldy] = yr[YR_R];
 }
 
-// Window staging for one frame from its six SO(3) knots (x,y,z,w) and six R^3 knots; `i` < 5 handles increment i.
-ICC_HD void stage_frame_increment(FrameWin& W, int i, Q4 qa, Q4 qb) {
+// The increment between two SO(3) knots: d = log(qa^-1 qb), |d| and its reciprocal (0 when the increment vanishes), the unit axis
+// and Jr^-1(d).  The one copy of this code: the window staging below and the increment table both call it.
+ICC_HD void so3_increment(Q4 qa, Q4 qb, V3& d_out, V3& dh, double& th_out, double& ith_out, M3& jri) {
   const V3 d = so3_log(qmul(qconj(qa), qb));
-  W.d[i] = d;
+  d_out = d;
   const double th = sqrt(dot(d, d)), ith = th > 1e-150 ? 1.0 / th : 0.0;
-  W.th[i] = th; W.ith[i] = ith; W.dh[i] = ith * d;
-  W.jri[i] = so3_jr_inv(d);
+  th_out = th; ith_out = ith; dh = ith * d;
+  jri = so3_jr_inv(d);
 }
+
+// Window staging for one frame from its six SO(3) knots (x,y,z,w) and six R^3 knots; `i` < 5 handles increment i.
+ICC_HD void stage_frame_increment(FrameWin& W, int i, Q4 qa, Q4 qb) { so3_increment(qa, qb, W.d[i], W.dh[i], W.th[i], W.ith[i], W.jri[i]); }
+
+// ---- SO(3) increment table ----------------------------------------------------------------------------------------------------
+// Entry i < n (= n_so3 - 1) is the increment between knots i and i + 1 of one state (so3_increment), formed once per evaluation by
+// incr_table_kernel (icc_eval_tmem.cu) instead of once per staged window.  It is stored field by field -- d (3n doubles), dh (3n),
+// th (n), ith (n), jri (9n) -- so that the five increments of the window that starts at knot s are five contiguous runs in FrameWin's
+// own order from FrameWin::d to FrameWin::jri: staging a window's increments is an 85-double copy.
+constexpr int INCR_DOUBLES = 17;                      // doubles per entry
+constexpr int WIN_INCR_DOUBLES = 5 * INCR_DOUBLES;    // FrameWin::d .. FrameWin::jri
+static_assert(offsetof(FrameWin, dh) == offsetof(FrameWin, d) + 15 * sizeof(double) && offsetof(FrameWin, th) == offsetof(FrameWin, d) + 30 * sizeof(double) &&
+              offsetof(FrameWin, ith) == offsetof(FrameWin, d) + 35 * sizeof(double) && offsetof(FrameWin, jri) == offsetof(FrameWin, d) + 40 * sizeof(double) &&
+              offsetof(FrameWin, p) == offsetof(FrameWin, d) + WIN_INCR_DOUBLES * sizeof(double), "FrameWin's increment block: d, dh, th, ith, jri back to back");
+
+ICC_HD void incr_table_entry(const double4* __restrict__ so3, int i, int n, double* __restrict__ tab) {
+  const double4 a = so3[i], b = so3[i + 1];
+  V3 d, dh; double th, ith; M3 jri;
+  so3_increment(q4(a.x, a.y, a.z, a.w), q4(b.x, b.y, b.z, b.w), d, dh, th, ith, jri);
+  tab[3 * i] = d.x; tab[3 * i + 1] = d.y; tab[3 * i + 2] = d.z;
+  tab[3 * n + 3 * i] = dh.x; tab[3 * n + 3 * i + 1] = dh.y; tab[3 * n + 3 * i + 2] = dh.z;
+  tab[6 * n + i] = th; tab[7 * n + i] = ith;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) tab[8 * n + 9 * i + k] = jri.m[k];
+}
+// Table index of double e (< WIN_INCR_DOUBLES) of the increment block of the window that starts at knot s.
+ICC_HD int incr_table_index(int e, int s, int n) {
+  if (e < 15) return 3 * s + e;
+  if (e < 30) return 3 * n + 3 * s + (e - 15);
+  if (e < 35) return 6 * n + s + (e - 30);
+  if (e < 40) return 7 * n + s + (e - 35);
+  return 8 * n + 9 * s + (e - 40);
+}
+ICC_HD double* win_incr(FrameWin& W) { return &W.d[0].x; }
 
 }  // namespace icc

@@ -36,30 +36,40 @@ struct WarpSlot {
   int finfo[2][4];                     // per staged frame: padded stream offset, first corner, corner count
 };
 
-struct StageArgs { const double4* so3; const double4* r3; const int* so3_col; const int* r3_col; int col_tic, col_ld; };
+// incr / n_incr: the evaluated state's SO(3) increment table (incr_table_entry) and its entry count
+struct StageArgs { const double* incr; const double4* so3; const double4* r3; const int* so3_col; const int* r3_col; int n_incr, col_tic, col_ld; };
 
-// Stage the knot windows of one frame: lanes 0..4 take one SO(3) increment each (log, unit axis, Jr^-1), lanes 8..13 the R^3 knots,
-// all lanes the tile-column -> solver-column map.  One copy of the log / Jr^-1 code for the three call sites.
+// Stage the knot windows of one frame: all lanes copy the five SO(3) increments (log, unit axis, Jr^-1) from the increment table,
+// lane 0 takes the first knot, lanes 8..13 the R^3 knots, all lanes the tile-column -> solver-column map.  Every load is issued before
+// the first store, so a window costs one L2 round trip and no arithmetic on the lanes.
 __device__ __noinline__ void stage_frame(WarpSlot* slot, int w, VisFrame F, StageArgs A) {
   const int lane = threadIdx.x & 31;
+  double inc[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { const int e = lane + 32 * k; inc[k] = e < WIN_INCR_DOUBLES ? A.incr[incr_table_index(e, F.s_so3, A.n_incr)] : 0.0; }
+  double4 k4 = make_double4(0, 0, 0, 1);
+  if (lane == 0) k4 = A.so3[F.s_so3];
+  else if (lane >= 8 && lane < 14) k4 = A.r3[F.s_r3 + lane - 8];
+  int g[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int c = lane + 32 * j;
+    g[j] = -1;
+    if (c < 18) { const int b = A.so3_col[F.s_so3 + c / 3]; g[j] = b < 0 ? -1 : b + c % 3; }
+    else if (c < 36) { const int b = A.r3_col[F.s_r3 + (c - 18) / 3]; g[j] = b < 0 ? -1 : b + (c - 18) % 3; }
+    else if (c < 42) g[j] = A.col_tic < 0 ? -1 : A.col_tic + (c - 36);
+    else if (c == 42) g[j] = A.col_ld;
+    else if (c == VIS_RES_COL) g[j] = -2;
+  }
   __syncwarp();                                   // every lane is done with whatever this window slot held before
   FrameWin& W = slot->win[w];
-  double4 k = make_double4(0, 0, 0, 1);
-  if (lane < 6) k = A.so3[F.s_so3 + lane];
-  const Q4 qa = q4(k.x, k.y, k.z, k.w);
-  const Q4 qb = q4(__shfl_down_sync(0xffffffffu, k.x, 1), __shfl_down_sync(0xffffffffu, k.y, 1), __shfl_down_sync(0xffffffffu, k.z, 1), __shfl_down_sync(0xffffffffu, k.w, 1));
-  if (lane < 5) stage_frame_increment(W, lane, qa, qb);
-  if (lane == 0) { W.q0 = qa; W.u_so3 = F.u_so3; W.u_r3 = F.u_r3; slot->finfo[w][0] = F.poff; slot->finfo[w][1] = F.c0; slot->finfo[w][2] = F.cn; }
-  if (lane >= 8 && lane < 14) { const double4 p = A.r3[F.s_r3 + lane - 8]; W.p[lane - 8] = v3(p.x, p.y, p.z); }
-  for (int c = lane; c < TCOLS; c += 32) {
-    int g = -1;
-    if (c < 18) { const int b = A.so3_col[F.s_so3 + c / 3]; g = b < 0 ? -1 : b + c % 3; }
-    else if (c < 36) { const int b = A.r3_col[F.s_r3 + (c - 18) / 3]; g = b < 0 ? -1 : b + (c - 18) % 3; }
-    else if (c < 42) g = A.col_tic < 0 ? -1 : A.col_tic + (c - 36);
-    else if (c == 42) g = A.col_ld;
-    else if (c == VIS_RES_COL) g = -2;
-    slot->gidx[w][c] = g;
-  }
+  double* wi = win_incr(W);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) if (lane + 32 * k < WIN_INCR_DOUBLES) wi[lane + 32 * k] = inc[k];
+  if (lane == 0) { W.q0 = q4(k4.x, k4.y, k4.z, k4.w); W.u_so3 = F.u_so3; W.u_r3 = F.u_r3; slot->finfo[w][0] = F.poff; slot->finfo[w][1] = F.c0; slot->finfo[w][2] = F.cn; }
+  if (lane >= 8 && lane < 14) W.p[lane - 8] = v3(k4.x, k4.y, k4.z);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) if (lane + 32 * j < TCOLS) slot->gidx[w][lane + 32 * j] = g[j];
   __syncwarp();
 }
 
@@ -112,7 +122,7 @@ ICC_D void init_const(VisConst* K, const DeviceProblem& P, const DeviceState& S,
 // One item = one contiguous run of 32-lane chunks of the packed corner stream, processed by one warp.
 template <int MODEL>
 ICC_D void run_item(const DeviceProblem& P, const TangentMeas& T, const DeviceState& S, const VisConst* K, WarpSlot* slot, double* __restrict__ tile, double* ta, const NeLayout& L, const VisItem it, double* __restrict__ res_out, int lane, int rounds, int bar_id, int bar_n) {
-  StageArgs A; A.so3 = S.so3; A.r3 = S.r3; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_tic = P.col_tic; A.col_ld = P.col_ld;
+  StageArgs A; A.incr = P.incr; A.n_incr = P.n_so3 - 1; A.so3 = S.so3; A.r3 = S.r3; A.so3_col = P.so3_col; A.r3_col = P.r3_col; A.col_tic = P.col_tic; A.col_ld = P.col_ld;
   double acc[2 * NBLK];                           // the current frame's tile accumulators, in registers for the whole run
 #pragma unroll
   for (int i = 0; i < 2 * NBLK; ++i) acc[i] = 0.0;
