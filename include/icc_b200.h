@@ -40,7 +40,10 @@ typedef enum {
  *   FOV                       [f, ar, cx, cy, omega]          (extension: the reference never dispatches FOV)
  *   DIVISION_UNDISTORTION     [f, ar, cx, cy, k]
  *   DOUBLE_SPHERE             [f, ar, skew, cx, cy, xi, alpha]
- *   EXTENDED_UNIFIED          [f, ar, skew, cx, cy, alpha, beta] */
+ *   EXTENDED_UNIFIED          [f, ar, skew, cx, cy, alpha, beta]
+ *   OMNI_RADIAL_TANGENTIAL    [f, ar, skew, cx, cy, xi, k1, k2, t1, t2]   (extension, no Theia counterpart: Kalibr's omni-radtan;
+ *                             n = z + xi |p|, (mx, my) = (x, y) / n radial-tangentially distorted, then the skewed affine; valid iff
+ *                             z > -w |p|, w = xi <= 1 ? xi : 1 / xi) */
 typedef enum {
   ICC_CAM_PINHOLE = 0,
   ICC_CAM_PINHOLE_RADIAL_TANGENTIAL = 1,
@@ -48,7 +51,8 @@ typedef enum {
   ICC_CAM_FOV = 3,
   ICC_CAM_DIVISION_UNDISTORTION = 4,
   ICC_CAM_DOUBLE_SPHERE = 5,
-  ICC_CAM_EXTENDED_UNIFIED = 6
+  ICC_CAM_EXTENDED_UNIFIED = 6,
+  ICC_CAM_OMNI_RADIAL_TANGENTIAL = 7
 } icc_camera_model;
 
 /* OpenICC::core::SplineOptimFlags (core/spline_trajectory_estimator.h:17-27), same numeric values. */
@@ -293,7 +297,8 @@ icc_status icc_get_board_points(const icc_handle* h, double* xyzw, int n);
 icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, double* xy_out, int32_t* ok);
 /* Unit bearing vectors of `n` pixels with the handle's camera: xyz_out[3n], ok[n] (nullable; 0 where the ray reprojects more than 1e-6 px
  * away).  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion give icc_pixels_to_normalized's ray normalised; Fisheye's ray
- * stays in z > 0 (the model maps p and -p to one pixel); DoubleSphere and ExtendedUnified reach their whole domain, z <= 0 included. */
+ * stays in z > 0 (the model maps p and -p to one pixel); DoubleSphere, ExtendedUnified and OmniRadialTangential reach their whole domain,
+ * z <= 0 included. */
 icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double* xyz_out, int32_t* ok);
 
 /* Residual of the per-view pose refinement, the inlier test and the board-point refinement of icc_estimate_board_poses and

@@ -10,6 +10,7 @@ from __future__ import annotations
 import numpy as np
 
 PINHOLE, PINHOLE_RADIAL_TANGENTIAL, FISHEYE, FOV, DIVISION_UNDISTORTION, DOUBLE_SPHERE, EXTENDED_UNIFIED = range(7)
+OMNI_RADIAL_TANGENTIAL = 7   # extension without a Theia counterpart: Kalibr's omni-radtan
 
 MODEL_NAMES = {
     PINHOLE: "PINHOLE",
@@ -19,10 +20,11 @@ MODEL_NAMES = {
     DIVISION_UNDISTORTION: "DIVISION_UNDISTORTION",
     DOUBLE_SPHERE: "DOUBLE_SPHERE",
     EXTENDED_UNIFIED: "EXTENDED_UNIFIED",
+    OMNI_RADIAL_TANGENTIAL: "OMNI_RADIAL_TANGENTIAL",
 }
 MODEL_IDS = {v: k for k, v in MODEL_NAMES.items()}
 NUM_PARAMS = {PINHOLE: 7, PINHOLE_RADIAL_TANGENTIAL: 10, FISHEYE: 9, FOV: 5, DIVISION_UNDISTORTION: 5,
-              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7}
+              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10}
 
 
 def _affine_skew(k, dx, dy):
@@ -97,4 +99,16 @@ def project(model: int, intr, pts):
         nrm = al * rho + (1.0 - al) * z
         valid = z > -_unified_w(al) * rho
         return _affine_skew(k, x / nrm, y / nrm), valid
+    if model == OMNI_RADIAL_TANGENTIAL:
+        # unit sphere, then a pinhole at distance xi behind its centre; Kalibr's RadialTangentialDistortion without k3
+        xi, k1, k2, t1, t2 = k[5], k[6], k[7], k[8], k[9]
+        d = np.sqrt(x * x + y * y + z * z)
+        valid = z > -(xi if xi <= 1.0 else 1.0 / xi) * d
+        n = z + xi * d
+        mx, my = x / n, y / n
+        r2 = mx * mx + my * my
+        radial = 1.0 + k1 * r2 + k2 * r2 * r2
+        dx = mx * radial + 2.0 * t1 * mx * my + t2 * (r2 + 2.0 * mx * mx)
+        dy = my * radial + 2.0 * t2 * mx * my + t1 * (r2 + 2.0 * my * my)
+        return _affine_skew(k, dx, dy), valid
     raise ValueError(f"unknown camera model {model}")

@@ -31,6 +31,7 @@ int model_from_string(const std::string& s) {   // theia::StringToCameraIntrinsi
   if (s == "EXTENDED_UNIFIED") return ICC_CAM_EXTENDED_UNIFIED;
   if (s == "FISHEYE") return ICC_CAM_FISHEYE;
   if (s == "FOV") return ICC_CAM_FOV;
+  if (s == "OMNI_RADIAL_TANGENTIAL") return ICC_CAM_OMNI_RADIAL_TANGENTIAL;   // extension: Kalibr's omni-radtan
   return -1;
 }
 }  // namespace
@@ -100,6 +101,8 @@ int main(int argc, char** argv) {
         case ICC_CAM_PINHOLE_RADIAL_TANGENTIAL: for (int i = 0; i < 3; ++i) in["radial_distortion_" + std::to_string(i + 1)] = Value(intr[5 + i]);
                                                 in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
         case ICC_CAM_FOV: in["radial_distortion_1"] = Value(intr[4]); break;   // extension: the layout this repository's readers use for FOV
+        case ICC_CAM_OMNI_RADIAL_TANGENTIAL: in["xi"] = Value(intr[5]); in["radial_distortion_1"] = Value(intr[6]); in["radial_distortion_2"] = Value(intr[7]);
+                                             in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
         default: break;
       }
       j["intrinsics"] = in;
@@ -134,6 +137,8 @@ int main(int argc, char** argv) {
     if (model == ICC_CAM_DIVISION_UNDISTORTION) std::cout << "DIVISION_UNDISTORTION model: Distortion: " << intr[4] << "\n";
     else if (model == ICC_CAM_DOUBLE_SPHERE) std::cout << "DOUBLE_SPHERE model: XI: " << intr[5] << " ALPHA: " << intr[6] << "\n";
     else if (model == ICC_CAM_EXTENDED_UNIFIED) std::cout << "EXTENDED_UNIFIED model: " << intr[5] << " BETA: " << intr[6] << "\n";
+    else if (model == ICC_CAM_OMNI_RADIAL_TANGENTIAL) std::cout << "OMNI_RADIAL_TANGENTIAL model: XI: " << intr[5] << " Radial distortion 1: " << intr[6] << " Radial distortion 2: " << intr[7]
+                                                                << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
     else if (model == ICC_CAM_FISHEYE) std::cout << "FISHEYE model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7] << " Radial distortion 4: " << intr[8] << "\n";
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   return 0;

@@ -68,12 +68,12 @@ ICC_HD double tangent_scale(int model, const double* k, bool dispatch_fov) {
 }
 
 // Unit ray b with project(b) within 1e-6 px of (px, py); false otherwise.  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion
-// cannot see past 90 degrees: their ray is unproject_gn's normalised-plane point, normalised.  Fisheye, DoubleSphere and ExtendedUnified run
+// cannot see past 90 degrees: their ray is unproject_gn's normalised-plane point, normalised.  Fisheye, DoubleSphere, ExtendedUnified and OmniRadtan run
 // damped Gauss-Newton on the sphere: the step lives in the tangent plane of the current b, its 2x2 Jacobian is the 2x3 projection Jacobian
 // times (e1, e2), and the new ray is b + dx e1 + dy e2 renormalised.  Theia's Fisheye projects p and -p to the same pixel, so its ray is held
-// in z > 0; the two unified models reach their whole forward domain, z <= 0 included.
+// in z > 0; the three unified models reach their whole forward domain, z <= 0 included (OmniRadtan: past 90 degrees for any xi > 0).
 ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, V3& b) {
-  if (model != CAM_FISHEYE && model != CAM_DOUBLE_SPHERE && model != CAM_EXTENDED_UNIFIED) {
+  if (model != CAM_FISHEYE && model != CAM_DOUBLE_SPHERE && model != CAM_EXTENDED_UNIFIED && model != CAM_OMNI_RADTAN) {
     double x = 0.0, y = 0.0;
     const bool good = unproject_gn(model, k, px, py, x, y);
     const double in = 1.0 / sqrt(x * x + y * y + 1.0);

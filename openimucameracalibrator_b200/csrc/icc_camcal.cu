@@ -361,6 +361,7 @@ IntrinsicSubsets intrinsic_subsets(int model) {
     case CAM_DIVISION_UNDISTORTION: return {bits({0}), bits({1}), bits({2, 3}), bits({4}), 0u};
     case CAM_DOUBLE_SPHERE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
     case CAM_EXTENDED_UNIFIED: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
+    case CAM_OMNI_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};   // radial = xi, k1, k2
     default: return {0u, 0u, 0u, 0u, 0u};
   }
 }
@@ -612,6 +613,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   if (model == CAM_FOV) k0[4] = distortion_init != 0.0 ? distortion_init : 1e-3;   // theia's FOV model has no gradient at omega = 0
   if (model == CAM_DOUBLE_SPHERE) { k0[5] = -0.25; k0[6] = 0.5; }
   if (model == CAM_EXTENDED_UNIFIED) { k0[5] = 0.5; k0[6] = 1.0; }
+  if (model == CAM_OMNI_RADTAN) { k0[5] = 1.0; k0[0] = 2.0 * f0; }   // xi = 1, f = (1 + xi) f0: magnification f / (1 + xi) = f0 at the image centre
   for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), 10 * sizeof(double), cudaMemcpyHostToDevice));
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :132-135
   const IntrinsicSubsets sub = intrinsic_subsets(model);
@@ -622,7 +624,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
   // 3. full optimisation (:181-198)
-  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN ? sub.tangential : 0u);
+  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN ? sub.tangential : 0u);
   rc = bundle_adjust(stage3_mask, true, 2);
   if (rc != ICC_OK) return rc;
   rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200

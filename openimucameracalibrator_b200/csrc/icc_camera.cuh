@@ -9,11 +9,13 @@
 
 namespace icc {
 
-enum CameraModel { CAM_PINHOLE = 0, CAM_PINHOLE_RADTAN = 1, CAM_FISHEYE = 2, CAM_FOV = 3, CAM_DIVISION_UNDISTORTION = 4, CAM_DOUBLE_SPHERE = 5, CAM_EXTENDED_UNIFIED = 6 };
+enum CameraModel { CAM_PINHOLE = 0, CAM_PINHOLE_RADTAN = 1, CAM_FISHEYE = 2, CAM_FOV = 3, CAM_DIVISION_UNDISTORTION = 4, CAM_DOUBLE_SPHERE = 5, CAM_EXTENDED_UNIFIED = 6,
+                   CAM_OMNI_RADTAN = 7 /* extension: Kalibr's omni-radtan, no Theia counterpart */ };
 
 ICC_HD int camera_num_params(int model) {
   switch (model) { case CAM_PINHOLE: return 7; case CAM_PINHOLE_RADTAN: return 10; case CAM_FISHEYE: return 9; case CAM_FOV: return 5;
-                   case CAM_DIVISION_UNDISTORTION: return 5; case CAM_DOUBLE_SPHERE: return 7; case CAM_EXTENDED_UNIFIED: return 7; default: return -1; }
+                   case CAM_DIVISION_UNDISTORTION: return 5; case CAM_DOUBLE_SPHERE: return 7; case CAM_EXTENDED_UNIFIED: return 7;
+                   case CAM_OMNI_RADTAN: return 10; default: return -1; }
 }
 
 // J is row-major 2x3: J[0..2] = d px / d(x,y,z), J[3..5] = d py / d(x,y,z).
@@ -166,7 +168,7 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
       const double ddx[2] = {-dx * in * dn[0], -dx * in * dn[1]}, ddy[2] = {-dy * in * dn[0], -dy * in * dn[1]};
       affine_skew_k(k, dx, dy, 2, idx, ddx, ddy, *pk);
     }
-  } else {  // CAM_EXTENDED_UNIFIED
+  } else if (MODEL == CAM_EXTENDED_UNIFIED) {
     const double al = k[5], be = k[6];
     const double r2 = p.x * p.x + p.y * p.y;
     const double rho = sqrt(be * r2 + p.z * p.z);
@@ -182,6 +184,29 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
       const double ddx[2] = {-dx * in * dn[0], -dx * in * dn[1]}, ddy[2] = {-dy * in * dn[0], -dy * in * dn[1]};
       affine_skew_k(k, dx, dy, 2, idx, ddx, ddy, *pk);
     }
+  } else if (MODEL == CAM_OMNI_RADTAN) {   // [f, ar, skew, cx, cy, xi, k1, k2, t1, t2]: unit sphere, then the pinhole from -xi on the axis
+    const double xi = k[5], k1 = k[6], k2 = k[7], t1 = k[8], t2 = k[9];
+    const double d = sqrt(p.x * p.x + p.y * p.y + p.z * p.z);
+    if (p.z <= -(xi <= 1.0 ? xi : 1.0 / xi) * d) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }   // EUCM's unified_w at alpha = xi / (1 + xi)
+    const double in = 1.0 / (p.z + xi * d), mx = p.x * in, my = p.y * in;
+    const double r2 = mx * mx + my * my;
+    const double rad = 1.0 + r2 * (k1 + k2 * r2), drad = k1 + 2.0 * k2 * r2;
+    const double dx = mx * rad + 2.0 * t1 * mx * my + t2 * (r2 + 2.0 * mx * mx);
+    const double dy = my * rad + 2.0 * t2 * mx * my + t1 * (r2 + 2.0 * my * my);
+    const double a00 = rad + 2.0 * mx * mx * drad + 2.0 * t1 * my + 6.0 * t2 * mx;   // a = d(dx,dy)/d(mx,my), symmetric
+    const double a01 = 2.0 * mx * my * drad + 2.0 * t1 * mx + 2.0 * t2 * my;
+    const double a11 = rad + 2.0 * my * my * drad + 2.0 * t2 * mx + 6.0 * t1 * my;
+    // d(mx,my)/dp = in ([I2 | 0] - (mx, my)^T dn/dp), dn/dp = xi p / d + ez;  so d(dx,dy)/dp = in ([a | 0] - (a m) dn/dp^T)
+    const double am0 = a00 * mx + a01 * my, am1 = a01 * mx + a11 * my;
+    const double s = xi / d, nx = s * p.x, ny = s * p.y, nz = s * p.z + 1.0;
+    double Dd[6] = {in * (a00 - am0 * nx), in * (a01 - am0 * ny), -in * am0 * nz, in * (a01 - am1 * nx), in * (a11 - am1 * ny), -in * am1 * nz};
+    affine_skew(k, dx, dy, Dd, o);
+    if (WITH_K) {   // d(mx,my)/d xi = -(mx,my) d / n
+      const int idx[5] = {5, 6, 7, 8, 9};
+      const double ddx[5] = {-am0 * d * in, mx * r2, mx * r2 * r2, 2.0 * mx * my, r2 + 2.0 * mx * mx};
+      const double ddy[5] = {-am1 * d * in, my * r2, my * r2 * r2, r2 + 2.0 * my * my, 2.0 * mx * my};
+      affine_skew_k(k, dx, dy, 5, idx, ddx, ddy, *pk);
+    }
   }
   return o;
 }
@@ -196,11 +221,12 @@ ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, 
     case CAM_EXTENDED_UNIFIED: return project_model<CAM_EXTENDED_UNIFIED, true>(k, p, dispatch_fov, pk);
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN, true>(k, p, dispatch_fov, pk);
     case CAM_FOV: return project_model<CAM_FOV, true>(k, p, dispatch_fov, pk);
+    case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN, true>(k, p, dispatch_fov, pk);
     default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 20; ++j) pk->Jk[j] = 0; return o; }
   }
 }
 
-// Runtime dispatch in the reference's order (residuals.h:366-389).
+// Runtime dispatch in the reference's order (residuals.h:366-389), then the extension CAM_OMNI_RADTAN.
 ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
   switch (model) {
     case CAM_DIVISION_UNDISTORTION: return project_model<CAM_DIVISION_UNDISTORTION>(k, p, dispatch_fov);
@@ -210,6 +236,7 @@ ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
     case CAM_EXTENDED_UNIFIED: return project_model<CAM_EXTENDED_UNIFIED>(k, p, dispatch_fov);
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN>(k, p, dispatch_fov);
     case CAM_FOV: return project_model<CAM_FOV>(k, p, dispatch_fov);
+    case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN>(k, p, dispatch_fov);
     default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
   }
 }
