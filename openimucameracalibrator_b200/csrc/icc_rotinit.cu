@@ -20,6 +20,7 @@
 #include "icc_reduce.cuh"
 
 #include "icc_rotinit_math.cuh"
+#include "icc_small_linalg.cuh"
 
 #include <cmath>
 
@@ -223,17 +224,6 @@ __global__ void init_state_kernel(RotInitProblem Q, double max_offset) {
   S->done = !(fabs(S->c - S->d) > Q.tolerance) ? 1 : 0;
 }
 
-void quat_from_rowmajor(const double* R, double* q) {    // -> x, y, z, w
-  const double m00 = R[0], m01 = R[1], m02 = R[2], m10 = R[3], m11 = R[4], m12 = R[5], m20 = R[6], m21 = R[7], m22 = R[8], tr = m00 + m11 + m22;
-  double x, y, z, w;
-  if (tr > 0.0) { const double s = std::sqrt(tr + 1.0) * 2.0; w = 0.25 * s; x = (m21 - m12) / s; y = (m02 - m20) / s; z = (m10 - m01) / s; }
-  else if (m00 > m11 && m00 > m22) { const double s = std::sqrt(1.0 + m00 - m11 - m22) * 2.0; w = (m21 - m12) / s; x = 0.25 * s; y = (m01 + m10) / s; z = (m02 + m20) / s; }
-  else if (m11 > m22) { const double s = std::sqrt(1.0 + m11 - m00 - m22) * 2.0; w = (m02 - m20) / s; x = (m01 + m10) / s; y = 0.25 * s; z = (m12 + m21) / s; }
-  else { const double s = std::sqrt(1.0 + m22 - m00 - m11) * 2.0; w = (m10 - m01) / s; x = (m02 + m20) / s; y = (m12 + m21) / s; z = 0.25 * s; }
-  const double n = std::sqrt(x * x + y * y + z * z + w * w);
-  q[0] = x / n; q[1] = y / n; q[2] = z / n; q[3] = w / n;
-}
-
 }  // namespace
 
 void launch_interp_quat(int n_old, const double* t_old, const double4* q_old, int n_new, const double* t_new, double4* q_new, cudaStream_t st) {
@@ -316,7 +306,9 @@ icc_status estimate_imu_to_camera_rotation(cudaStream_t st, int sm_count, int n_
   CU(cudaStreamSynchronize(st));
   if (cudaGetLastError() != cudaSuccess) { err = "rotation initialiser kernels failed"; return ICC_ERR_CUDA; }
   if (!S.done) { err = "golden-section search did not terminate"; return ICC_ERR_NUMERIC; }
-  quat_from_rowmajor(S.R_best, q_out);
+  const double* R = S.R_best;                                                              // row-major
+  const Q4 q = quat_from_columns(v3(R[0], R[3], R[6]), v3(R[1], R[4], R[7]), v3(R[2], R[5], R[8]));
+  q_out[0] = q.x; q_out[1] = q.y; q_out[2] = q.z; q_out[3] = q.w;
   *td_out = (S.b + S.a) / 2;                                                               // :259
   if (bias_out) for (int d = 0; d < 3; ++d) bias_out[d] = S.bias_best[d];
   if (err_out) *err_out = S.error;

@@ -20,17 +20,21 @@ def _rot(q, v):
     return v + q[3] * uv + np.cross(qv, uv)
 
 
-def _analytic(duration=40.0, fps=30.0, imu_hz=200.0, td=0.037, bias=(0.004, -0.002, 0.001), seed=0):
+def _analytic(duration=40.0, fps=30.0, imu_hz=200.0, td=0.037, bias=(0.004, -0.002, 0.001), seed=0, q_ic=Q_IC, extra=None, imu_t=None):
+    """Views, q_cw, gyroscope times and rates of the analytic scene; q_ic is the mounting (x y z w), extra(t) -> (a, da) adds a
+    rotation-vector term (a burst), imu_t replaces the regular gyroscope clock."""
     rng = np.random.default_rng(seed)
     f = np.array([0.13, 0.31, 0.47, 0.71, 0.97]); A = rng.uniform(0.05, 0.12, (3, 5)); ph = rng.uniform(0, 2 * np.pi, (3, 5))
-    a = lambda t: (A[None] * np.sin(2 * np.pi * f[None, None] * t[:, None, None] + ph[None])).sum(-1)                       # noqa: E731
-    da = lambda t: (A[None] * 2 * np.pi * f[None, None] * np.cos(2 * np.pi * f[None, None] * t[:, None, None] + ph[None])).sum(-1)  # noqa: E731
+    a0 = lambda t: (A[None] * np.sin(2 * np.pi * f[None, None] * t[:, None, None] + ph[None])).sum(-1)                       # noqa: E731
+    da0 = lambda t: (A[None] * 2 * np.pi * f[None, None] * np.cos(2 * np.pi * f[None, None] * t[:, None, None] + ph[None])).sum(-1)  # noqa: E731
+    a = a0 if extra is None else (lambda t: a0(t) + extra(t)[0])                                                          # noqa: E731
+    da = da0 if extra is None else (lambda t: da0(t) + extra(t)[1])                                                       # noqa: E731
     tv = np.arange(int(duration * fps)) / fps
     q_wc = syn.matrix_to_quat_xyzw(syn.so3_exp(a(tv)))
-    ti = np.arange(int(duration * imu_hz)) / imu_hz - 0.2
+    ti = np.arange(int(duration * imu_hz)) / imu_hz - 0.2 if imu_t is None else np.asarray(imu_t, dtype=np.float64)
     tq = ti + td                                                     # camera-clock time of IMU sample i: t_cam = t_imu + td
     w_c = np.einsum("nij,nj->ni", syn.so3_right_jacobian(a(tq)), da(tq))      # body rate of the camera frame
-    w_i = np.array([_rot(Q_IC, w) for w in w_c]) + np.asarray(bias)   # omega_c = R_ci omega_i
+    w_i = _rot(np.asarray(q_ic, dtype=np.float64), w_c) + np.asarray(bias)           # omega_c = R_ci omega_i (row-wise)
     return tv, q_wc * CONJ, ti, w_i
 
 
