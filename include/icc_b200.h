@@ -186,6 +186,33 @@ icc_status icc_set_knots(icc_handle* h, const double* so3_xyzw, const double* r3
 icc_status icc_set_T_i_c(icc_handle* h, const double T_i_c[7]);
 icc_status icc_set_line_delay(icc_handle* h, double line_delay_s);
 icc_status icc_get_mean_reprojection_error(icc_handle* h, double* err);
+
+/* ---- outlier corners between spline solves (extension: the reference has no per-corner rejection) -----------------------------------
+ * The error of a corner is e = sqrt(rx^2 + ry^2) of its unweighted residual pair at the current state with rolling-shutter timing: in the
+ * pixel mode exactly the terms icc_get_mean_reprojection_error averages, with ICC_REPROJ_ERROR_TANGENT the scaled tangent residual the solve
+ * minimises.  A pair with rx == 0 || ry == 0 (the reference's quirk in GetMeanReprojectionError, impl.h:1058-1064) is neither counted nor
+ * rejected; a failed projection (the constant 1e10 pair) is not counted and always rejected.
+ * icc_reject_outlier_corners sums e^2 and the count of the counted corners over the shards (the cross-rank sum of the solve), so every rank
+ * uses the same threshold = max(min_px, k_sigma * rms_px), and removes from this shard's solve every corner with e > threshold.  The state,
+ * the solver options and the inputs of icc_set_frames are not changed; icc_num_residuals, icc_evaluate, icc_get_eval_schedule and the next
+ * icc_optimize see the reduced set until icc_batch_init_spline assembles the problem again.  A frame left without corners keeps its knots
+ * (the IMU holds them).  ICC_ERR_STATE before icc_batch_init_spline; k_sigma <= 0 or non-finite, min_px negative or non-finite:
+ * ICC_ERR_INVALID_ARGUMENT. */
+typedef struct {
+  int64_t n_corners;        /* corners in the solve before this call (all shards) */
+  int64_t n_rejected;       /* removed by this call (all shards), failed projections included */
+  int64_t n_failed;         /* of those: corners whose projection failed (the 1e10 residuals) */
+  int32_t n_frames_emptied; /* frames left without corners (they leave the vision schedule; their knots stay, held by the IMU) */
+  int32_t reserved;
+  double rms_px;            /* sqrt(mean e^2) over the counted corners (all shards) */
+  double threshold_px;      /* max(min_px, k_sigma * rms_px) */
+} icc_outlier_summary;
+/* e of every corner in this shard's solve, in frame order; n = that count (icc_num_residuals' n_vision / 2 on the rolling-shutter path) */
+icc_status icc_get_corner_errors(icc_handle* h, int n, double* err_px);
+icc_status icc_reject_outlier_corners(icc_handle* h, double k_sigma, double min_px, icc_outlier_summary* out /* nullable */);
+/* per corner given to icc_set_frames (n_input = their count): 1 in this shard's solve, 0 rejected, -1 not assembled here (other shard,
+ * frame outside the spline).  Host only. */
+icc_status icc_get_corner_status(const icc_handle* h, int n_input, int32_t* status);
 /* number of IMU samples kept by BatchInitSpline and their (offset-corrected) timestamps / raw readings (app :265-327) */
 icc_status icc_get_num_imu_used(const icc_handle* h, int* n);
 icc_status icc_get_imu_used(const icc_handle* h, double* t_s, double* accel_xyz, double* gyro_xyz);

@@ -54,6 +54,15 @@ class Summary(C.Structure):
         return d
 
 
+class OutlierSummary(C.Structure):
+    """icc_outlier_summary (include/icc_b200.h): what one icc_reject_outlier_corners call did, summed over the shards."""
+    _fields_ = [("n_corners", C.c_int64), ("n_rejected", C.c_int64), ("n_failed", C.c_int64), ("n_frames_emptied", C.c_int32),
+                ("reserved", C.c_int32), ("rms_px", C.c_double), ("threshold_px", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 class CamCalOptions(C.Structure):
     """icc_camcal_options (include/icc_b200.h): zero / negative fields select the reference's defaults."""
     _fields_ = [("grid_size", C.c_double), ("function_tolerance", C.c_double), ("parameter_tolerance", C.c_double), ("gradient_tolerance", C.c_double),
@@ -199,6 +208,7 @@ class CApi:
         t = _f64(t_s); off = np.ascontiguousarray(corner_offsets, dtype=np.int32); ids = np.ascontiguousarray(point_ids, dtype=np.int32)
         uv = _f64(uv); q = _f64(q_wc); p = _f64(p_wc)
         assert off.size == t.size + 1 and ids.size == off[-1] and uv.size == 2 * ids.size and q.size == 4 * t.size and p.size == 3 * t.size
+        self._n_corners_in = int(ids.size)
         self._call("set_frames", [C.c_int, c_double_p, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p], t.size, _dp(t),
                    off.ctypes.data_as(c_int32_p), ids.ctypes.data_as(c_int32_p), _dp(uv), _dp(q), _dp(p))
 
@@ -492,6 +502,25 @@ class CApi:
 
     def mean_reprojection_error(self):
         v = C.c_double(); self._call("get_mean_reprojection_error", [c_double_p], C.byref(v)); return v.value
+
+    def corner_status(self):
+        """Per corner given to set_frames: 1 in this shard's solve, 0 rejected by reject_outlier_corners, -1 not assembled here."""
+        st = np.zeros(self._n_corners_in, dtype=np.int32)
+        self._call("get_corner_status", [C.c_int, c_int32_p], st.size, st.ctypes.data_as(c_int32_p))
+        return st
+
+    def corner_errors(self):
+        """|(rx, ry)| of every corner in this shard's solve at the current state, in frame order."""
+        n = int(np.count_nonzero(self.corner_status() == 1))
+        e = np.zeros(n)
+        self._call("get_corner_errors", [C.c_int, c_double_p], n, _dp(e))
+        return e
+
+    def reject_outlier_corners(self, k_sigma, min_px=1.0) -> dict:
+        """Remove from the solve every corner whose error exceeds max(min_px, k_sigma * rms) (failed projections always)."""
+        o = OutlierSummary()
+        self._call("reject_outlier_corners", [C.c_double, C.c_double, C.POINTER(OutlierSummary)], float(k_sigma), float(min_px), C.byref(o))
+        return o.as_dict()
 
     def imu_used(self):
         n = C.c_int(); self._call("get_num_imu_used", [C.POINTER(C.c_int)], C.byref(n))

@@ -87,6 +87,18 @@ class ImuCameraCalibrator:
         self.last_summary = self.api.optimize(iterations, int(optim_flags))
         return self.last_summary.mean_reproj_error
 
+    def GetCornerErrors(self):
+        """Per-corner reprojection error |(rx, ry)| [px, or scaled tangent units] of the corners in the solve, in frame order."""
+        return self.api.corner_errors()
+
+    def RejectOutlierCorners(self, k_sigma: float, min_px: float = 1.0) -> dict:
+        """Drop the corners whose error exceeds max(min_px, k_sigma * rms) until the next BatchInitSpline (icc_reject_outlier_corners)."""
+        return self.api.reject_outlier_corners(k_sigma, min_px)
+
+    def GetCornerStatus(self):
+        """Per input corner: 1 in the solve, 0 rejected, -1 not assembled (icc_get_corner_status)."""
+        return self.api.corner_status()
+
     def GetCamTimestamps(self):
         return self._cam_timestamps
 

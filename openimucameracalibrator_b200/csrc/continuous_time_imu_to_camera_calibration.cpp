@@ -20,6 +20,10 @@
 // --gpus N (residual blocks sharded by time slice over devices device..device+N-1 of this host: the binary spawns one rank process per
 // extra device -- hidden flags --shard_rank / --shard_world / --comm_id_hex -- each with the library's own NCCL communicator; one
 // all-reduce of the packed normal equations per Jacobian evaluation).
+// --outlier_sigma k (default 0 = off), --outlier_min_px m (default 1), --outlier_rounds n (default 2): after stage 1, up to n rounds of
+// icc_reject_outlier_corners (corners whose reprojection error exceeds max(m, k * rms) leave the solve) each followed by stage 1 again with
+// the same flags and iteration limit, until a round rejects nothing; stage 2 then runs as before.  With k > 0 the result JSON also holds
+// "outlier_corners_rejected" (all rounds) and "outlier_threshold_px" (the last round's threshold).
 #include "../../include/icc_b200.h"
 #include "icc_cli_common.hpp"
 
@@ -47,7 +51,8 @@ icccli::Flags default_flags() {
     {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"},
     {"pose_shutter", "global"}, {"reprojection_error", "pixel"}};
   f.boolean = {{"global_shutter", false}, {"calibrate_cam_line_delay", false}, {"reestimate_biases", false}, {"parse_only", false}, {"json_selftest", false}};
-  f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0}};
+  f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0},
+    {"outlier_sigma", 0.0}, {"outlier_min_px", 1.0}, {"outlier_rounds", 2.0}};
   return f;
 }
 
@@ -165,9 +170,16 @@ int main(int argc, char** argv) {
   icccli::Flags F = default_flags();
   int pose_error = ICC_POSE_ERROR_NORMALIZED, reproj_error = ICC_REPROJ_ERROR_PIXEL;
   bool pose_rolling = false;
+  double outlier_sigma = 0.0, outlier_min_px = 1.0; int outlier_rounds = 2;
   try {
     icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); pose_rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]);
     reproj_error = icccli::parse_reprojection_error(F.str["reprojection_error"]);
+    outlier_sigma = F.num["outlier_sigma"]; outlier_min_px = F.num["outlier_min_px"];
+    if (!(outlier_sigma >= 0.0) || !std::isfinite(outlier_sigma)) throw std::runtime_error("--outlier_sigma must be a finite number >= 0 (0 = off)");
+    if (!(outlier_min_px >= 0.0) || !std::isfinite(outlier_min_px)) throw std::runtime_error("--outlier_min_px must be a finite number >= 0");
+    if (!(F.num["outlier_rounds"] >= 0.0) || F.num["outlier_rounds"] > 1000.0 || F.num["outlier_rounds"] != std::floor(F.num["outlier_rounds"]))
+      throw std::runtime_error("--outlier_rounds must be a whole number >= 0");
+    outlier_rounds = (int)F.num["outlier_rounds"];
     if (pose_rolling && F.boolean["global_shutter"]) throw std::runtime_error("--pose_shutter rolling contradicts --global_shutter");
     if (pose_rolling && !F.str["input_pose_dataset"].empty()) throw std::runtime_error("--pose_shutter rolling applies to the in-process pose step, which --input_pose_dataset skips");
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
@@ -318,6 +330,7 @@ int main(int argc, char** argv) {
       s["views"] = Value((int64_t)frame_t.size()); s["corners"] = Value((int64_t)ids.size()); s["imu_samples"] = Value((int64_t)imu_t.size());
       s["board_points"] = Value((int64_t)(max_id + 1)); s["camera_model"] = Value(model); s["intrinsics"] = Value::array();
       for (double v : intr) s["intrinsics"].push_back(Value(v));
+      if (outlier_sigma > 0.0) { s["outlier_sigma"] = Value(outlier_sigma); s["outlier_min_px"] = Value(outlier_min_px); s["outlier_rounds"] = Value((int64_t)outlier_rounds); }
       s["init_line_delay_s"] = Value(init_line_delay); s["dt_so3"] = Value(ip.dt_so3_s); s["dt_r3"] = Value(ip.dt_r3_s); s["first_view_t_s"] = Value(frame_t.front());
       s["uv_sum"] = Value([&] { double a = 0; for (double v : uv) a += v; return a; }());
       // order-sensitive digests: the views must arrive in std::map key order, the corners of a view in the order of their id strings
@@ -384,6 +397,17 @@ int main(int argc, char** argv) {
       if (grav_dir_axis != -1) { double g[3] = {0, 0, 0}; g[grav_dir_axis] = F.num["gravity_const"]; ICC(icc_set_known_gravity_dir(h, g)); }
     }
     ICC(icc_optimize(h, 50, flags, &s1));
+    // --outlier_sigma: reject, and solve stage 1 again, until a round rejects nothing (every rank runs the same calls: the threshold is global)
+    int64_t outliers_rejected = 0; double outlier_threshold = 0.0;
+    for (int round = 1; outlier_sigma > 0.0 && round <= outlier_rounds; ++round) {
+      icc_outlier_summary os;
+      ICC(icc_reject_outlier_corners(h, outlier_sigma, outlier_min_px, &os));
+      outliers_rejected += os.n_rejected; outlier_threshold = os.threshold_px;
+      std::cout << "Outlier round " << round << ": threshold " << os.threshold_px << " px, rejected " << os.n_rejected << " of " << os.n_corners
+                << " corners (" << os.n_failed << " failed projections, " << os.n_frames_emptied << " views emptied)\n";
+      if (os.n_rejected == 0) break;
+      ICC(icc_optimize(h, 50, flags, &s1));
+    }
     if (stage2) ICC(icc_optimize(h, 10, ICC_FLAG_CAM_LINE_DELAY, &s2));
     if (shard_rank > 0) { icc_destroy(h); icc_comm_destroy(comm); return 0; }   // only rank 0 reports
     double reproj_error = s1.mean_reproj_error, reproj_error_after_ld = stage2 ? s2.mean_reproj_error : reproj_error;
@@ -403,6 +427,7 @@ int main(int argc, char** argv) {
     out["r3_dt"] = Value(ip.dt_r3_s); out["so3_dt"] = Value(ip.dt_so3_s);
     out["init_line_delay_us"] = Value(init_line_delay * S_TO_US); out["calib_line_delay_us"] = Value(calib_line_delay_us);
     out["time_offset_imu_to_cam_s"] = Value(time_offset_imu_to_cam);
+    if (outlier_sigma > 0.0) { out["outlier_corners_rejected"] = Value(outliers_rejected); out["outlier_threshold_px"] = Value(outlier_threshold); }
     int n_used = 0; ICC(icc_get_num_imu_used(h, &n_used));
     std::vector<double> ut(n_used), ua(3 * (size_t)n_used), ug(3 * (size_t)n_used);
     ICC(icc_get_imu_used(h, ut.data(), ua.data(), ug.data()));

@@ -133,6 +133,9 @@ struct icc_handle {
   std::vector<double> used_uv; std::vector<int> used_pid;   // gathered corners -- only when the used frames are not one contiguous run
   bool used_contig = false; int used_c0 = 0, used_n = 0;    // ... otherwise corners [used_c0, used_c0 + used_n) of uv / point_ids are used in place
   bool imu_contig = false; int imu_src0 = 0;                // same for the accelerometer / gyroscope samples
+  std::vector<std::pair<int, int>> frame_in;               // input corner range (icc_set_frames) of every frame in the problem
+  size_t n_corners_assembled = 0;                           // corners given to icc_set_frames when the problem was assembled
+  bool corners_rejected = false;                            // icc_reject_outlier_corners has compacted the corners since batch_init
   std::vector<double> imu_used_t, imu_used_acc, imu_used_gyr; HostBuf<int64_t> imu_used_st;
   size_t n_imu_used = 0;                     // kept samples; imu_used_t / imu_used_st are only materialised off the sorted fast path (imu_lazy == false)
   bool imu_lazy = false;                     // sorted fast path: kept samples = imu_t[imu_src0 .. +n_imu_used) + time offset, relative times derived on the device
@@ -151,6 +154,9 @@ struct icc_handle {
   DevBuf<double> d_view_t, d_view_q, d_view_p;   // per-view pose priors in time order (knot initialisation kernel)
   DevBuf<VisFrame> d_vframes; DevBuf<VisItem> d_vitems;
   DevBuf<double4> d_bear; DevBuf<int> d_bear_ok;   // tangent mode: the used corners' bearings, in stream order next to P.uv
+  // outlier corners: residual pairs, errors and sums of the error pass; input index of every corner (once rejected); compaction targets
+  DevBuf<double> d_cres, d_cerr, d_osum; DevBuf<int> d_csrc, d_ckept, d_in_off, d_foff_new;
+  DevBuf<double2> d_uv_new; DevBuf<int> d_pid_new, d_bear_ok_new, d_csrc_new; DevBuf<double4> d_bear_new;
   TangentMeas tan{nullptr, nullptr, 0.0};          // ... and what the evaluation kernels read of them (tangent_meas)
   DevBuf<ImuCellP> d_icells; DevBuf<VisItem> d_iitems;
   std::vector<VisItem> vitems, iitems;   // host copies of the per-warp runs (icc_get_eval_schedule)
@@ -812,7 +818,8 @@ icc_status select_general(icc_handle* h, const KnotCounts& n, const std::vector<
 // shard), else gathered on the host
 icc_status gather_corners(icc_handle* h, const std::vector<FrameHost>& frames, const std::vector<int>& frame_sel) {
   h->frames.clear(); h->used_uv.clear(); h->used_pid.clear();
-  h->frames.reserve(frame_sel.size());
+  h->frames.reserve(frame_sel.size()); h->corners_rejected = false; h->n_corners_assembled = h->n_corners_in;
+  h->frame_in.clear(); for (int fi : frame_sel) h->frame_in.push_back({frames[fi].c0, frames[fi].c1});
   bool consecutive = !frame_sel.empty();
   for (size_t k = 1; k < frame_sel.size() && consecutive; ++k) consecutive = frame_sel[k] == frame_sel[k - 1] + 1;
   h->used_contig = consecutive; h->used_c0 = 0; h->used_n = 0;
@@ -916,9 +923,32 @@ EvalStreams eval_schedule(icc_handle* h) {
   return es;
 }
 
+// work lists: one warp per item; items sized so that the grid fills the GPU but every item amortises its tile flush
+int work_items_target(const icc_handle* h) { return h->sm_count * 8; }
+int round32(long v) { return (int)((v + 31) / 32 * 32); }
+// the one-warp vision kernels' items: runs of at most per_v corners of one frame (after batch_init and after a corner rejection)
+icc_status upload_vision_work(icc_handle* h) {
+  DeviceProblem& P = h->P;
+  const int per_v = std::max(32, round32(P.n_corners / std::max(1, work_items_target(h))));
+  std::vector<VisionWork> vw;
+  for (int fi = 0; fi < P.n_frames; ++fi) for (int c = h->frames[fi].c0; c < h->frames[fi].c1; c += per_v) vw.push_back({fi, c, std::min(c + per_v, h->frames[fi].c1), 0});
+  CU(upload_staged(h, h->d_vwork, vw)); P.vwork = h->d_vwork.p; P.n_vwork = (int)vw.size();
+  return ICC_OK;
+}
+// the persistent kernel's unit tables and per-warp runs (eval_schedule)
+icc_status upload_schedule(icc_handle* h, const EvalStreams& es) {
+  DeviceProblem& P = h->P;
+  CU(upload_staged(h, h->d_vframes, es.vf)); P.vframes = h->d_vframes.p;
+  CU(upload_staged(h, h->d_vitems, h->vitems)); P.vitems = h->d_vitems.p;
+  CU(upload_staged(h, h->d_icells, es.ic)); P.icells = h->d_icells.p;
+  CU(upload_staged(h, h->d_iitems, h->iitems)); P.iitems = h->d_iitems.p;
+  return ICC_OK;
+}
+
 // Device upload: the problem arrays and work lists, both state copies, and the knots by init_knots_kernel from the view table.  The small
 // arrays are staged through the pinned arena: its size below must cover everything staged through it until the next batch_init (each
-// array takes a multiple of 256 bytes), else upload_staged falls back to blocking copies.
+// array takes a multiple of 256 bytes), else upload_staged falls back to blocking copies.  A corner rejection restarts the arena once the
+// stream has drained and stages only the vision work list and the schedule again, both within what this budget gives them.
 icc_status upload_problem(icc_handle* h, const ViewTable& v, const Pose& Tci, const EvalStreams& es, PhaseTrace& trace) {
   DeviceProblem& P = h->P;
   const size_t nf = h->frame_t.size();
@@ -953,22 +983,13 @@ icc_status upload_problem(icc_handle* h, const ViewTable& v, const Pose& Tci, co
       launch_bearings(h->model, h->intr, P.n_corners, P.uv, h->d_bear.p, h->d_bear_ok.p, h->stream);
       h->tan = TangentMeas{h->d_bear.p, h->d_bear_ok.p, tangent_scale(h->model, h->intr, P.dispatch_fov != 0)};
     }
-    // work lists: one warp per item; items sized so that the grid fills the GPU but every item amortises its tile flush
-    const int target_items = h->sm_count * 8;
-    auto round32 = [](long v) { return (int)((v + 31) / 32 * 32); };
-    const int per_v = std::max(32, round32(P.n_corners / std::max(1, target_items)));
-    std::vector<VisionWork> vw;
-    for (int fi = 0; fi < P.n_frames; ++fi) for (int c = h->frames[fi].c0; c < h->frames[fi].c1; c += per_v) vw.push_back({fi, c, std::min(c + per_v, h->frames[fi].c1), 0});
-    CU(upload_staged(h, h->d_vwork, vw)); P.vwork = h->d_vwork.p; P.n_vwork = (int)vw.size();
-    const int per_i = std::max(32, round32(P.n_imu / std::max(1, target_items)));
+    { icc_status r = upload_vision_work(h); if (r != ICC_OK) return r; }
+    const int per_i = std::max(32, round32(P.n_imu / std::max(1, work_items_target(h))));
     std::vector<ImuCell> iw;
     for (const auto& c : h->cells) for (int i = c.i_begin; i < c.i_end; i += per_i) { ImuCell s = c; s.i_begin = i; s.i_end = std::min(i + per_i, c.i_end); iw.push_back(s); }
     CU(upload_staged(h, h->d_iwork, iw)); P.iwork = h->d_iwork.p; P.n_iwork = (int)iw.size();
     CU(upload_staged(h, h->d_cells, h->cells)); P.cells = h->d_cells.p;
-    CU(upload_staged(h, h->d_vframes, es.vf)); P.vframes = h->d_vframes.p;
-    CU(upload_staged(h, h->d_vitems, h->vitems)); P.vitems = h->d_vitems.p;
-    CU(upload_staged(h, h->d_icells, es.ic)); P.icells = h->d_icells.p;
-    CU(upload_staged(h, h->d_iitems, h->iitems)); P.iitems = h->d_iitems.p;
+    { icc_status r = upload_schedule(h, es); if (r != ICC_OK) return r; }
     CU(h->d_imu_t.alloc(h->n_imu_used));
     if (h->imu_lazy && h->n_imu_used) {   // sorted stream: the raw stamps go up, the relative integer times are derived there
       CU(h->d_imu_traw.alloc(h->n_imu_used));
@@ -998,6 +1019,85 @@ icc_status upload_problem(icc_handle* h, const ViewTable& v, const Pose& Tci, co
     h->knots_dirty_host = true;     // the device holds the knots; the host mirror is refreshed on demand (getters / setters)
   }
   trace.lap("batch_init: knot init");
+  return ICC_OK;
+}
+
+
+// ---- outlier corners (icc_get_corner_errors / icc_reject_outlier_corners) ------------------------------------------------------------------
+template <class T> void swap_dev(DevBuf<T>& a, DevBuf<T>& b) { std::swap(a.p, b.p); std::swap(a.n, b.n); std::swap(a.cap_bytes, b.cap_bytes); }
+
+// Residual pair of every corner at the current state (the cost-only vision kernel, rolling-shutter timing in either shutter mode, the
+// residual of the solve: tangent or pixel), then e = |pair| per corner into d_cerr and {sum e^2, count, failed} into d_osum[0..2]
+icc_status corner_error_pass(icc_handle* h) {
+  const DeviceProblem& P = h->P;
+  const int n = P.n_corners;
+  CU(h->d_osum.alloc(4)); CU(cudaMemsetAsync(h->d_osum.p, 0, 4 * sizeof(double), h->stream));
+  CU(h->d_cres.alloc(2 * (size_t)n)); CU(h->d_cerr.alloc((size_t)n));
+  if (n > 0 && P.n_vwork > 0) {
+    DeviceProblem Q = P; Q.n_iwork = 0; Q.rolling = 1;
+    if (launch_eval(Q, h->st[h->cur].view(), false, nullptr, h->d_cres.p, nullptr, h->stream, nullptr, tangent_meas(h))) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
+    launch_corner_errors(n, h->d_cres.p, h->d_cerr.p, h->d_osum.p, h->stream);
+  }
+  return ICC_OK;
+}
+
+icc_status reject_outliers(icc_handle* h, double k_sigma, double min_px, icc_outlier_summary* out) {
+  DeviceProblem& P = h->P;
+  const int n = P.n_corners, nf = P.n_frames;
+  const bool tangent = h->reproj_error == ICC_REPROJ_ERROR_TANGENT;
+  { icc_status r = corner_error_pass(h); if (r != ICC_OK) return r; }
+  double sums[4] = {0.0, 0.0, 0.0, double(n)};
+  CU(cudaMemcpyAsync(h->d_osum.p + 3, sums + 3, sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  { icc_status r = cross_rank_sum(h, h->d_osum.p, 4); if (r != ICC_OK) return r; }   // every rank enters, with or without corners
+  CU(cudaMemcpyAsync(sums, h->d_osum.p, sizeof sums, cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  const double rms = sums[1] > 0.0 ? std::sqrt(sums[0] / sums[1]) : 0.0, thr = std::max(min_px, k_sigma * rms);
+  int n_new = n, emptied = 0;
+  if (n > 0) {
+    CU(h->d_ckept.alloc((size_t)nf)); CU(h->d_foff_new.alloc((size_t)nf + 1));
+    CU(h->d_uv_new.alloc((size_t)n)); CU(h->d_pid_new.alloc((size_t)n)); CU(h->d_csrc_new.alloc((size_t)n));
+    if (tangent) { CU(h->d_bear_new.alloc((size_t)n)); CU(h->d_bear_ok_new.alloc((size_t)n)); }
+    if (!h->corners_rejected) {   // the corners still lie as assembled: the input index follows from each frame's first input corner
+      std::vector<int> in_off(nf); for (int k = 0; k < nf; ++k) in_off[k] = h->frame_in[k].first;
+      CU(h->d_in_off.upload(in_off));
+    }
+    CornerCompaction C{nf, thr, P.f_off, h->d_cres.p, h->d_cerr.p, P.uv, P.pid, tangent ? h->tan.bear : nullptr, tangent ? h->tan.ok : nullptr,
+                       h->corners_rejected ? h->d_csrc.p : nullptr, h->d_in_off.p, h->d_ckept.p, h->d_foff_new.p, h->d_uv_new.p, h->d_pid_new.p,
+                       tangent ? h->d_bear_new.p : nullptr, tangent ? h->d_bear_ok_new.p : nullptr, h->d_csrc_new.p};
+    launch_compact_corners(C, h->stream);
+    std::vector<int> kept((size_t)nf);   // the only per-frame data that comes back
+    CU(cudaMemcpyAsync(kept.data(), h->d_ckept.p, (size_t)nf * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->arena.reset(0, true);   // the stream has drained: every staged copy is done, so the vision tables below are staged from the arena's start
+    // the compacted arrays become the problem's own (the inputs of icc_set_frames, d_uv_all included, are never written)
+    swap_dev(h->d_uv, h->d_uv_new); swap_dev(h->d_pid, h->d_pid_new); swap_dev(h->d_csrc, h->d_csrc_new); swap_dev(h->d_f_off, h->d_foff_new);
+    if (tangent) { swap_dev(h->d_bear, h->d_bear_new); swap_dev(h->d_bear_ok, h->d_bear_ok_new); h->tan.bear = h->d_bear.p; h->tan.ok = h->d_bear_ok.p; }
+    h->corners_rejected = true;
+    int c = 0;
+    for (int k = 0; k < nf; ++k) {
+      FrameHost& f = h->frames[k];
+      if (f.c1 > f.c0 && kept[k] == 0) ++emptied;
+      f.c0 = c; c += kept[k]; f.c1 = c;
+    }
+    n_new = c;
+    P.uv = h->d_uv.p; P.pid = h->d_pid.p; P.f_off = h->d_f_off.p;
+    P.n_corners = n_new; P.n_res_vis = P.rolling ? 2 * n_new : 0;
+    { icc_status r = upload_vision_work(h); if (r != ICC_OK) return r; }
+    const EvalStreams es = eval_schedule(h);
+    { icc_status r = upload_schedule(h, es); if (r != ICC_OK) return r; }
+    h->ne_flags = -1;
+  }
+  double moved[2] = {double(n - n_new), double(emptied)};
+  if (h->shard_world > 1) {
+    CU(cudaMemcpyAsync(h->d_osum.p, moved, sizeof moved, cudaMemcpyHostToDevice, h->stream));
+    { icc_status r = cross_rank_sum(h, h->d_osum.p, 2); if (r != ICC_OK) return r; }
+    CU(cudaMemcpyAsync(moved, h->d_osum.p, sizeof moved, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+  }
+  if (out) {
+    out->n_corners = (int64_t)llround(sums[3]); out->n_rejected = (int64_t)llround(moved[0]); out->n_failed = (int64_t)llround(sums[2]);
+    out->n_frames_emptied = (int32_t)llround(moved[1]); out->rms_px = rms; out->threshold_px = thr;
+  }
   return ICC_OK;
 }
 
@@ -1729,6 +1829,43 @@ icc_status icc_get_allan_curves(const icc_handle* h, int channel, int32_t* facto
   std::copy(C.sigma2[channel].begin(), C.sigma2[channel].end(), sigma2);
   std::copy(C.fit_deviation[channel].begin(), C.fit_deviation[channel].end(), fit_deviation);
   *len = need;
+  return ICC_OK;
+}
+
+icc_status icc_get_corner_errors(icc_handle* h, int n, double* err) {
+  if (!h || (!err && n != 0)) return ICC_ERR_INVALID_ARGUMENT;
+  NEED_DEVICE();
+  if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
+  if (n != h->P.n_corners) return fail(h, ICC_ERR_INVALID_ARGUMENT, "n must be the number of corners in this shard's solve (icc_num_residuals)");
+  CU(cudaSetDevice(h->device));
+  { icc_status r = corner_error_pass(h); if (r != ICC_OK) return r; }
+  if (n > 0) CU(cudaMemcpyAsync(err, h->d_cerr.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU(cudaStreamSynchronize(h->stream));
+  return ICC_OK;
+}
+icc_status icc_reject_outlier_corners(icc_handle* h, double k_sigma, double min_px, icc_outlier_summary* out) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (!(k_sigma > 0.0) || !std::isfinite(k_sigma) || !(min_px >= 0.0) || !std::isfinite(min_px))
+    return fail(h, ICC_ERR_INVALID_ARGUMENT, "k_sigma must be positive and finite, min_px non-negative and finite");
+  NEED_DEVICE();
+  if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
+  CU(cudaSetDevice(h->device));
+  return reject_outliers(h, k_sigma, min_px, out);
+}
+icc_status icc_get_corner_status(const icc_handle* hc, int n_input, int32_t* status) {
+  icc_handle* h = const_cast<icc_handle*>(hc);
+  if (!h || !status) return ICC_ERR_INVALID_ARGUMENT;
+  if (!h->initialised) return fail(h, ICC_ERR_STATE, "icc_batch_init_spline must be called first");
+  if (n_input < 0 || (size_t)n_input != h->n_corners_assembled) return fail(h, ICC_ERR_INVALID_ARGUMENT, "n_input must be the number of corners given to icc_set_frames");
+  std::fill(status, status + n_input, -1);
+  for (const auto& r : h->frame_in) std::fill(status + r.first, status + r.second, h->corners_rejected ? 0 : 1);
+  if (h->corners_rejected && h->P.n_corners > 0) {
+    std::vector<int> src((size_t)h->P.n_corners);
+    CU(cudaSetDevice(h->device));
+    CU(cudaMemcpyAsync(src.data(), h->d_csrc.p, src.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    for (const int c : src) status[c] = 1;
+  }
   return ICC_OK;
 }
 

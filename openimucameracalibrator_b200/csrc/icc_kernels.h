@@ -163,6 +163,20 @@ void launch_board_focal(const PoseProblem& Q, const double2* uv, double cx, doub
 void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, double f, double2* xy, int* ok, cudaStream_t st);
 // unit bearings of pixels (icc_bearing_math.cuh); ok[i] = 1 when b[i] could be formed (icc_pose.cu)
 void launch_bearings(int model, const double* intr10, int n, const double2* uv, double4* b, int* ok, cudaStream_t st);
+// ---- outlier corners (icc_outliers.cu) -----------------------------------------------------------------------------
+// err[c] = |(rx, ry)| of the residual pairs res2 (2 per corner); sums[0..2] += sum e^2 and the count over the counted corners (no zero
+// component, no failed projection), the failed projections
+void launch_corner_errors(int n, const double* res2, double* err, double* sums, cudaStream_t st);
+// The corners of every frame that the rule keeps, in order, written to the *_out arrays (bear_* may be null: pixel mode); kept[f] and
+// off_new (n_frames + 1) are the new per-frame counts and offsets; src_out = input corner index (src_in, or in_off[f] + position)
+struct CornerCompaction {
+  int n_frames; double threshold;
+  const int* off_old; const double* res2; const double* err;
+  const double2* uv_in; const int* pid_in; const double4* bear_in; const int* bear_ok_in; const int* src_in; const int* in_off;
+  int* kept; int* off_new;
+  double2* uv_out; int* pid_out; double4* bear_out; int* bear_ok_out; int* src_out;
+};
+void launch_compact_corners(const CornerCompaction& C, cudaStream_t st);
 int kernel_launch_count();   // kernels launched so far in this process (icc_eval.cu)
 void count_launch();         // every launcher calls it once per kernel it enqueues
 

@@ -7,7 +7,7 @@
 per_kernel=0; if [ "$1" = "-k" ]; then per_kernel=1; shift; fi
 dir="${1:-$(dirname "$0")/../openimucameracalibrator_b200/csrc}"
 sass=$(mktemp); trap 'rm -f "$sass"' EXIT
-for f in icc_eval icc_eval_tmem icc_init icc_points icc_solver icc_pose icc_camcal icc_rotinit icc_sew icc_static_imu icc_allan; do
+for f in icc_eval icc_eval_tmem icc_init icc_points icc_solver icc_pose icc_camcal icc_rotinit icc_sew icc_static_imu icc_allan icc_outliers; do
   cuobjdump -sass "$dir/$f.o" | grep -v '^\s*/\*[0-9a-f]\{4\}\*/\s*$' | sed -E 's/_GLOBAL__N__[0-9a-f]+_[0-9]+_[A-Za-z0-9_]+_cu_[0-9a-f]+/_ANON_/g' > "$sass"
   echo "$(md5sum < "$sass" | cut -d' ' -f1)  $f.o"
   if [ "$per_kernel" = 1 ]; then
