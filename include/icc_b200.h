@@ -43,7 +43,11 @@ typedef enum {
  *   EXTENDED_UNIFIED          [f, ar, skew, cx, cy, alpha, beta]
  *   OMNI_RADIAL_TANGENTIAL    [f, ar, skew, cx, cy, xi, k1, k2, t1, t2]   (extension, no Theia counterpart: Kalibr's omni-radtan;
  *                             n = z + xi |p|, (mx, my) = (x, y) / n radial-tangentially distorted, then the skewed affine; valid iff
- *                             z > -w |p|, w = xi <= 1 ? xi : 1 / xi) */
+ *                             z > -w |p|, w = xi <= 1 ? xi : 1 / xi)
+ *   SCARAMUZZA                [a0, c, e, cx, cy, a2, a3, a4, d]   (extension, no Theia counterpart: Scaramuzza's omnidirectional model as
+ *                             OCamCalib calibrates it; the pixel's sensor point (u', v') = A^-1 (u - cx, v - cy), A = [[1, e], [d, c]], sees the ray
+ *                             (u', v', a0 + a2 rho^2 + a3 rho^3 + a4 rho^4), rho = |(u', v')|; a point projects through the root of that quartic,
+ *                             valid iff z / |(x, y)| > F(rho_max) / rho_max, rho_max = the first stationary point of F(rho) / rho) */
 typedef enum {
   ICC_CAM_PINHOLE = 0,
   ICC_CAM_PINHOLE_RADIAL_TANGENTIAL = 1,
@@ -52,7 +56,8 @@ typedef enum {
   ICC_CAM_DIVISION_UNDISTORTION = 4,
   ICC_CAM_DOUBLE_SPHERE = 5,
   ICC_CAM_EXTENDED_UNIFIED = 6,
-  ICC_CAM_OMNI_RADIAL_TANGENTIAL = 7
+  ICC_CAM_OMNI_RADIAL_TANGENTIAL = 7,
+  ICC_CAM_SCARAMUZZA = 8
 } icc_camera_model;
 
 /* OpenICC::core::SplineOptimFlags (core/spline_trajectory_estimator.h:17-27), same numeric values. */
@@ -325,7 +330,7 @@ icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, doub
 /* Unit bearing vectors of `n` pixels with the handle's camera: xyz_out[3n], ok[n] (nullable; 0 where the ray reprojects more than 1e-6 px
  * away).  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion give icc_pixels_to_normalized's ray normalised; Fisheye's ray
  * stays in z > 0 (the model maps p and -p to one pixel); DoubleSphere, ExtendedUnified and OmniRadialTangential reach their whole domain,
- * z <= 0 included. */
+ * z <= 0 included; Scaramuzza back-projects in closed form (ok = 0 beyond rho_max). */
 icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double* xyz_out, int32_t* ok);
 
 /* Residual of the per-view pose refinement, the inlier test and the board-point refinement of icc_estimate_board_poses and

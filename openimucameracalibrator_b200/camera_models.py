@@ -11,6 +11,7 @@ import numpy as np
 
 PINHOLE, PINHOLE_RADIAL_TANGENTIAL, FISHEYE, FOV, DIVISION_UNDISTORTION, DOUBLE_SPHERE, EXTENDED_UNIFIED = range(7)
 OMNI_RADIAL_TANGENTIAL = 7   # extension without a Theia counterpart: Kalibr's omni-radtan
+SCARAMUZZA = 8               # extension without a Theia counterpart: Scaramuzza's omnidirectional polynomial model (OCamCalib)
 
 MODEL_NAMES = {
     PINHOLE: "PINHOLE",
@@ -21,10 +22,11 @@ MODEL_NAMES = {
     DOUBLE_SPHERE: "DOUBLE_SPHERE",
     EXTENDED_UNIFIED: "EXTENDED_UNIFIED",
     OMNI_RADIAL_TANGENTIAL: "OMNI_RADIAL_TANGENTIAL",
+    SCARAMUZZA: "SCARAMUZZA",
 }
 MODEL_IDS = {v: k for k, v in MODEL_NAMES.items()}
 NUM_PARAMS = {PINHOLE: 7, PINHOLE_RADIAL_TANGENTIAL: 10, FISHEYE: 9, FOV: 5, DIVISION_UNDISTORTION: 5,
-              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10}
+              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10, SCARAMUZZA: 9}
 
 
 def _affine_skew(k, dx, dy):
@@ -33,6 +35,79 @@ def _affine_skew(k, dx, dy):
 
 def _unified_w(alpha):
     return (1.0 - alpha) / alpha if alpha > 0.5 else alpha / (1.0 - alpha)
+
+
+def scaramuzza_F(k, rho):
+    """F(rho) = a0 + a2 rho^2 + a3 rho^3 + a4 rho^4 of SCARAMUZZA's [a0, c, e, cx, cy, a2, a3, a4, d]"""
+    return k[0] + rho * rho * (k[5] + rho * (k[6] + rho * k[7]))
+
+
+def scaramuzza_rho_max(k) -> float:
+    """First stationary point of F(rho) / rho: the smallest positive root of 3 a4 rho^4 + 2 a3 rho^3 + a2 rho^2 - a0 (np.roots, polished by
+    Newton's method), inf when there is none."""
+    a0, a2, a3, a4 = (float(k[i]) for i in (0, 5, 6, 7))
+    roots = np.roots([3.0 * a4, 2.0 * a3, a2, 0.0, -a0])
+    pos = roots.real[(np.abs(roots.imag) <= 1e-8 * np.abs(roots)) & (roots.real > 0.0)]
+    if pos.size == 0:
+        return np.inf
+    x = float(pos.min())
+    for _ in range(4):
+        dq = x * (2.0 * a2 + x * (6.0 * a3 + 12.0 * a4 * x))
+        if dq != 0.0:
+            x -= (x * x * (a2 + x * (2.0 * a3 + 3.0 * a4 * x)) - a0) / dq
+    return x
+
+
+def scaramuzza_scale(k, r, z):
+    """(s, valid): the projection's scale s (sensor point = s (x, y)), the smallest positive root of a0 - z s + a2 (r s)^2 + a3 (r s)^3 +
+    a4 (r s)^4 for points at distance r from the optical axis and depth z, by bisection and Newton's method over whole arrays.  A point is
+    valid iff z / r > F(rho_max) / rho_max (z > 0 on the axis); with rho_max = inf that bound is 0 for a constant F and -inf otherwise."""
+    k = np.asarray(k, dtype=np.float64)
+    r, z = np.broadcast_arrays(np.asarray(r, dtype=np.float64), np.asarray(z, dtype=np.float64))
+    a0, a2, a3, a4 = k[0], k[5], k[6], k[7]
+    rmax = scaramuzza_rho_max(k)
+    if np.isfinite(rmax):
+        valid = z * rmax > r * scaramuzza_F(k, rmax)
+    elif a2 == 0.0 and a3 == 0.0 and a4 == 0.0:
+        valid = z > 0.0
+    else:
+        valid = (z > 0.0) | (r > 0.0)
+    valid = valid & (a0 > 0.0)
+    s = np.zeros(r.shape)
+    if not valid.any():
+        return s, valid
+    rv, zv = r[valid], z[valid]
+
+    def h(x, i):    # -G(x) and -G_s(x) of the points i, increasing along the branch
+        rho = rv[i] * x
+        return zv[i] * x - scaramuzza_F(k, rho), zv[i] - rv[i] * rho * (2.0 * a2 + rho * (3.0 * a3 + 4.0 * a4 * rho))
+
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        cap = np.where(rv > 0.0, rmax / rv, np.inf)
+        lo, hi = np.zeros(rv.shape), np.minimum(a0 / np.hypot(rv, zv), cap)
+        i = np.arange(rv.size)
+        for _ in range(1100):              # grow the bracket until -G(hi) >= 0 or hi reaches rho_max / r
+            i = i[(h(hi[i], i)[0] < 0.0) & (hi[i] < cap[i])]
+            if i.size == 0:
+                break
+            lo[i] = hi[i]
+            hi[i] = np.minimum(2.0 * hi[i], cap[i])
+        x = 0.5 * (lo + hi)
+        i = np.arange(rv.size)
+        for _ in range(200):               # Newton's method, bisection where a step leaves the bracket, until the step is an ulp or two
+            xi, li, hi_ = x[i], lo[i], hi[i]
+            f, df = h(xi, i)
+            li = np.where(f < 0.0, xi, li)
+            hi_ = np.where(f > 0.0, xi, hi_)
+            xn = xi - f / df
+            xn = np.where((xn > li) & (xn < hi_), xn, 0.5 * (li + hi_))
+            xn = np.where(f == 0.0, xi, xn)
+            x[i], lo[i], hi[i] = xn, li, hi_
+            i = i[np.abs(xn - xi) > 2.5e-16 * np.abs(xn)]
+            if i.size == 0:
+                break
+    s[valid] = x
+    return s, valid
 
 
 def project(model: int, intr, pts):
@@ -111,4 +186,9 @@ def project(model: int, intr, pts):
         dx = mx * radial + 2.0 * t1 * mx * my + t2 * (r2 + 2.0 * mx * mx)
         dy = my * radial + 2.0 * t2 * mx * my + t1 * (r2 + 2.0 * my * my)
         return _affine_skew(k, dx, dy), valid
+    if model == SCARAMUZZA:
+        # OCamCalib's world2cam with the exact root: the sensor point s (x, y), then the stretch [[1, e], [d, c]] and the centre
+        s, valid = scaramuzza_scale(k, np.hypot(x, y), z)
+        up, vp = s * x, s * y
+        return np.stack([up + k[2] * vp + k[3], k[8] * up + k[1] * vp + k[4]], axis=-1), valid
     raise ValueError(f"unknown camera model {model}")

@@ -32,6 +32,7 @@ int model_from_string(const std::string& s) {   // theia::StringToCameraIntrinsi
   if (s == "FISHEYE") return ICC_CAM_FISHEYE;
   if (s == "FOV") return ICC_CAM_FOV;
   if (s == "OMNI_RADIAL_TANGENTIAL") return ICC_CAM_OMNI_RADIAL_TANGENTIAL;   // extension: Kalibr's omni-radtan
+  if (s == "SCARAMUZZA") return ICC_CAM_SCARAMUZZA;                           // extension: Scaramuzza's omnidirectional model (OCamCalib)
   return -1;
 }
 }  // namespace
@@ -103,6 +104,8 @@ int main(int argc, char** argv) {
         case ICC_CAM_FOV: in["radial_distortion_1"] = Value(intr[4]); break;   // extension: the layout this repository's readers use for FOV
         case ICC_CAM_OMNI_RADIAL_TANGENTIAL: in["xi"] = Value(intr[5]); in["radial_distortion_1"] = Value(intr[6]); in["radial_distortion_2"] = Value(intr[7]);
                                              in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
+        case ICC_CAM_SCARAMUZZA: in["stretch_e"] = Value(intr[2]); in["stretch_d"] = Value(intr[8]);   // `skew` stays 0: the stretch is e, d
+                                 in["polynomial_a2"] = Value(intr[5]); in["polynomial_a3"] = Value(intr[6]); in["polynomial_a4"] = Value(intr[7]); break;
         default: break;
       }
       j["intrinsics"] = in;
@@ -139,6 +142,8 @@ int main(int argc, char** argv) {
     else if (model == ICC_CAM_EXTENDED_UNIFIED) std::cout << "EXTENDED_UNIFIED model: " << intr[5] << " BETA: " << intr[6] << "\n";
     else if (model == ICC_CAM_OMNI_RADIAL_TANGENTIAL) std::cout << "OMNI_RADIAL_TANGENTIAL model: XI: " << intr[5] << " Radial distortion 1: " << intr[6] << " Radial distortion 2: " << intr[7]
                                                                 << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
+    else if (model == ICC_CAM_SCARAMUZZA) std::cout << "SCARAMUZZA model: A2: " << intr[5] << " A3: " << intr[6] << " A4: " << intr[7] << " Stretch c: " << intr[1]
+                                                    << " d: " << intr[8] << " e: " << intr[2] << "\n";
     else if (model == ICC_CAM_FISHEYE) std::cout << "FISHEYE model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7] << " Radial distortion 4: " << intr[8] << "\n";
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   return 0;

@@ -72,7 +72,19 @@ ICC_HD double tangent_scale(int model, const double* k, bool dispatch_fov) {
 // damped Gauss-Newton on the sphere: the step lives in the tangent plane of the current b, its 2x2 Jacobian is the 2x3 projection Jacobian
 // times (e1, e2), and the new ray is b + dx e1 + dy e2 renormalised.  Theia's Fisheye projects p and -p to the same pixel, so its ray is held
 // in z > 0; the three unified models reach their whole forward domain, z <= 0 included (OmniRadtan: past 90 degrees for any xi > 0).
+// Scaramuzza's model back-projects in closed form: the sensor point (u', v') = A^-1 (u - cx, v - cy) sees (u', v', F(rho)), for every
+// rho = |(u', v')| below rho_max (beyond it the pixel is not the image of any point) and det A = c - d e != 0.
 ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, V3& b) {
+  if (model == CAM_SCARAMUZZA) {
+    const double det = k[1] - k[8] * k[2], du = px - k[3], dv = py - k[4];
+    b = v3(0.0, 0.0, 1.0);
+    if (!(det != 0.0) || !(k[0] > 0.0)) return false;
+    const double up = (k[1] * du - k[2] * dv) / det, vp = (dv - k[8] * du) / det, rho = sqrt(up * up + vp * vp);
+    if (!(rho < scaramuzza_rho_max(k))) return false;
+    const V3 ray = v3(up, vp, scaramuzza_F(k, rho));
+    b = (1.0 / sqrt(dot(ray, ray))) * ray;
+    return true;
+  }
   if (model != CAM_FISHEYE && model != CAM_DOUBLE_SPHERE && model != CAM_EXTENDED_UNIFIED && model != CAM_OMNI_RADTAN) {
     double x = 0.0, y = 0.0;
     const bool good = unproject_gn(model, k, px, py, x, y);

@@ -362,6 +362,7 @@ IntrinsicSubsets intrinsic_subsets(int model) {
     case CAM_DOUBLE_SPHERE: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
     case CAM_EXTENDED_UNIFIED: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
     case CAM_OMNI_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};   // radial = xi, k1, k2
+    case CAM_SCARAMUZZA: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({2, 8})};    // radial = a2, a3, a4; the stretch e, d as tangential
     default: return {0u, 0u, 0u, 0u, 0u};
   }
 }
@@ -614,6 +615,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   if (model == CAM_DOUBLE_SPHERE) { k0[5] = -0.25; k0[6] = 0.5; }
   if (model == CAM_EXTENDED_UNIFIED) { k0[5] = 0.5; k0[6] = 1.0; }
   if (model == CAM_OMNI_RADTAN) { k0[5] = 1.0; k0[0] = 2.0 * f0; }   // xi = 1, f = (1 + xi) f0: magnification f / (1 + xi) = f0 at the image centre
+  if (model == CAM_SCARAMUZZA) k0[5] = -0.25 / f0;                    // the stereographic member a2 = -1 / (4 a0): magnification a0 = f0 at the image centre
   for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), 10 * sizeof(double), cudaMemcpyHostToDevice));
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :132-135
   const IntrinsicSubsets sub = intrinsic_subsets(model);
@@ -624,7 +626,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
   // 3. full optimisation (:181-198)
-  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN ? sub.tangential : 0u);
+  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN || model == CAM_SCARAMUZZA ? sub.tangential : 0u);
   rc = bundle_adjust(stage3_mask, true, 2);
   if (rc != ICC_OK) return rc;
   rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200

@@ -10,12 +10,13 @@
 namespace icc {
 
 enum CameraModel { CAM_PINHOLE = 0, CAM_PINHOLE_RADTAN = 1, CAM_FISHEYE = 2, CAM_FOV = 3, CAM_DIVISION_UNDISTORTION = 4, CAM_DOUBLE_SPHERE = 5, CAM_EXTENDED_UNIFIED = 6,
-                   CAM_OMNI_RADTAN = 7 /* extension: Kalibr's omni-radtan, no Theia counterpart */ };
+                   CAM_OMNI_RADTAN = 7 /* extension: Kalibr's omni-radtan, no Theia counterpart */,
+                   CAM_SCARAMUZZA = 8 /* extension: Scaramuzza's omnidirectional polynomial model (OCamCalib), no Theia counterpart */ };
 
 ICC_HD int camera_num_params(int model) {
   switch (model) { case CAM_PINHOLE: return 7; case CAM_PINHOLE_RADTAN: return 10; case CAM_FISHEYE: return 9; case CAM_FOV: return 5;
                    case CAM_DIVISION_UNDISTORTION: return 5; case CAM_DOUBLE_SPHERE: return 7; case CAM_EXTENDED_UNIFIED: return 7;
-                   case CAM_OMNI_RADTAN: return 10; default: return -1; }
+                   case CAM_OMNI_RADTAN: return 10; case CAM_SCARAMUZZA: return 9; default: return -1; }
 }
 
 // J is row-major 2x3: J[0..2] = d px / d(x,y,z), J[3..5] = d py / d(x,y,z).
@@ -41,6 +42,82 @@ ICC_HD void affine_skew_k(const double* k, double dx, double dy, int nd, const i
 }
 
 ICC_HD double unified_w(double alpha) { return alpha > 0.5 ? (1.0 - alpha) / alpha : alpha / (1.0 - alpha); }
+
+// ---- Scaramuzza's omnidirectional polynomial model, [a0, c, e, cx, cy, a2, a3, a4, d] ------------------------------------------------
+// A pixel's sensor point (u', v') = A^-1 (u - cx, v - cy), A = [[1, e], [d, c]], sees the ray (u', v', F(rho)), rho = |(u', v')|,
+// F(rho) = a0 + a2 rho^2 + a3 rho^3 + a4 rho^4.  A point p = (x, y, z) at r = |(x, y)| projects to (u', v') = s (x, y), where s is the
+// root of G(s) = F(r s) - z s on the branch where F(rho) / rho still falls: rho < rho_max, the first stationary point of F(rho) / rho.
+ICC_HD double scaramuzza_F(const double* k, double rho) { return k[0] + rho * rho * (k[5] + rho * (k[6] + rho * k[7])); }
+
+// Root of fn on [lo, hi], where fn(x, f, df) is increasing with f(lo) < 0 <= f(hi): Newton's method safeguarded by bisection, run until
+// a step moves the iterate by at most an ulp or two.
+template <class Fn> ICC_HD double bracketed_newton(const Fn& fn, double lo, double hi) {
+  double x = 0.5 * (lo + hi);
+  for (int it = 0; it < 100; ++it) {
+    double f, df;
+    fn(x, f, df);
+    if (f < 0.0) lo = x; else if (f > 0.0) hi = x; else return x;
+    double xn = x - f / df;
+    if (!(xn > lo && xn < hi)) xn = 0.5 * (lo + hi);
+    if (!(fabs(xn - x) > 2.5e-16 * fabs(xn))) return xn;
+    x = xn;
+  }
+  return x;
+}
+
+// rho_max: the smallest positive root of q(rho) = rho F'(rho) - F(rho) = 3 a4 rho^4 + 2 a3 rho^3 + a2 rho^2 - a0 (q / rho^2 is the slope of
+// F(rho) / rho), or +inf when q has none.  q(0) = -a0 < 0; q is monotone between its stationary points, the positive roots of
+// q'(rho) / rho = 12 a4 rho^2 + 6 a3 rho + 2 a2, so the first piece on which q reaches 0 brackets the root.  A function of the intrinsics only.
+ICC_HD double scaramuzza_rho_max(const double* k) {
+  const double a0 = k[0], a2 = k[5], a3 = k[6], a4 = k[7];
+  const auto fq = [&](double x, double& f, double& df) { f = x * x * (a2 + x * (2.0 * a3 + 3.0 * a4 * x)) - a0; df = x * (2.0 * a2 + x * (6.0 * a3 + 12.0 * a4 * x)); };
+  double c0 = -1.0, c1 = -1.0;   // stationary points, ascending; <= 0 = none
+  if (a4 != 0.0) {
+    const double disc = 36.0 * a3 * a3 - 96.0 * a4 * a2;
+    if (disc >= 0.0) {
+      const double t = -0.5 * (6.0 * a3 + copysign(sqrt(disc), a3));
+      if (t != 0.0) { const double x0 = t / (12.0 * a4), x1 = 2.0 * a2 / t; c0 = fmin(x0, x1); c1 = fmax(x0, x1); }
+    }
+  } else if (a3 != 0.0) {
+    c1 = -a2 / (3.0 * a3);
+  }
+  double lo = 0.0, f, df;
+  if (c0 > 0.0) { fq(c0, f, df); if (f >= 0.0) return bracketed_newton(fq, lo, c0); lo = c0; }
+  if (c1 > 0.0) { fq(c1, f, df); if (f >= 0.0) return bracketed_newton(fq, lo, c1); lo = c1; }
+  const double lead = a4 != 0.0 ? a4 : (a3 != 0.0 ? a3 : a2);   // q's leading coefficient has this sign
+  if (!(lead > 0.0)) return INFINITY;
+  double hi = fmax(2.0 * lo, 1.0);
+  for (int i = 0; i < 2100; ++i) { fq(hi, f, df); if (f >= 0.0) break; lo = hi; hi *= 2.0; }
+  return bracketed_newton(fq, lo, hi);
+}
+
+// The projection's scale s > 0 (G(s) = 0) of a point at distance r from the optical axis and depth z, and G_s = dG/ds < 0 there.
+// The point is in the domain iff z / r > F(rho_max) / rho_max (z > 0 on the axis), the limit of F(rho) / rho standing in for rho_max = inf:
+// 0 for a constant F, -inf otherwise.  There G falls through 0 exactly once on (0, rho_max / r): a bracket grown from a0 / |p| holds the root.
+ICC_HD bool scaramuzza_scale(const double* k, double r, double z, double& s, double& gs) {
+  const double a0 = k[0], a2 = k[5], a3 = k[6], a4 = k[7];
+  const double rmax = scaramuzza_rho_max(k);
+  const bool in = rmax < INFINITY ? z * rmax > r * scaramuzza_F(k, rmax) : (z > 0.0 || (r > 0.0 && !(a2 == 0.0 && a3 == 0.0 && a4 == 0.0)));
+  const double pn = sqrt(r * r + z * z);
+  if (!in || !(a0 > 0.0) || !(pn > 0.0)) return false;
+  const auto fg = [&](double x, double& f, double& df) {   // -G and -G_s, increasing in s on the branch
+    const double rho = r * x;
+    f = z * x - (a0 + rho * rho * (a2 + rho * (a3 + rho * a4)));
+    df = z - r * rho * (2.0 * a2 + rho * (3.0 * a3 + 4.0 * a4 * rho));
+  };
+  double lo = 0.0, hi = a0 / pn, f, df;
+  bool bracketed = false;
+  for (int i = 0; i < 128 && !bracketed; ++i) {
+    if (r * hi >= rmax) { hi = rmax / r; bracketed = true; break; }
+    fg(hi, f, df);
+    if (f >= 0.0) bracketed = true; else { lo = hi; hi *= 4.0; }
+  }
+  if (!bracketed) return false;
+  s = bracketed_newton(fg, lo, hi);
+  fg(s, f, df);
+  gs = -df;
+  return true;
+}
 
 template <int MODEL, bool WITH_K = false>
 ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = nullptr) {
@@ -207,9 +284,38 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
       const double ddy[5] = {-am1 * d * in, my * r2, my * r2 * r2, r2 + 2.0 * my * my, 2.0 * mx * my};
       affine_skew_k(k, dx, dy, 5, idx, ddx, ddy, *pk);
     }
+  } else if (MODEL == CAM_SCARAMUZZA) {   // [a0, c, e, cx, cy, a2, a3, a4, d]: (u', v') = s (x, y), G(s) = 0; u = u' + e v' + cx, v = d u' + c v' + cy
+    const double r = sqrt(p.x * p.x + p.y * p.y);
+    double s, gs;
+    if (!scaramuzza_scale(k, r, p.z, s, gs)) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
+    const double c = k[1], e = k[2], d = k[8];
+    const double up = s * p.x, vp = s * p.y;
+    o.u = up + e * vp + k[3];
+    o.v = d * up + c * vp + k[4];
+    // implicit function theorem on G(s; p, k) = 0: ds = -dG / G_s, with dG/dx = x g, dG/dy = y g, dG/dz = -s, g = s^2 (2 a2 + 3 a3 rho + 4 a4 rho^2)
+    const double rho = r * s, ig = -1.0 / gs;
+    const double sg = s * s * (2.0 * k[5] + rho * (3.0 * k[6] + 4.0 * k[7] * rho)) * ig;
+    const double sx = p.x * sg, sy = p.y * sg, sz = -s * ig;
+    const double Du[3] = {s + p.x * sx, p.x * sy, p.x * sz}, Dv[3] = {p.y * sx, s + p.y * sy, p.y * sz};   // d(u', v')/dp
+    for (int j = 0; j < 3; ++j) { o.J[j] = Du[j] + e * Dv[j]; o.J[3 + j] = d * Du[j] + c * Dv[j]; }
+    if (WITH_K) {   // ds/da0 = -1 / G_s, ds/da_i = -rho^i / G_s
+      const double wu = p.x + e * p.y, wv = d * p.x + c * p.y, rho2 = rho * rho;   // d(u, v)/ds
+      pk->Jk[0] = wu * ig; pk->Jk[10] = wv * ig;
+      pk->Jk[11] = vp;                                  // c
+      pk->Jk[2] = vp;                                   // e
+      pk->Jk[3] = 1.0; pk->Jk[14] = 1.0;                // principal point
+      pk->Jk[5] = wu * rho2 * ig; pk->Jk[15] = wv * rho2 * ig;
+      pk->Jk[6] = wu * rho2 * rho * ig; pk->Jk[16] = wv * rho2 * rho * ig;
+      pk->Jk[7] = wu * rho2 * rho2 * ig; pk->Jk[17] = wv * rho2 * rho2 * ig;
+      pk->Jk[18] = up;                                  // d
+    }
   }
   return o;
 }
+
+// CAM_SCARAMUZZA out of line for the runtime dispatchers: its root solves stay out of the kernels that inline project() for every model
+__host__ __device__ inline __noinline__ Proj project_scaramuzza(const double* k, V3 p) { return project_model<CAM_SCARAMUZZA>(k, p, true); }
+__host__ __device__ inline __noinline__ Proj project_scaramuzza_with_k(const double* k, V3 p, ProjK* pk) { return project_model<CAM_SCARAMUZZA, true>(k, p, true, pk); }
 
 // Same dispatch, additionally returning d(u,v)/d(intrinsics) (CAM_INTRINSICS extension).
 ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, ProjK* pk) {
@@ -222,11 +328,12 @@ ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, 
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN, true>(k, p, dispatch_fov, pk);
     case CAM_FOV: return project_model<CAM_FOV, true>(k, p, dispatch_fov, pk);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN, true>(k, p, dispatch_fov, pk);
+    case CAM_SCARAMUZZA: return project_scaramuzza_with_k(k, p, pk);
     default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 20; ++j) pk->Jk[j] = 0; return o; }
   }
 }
 
-// Runtime dispatch in the reference's order (residuals.h:366-389), then the extension CAM_OMNI_RADTAN.
+// Runtime dispatch in the reference's order (residuals.h:366-389), then the extensions CAM_OMNI_RADTAN and CAM_SCARAMUZZA.
 ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
   switch (model) {
     case CAM_DIVISION_UNDISTORTION: return project_model<CAM_DIVISION_UNDISTORTION>(k, p, dispatch_fov);
@@ -237,6 +344,7 @@ ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN>(k, p, dispatch_fov);
     case CAM_FOV: return project_model<CAM_FOV>(k, p, dispatch_fov);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN>(k, p, dispatch_fov);
+    case CAM_SCARAMUZZA: return project_scaramuzza(k, p);
     default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
   }
 }

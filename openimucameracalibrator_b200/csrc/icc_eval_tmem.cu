@@ -143,6 +143,7 @@ int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* resid
       case CAM_DOUBLE_SPHERE: e = launch_model<CAM_DOUBLE_SPHERE>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       case CAM_EXTENDED_UNIFIED: e = launch_model<CAM_EXTENDED_UNIFIED>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       case CAM_OMNI_RADTAN: e = launch_model<CAM_OMNI_RADTAN>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
+      case CAM_SCARAMUZZA: e = launch_model<CAM_SCARAMUZZA>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       default: return 1;
     }
     if (e) return 1;
