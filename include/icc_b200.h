@@ -47,7 +47,14 @@ typedef enum {
  *   SCARAMUZZA                [a0, c, e, cx, cy, a2, a3, a4, d]   (extension, no Theia counterpart: Scaramuzza's omnidirectional model as
  *                             OCamCalib calibrates it; the pixel's sensor point (u', v') = A^-1 (u - cx, v - cy), A = [[1, e], [d, c]], sees the ray
  *                             (u', v', a0 + a2 rho^2 + a3 rho^3 + a4 rho^4), rho = |(u', v')|; a point projects through the root of that quartic,
- *                             valid iff z / |(x, y)| > F(rho_max) / rho_max, rho_max = the first stationary point of F(rho) / rho) */
+ *                             valid iff z / |(x, y)| > F(rho_max) / rho_max, rho_max = the first stationary point of F(rho) / rho)
+ *   PINHOLE_RATIONAL          [f, ar, skew, cx, cy, k1, k2, k3, t1, t2, k4, k5, k6]   (extension, no Theia counterpart: OpenCV's rational
+ *                             polynomial model, CALIB_RATIONAL_MODEL, with t1, t2 = OpenCV's p1, p2; (xn, yn) = (x, y) / z, s = xn^2 + yn^2,
+ *                             R = (1 + k1 s + k2 s^2 + k3 s^3) / (1 + k4 s + k5 s^2 + k6 s^3), dx = xn R + 2 t1 xn yn + t2 (s + 2 xn^2),
+ *                             dy = yn R + t1 (s + 2 yn^2) + 2 t2 xn yn, then the skewed affine; valid iff z > 0 and s < s_max, the first
+ *                             s > 0 at which r R(r^2) stops increasing (a root of d(r R)/dr or a pole of R), +inf when there is none)
+ * ICC_MAX_INTRINSICS is the longest of these vectors. */
+#define ICC_MAX_INTRINSICS 13
 typedef enum {
   ICC_CAM_PINHOLE = 0,
   ICC_CAM_PINHOLE_RADIAL_TANGENTIAL = 1,
@@ -57,7 +64,8 @@ typedef enum {
   ICC_CAM_DOUBLE_SPHERE = 5,
   ICC_CAM_EXTENDED_UNIFIED = 6,
   ICC_CAM_OMNI_RADIAL_TANGENTIAL = 7,
-  ICC_CAM_SCARAMUZZA = 8
+  ICC_CAM_SCARAMUZZA = 8,
+  ICC_CAM_PINHOLE_RATIONAL = 9
 } icc_camera_model;
 
 /* OpenICC::core::SplineOptimFlags (core/spline_trajectory_estimator.h:17-27), same numeric values. */
@@ -330,7 +338,8 @@ icc_status icc_pixels_to_normalized(icc_handle* h, int n, const double* uv, doub
 /* Unit bearing vectors of `n` pixels with the handle's camera: xyz_out[3n], ok[n] (nullable; 0 where the ray reprojects more than 1e-6 px
  * away).  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion give icc_pixels_to_normalized's ray normalised; Fisheye's ray
  * stays in z > 0 (the model maps p and -p to one pixel); DoubleSphere, ExtendedUnified and OmniRadialTangential reach their whole domain,
- * z <= 0 included; Scaramuzza back-projects in closed form (ok = 0 beyond rho_max). */
+ * z <= 0 included; Scaramuzza back-projects in closed form (ok = 0 beyond rho_max); PinholeRational gives icc_pixels_to_normalized's
+ * ray normalised, ok = 0 where it would land outside the model's domain. */
 icc_status icc_pixels_to_bearings(icc_handle* h, int n, const double* uv, double* xyz_out, int32_t* ok);
 
 /* Residual of the per-view pose refinement, the inlier test and the board-point refinement of icc_estimate_board_poses and
@@ -429,7 +438,8 @@ icc_status icc_spline_error_weighting(icc_handle* h, int n, const double* times_
  * non-pinhole models focal length, a division-model distortion and the poses are then refined jointly (the quantities
  * utils::initialize_radial_undistortion_camera hands the reference, :283-306) before the target model takes over.
  * Needs icc_set_board_points (planar board for the internal initialiser).
- * Outputs (caller-owned): intrinsics[10] in Theia's order for `model`; per view q_wc / p_wc (as icc_set_frames consumes them),
+ * Outputs (caller-owned): intrinsics in Theia's order for `model`, max(10, its parameter count) entries (10 for every model but
+ * PINHOLE_RATIONAL, 13 for it; unused entries zero); per view q_wc / p_wc (as icc_set_frames consumes them),
  * the mean reprojection error [px] (GetReprojErrorOfView) and used[v] = 1 for the views that survive to the end.
  * summary->success = 0 (status still ICC_OK) when fewer than min_num_views views remain, like RunCalibration returning false. */
 typedef struct icc_camcal_options {
@@ -467,7 +477,7 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int image_width, int i
                                 int n_views, const int32_t* corner_offsets /* n_views+1 */, const int32_t* point_ids, const double* uv,
                                 const double* q_wc_init_xyzw /* nullable */, const double* p_wc_init /* nullable */, const int32_t* init_valid /* nullable */,
                                 double focal_length_init, double distortion_init, const icc_camcal_options* options /* nullable */,
-                                double* intrinsics /* 10 */, double* q_wc_xyzw, double* p_wc, double* view_reproj_error_px, int32_t* view_used,
+                                double* intrinsics /* max(10, n_params(model)) */, double* q_wc_xyzw, double* p_wc, double* view_reproj_error_px, int32_t* view_used,
                                 icc_camcal_summary* summary /* nullable */);
 /* Shutter of icc_calibrate_camera.  line_delay_s = 0 (the default) is the global shutter and leaves the calibration exactly as above.
  * line_delay_s > 0 is a rolling shutter with the model of icc_set_pose_rolling_shutter: corner c of view i is seen tau = uv_c.y * line_delay_s

@@ -10,6 +10,8 @@ import ctypes as C
 
 import numpy as np
 
+from .camera_models import MAX_INTRINSICS
+
 c_double_p = C.POINTER(C.c_double)
 c_int32_p = C.POINTER(C.c_int32)
 c_int64_p = C.POINTER(C.c_int64)
@@ -320,7 +322,7 @@ class CApi:
             setattr(o, k, v)
         qi = None if q_wc_init is None else _f64(q_wc_init); pi = None if p_wc_init is None else _f64(p_wc_init)
         vi = None if init_valid is None else np.ascontiguousarray(init_valid, dtype=np.int32)
-        intr = np.zeros(10); q = np.zeros((nv, 4)); p = np.zeros((nv, 3)); e = np.zeros(nv); used = np.zeros(nv, dtype=np.int32); s = CamCalSummary()
+        intr = np.zeros(MAX_INTRINSICS); q = np.zeros((nv, 4)); p = np.zeros((nv, 3)); e = np.zeros(nv); used = np.zeros(nv, dtype=np.int32); s = CamCalSummary()
         self._call("calibrate_camera", [C.c_int, C.c_int, C.c_int, C.c_int, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_int32_p, C.c_double, C.c_double,
                                         C.POINTER(CamCalOptions), c_double_p, c_double_p, c_double_p, c_double_p, c_int32_p, C.POINTER(CamCalSummary)],
                    int(model), int(image_width), int(image_height), nv, off.ctypes.data_as(c_int32_p), ids.ctypes.data_as(c_int32_p), _dp(uv),

@@ -247,7 +247,9 @@ class CameraCalibrator:
                      cm.FISHEYE: {f"radial_distortion_{i + 1}": 5 + i for i in range(4)}, cm.FOV: {"radial_distortion_1": 4},
                      cm.PINHOLE_RADIAL_TANGENTIAL: {"radial_distortion_1": 5, "radial_distortion_2": 6, "radial_distortion_3": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9},
                      cm.OMNI_RADIAL_TANGENTIAL: {"xi": 5, "radial_distortion_1": 6, "radial_distortion_2": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9},
-                     cm.SCARAMUZZA: {"stretch_d": 8, "stretch_e": 2, "polynomial_a2": 5, "polynomial_a3": 6, "polynomial_a4": 7}}
+                     cm.SCARAMUZZA: {"stretch_d": 8, "stretch_e": 2, "polynomial_a2": 5, "polynomial_a3": 6, "polynomial_a4": 7},
+                     cm.PINHOLE_RATIONAL: {"radial_distortion_1": 5, "radial_distortion_2": 6, "radial_distortion_3": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9,
+                                           "radial_distortion_4": 10, "radial_distortion_5": 11, "radial_distortion_6": 12}}
             for name, idx in extra.get(self.model, {}).items():
                 intr[name] = k[idx]
             doc = {"stabelized": False, "fps": scene_json["camera_fps"], "nr_calib_images": s["n_views_used"], "final_reproj_error": s["final_reproj_error"],
@@ -269,6 +271,9 @@ class CameraCalibrator:
             print(f"EXTENDED_UNIFIED model: {k[5]} BETA: {k[6]}")
         elif self.model == cm.OMNI_RADIAL_TANGENTIAL:
             print(f"OMNI_RADIAL_TANGENTIAL model: XI: {k[5]} Radial distortion 1: {k[6]} Radial distortion 2: {k[7]} Tangential distortion 1: {k[8]} Tangential distortion 2: {k[9]}")
+        elif self.model == cm.PINHOLE_RATIONAL:
+            print("PINHOLE_RATIONAL model: " + " ".join(f"Radial distortion {i + 1}: {k[(5, 6, 7, 10, 11, 12)[i]]}" for i in range(6))
+                  + f" Tangential distortion 1: {k[8]} Tangential distortion 2: {k[9]}")
         elif self.model == cm.SCARAMUZZA:
             print(f"SCARAMUZZA model: A2: {k[5]} A3: {k[6]} A4: {k[7]} Stretch c: {k[1]} d: {k[8]} e: {k[2]}")
         elif self.model == cm.FISHEYE:

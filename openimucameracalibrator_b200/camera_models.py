@@ -12,6 +12,7 @@ import numpy as np
 PINHOLE, PINHOLE_RADIAL_TANGENTIAL, FISHEYE, FOV, DIVISION_UNDISTORTION, DOUBLE_SPHERE, EXTENDED_UNIFIED = range(7)
 OMNI_RADIAL_TANGENTIAL = 7   # extension without a Theia counterpart: Kalibr's omni-radtan
 SCARAMUZZA = 8               # extension without a Theia counterpart: Scaramuzza's omnidirectional polynomial model (OCamCalib)
+PINHOLE_RATIONAL = 9         # extension without a Theia counterpart: OpenCV's rational polynomial model (k1..k6, p1, p2)
 
 MODEL_NAMES = {
     PINHOLE: "PINHOLE",
@@ -23,10 +24,12 @@ MODEL_NAMES = {
     EXTENDED_UNIFIED: "EXTENDED_UNIFIED",
     OMNI_RADIAL_TANGENTIAL: "OMNI_RADIAL_TANGENTIAL",
     SCARAMUZZA: "SCARAMUZZA",
+    PINHOLE_RATIONAL: "PINHOLE_RATIONAL",
 }
 MODEL_IDS = {v: k for k, v in MODEL_NAMES.items()}
 NUM_PARAMS = {PINHOLE: 7, PINHOLE_RADIAL_TANGENTIAL: 10, FISHEYE: 9, FOV: 5, DIVISION_UNDISTORTION: 5,
-              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10, SCARAMUZZA: 9}
+              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10, SCARAMUZZA: 9, PINHOLE_RATIONAL: 13}
+MAX_INTRINSICS = 13   # ICC_MAX_INTRINSICS: the longest intrinsic vector
 
 
 def _affine_skew(k, dx, dy):
@@ -110,6 +113,74 @@ def scaramuzza_scale(k, r, z):
     return s, valid
 
 
+def rational_s_max(k) -> float:
+    """PINHOLE_RATIONAL's [f, ar, skew, cx, cy, k1, k2, k3, t1, t2, k4, k5, k6]: the first s = xn^2 + yn^2 > 0 at which the radial map
+    r R(r^2), R = N / M, stops increasing: the smallest positive real root of M or of h = N M + 2 s (N' M - N M') (np.roots), inf when
+    there is none."""
+    k = np.asarray(k, dtype=np.float64)
+    n = np.array([1.0, k[5], k[6], k[7]])                # ascending powers of s
+    m = np.array([1.0, k[10], k[11], k[12]])
+    nm = np.convolve(n, m)
+    dn, dm = n[1:] * np.arange(1, 4), m[1:] * np.arange(1, 4)
+    h = nm.copy()
+    h[1:] += 2.0 * (np.convolve(dn, m) - np.convolve(n, dm))   # s (N' M - N M')
+    best = np.inf
+    for c in (m, h):
+        c = np.trim_zeros(c, "b")
+        if c.size < 2:
+            continue
+        roots = np.roots(c[::-1])
+        pos = roots.real[(np.abs(roots.imag) <= 1e-9 * np.maximum(np.abs(roots), 1.0)) & (roots.real > 0.0)]
+        if pos.size:
+            best = min(best, float(pos.min()))
+    return best
+
+
+def rational_distort(k, xn, yn):
+    """PINHOLE_RATIONAL's distorted normalised point (dx, dy) of (xn, yn)"""
+    s = xn * xn + yn * yn
+    R = (1.0 + s * (k[5] + s * (k[6] + s * k[7]))) / (1.0 + s * (k[10] + s * (k[11] + s * k[12])))
+    return (xn * R + 2.0 * k[8] * xn * yn + k[9] * (s + 2.0 * xn * xn),
+            yn * R + k[8] * (s + 2.0 * yn * yn) + 2.0 * k[9] * xn * yn)
+
+
+def rational_unproject(k, uv):
+    """PINHOLE_RATIONAL: (xn, yn) = (x / z, y / z) of pixels uv (..., 2) and ok (...,): the skewed affine inverted, then damped Newton's
+    method on the distortion over whole arrays (Jacobian by central differences), started at the distorted point pulled inside the domain;
+    ok iff the point converged to 1e-12 of the distorted point and lies inside the domain s < s_max."""
+    k = np.asarray(k, dtype=np.float64)
+    uv = np.asarray(uv, dtype=np.float64)
+    dy = (uv[..., 1] - k[4]) / (k[0] * k[1])
+    dx = (uv[..., 0] - k[3] - k[2] * dy) / k[0]
+    smax = rational_s_max(k)
+    shrink = np.where(dx * dx + dy * dy < 0.5 * smax, 1.0, np.sqrt(0.5 * smax / np.maximum(dx * dx + dy * dy, 1e-300)))
+    x, y = dx * shrink, dy * shrink                      # a start inside the domain
+
+    def err(x, y):
+        fx, fy = rational_distort(k, x, y)
+        return np.where(x * x + y * y < smax, np.hypot(fx - dx, fy - dy), np.inf), fx - dx, fy - dy
+
+    with np.errstate(all="ignore"):
+        for _ in range(100):                             # Newton's method, each step halved until it stays inside and improves
+            e, ex, ey = err(x, y)
+            h = 1e-7 * np.maximum(1.0, np.hypot(x, y))
+            ax = (np.array(rational_distort(k, x + h, y)) - np.array(rational_distort(k, x - h, y))) / (2.0 * h)
+            ay = (np.array(rational_distort(k, x, y + h)) - np.array(rational_distort(k, x, y - h))) / (2.0 * h)
+            det = ax[0] * ay[1] - ay[0] * ax[1]
+            sx, sy = -(ay[1] * ex - ay[0] * ey) / det, -(-ax[1] * ex + ax[0] * ey) / det
+            t = np.ones_like(x)
+            for _ in range(40):
+                bad = ~(err(x + t * sx, y + t * sy)[0] <= e)
+                if not bad.any():
+                    break
+                t = np.where(bad, 0.5 * t, t)
+            moved = err(x + t * sx, y + t * sy)[0] <= e
+            x, y = np.where(moved, x + t * sx, x), np.where(moved, y + t * sy, y)
+        fx, fy = rational_distort(k, x, y)
+        ok = (np.hypot(fx - dx, fy - dy) <= 1e-12 * np.maximum(1.0, np.hypot(dx, dy))) & (x * x + y * y < smax)
+    return np.stack([x, y], axis=-1), ok
+
+
 def project(model: int, intr, pts):
     """pts: (..., 3) camera-frame points -> (uv (..., 2), valid (...,))."""
     k = np.asarray(intr, dtype=np.float64)
@@ -191,4 +262,12 @@ def project(model: int, intr, pts):
         s, valid = scaramuzza_scale(k, np.hypot(x, y), z)
         up, vp = s * x, s * y
         return np.stack([up + k[2] * vp + k[3], k[8] * up + k[1] * vp + k[4]], axis=-1), valid
+    if model == PINHOLE_RATIONAL:
+        # OpenCV's projectPoints with CALIB_RATIONAL_MODEL (t1, t2 = p1, p2), valid iff z > 0 and s < s_max (which implies M(s) > 0)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xn, yn = x / z, y / z
+            s = xn * xn + yn * yn
+            dx, dy = rational_distort(k, xn, yn)
+            valid = (z > 0.0) & (s < rational_s_max(k)) & (1.0 + s * (k[10] + s * (k[11] + s * k[12])) > 0.0)
+        return _affine_skew(k, dx, dy), valid
     raise ValueError(f"unknown camera model {model}")

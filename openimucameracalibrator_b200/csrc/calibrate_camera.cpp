@@ -33,6 +33,7 @@ int model_from_string(const std::string& s) {   // theia::StringToCameraIntrinsi
   if (s == "FOV") return ICC_CAM_FOV;
   if (s == "OMNI_RADIAL_TANGENTIAL") return ICC_CAM_OMNI_RADIAL_TANGENTIAL;   // extension: Kalibr's omni-radtan
   if (s == "SCARAMUZZA") return ICC_CAM_SCARAMUZZA;                           // extension: Scaramuzza's omnidirectional model (OCamCalib)
+  if (s == "PINHOLE_RATIONAL") return ICC_CAM_PINHOLE_RATIONAL;               // extension: OpenCV's rational polynomial model
   return -1;
 }
 }  // namespace
@@ -61,7 +62,7 @@ int main(int argc, char** argv) {
     icc_handle* h = nullptr;
     icc_status st = icc_create(&h, (int)F.num["device"]);
     if (st != ICC_OK) { std::cerr << "icc_create failed (" << st << "): " << icc_last_error(h) << std::endl; return 2; }
-    std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), err(nv), intr(10, 0.0); std::vector<int32_t> used(nv);
+    std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), err(nv), intr(ICC_MAX_INTRINSICS, 0.0); std::vector<int32_t> used(nv);
     icc_camcal_options opt{}; opt.grid_size = F.num["grid_size"]; opt.optimize_board_points = F.boolean["optimize_board_points"] ? 1 : 0;
     icc_camcal_summary S{};
     st = icc_set_board_points(h, np, board.data());
@@ -106,6 +107,8 @@ int main(int argc, char** argv) {
                                              in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
         case ICC_CAM_SCARAMUZZA: in["stretch_e"] = Value(intr[2]); in["stretch_d"] = Value(intr[8]);   // `skew` stays 0: the stretch is e, d
                                  in["polynomial_a2"] = Value(intr[5]); in["polynomial_a3"] = Value(intr[6]); in["polynomial_a4"] = Value(intr[7]); break;
+        case ICC_CAM_PINHOLE_RATIONAL: for (int i = 0; i < 3; ++i) { in["radial_distortion_" + std::to_string(i + 1)] = Value(intr[5 + i]); in["radial_distortion_" + std::to_string(i + 4)] = Value(intr[10 + i]); }
+                                       in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
         default: break;
       }
       j["intrinsics"] = in;
@@ -142,6 +145,9 @@ int main(int argc, char** argv) {
     else if (model == ICC_CAM_EXTENDED_UNIFIED) std::cout << "EXTENDED_UNIFIED model: " << intr[5] << " BETA: " << intr[6] << "\n";
     else if (model == ICC_CAM_OMNI_RADIAL_TANGENTIAL) std::cout << "OMNI_RADIAL_TANGENTIAL model: XI: " << intr[5] << " Radial distortion 1: " << intr[6] << " Radial distortion 2: " << intr[7]
                                                                 << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
+    else if (model == ICC_CAM_PINHOLE_RATIONAL) std::cout << "PINHOLE_RATIONAL model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7]
+                                                          << " Radial distortion 4: " << intr[10] << " Radial distortion 5: " << intr[11] << " Radial distortion 6: " << intr[12]
+                                                          << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
     else if (model == ICC_CAM_SCARAMUZZA) std::cout << "SCARAMUZZA model: A2: " << intr[5] << " A3: " << intr[6] << " A4: " << intr[7] << " Stretch c: " << intr[1]
                                                     << " d: " << intr[8] << " e: " << intr[2] << "\n";
     else if (model == ICC_CAM_FISHEYE) std::cout << "FISHEYE model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7] << " Radial distortion 4: " << intr[8] << "\n";

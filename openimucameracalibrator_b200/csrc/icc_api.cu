@@ -102,7 +102,7 @@ struct icc_handle {
   int device = -1;
   icc_solver_options opt;
   // ---- raw inputs -------------------------------------------------------------------------------------------
-  int model = -1, n_intr = 0, width = 0, height = 0; double intr[10] = {0};
+  int model = -1, n_intr = 0, width = 0, height = 0; double intr[MAX_INTR] = {0};
   int pose_error = ICC_POSE_ERROR_NORMALIZED;   // residual of icc_estimate_board_poses / icc_optimize_board_points (icc_set_pose_error)
   int reproj_error = ICC_REPROJ_ERROR_PIXEL;     // vision residual of the spline solve (icc_set_reprojection_error), fixed at batch_init
   double pose_line_delay = 0.0; std::vector<double> pose_frame_t;   // their shutter (icc_set_pose_rolling_shutter; 0 = global)
@@ -601,7 +601,7 @@ icc_status init_globals_and_knot_counts(icc_handle* h, KnotCounts& n) {
   for (int i = 0; i < 6; ++i) h->glob[G_ACC_INTR + i] = ip.acc_intrinsics[i];
   for (int i = 0; i < 9; ++i) h->glob[G_GYR_INTR + i] = ip.gyr_intrinsics[i];
   h->glob[G_LD] = ip.init_line_delay_s;
-  for (int i = 0; i < 10; ++i) h->glob[G_CAM_INTR + i] = i < h->n_intr ? h->intr[i] : 0.0;
+  for (int i = 0; i < MAX_INTR; ++i) h->glob[G_CAM_INTR + i] = i < h->n_intr ? h->intr[i] : 0.0;
   h->glob[G_TOFF] = 0.0;
   const auto range = std::minmax_element(h->frame_t.begin(), h->frame_t.end());
   h->t0_s = *range.first; h->tend_s = *range.second;
@@ -1725,11 +1725,11 @@ icc_status icc_calibrate_camera(icc_handle* h, int model, int W, int H, int nv, 
     if (!h->camcal_w_u.empty()) { vel = h->camcal_w_u; return calibrate(CamCalShutter{h->camcal_line_delay, vel.data()}); }
     // automatic mode: global-shutter round 0, then two rounds of (rolling-shutter pose step under the last intrinsics, calibration)
     icc_status r = calibrate(CamCalShutter{}); if (r != ICC_OK || !S.success) return r;
-    std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), intr(10);
+    std::vector<double> q(4 * (size_t)nv), p(3 * (size_t)nv), intr(MAX_INTR);
     std::vector<int32_t> valid(nv);
     vel.assign(6 * (size_t)nv, 0.0);
     for (int round = 1; round <= 2; ++round) {
-      std::copy(intr_out, intr_out + 10, intr.begin());
+      std::copy(intr_out, intr_out + std::max(10, camera_num_params(model)), intr.begin());
       const PoseShutter ps{h->camcal_line_delay, h->camcal_frame_t.data(), vel.data(), &n_static};
       r = estimate_board_poses(h->stream, model, intr.data(), W, H, np, h->points.data(), nv, off, ids, uv, 0.0, 0, h->pose_error, ps, q.data(), p.data(), nullptr, valid.data(), err);
       if (r != ICC_OK) return r;

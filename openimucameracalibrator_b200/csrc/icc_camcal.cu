@@ -5,16 +5,16 @@
 //   utils::GetReprojErrorOfView                 src/utils/utils.cc:163-177              (per-view mean reprojection error)
 // with the residual of theia::ReprojectionError (external): r = CameraToPixelCoordinates(intr, R_cw (X - c)) - feature.
 //
-// Mapping to the machine.  The normal equations are an arrow: 6x6 pose blocks on the diagonal, a border of <= 10 intrinsics.
-//   camcal_accumulate_kernel : one WARP per view.  Each lane evaluates one corner (projection + closed-form 2x3 and 2x10
+// Mapping to the machine.  The normal equations are an arrow: 6x6 pose blocks on the diagonal, a border of <= MAX_INTR (13) intrinsics.
+//   camcal_accumulate_kernel : one WARP per view.  Each lane evaluates one corner (projection + closed-form 2x3 and 2xMAX_INTR
 //       Jacobians of icc_camera.cuh, Huber weight) and writes its weighted rows [J_pose | J_intr | r] (17 columns, padded to three
 //       8-column blocks) into the warp's shared-memory tile -- x rows, then y rows; each half is folded into the symmetric product
 //       with FP64 tensor-core MMAs (mma.sync m8n8k4: 6 block products per 4 rows, the accumulator fragments stay in registers for
 //       the whole view), so J^T J, J^T r and r^T r come out of one contraction.  The view's 17x17 block goes to HBM, its intrinsics
 //       part is summed into the global system with RED.ADD.F64.
 //   camcal_reduce_kernel     : one thread per view: damped 6x6 Cholesky, Y = A^-1 [H_pk | g_p], Schur complement of the view
-//       onto the intrinsics, summed over the CTA through shared memory and added to the reduced 10x10 system.
-//   camcal_solve_kernel      : the reduced system (<= 10 unknowns) by Cholesky, intrinsics step, candidate intrinsics.
+//       onto the intrinsics, summed over the CTA through shared memory and added to the reduced MAX_INTR x MAX_INTR system.
+//   camcal_solve_kernel      : the reduced system (<= MAX_INTR unknowns) by Cholesky, intrinsics step, candidate intrinsics.
 //   camcal_update_kernel     : back-substitution of every view's pose step, candidate poses, step / model-decrease sums.
 // The host only sequences these launches and applies Ceres' trust-region logic to eight scalars per iteration (calibrate_camera below).
 #include "icc_camera.cuh"
@@ -30,8 +30,11 @@
 
 namespace icc {
 
-// Column order of a view's [J | r] rows: 0-2 rotation increment, 3-5 camera centre, 6-15 intrinsics (Theia order), 16 residual.
-constexpr int CC_COLS = 17, CC_PACK = CC_COLS * (CC_COLS + 1) / 2, CC_Y = 66;   // packed upper triangle; Y = A^-1 [H_pk | g_p] (6 x 11)
+// Column order of a view's [J | r] rows: 0-2 rotation increment, 3-5 camera centre, 6.. intrinsics (Theia order, MAX_INTR columns), residual.
+constexpr int CC_RES = 6 + MAX_INTR, CC_COLS = CC_RES + 1, CC_PACK = CC_COLS * (CC_COLS + 1) / 2;   // packed upper triangle
+constexpr int CC_Y = 6 * (MAX_INTR + 1);                                                           // Y = A^-1 [H_pk | g_p] (6 x (MAX_INTR + 1))
+// the intrinsics' Schur complement: the packed upper triangle of the reduced system, then its gradient
+constexpr int CC_RED_G = MAX_INTR * (MAX_INTR + 1) / 2, CC_RED = CC_RED_G + MAX_INTR;
 enum { CC_CAND_COST = 0, CC_G_DELTA = 1, CC_D_DELTA = 2, CC_STEP_SQ = 3, CC_X_SQ = 4, CC_FAIL = 5, CC_GRAD_MAX = 6, CC_X_COST = 7, CC_SCAL_COUNT = 8 };
 struct CamCalProblem {
   int model, n_points, n_active, pose_free;
@@ -40,13 +43,13 @@ struct CamCalProblem {
   const double4* board; const int* f_off; const int* pid; const double2* uv;
   const int* active;           // indices of the views that take part (n_active)
 };
-struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) per view, camera centre per view, 10 intrinsics
+struct CamCalState { double* q; double* c; double* k; };   // R_cw as (x,y,z,w) per view, camera centre per view, MAX_INTR intrinsics
 struct CamCalRs { const double* vel; double line_delay; };  // rolling shutter: (w, u) per view (6 doubles), line delay [s]; vel == nullptr: global
 
 namespace {
 
-ICC_HD int pk(int i, int j) { return i * CC_COLS - i * (i - 1) / 2 + (j - i); }   // packed upper triangle of the 17x17 block, i <= j
-ICC_HD int pk10(int a, int b) { return a * 10 - a * (a - 1) / 2 + (b - a); }       // packed upper triangle of the 10x10 reduced system
+ICC_HD int pk(int i, int j) { return i * CC_COLS - i * (i - 1) / 2 + (j - i); }              // packed upper triangle of a view's block, i <= j
+ICC_HD int pkr(int a, int b) { return a * MAX_INTR - a * (a - 1) / 2 + (b - a); }             // packed upper triangle of the reduced system
 
 ICC_D void atomic_max_nonneg(double* addr, double v) {   // v >= 0: the bit patterns of non-negative doubles order like integers
   atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
@@ -84,14 +87,14 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
   const int slot = blockIdx.x * 4 + warp;
   if (slot >= Q.n_active) return;
   double* tile = tile_all + (JAC ? warp * CC_TCOLS * LDT : 0);
-  if (JAC) { for (int i = lane; i < CC_TCOLS * LDT; i += 32) tile[i] = 0.0; __syncwarp(); }   // the padding columns 17..23 stay zero
+  if (JAC) { for (int i = lane; i < CC_TCOLS * LDT; i += 32) tile[i] = 0.0; __syncwarp(); }   // the padding columns past CC_COLS stay zero
   const int v = Q.active[slot];
   const int c0 = Q.f_off[v], c1 = Q.f_off[v + 1];
   const Q4 q = q4(S.q[4 * v], S.q[4 * v + 1], S.q[4 * v + 2], S.q[4 * v + 3]);
   const V3 cc = v3(S.c[3 * v], S.c[3 * v + 1], S.c[3 * v + 2]);
-  double k[10];
+  double k[MAX_INTR];
 #pragma unroll
-  for (int i = 0; i < 10; ++i) k[i] = S.k[i];
+  for (int i = 0; i < MAX_INTR; ++i) k[i] = S.k[i];
   double acc[CC_NACC][2];
 #pragma unroll
   for (int i = 0; i < CC_NACC; ++i) { acc[i][0] = 0.0; acc[i][1] = 0.0; }
@@ -110,7 +113,7 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
       const double* vel = rs.vel + 6 * v;
       RsMotion m; m.w = v3(vel[0], vel[1], vel[2]); m.u = v3(vel[3], vel[4], vel[5]);
       const double2 uv = Q.uv[c];
-      double r0, r1, J0[6], J1[6], Jk0[10], Jk1[10];
+      double r0, r1, J0[6], J1[6], Jk0[MAX_INTR], Jk1[MAX_INTR];
       const bool ok = rs_camera_residual(Q.model, k, q, cc, v3(Xb.x * iw, Xb.y * iw, Xb.z * iw), m, uv.y * rs.line_delay, uv, r0, r1,
                                          JAC ? J0 : nullptr, JAC ? J1 : nullptr, JAC ? Jk0 : nullptr, JAC ? Jk1 : nullptr);
       if (!ok) { cost += 1e10; esum += 1e10; }
@@ -125,8 +128,8 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
 #pragma unroll
             for (int i = 0; i < 6; ++i) { rx[i] = sw * J0[i]; ry[i] = sw * J1[i]; }
 #pragma unroll
-          for (int i = 0; i < 10; ++i) if ((Q.intr_mask >> i) & 1u) { rx[6 + i] = sw * Jk0[i]; ry[6 + i] = sw * Jk1[i]; }
-          rx[16] = sw * r0; ry[16] = sw * r1;
+          for (int i = 0; i < MAX_INTR; ++i) if ((Q.intr_mask >> i) & 1u) { rx[6 + i] = sw * Jk0[i]; ry[6 + i] = sw * Jk1[i]; }
+          rx[CC_RES] = sw * r0; ry[CC_RES] = sw * r1;
         }
       }
     } else if (!RS && c < c1) {
@@ -156,8 +159,8 @@ __global__ void __launch_bounds__(128) camcal_accumulate_kernel(CamCalProblem Q,
             ry[0] = sw * b1.x; ry[1] = sw * b1.y; ry[2] = sw * b1.z; ry[3] = -sw * t1.x; ry[4] = -sw * t1.y; ry[5] = -sw * t1.z;
           }
 #pragma unroll
-          for (int i = 0; i < 10; ++i) if ((Q.intr_mask >> i) & 1u) { rx[6 + i] = sw * pkk.Jk[i]; ry[6 + i] = sw * pkk.Jk[10 + i]; }
-          rx[16] = sw * r0; ry[16] = sw * r1;
+          for (int i = 0; i < MAX_INTR; ++i) if ((Q.intr_mask >> i) & 1u) { rx[6 + i] = sw * pkk.Jk[jk_at(0, i)]; ry[6 + i] = sw * pkk.Jk[jk_at(1, i)]; }
+          rx[CC_RES] = sw * r0; ry[CC_RES] = sw * r1;
         }
       }
     }
@@ -213,14 +216,14 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
                                                            double* __restrict__ scale, int compute_scale, double radius, double mind, double maxd, double* __restrict__ scal) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
   const bool live = slot < Q.n_active && Q.pose_free;
-  double Yl[11][6];   // Yl[c] = column c of Y = A^-1 [H_pk | g_p]: one right-hand side of the 6x6 system each
-  double Hpk[6][10];
+  double Yl[MAX_INTR + 1][6];   // Yl[c] = column c of Y = A^-1 [H_pk | g_p]: one right-hand side of the 6x6 system each
+  double Hpk[6][MAX_INTR];
 #pragma unroll
   for (int i = 0; i < 6; ++i) {
 #pragma unroll
-    for (int c = 0; c < 11; ++c) Yl[c][i] = 0.0;
+    for (int c = 0; c <= MAX_INTR; ++c) Yl[c][i] = 0.0;
 #pragma unroll
-    for (int c = 0; c < 10; ++c) Hpk[i][c] = 0.0;
+    for (int c = 0; c < MAX_INTR; ++c) Hpk[i][c] = 0.0;
   }
   double gmax = 0.0;
   if (live) {
@@ -231,9 +234,9 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
 #pragma unroll
       for (int j = 0; j < 6; ++j) if (j >= i) { A[j][i] = B[pk(i, j)]; }
 #pragma unroll
-      for (int c = 0; c < 10; ++c) { Hpk[i][c] = B[pk(i, 6 + c)]; Yl[c][i] = Hpk[i][c]; }
-      Yl[10][i] = B[pk(i, 16)];
-      gmax = fmax(gmax, fabs(Yl[10][i]));
+      for (int c = 0; c < MAX_INTR; ++c) { Hpk[i][c] = B[pk(i, 6 + c)]; Yl[c][i] = Hpk[i][c]; }
+      Yl[MAX_INTR][i] = B[pk(i, CC_RES)];
+      gmax = fmax(gmax, fabs(Yl[MAX_INTR][i]));
     }
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
@@ -243,42 +246,46 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
     }
     const bool ok = chol_factor<6>(A);
 #pragma unroll
-    for (int c = 0; c < 11; ++c) chol_substitute<6>(A, Yl[c]);
+    for (int c = 0; c <= MAX_INTR; ++c) chol_substitute<6>(A, Yl[c]);
     if (!ok) atomicAdd(&scal[CC_FAIL], 1.0);
     double* Yo = Y + (size_t)slot * CC_Y;
 #pragma unroll
     for (int i = 0; i < 6; ++i)
 #pragma unroll
-      for (int c = 0; c < 11; ++c) Yo[i * 11 + c] = Yl[c][i];
+      for (int c = 0; c <= MAX_INTR; ++c) Yo[i * (MAX_INTR + 1) + c] = Yl[c][i];
   } else if (slot < Q.n_active) {
     double* Yo = Y + (size_t)slot * CC_Y;
     for (int i = 0; i < CC_Y; ++i) Yo[i] = 0.0;
   }
-  // Schur complement of this view onto the intrinsics: -H_pk^T Y  (matrix and gradient part); the 65 sums of the CTA's views are
-  // formed through shared memory (one column per thread, then one thread per output), 65 RED.ADD.F64 per CTA
-  __shared__ double part[65][RED_THREADS + 1];
-  {
+  // Schur complement of this view onto the intrinsics: -H_pk^T Y  (matrix and gradient part); the CC_RED sums of the CTA's views are
+  // formed through shared memory (one column per thread, then one thread per output), RED_ROWS of them per pass, one RED.ADD.F64 each
+  constexpr int RED_ROWS = 65;
+  __shared__ double part[RED_ROWS][RED_THREADS + 1];
+  for (int o0 = 0; o0 < CC_RED; o0 += RED_ROWS) {
     int o = 0;
 #pragma unroll
-    for (int a = 0; a < 10; ++a) {
+    for (int a = 0; a < MAX_INTR; ++a) {
 #pragma unroll
-      for (int b = 0; b < 11; ++b) if (b >= a) {
-        double sacc = 0.0;
+      for (int b = 0; b <= MAX_INTR; ++b) if (b >= a) {
+        if (o >= o0 && o < o0 + RED_ROWS) {
+          double sacc = 0.0;
 #pragma unroll
-        for (int i = 0; i < 6; ++i) sacc -= Hpk[i][a] * Yl[b][i];
-        part[o][threadIdx.x] = sacc;
+          for (int i = 0; i < 6; ++i) sacc -= Hpk[i][a] * Yl[b][i];
+          part[o - o0][threadIdx.x] = sacc;
+        }
         ++o;
       }
     }
-  }
-  __syncthreads();
-  for (int o = threadIdx.x; o < 65; o += RED_THREADS) {
-    double sacc = 0.0;
-    for (int t = 0; t < RED_THREADS; ++t) sacc += part[o][t];
-    // o enumerates (a, b >= a) row by row with b = 10 the gradient column
-    int a = 0, r = o; while (r >= 11 - a) { r -= 11 - a; ++a; }
-    const int b = a + r;
-    if (sacc != 0.0) atomicAdd(&red[b < 10 ? pk10(a, b) : 55 + a], sacc);
+    __syncthreads();
+    for (int o = o0 + threadIdx.x; o < o0 + RED_ROWS && o < CC_RED; o += RED_THREADS) {
+      double sacc = 0.0;
+      for (int t = 0; t < RED_THREADS; ++t) sacc += part[o - o0][t];
+      // o enumerates (a, b >= a) row by row with b = MAX_INTR the gradient column
+      int a = 0, r = o; while (r >= MAX_INTR + 1 - a) { r -= MAX_INTR + 1 - a; ++a; }
+      const int b = a + r;
+      if (sacc != 0.0) atomicAdd(&red[b < MAX_INTR ? pkr(a, b) : CC_RED_G + a], sacc);
+    }
+    __syncthreads();
   }
   gmax = warp_max(gmax);
   if (lane == 0 && gmax > 0.0) atomic_max_nonneg(&scal[CC_GRAD_MAX], gmax);
@@ -287,26 +294,26 @@ __global__ void __launch_bounds__(RED_THREADS) camcal_reduce_kernel(CamCalProble
 __global__ void camcal_solve_kernel(CamCalProblem Q, CamCalState cur, CamCalState cand, const double* __restrict__ sys, const double* __restrict__ red,
                                     double* __restrict__ scale_k, int compute_scale, double radius, double mind, double maxd, double* __restrict__ dk, double* __restrict__ scal) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  double A[10][10], b[10], D[10], g[10];
+  double A[MAX_INTR][MAX_INTR], b[MAX_INTR], D[MAX_INTR], g[MAX_INTR];
   double gmax = 0.0;
-  for (int a = 0; a < 10; ++a) {
+  for (int a = 0; a < MAX_INTR; ++a) {
     const bool act = (Q.intr_mask >> a) & 1u;
-    g[a] = act ? sys[pk(6 + a, 16)] : 0.0;
+    g[a] = act ? sys[pk(6 + a, CC_RES)] : 0.0;
     gmax = fmax(gmax, fabs(g[a]));
-    for (int c = a; c < 10; ++c) { const double v = sys[pk(6 + a, 6 + c)] + red[pk10(a, c)]; A[c][a] = v; A[a][c] = v; }
+    for (int c = a; c < MAX_INTR; ++c) { const double v = sys[pk(6 + a, 6 + c)] + red[pkr(a, c)]; A[c][a] = v; A[a][c] = v; }
     if (act) {
       const double hii = sys[pk(6 + a, 6 + a)];
       const double s = compute_scale ? 1.0 / (1.0 + sqrt(hii)) : scale_k[a];
       if (compute_scale) scale_k[a] = s;
       D[a] = lm_damping(hii, s, radius, mind, maxd);
       A[a][a] += D[a];
-      b[a] = -(g[a] + red[55 + a]);
+      b[a] = -(g[a] + red[CC_RED_G + a]);
     } else { D[a] = 0.0; b[a] = 0.0; }
   }
-  for (int a = 0; a < 10; ++a) if (!((Q.intr_mask >> a) & 1u)) { for (int c = 0; c < 10; ++c) { A[a][c] = 0.0; A[c][a] = 0.0; } A[a][a] = 1.0; }
-  const bool ok = chol_solve<10>(A, b);
+  for (int a = 0; a < MAX_INTR; ++a) if (!((Q.intr_mask >> a) & 1u)) { for (int c = 0; c < MAX_INTR; ++c) { A[a][c] = 0.0; A[c][a] = 0.0; } A[a][a] = 1.0; }
+  const bool ok = chol_solve<MAX_INTR>(A, b);
   double gd = 0.0, dd = 0.0, st = 0.0, xs = 0.0;
-  for (int a = 0; a < 10; ++a) {
+  for (int a = 0; a < MAX_INTR; ++a) {
     dk[a] = b[a]; cand.k[a] = cur.k[a] + b[a];
     gd += g[a] * b[a]; dd += D[a] * b[a] * b[a]; st += b[a] * b[a]; xs += cur.k[a] * cur.k[a];
   }
@@ -330,12 +337,12 @@ __global__ void __launch_bounds__(128) camcal_update_kernel(CamCalProblem Q, Cam
       const double* B = blocks + (size_t)slot * CC_PACK;
 #pragma unroll
       for (int i = 0; i < 6; ++i) {
-        double s = Yi[i * 11 + 10];
+        double s = Yi[i * (MAX_INTR + 1) + MAX_INTR];
 #pragma unroll
-        for (int a = 0; a < 10; ++a) s += Yi[i * 11 + a] * dk[a];
+        for (int a = 0; a < MAX_INTR; ++a) s += Yi[i * (MAX_INTR + 1) + a] * dk[a];
         dp[i] = -s;
         const double hii = B[pk(i, i)];
-        gd += B[pk(i, 16)] * dp[i];
+        gd += B[pk(i, CC_RES)] * dp[i];
         dd += lm_damping(hii, scale[6 * slot + i], radius, mind, maxd) * dp[i] * dp[i];
         st += dp[i] * dp[i];
       }
@@ -363,6 +370,7 @@ IntrinsicSubsets intrinsic_subsets(int model) {
     case CAM_EXTENDED_UNIFIED: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6}), 0u};
     case CAM_OMNI_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};   // radial = xi, k1, k2
     case CAM_SCARAMUZZA: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({2, 8})};    // radial = a2, a3, a4; the stretch e, d as tangential
+    case CAM_PINHOLE_RATIONAL: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7, 10, 11, 12}), bits({8, 9})};   // radial = k1..k6
     default: return {0u, 0u, 0u, 0u, 0u};
   }
 }
@@ -387,8 +395,8 @@ void launch_camcal_accumulate(const CamCalProblem& Q, const CamCalState& S, bool
 }
 
 // one damped step: per-view Schur elimination, reduced intrinsics system, back-substitution into the candidate state
-void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const CamCalState& cand, const double* blocks, const double* sys, double* red /* 66 */, double* Y,
-                        double* scale /* 6 n_active + 10 */, int compute_scale, double radius, double min_diag, double max_diag, double* dk /* 10 */, double* scal, cudaStream_t st) {
+void launch_camcal_step(const CamCalProblem& Q, const CamCalState& cur, const CamCalState& cand, const double* blocks, const double* sys, double* red /* CC_RED */, double* Y,
+                        double* scale /* 6 n_active + MAX_INTR */, int compute_scale, double radius, double min_diag, double max_diag, double* dk /* MAX_INTR */, double* scal, cudaStream_t st) {
   if (Q.n_active <= 0) return;
   const int grid = (Q.n_active + 127) / 128;
   camcal_reduce_kernel<<<(Q.n_active + RED_THREADS - 1) / RED_THREADS, RED_THREADS, 0, st>>>(Q, blocks, red, Y, scale, compute_scale, radius, min_diag, max_diag, scal);
@@ -462,7 +470,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     if (init_valid) for (int i = 0; i < nv; ++i) ok0[i] = init_valid[i] != 0;
   }
   // ---- state: R_cw = conj(q_wc), camera centre, shared intrinsics ---------------------------------------------------------------
-  std::vector<double> qs(4 * (size_t)nv), k0(10, 0.0);
+  std::vector<double> qs(4 * (size_t)nv), k0(MAX_INTR, 0.0);
   for (int v = 0; v < nv; ++v) {
     const Q4 q = qnormalized(q4(q0[4 * v], q0[4 * v + 1], q0[4 * v + 2], q0[4 * v + 3]));
     qs[4 * v] = -q.x; qs[4 * v + 1] = -q.y; qs[4 * v + 2] = -q.z; qs[4 * v + 3] = q.w;
@@ -478,8 +486,8 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   DevBuf<double> d_q[2], d_c[2], d_k[2], d_blocks, d_Y, d_scale, d_sys, d_red, d_dk, d_scal, d_verr;
   for (int i = 0; i < 2; ++i) { CU(d_q[i].upload(qs)); CU(d_c[i].upload(p0)); CU(d_k[i].upload(k0)); }
   const size_t na0 = std::max<size_t>(1, active.size());
-  CU(d_blocks.alloc(na0 * CC_PACK)); CU(d_Y.alloc(na0 * CC_Y)); CU(d_scale.alloc(6 * na0 + 10)); CU(d_sys.alloc(CC_PACK + 1)); CU(d_red.alloc(66));
-  CU(d_dk.alloc(10)); CU(d_scal.alloc(CC_SCAL_COUNT)); CU(d_verr.alloc(nv));
+  CU(d_blocks.alloc(na0 * CC_PACK)); CU(d_Y.alloc(na0 * CC_Y)); CU(d_scale.alloc(6 * na0 + MAX_INTR)); CU(d_sys.alloc(CC_PACK + 1)); CU(d_red.alloc(CC_RED));
+  CU(d_dk.alloc(MAX_INTR)); CU(d_scal.alloc(CC_SCAL_COUNT)); CU(d_verr.alloc(nv));
   int cur = 0;
   CamCalProblem Q; memset(&Q, 0, sizeof Q);
   Q.model = model; Q.n_points = np; Q.huber = o.huber_width; Q.board = B.board.p; Q.f_off = B.off.p; Q.pid = B.pid.p; Q.uv = B.uv.p; Q.active = d_active.p;
@@ -521,7 +529,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
         CU(cudaMemsetAsync(d_sys.p, 0, (CC_PACK + 1) * sizeof(double), st));
         launch_camcal_accumulate(Q, state(cur), true, d_blocks.p, d_sys.p, nullptr, nullptr, rs, st);
       }
-      CU(cudaMemsetAsync(d_red.p, 0, 66 * sizeof(double), st));
+      CU(cudaMemsetAsync(d_red.p, 0, CC_RED * sizeof(double), st));
       CU(cudaMemsetAsync(d_scal.p, 0, CC_SCAL_COUNT * sizeof(double), st));
       launch_camcal_step(Q, state(cur), state(1 - cur), d_blocks.p, d_sys.p, d_red.p, d_Y.p, d_scale.p, T.iterations == 0 ? 1 : 0, T.radius, to.min_diagonal, to.max_diagonal, d_dk.p, d_scal.p, st);
       launch_camcal_accumulate(Q, state(1 - cur), false, nullptr, nullptr, d_scal.p + CC_CAND_COST, nullptr, rs, st);
@@ -538,17 +546,17 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     // a rejected candidate are stale): bring the spare copy back to the current state
     CU(cudaMemcpyAsync(d_q[1 - cur].p, d_q[cur].p, 4 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
     CU(cudaMemcpyAsync(d_c[1 - cur].p, d_c[cur].p, 3 * (size_t)nv * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(d_k[1 - cur].p, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(d_k[1 - cur].p, d_k[cur].p, MAX_INTR * sizeof(double), cudaMemcpyDeviceToDevice, st));
     if (stage == 0) S.initial_cost = T.initial_cost;
     if (stage >= 0) { S.final_cost[stage] = T.cost; S.iterations[stage] = T.iterations; S.termination[stage] = T.termination; } else S.init_iterations = T.iterations;
     return ICC_OK;
   };
   auto finish = [&](bool success) -> icc_status {
     icc_status r = view_errors(); if (r != ICC_OK) return r;
-    std::vector<double> qh(4 * (size_t)nv), ch(3 * (size_t)nv), kh(10);
+    std::vector<double> qh(4 * (size_t)nv), ch(3 * (size_t)nv), kh(MAX_INTR);
     CU(cudaMemcpy(qh.data(), d_q[cur].p, qh.size() * sizeof(double), cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(ch.data(), d_c[cur].p, ch.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(kh.data(), d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(kh.data(), d_k[cur].p, MAX_INTR * sizeof(double), cudaMemcpyDeviceToHost));
     for (int v = 0; v < nv; ++v) {
       q_out[4 * v] = -qh[4 * v]; q_out[4 * v + 1] = -qh[4 * v + 1]; q_out[4 * v + 2] = -qh[4 * v + 2]; q_out[4 * v + 3] = qh[4 * v + 3];
       for (int d = 0; d < 3; ++d) p_out[3 * v + d] = ch[3 * v + d];
@@ -556,7 +564,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     }
     double tot = 0.0;
     for (int v : active) { used_out[v] = 1; if (err_out) err_out[v] = verr[v]; tot += verr[v]; }
-    for (int i = 0; i < 10; ++i) intr_out[i] = kh[i];
+    for (int i = 0; i < std::max(10, camera_num_params(model)); ++i) intr_out[i] = kh[i];   // icc_b200.h: max(10, parameter count) entries
     S.success = success ? 1 : 0; S.n_views_used = (int)active.size();
     S.final_reproj_error = active.empty() ? 0.0 : tot / (double)active.size();                 // :352-366
     S.gpu_launches = kernel_launch_count() - launches0;
@@ -568,7 +576,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     Q.model = CAM_DIVISION_UNDISTORTION;
     rc = bundle_adjust((1u << 0) | (1u << 4), true, -1); if (rc != ICC_OK) return rc;
     Q.model = model;
-    double kd[10];
+    double kd[MAX_INTR];
     CU(cudaMemcpy(kd, d_k[cur].p, sizeof kd, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(p0.data(), d_c[cur].p, p0.size() * sizeof(double), cudaMemcpyDeviceToHost));
     if (kd[0] > 0.0 && std::isfinite(kd[0])) { f0 = kd[0]; if (model == CAM_DIVISION_UNDISTORTION) distortion_init = kd[4]; }
@@ -616,7 +624,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   if (model == CAM_EXTENDED_UNIFIED) { k0[5] = 0.5; k0[6] = 1.0; }
   if (model == CAM_OMNI_RADTAN) { k0[5] = 1.0; k0[0] = 2.0 * f0; }   // xi = 1, f = (1 + xi) f0: magnification f / (1 + xi) = f0 at the image centre
   if (model == CAM_SCARAMUZZA) k0[5] = -0.25 / f0;                    // the stereographic member a2 = -1 / (4 a0): magnification a0 = f0 at the image centre
-  for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), 10 * sizeof(double), cudaMemcpyHostToDevice));
+  for (int i = 0; i < 2; ++i) CU(cudaMemcpy(d_k[i].p, k0.data(), MAX_INTR * sizeof(double), cudaMemcpyHostToDevice));
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :132-135
   const IntrinsicSubsets sub = intrinsic_subsets(model);
   // 1. focal length and radial distortion, principal point fixed (:146-160)
@@ -626,7 +634,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
   // 3. full optimisation (:181-198)
-  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN || model == CAM_SCARAMUZZA ? sub.tangential : 0u);
+  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN || model == CAM_SCARAMUZZA || model == CAM_PINHOLE_RATIONAL ? sub.tangential : 0u);
   rc = bundle_adjust(stage3_mask, true, 2);
   if (rc != ICC_OK) return rc;
   rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200
@@ -636,7 +644,7 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
     std::vector<int> obs_view(std::max(1, nc), -1);
     for (int v : active) for (int c = off[v]; c < off[v + 1]; ++c) obs_view[c] = v;
     PointProblem PQ; memset(&PQ, 0, sizeof PQ);
-    PQ.model = model; CU(cudaMemcpy(PQ.intr, d_k[cur].p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
+    PQ.model = model; CU(cudaMemcpy(PQ.intr, d_k[cur].p, MAX_INTR * sizeof(double), cudaMemcpyDeviceToHost));
     PQ.normalized = 0; PQ.n_points = np; PQ.min_obs = 1; PQ.huber = o.huber_width;
     PQ.board_in = B.board.p; PQ.meas = B.uv.p; PQ.q_cw = d_q[cur].p; PQ.cam_c = d_c[cur].p;
     const RsPass rsp{B.uv.p, d_vel.p, shutter.line_delay};

@@ -6,23 +6,30 @@
 // Return value = Theia's `bool` (false => the reference writes the constant 1e10 residual, quirk q12).
 #pragma once
 #include "icc_device_math.cuh"
+#include "../../include/icc_b200.h"
 
 namespace icc {
 
 enum CameraModel { CAM_PINHOLE = 0, CAM_PINHOLE_RADTAN = 1, CAM_FISHEYE = 2, CAM_FOV = 3, CAM_DIVISION_UNDISTORTION = 4, CAM_DOUBLE_SPHERE = 5, CAM_EXTENDED_UNIFIED = 6,
                    CAM_OMNI_RADTAN = 7 /* extension: Kalibr's omni-radtan, no Theia counterpart */,
-                   CAM_SCARAMUZZA = 8 /* extension: Scaramuzza's omnidirectional polynomial model (OCamCalib), no Theia counterpart */ };
+                   CAM_SCARAMUZZA = 8 /* extension: Scaramuzza's omnidirectional polynomial model (OCamCalib), no Theia counterpart */,
+                   CAM_PINHOLE_RATIONAL = 9 /* extension: OpenCV's rational polynomial model (k1..k6, p1, p2), no Theia counterpart */ };
+
+// Width of every intrinsic vector, buffer and Jacobian row in this library: the longest model's parameter count.
+constexpr int MAX_INTR = ICC_MAX_INTRINSICS;
 
 ICC_HD int camera_num_params(int model) {
   switch (model) { case CAM_PINHOLE: return 7; case CAM_PINHOLE_RADTAN: return 10; case CAM_FISHEYE: return 9; case CAM_FOV: return 5;
                    case CAM_DIVISION_UNDISTORTION: return 5; case CAM_DOUBLE_SPHERE: return 7; case CAM_EXTENDED_UNIFIED: return 7;
-                   case CAM_OMNI_RADTAN: return 10; case CAM_SCARAMUZZA: return 9; default: return -1; }
+                   case CAM_OMNI_RADTAN: return 10; case CAM_SCARAMUZZA: return 9; case CAM_PINHOLE_RATIONAL: return 13; default: return -1; }
 }
 
 // J is row-major 2x3: J[0..2] = d px / d(x,y,z), J[3..5] = d py / d(x,y,z).
-// Jk (only filled when requested) is row-major 2 x 10: d(u,v)/d intrinsics in Theia's parameter order, unused entries zero.
+// Jk (only filled when requested): d(u,v)/d intrinsics in Theia's parameter order, unused entries zero.  The first ten columns are
+// row-major 2 x 10 in Jk[0..19]; the columns past ten (CAM_PINHOLE_RATIONAL's k4..k6) follow as row-major 2 x (MAX_INTR - 10): jk_at.
 struct Proj { double u, v; double J[6]; bool ok; };
-struct ProjK { double Jk[20]; };
+struct ProjK { double Jk[2 * MAX_INTR]; };
+ICC_HD constexpr int jk_at(int row, int col) { return col < 10 ? 10 * row + col : 20 + (MAX_INTR - 10) * row + (col - 10); }
 
 // final affine of the skewed models: u = f dx + s dy + cx, v = f ar dy + cy, given d(dx,dy)/dp
 ICC_HD void affine_skew(const double* k, double dx, double dy, const double* Dd /*2x3*/, Proj& o) {
@@ -33,12 +40,12 @@ ICC_HD void affine_skew(const double* k, double dx, double dy, const double* Dd 
 }
 // intrinsic Jacobian of the skewed models: [f, ar, skew, cx, cy] columns + distortion columns idx[q] with d(dx,dy)/dk_q = (ddx[q], ddy[q])
 ICC_HD void affine_skew_k(const double* k, double dx, double dy, int nd, const int* idx, const double* ddx, const double* ddy, ProjK& o) {
-  for (int j = 0; j < 20; ++j) o.Jk[j] = 0.0;
+  for (int j = 0; j < 2 * MAX_INTR; ++j) o.Jk[j] = 0.0;
   o.Jk[0] = dx; o.Jk[10] = k[1] * dy;          // f
   o.Jk[11] = k[0] * dy;                        // aspect ratio
   o.Jk[2] = dy;                                // skew
   o.Jk[3] = 1.0; o.Jk[14] = 1.0;               // principal point
-  for (int q = 0; q < nd; ++q) { o.Jk[idx[q]] = k[0] * ddx[q] + k[2] * ddy[q]; o.Jk[10 + idx[q]] = k[0] * k[1] * ddy[q]; }
+  for (int q = 0; q < nd; ++q) { o.Jk[jk_at(0, idx[q])] = k[0] * ddx[q] + k[2] * ddy[q]; o.Jk[jk_at(1, idx[q])] = k[0] * k[1] * ddy[q]; }
 }
 
 ICC_HD double unified_w(double alpha) { return alpha > 0.5 ? (1.0 - alpha) / alpha : alpha / (1.0 - alpha); }
@@ -119,14 +126,76 @@ ICC_HD bool scaramuzza_scale(const double* k, double r, double z, double& s, dou
   return true;
 }
 
+// ---- OpenCV's rational polynomial model, [f, ar, skew, cx, cy, k1, k2, k3, t1, t2, k4, k5, k6] -------------------------------------------
+// R(s) = N(s) / M(s), N = 1 + k1 s + k2 s^2 + k3 s^3, M = 1 + k4 s + k5 s^2 + k6 s^3, s = xn^2 + yn^2.  A rational fit folds outside the
+// field it was calibrated on, so the model is valid only for s < s_max: the first s > 0 at which the radial map r R(r^2) stops increasing,
+// i.e. the first positive root of h = N M + 2 s (N' M - N M') (= M^2 d(r R) / dr) or of M (a pole); +inf when there is none.
+
+// Whether the polynomial c[0] + c[1] x + ... + c[D] x^D (c[0] > 0) has no root in (0, s]: Descartes' rule of signs on the Moebius image
+// q(y) = (1 + y)^D p((a + b y) / (1 + y)), whose positive roots are the roots of p in (a, b), bounds their number by the sign variations of
+// q's coefficients, with equal parity.  0: (a, b) is clear; odd: a root; otherwise (a, b) is halved (Vincent's theorem: a small enough
+// interval around simple roots counts exactly).  Left to right over (0, s]; a root cluster too tight to separate within the cap counts as a root.
+template <int D> ICC_HD double poly_at(const double* c, double x) { double v = c[D]; for (int j = D - 1; j >= 0; --j) v = v * x + c[j]; return v; }
+template <int D> ICC_HD int interval_sign_changes(const double* c, double a, double b) {
+  double q[D + 1];
+  for (int j = 0; j <= D; ++j) q[j] = c[j];
+  for (int i = 0; i < D; ++i)                       // Taylor shift to a: q[j] = p^(j)(a) / j!
+    for (int j = D - 1; j >= i; --j) q[j] += a * q[j + 1];
+  double w = 1.0;
+  for (int j = 1; j <= D; ++j) { w *= b - a; q[j] *= w; }   // p(a + (b - a) y)
+  for (int j = 0; j < D / 2 + 1 && j < D - j; ++j) { const double t = q[j]; q[j] = q[D - j]; q[D - j] = t; }   // y^D p(1 / y)
+  for (int i = 0; i < D; ++i)                       // Taylor shift by 1
+    for (int j = D - 1; j >= i; --j) q[j] += q[j + 1];
+  int v = 0; double prev = 0.0;
+  for (int j = 0; j <= D; ++j) if (q[j] != 0.0) { if (prev != 0.0 && (q[j] > 0.0) != (prev > 0.0)) ++v; prev = q[j]; }
+  return v;
+}
+template <int D> ICC_HD bool poly_root_free(const double* c, double s) {
+  if (!(poly_at<D>(c, s) > 0.0)) return false;
+  double a = 0.0, b = s;
+  for (int it = 0; it < 200; ++it) {
+    const int n = interval_sign_changes<D>(c, a, b);
+    if (n == 0) {
+      if (b >= s) return true;
+      if (!(poly_at<D>(c, b) > 0.0)) return false;
+      const double w = b - a;
+      a = b; b = fmin(s, b + 2.0 * w);
+      continue;
+    }
+    if (n & 1) return false;
+    const double m = 0.5 * (a + b);
+    if (!(m > a && m < b)) return false;
+    b = m;
+  }
+  return false;
+}
+// The domain test at s >= 0: M(s) > 0 and s < s_max.
+ICC_HD bool rational_in_domain(const double* k, double s) {
+  const double k1 = k[5], k2 = k[6], k3 = k[7], k4 = k[10], k5 = k[11], k6 = k[12];
+  if (!(1.0 + s * (k4 + s * (k5 + s * k6)) > 0.0)) return false;
+  const double m[4] = {1.0, k4, k5, k6};
+  // h = N M + 2 s (N' M - N M'): coefficient of s^j of N M is sum n_i m_(j-i), of s (N' M - N M') it is sum (i - (j - i)) n_i m_(j-i)
+  const double n[4] = {1.0, k1, k2, k3};
+  double h[7];
+  for (int j = 0; j <= 6; ++j) {
+    double acc = 0.0;
+    for (int i = 0; i <= 3; ++i) if (j - i >= 0 && j - i <= 3) acc += (1.0 + 2.0 * (2 * i - j)) * n[i] * m[j - i];
+    h[j] = acc;
+  }
+  return poly_root_free<3>(m, s) && poly_root_free<6>(h, s);
+}
+
 template <int MODEL, bool WITH_K = false>
 ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = nullptr) {
   Proj o; o.ok = true;
-  if (WITH_K) for (int j = 0; j < 20; ++j) pk->Jk[j] = 0.0;
-  if (MODEL == CAM_PINHOLE || MODEL == CAM_PINHOLE_RADTAN) {
+  if (WITH_K) for (int j = 0; j < 2 * MAX_INTR; ++j) pk->Jk[j] = 0.0;
+  if (MODEL == CAM_PINHOLE || MODEL == CAM_PINHOLE_RADTAN || MODEL == CAM_PINHOLE_RATIONAL) {
+    if (MODEL == CAM_PINHOLE_RATIONAL && !(p.z > 0.0)) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
     const double iz = 1.0 / p.z, xn = p.x * iz, yn = p.y * iz;
     const double r2 = xn * xn + yn * yn;
     double d, dd, dx, dy, a00, a01, a10, a11;   // a = d(dx,dy)/d(xn,yn)
+    double iM = 1.0;                            // CAM_PINHOLE_RATIONAL: 1 / M
+    if (MODEL == CAM_PINHOLE_RATIONAL && !rational_in_domain(k, r2)) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
     if (MODEL == CAM_PINHOLE) {
       d = 1.0 + r2 * (k[5] + k[6] * r2); dd = k[5] + 2.0 * k[6] * r2;
       dx = xn * d; dy = yn * d;
@@ -134,6 +203,11 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
     } else {
       const double k1 = k[5], k2 = k[6], k3 = k[7], t1 = k[8], t2 = k[9];
       d = 1.0 + r2 * (k1 + r2 * (k2 + r2 * k3)); dd = k1 + r2 * (2.0 * k2 + 3.0 * k3 * r2);
+      if (MODEL == CAM_PINHOLE_RATIONAL) {        // d = N / M, dd = (N' - d M') / M
+        const double k4 = k[10], k5 = k[11], k6 = k[12];
+        iM = 1.0 / (1.0 + r2 * (k4 + r2 * (k5 + r2 * k6)));
+        d *= iM; dd = (dd - d * (k4 + r2 * (2.0 * k5 + 3.0 * k6 * r2))) * iM;
+      }
       dx = xn * d + 2.0 * t1 * xn * yn + t2 * (r2 + 2.0 * xn * xn);
       dy = yn * d + 2.0 * t2 * xn * yn + t1 * (r2 + 2.0 * yn * yn);
       a00 = d + 2.0 * xn * xn * dd + 2.0 * t1 * yn + 6.0 * t2 * xn;
@@ -146,9 +220,15 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
     affine_skew(k, dx, dy, Dd, o);
     if (WITH_K) {
       if (MODEL == CAM_PINHOLE) { const int idx[2] = {5, 6}; const double ddx[2] = {xn * r2, xn * r2 * r2}, ddy[2] = {yn * r2, yn * r2 * r2}; affine_skew_k(k, dx, dy, 2, idx, ddx, ddy, *pk); }
-      else { const int idx[5] = {5, 6, 7, 8, 9};
+      else if (MODEL == CAM_PINHOLE_RADTAN) { const int idx[5] = {5, 6, 7, 8, 9};
              const double ddx[5] = {xn * r2, xn * r2 * r2, xn * r2 * r2 * r2, 2.0 * xn * yn, r2 + 2.0 * xn * xn}, ddy[5] = {yn * r2, yn * r2 * r2, yn * r2 * r2 * r2, r2 + 2.0 * yn * yn, 2.0 * xn * yn};
              affine_skew_k(k, dx, dy, 5, idx, ddx, ddy, *pk); }
+      else {   // dR/dk_i = s^i / M (k1..k3), -R s^i / M (k4..k6)
+        const int idx[8] = {5, 6, 7, 8, 9, 10, 11, 12};
+        const double ddx[8] = {xn * r2 * iM, xn * r2 * r2 * iM, xn * r2 * r2 * r2 * iM, 2.0 * xn * yn, r2 + 2.0 * xn * xn, -xn * d * r2 * iM, -xn * d * r2 * r2 * iM, -xn * d * r2 * r2 * r2 * iM};
+        const double ddy[8] = {yn * r2 * iM, yn * r2 * r2 * iM, yn * r2 * r2 * r2 * iM, r2 + 2.0 * yn * yn, 2.0 * xn * yn, -yn * d * r2 * iM, -yn * d * r2 * r2 * iM, -yn * d * r2 * r2 * r2 * iM};
+        affine_skew_k(k, dx, dy, 8, idx, ddx, ddy, *pk);
+      }
     }
   } else if (MODEL == CAM_FISHEYE) {
     const double r2 = p.x * p.x + p.y * p.y;
@@ -301,21 +381,26 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
     if (WITH_K) {   // ds/da0 = -1 / G_s, ds/da_i = -rho^i / G_s
       const double wu = p.x + e * p.y, wv = d * p.x + c * p.y, rho2 = rho * rho;   // d(u, v)/ds
       pk->Jk[0] = wu * ig; pk->Jk[10] = wv * ig;
-      pk->Jk[11] = vp;                                  // c
+      pk->Jk[11] = vp;                        // c
       pk->Jk[2] = vp;                                   // e
-      pk->Jk[3] = 1.0; pk->Jk[14] = 1.0;                // principal point
+      pk->Jk[3] = 1.0; pk->Jk[14] = 1.0;      // principal point
       pk->Jk[5] = wu * rho2 * ig; pk->Jk[15] = wv * rho2 * ig;
       pk->Jk[6] = wu * rho2 * rho * ig; pk->Jk[16] = wv * rho2 * rho * ig;
       pk->Jk[7] = wu * rho2 * rho2 * ig; pk->Jk[17] = wv * rho2 * rho2 * ig;
-      pk->Jk[18] = up;                                  // d
+      pk->Jk[18] = up;                        // d
     }
   }
   return o;
 }
 
-// CAM_SCARAMUZZA out of line for the runtime dispatchers: its root solves stay out of the kernels that inline project() for every model
-__host__ __device__ inline __noinline__ Proj project_scaramuzza(const double* k, V3 p) { return project_model<CAM_SCARAMUZZA>(k, p, true); }
-__host__ __device__ inline __noinline__ Proj project_scaramuzza_with_k(const double* k, V3 p, ProjK* pk) { return project_model<CAM_SCARAMUZZA, true>(k, p, true, pk); }
+// CAM_SCARAMUZZA and CAM_PINHOLE_RATIONAL out of line for the runtime dispatchers, behind one call: their root solves / root isolation
+// stay out of the kernels that inline project() for every model
+__host__ __device__ inline __noinline__ Proj project_out_of_line(int model, const double* k, V3 p) {
+  return model == CAM_SCARAMUZZA ? project_model<CAM_SCARAMUZZA>(k, p, true) : project_model<CAM_PINHOLE_RATIONAL>(k, p, true);
+}
+__host__ __device__ inline __noinline__ Proj project_out_of_line_with_k(int model, const double* k, V3 p, ProjK* pk) {
+  return model == CAM_SCARAMUZZA ? project_model<CAM_SCARAMUZZA, true>(k, p, true, pk) : project_model<CAM_PINHOLE_RATIONAL, true>(k, p, true, pk);
+}
 
 // Same dispatch, additionally returning d(u,v)/d(intrinsics) (CAM_INTRINSICS extension).
 ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, ProjK* pk) {
@@ -328,12 +413,12 @@ ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, 
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN, true>(k, p, dispatch_fov, pk);
     case CAM_FOV: return project_model<CAM_FOV, true>(k, p, dispatch_fov, pk);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN, true>(k, p, dispatch_fov, pk);
-    case CAM_SCARAMUZZA: return project_scaramuzza_with_k(k, p, pk);
-    default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 20; ++j) pk->Jk[j] = 0; return o; }
+    case CAM_SCARAMUZZA: case CAM_PINHOLE_RATIONAL: return project_out_of_line_with_k(model, k, p, pk);
+    default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 2 * MAX_INTR; ++j) pk->Jk[j] = 0; return o; }
   }
 }
 
-// Runtime dispatch in the reference's order (residuals.h:366-389), then the extensions CAM_OMNI_RADTAN and CAM_SCARAMUZZA.
+// Runtime dispatch in the reference's order (residuals.h:366-389), then the extensions CAM_OMNI_RADTAN, CAM_SCARAMUZZA and CAM_PINHOLE_RATIONAL.
 ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
   switch (model) {
     case CAM_DIVISION_UNDISTORTION: return project_model<CAM_DIVISION_UNDISTORTION>(k, p, dispatch_fov);
@@ -344,7 +429,7 @@ ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
     case CAM_PINHOLE_RADTAN: return project_model<CAM_PINHOLE_RADTAN>(k, p, dispatch_fov);
     case CAM_FOV: return project_model<CAM_FOV>(k, p, dispatch_fov);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN>(k, p, dispatch_fov);
-    case CAM_SCARAMUZZA: return project_scaramuzza(k, p);
+    case CAM_SCARAMUZZA: case CAM_PINHOLE_RATIONAL: return project_out_of_line(model, k, p);
     default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
   }
 }

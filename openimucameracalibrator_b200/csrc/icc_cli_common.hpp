@@ -83,6 +83,11 @@ int read_camera(const Value& j, std::vector<double>& k, int& width, int& height,
   if (type == "PINHOLE") { k = {f, ar(), 0.0, cx, cy, 0.0, 0.0}; return ICC_CAM_PINHOLE; }
   if (type == "OMNI_RADIAL_TANGENTIAL") { k = {f, ar(), 0.0, cx, cy, in.at("xi").num(), in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("tangential_distortion_1").num(), in.at("tangential_distortion_2").num()}; return ICC_CAM_OMNI_RADIAL_TANGENTIAL; }
   if (type == "SCARAMUZZA") { k = {f, ar(), in.at("stretch_e").num(), cx, cy, in.at("polynomial_a2").num(), in.at("polynomial_a3").num(), in.at("polynomial_a4").num(), in.at("stretch_d").num()}; return ICC_CAM_SCARAMUZZA; }
+  if (type == "PINHOLE_RATIONAL") {   // extension: OpenCV's rational polynomial model, k1..k6 = radial_distortion_1..6, p1, p2 = tangential_distortion_1, 2
+    k = {f, ar(), 0.0, cx, cy, in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("radial_distortion_3").num(), in.at("tangential_distortion_1").num(),
+         in.at("tangential_distortion_2").num(), in.at("radial_distortion_4").num(), in.at("radial_distortion_5").num(), in.at("radial_distortion_6").num()};
+    return ICC_CAM_PINHOLE_RATIONAL;
+  }
   if (type == "FOV") { k = {f, in.contains("aspect_ratio") ? ar() : 1.0, cx, cy, in.at("radial_distortion_1").num()}; return ICC_CAM_FOV; }
   throw std::runtime_error("unknown intrinsic_type " + type);
 }

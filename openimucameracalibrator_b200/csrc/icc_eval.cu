@@ -35,6 +35,8 @@ void count_launch() { g_launches.fetch_add(1); }
 namespace {
 
 constexpr int WARPS = 4;
+// tile columns of the CAM_INTRINSICS vision kernel (JAC == 2): [so3 | r3 | T_i_c | ld | MAX_INTR intrinsics | r] in 8-column blocks
+constexpr int VIS_K_TILE_COLS = 8 * ((43 + MAX_INTR + 1 + 7) / 8);
 
 ICC_D void mma_f64(double (&c)[2], double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
@@ -113,12 +115,12 @@ __global__ void __launch_bounds__(WARPS * 32) vision_kernel(DeviceProblem P, Dev
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   WarpCtx* wc = reinterpret_cast<WarpCtx*>(smem_raw) + warp;
-  constexpr int NB = JAC == 2 ? 7 : 6, TILE_COLS = 8 * NB;
+  constexpr int NB = JAC == 2 ? VIS_K_TILE_COLS / 8 : 6, TILE_COLS = 8 * NB;
   double* Jt = reinterpret_cast<double*>(smem_raw + WARPS * sizeof(WarpCtx)) + warp * (TILE_COLS * LDJ);
   const int RES = JAC == 2 ? 43 + P.n_intr : 43, NCOL = RES + 1;
-  double intr[10];
+  double intr[MAX_INTR];
 #pragma unroll
-  for (int i = 0; i < 10; ++i) intr[i] = S.glob[G_CAM_INTR + i];
+  for (int i = 0; i < MAX_INTR; ++i) intr[i] = S.glob[G_CAM_INTR + i];
 
   const Q4 q_ic = q4(S.glob[G_TIC + 0], S.glob[G_TIC + 1], S.glob[G_TIC + 2], S.glob[G_TIC + 3]);
   const V3 t_ic = v3(S.glob[G_TIC + 4], S.glob[G_TIC + 5], S.glob[G_TIC + 6]);
@@ -206,7 +208,7 @@ __global__ void __launch_bounds__(WARPS * 32) vision_kernel(DeviceProblem P, Dev
             Jt[36 * LDJ + lane] = -Dp.x; Jt[37 * LDJ + lane] = -Dp.y; Jt[38 * LDJ + lane] = -Dp.z;
             Jt[39 * LDJ + lane] = om.x; Jt[40 * LDJ + lane] = om.y; Jt[41 * LDJ + lane] = om.z;
             Jt[42 * LDJ + lane] = y * (du - dot(m_t, tdot));
-            if (JAC == 2) { for (int q = 0; q < P.n_intr; ++q) Jt[(43 + q) * LDJ + lane] = pk.Jk[10 * row + q]; }
+            if (JAC == 2) { for (int q = 0; q < P.n_intr; ++q) Jt[(43 + q) * LDJ + lane] = pk.Jk[jk_at(row, q)]; }
             Jt[RES * LDJ + lane] = row == 0 ? r0 : r1;
           } else {
             for (int k = 0; k < RES; ++k) Jt[k * LDJ + lane] = 0.0;
@@ -533,7 +535,7 @@ int launch_eval(const DeviceProblem& P_in, const DeviceState& S, bool with_jacob
   static int sm_count = 0;
   if (!sm_count) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev); if (sm_count <= 0) sm_count = 132; }
   const size_t sm_vis = WARPS * sizeof(WarpCtx) + WARPS * 48 * LDJ * sizeof(double);
-  const size_t sm_vis_k = WARPS * sizeof(WarpCtx) + WARPS * 56 * LDJ * sizeof(double);
+  const size_t sm_vis_k = WARPS * sizeof(WarpCtx) + WARPS * VIS_K_TILE_COLS * LDJ * sizeof(double);
   const size_t sm_imu_nb = WARPS * sizeof(WarpCtx) + WARPS * 40 * LDJ * sizeof(double);
   const size_t sm_imu_b = WARPS * sizeof(WarpCtx) + WARPS * 56 * LDJ * sizeof(double);
   const size_t sm_cost = WARPS * sizeof(WarpCtx);   // the cost-only kernels never touch a tile: more CTAs per SM

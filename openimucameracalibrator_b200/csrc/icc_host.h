@@ -91,16 +91,16 @@ icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const in
                                const double4* bear = nullptr, const RsPass* rs = nullptr);
 
 // ---- the upstream tools' host drivers, each in the .cu file of its kernels -----------------------------------------------------
-icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err);
-icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err);
+icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err);
+icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err);
 // pose_error: ICC_POSE_ERROR_NORMALIZED or ICC_POSE_ERROR_TANGENT (the residual of the per-view refinement and of the board points)
 // The shutter of the pose step (icc_set_pose_rolling_shutter): line_delay = 0 is the global shutter; otherwise frame_t holds the nf view times,
 // and vel (6 per view: w, u) and n_static (valid views without a neighbour in time) receive what the last rolling-shutter pass used.
 struct PoseShutter { double line_delay = 0.0; const double* frame_t = nullptr; double* vel = nullptr; int32_t* n_static = nullptr; };
-icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
+icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int W, int H, int np, const double* points, int nf, const int32_t* off,
                                 const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc, double* mean_err,
                                 int32_t* valid, std::string& err);
-icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
+icc_status optimize_board_points(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
                                  const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc,
                                  double* mean_err, int32_t* valid, std::vector<double>& points_out, int32_t* n_opt_out, std::string& err);
 void filter_bad_poses(int nv, const double* p_wc, int32_t* valid);

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/icc_b200.h"
+
 struct icc_solver_plan_info;   // include/icc_b200.h
 
 namespace icc {
@@ -11,8 +13,8 @@ constexpr int SPLINE_N = 6;   // core/imu_camera_calibrator.h:27
 constexpr int BIAS_N = 3;     // basalt_spline/ceres_calib_split_residuals.h:21
 
 // Offsets inside the "globals" block of a state: T_i_c (7), gravity (3), line delay, accelerometer / gyroscope intrinsics (6 / 9),
-// camera intrinsics (<= 10, Theia order) and the time-offset increment [s] (both constant unless the extension flags free them).
-enum { G_TIC = 0, G_GRAV = 7, G_LD = 10, G_ACC_INTR = 11, G_GYR_INTR = 17, G_CAM_INTR = 26, G_TOFF = 36, G_COUNT = 37 };
+// camera intrinsics (ICC_MAX_INTRINSICS slots, Theia order) and the time-offset increment [s] (both constant unless the extension flags free them).
+enum { G_TIC = 0, G_GRAV = 7, G_LD = 10, G_ACC_INTR = 11, G_GYR_INTR = 17, G_CAM_INTR = 26, G_TOFF = G_CAM_INTR + ICC_MAX_INTRINSICS, G_COUNT = G_TOFF + 1 };
 
 // One LM state in HBM.  Knots are padded to 32 B (x,y,z,w / x,y,z,0) for 16-byte vector loads.
 struct DeviceState {
@@ -135,7 +137,7 @@ void launch_eval_trajectory(const DeviceProblem& P, const DeviceState& S, int n,
                             double* bg, double* ba, double* pose_q, double* pose_p, int* valid, cudaStream_t st);
 // ---- per-view board poses (icc_pose.cu) ---------------------------------------------------------------------------
 struct PoseProblem {
-  int model; double intr[10];
+  int model; double intr[ICC_MAX_INTRINSICS];
   int n_frames, n_points, min_points;
   const double4* board; const int* f_off; const int* pid;
   double thresh_sq;            // squared normalised reprojection error of an inlier (pose_estimator.cc:100-101)
@@ -146,7 +148,7 @@ struct PoseProblem {
 void launch_board_poses(const PoseProblem& Q, const double2* xy, const int* ok, unsigned char* use, double* q_wc, double* p_wc, double* err, int* valid, cudaStream_t st);
 // board point refinement with constant cameras (theia::BundleAdjustTracks), one warp per point
 struct PointProblem {
-  int model; double intr[10];
+  int model; double intr[ICC_MAX_INTRINSICS];
   int normalized;              // 1: measurements are undistorted normalised coordinates (unit pinhole), 0: pixels through `model`
   int n_points, min_obs;       // points with more than min_obs observations are optimised
   double huber;
@@ -162,7 +164,7 @@ struct RsPass { const double2* uv; const double* vel; double line_delay; };
 void launch_board_focal(const PoseProblem& Q, const double2* uv, double cx, double cy, double2* xy, unsigned char* use, double* f2, cudaStream_t st);
 void launch_pinhole_normalize(int n, const double2* uv, double cx, double cy, double f, double2* xy, int* ok, cudaStream_t st);
 // unit bearings of pixels (icc_bearing_math.cuh); ok[i] = 1 when b[i] could be formed (icc_pose.cu)
-void launch_bearings(int model, const double* intr10, int n, const double2* uv, double4* b, int* ok, cudaStream_t st);
+void launch_bearings(int model, const double* intr, int n, const double2* uv, double4* b, int* ok, cudaStream_t st);
 // ---- outlier corners (icc_outliers.cu) -----------------------------------------------------------------------------
 // err[c] = |(rx, ry)| of the residual pairs res2 (2 per corner); sums[0..2] += sum e^2 and the count over the counted corners (no zero
 // component, no failed projection), the failed projections

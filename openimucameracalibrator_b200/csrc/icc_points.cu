@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(128) points_jac_kernel(DeviceProblem P, Device
   __shared__ FrameWin wins[4];
   __shared__ VisConst K;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x < 10) K.intr[threadIdx.x] = S.glob[G_CAM_INTR + threadIdx.x];
+  if (threadIdx.x < MAX_INTR) K.intr[threadIdx.x] = S.glob[G_CAM_INTR + threadIdx.x];
   if (threadIdx.x == 32) {
     const Q4 q_ic = q4(S.glob[G_TIC + 0], S.glob[G_TIC + 1], S.glob[G_TIC + 2], S.glob[G_TIC + 3]);
     K.Ric = qmat(q_ic); K.tic = v3(S.glob[G_TIC + 4], S.glob[G_TIC + 5], S.glob[G_TIC + 6]);

@@ -37,7 +37,7 @@ namespace icc {
 
 namespace {
 
-struct Intr { double k[10]; };
+struct Intr { double k[MAX_INTR]; };
 
 __global__ void unproject_kernel(int model, Intr K, int n, const double2* __restrict__ uv, double2* __restrict__ xy, int* __restrict__ ok) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -615,16 +615,16 @@ __global__ void view_velocity_kernel(int n, const int* __restrict__ order, const
 
 }  // namespace
 
-void launch_unproject(int model, const double* intr10, int n, const double2* uv, double2* xy, int* ok, cudaStream_t st) {
+void launch_unproject(int model, const double* intr, int n, const double2* uv, double2* xy, int* ok, cudaStream_t st) {
   if (n <= 0) return;
-  Intr K; for (int i = 0; i < 10; ++i) K.k[i] = intr10[i];
+  Intr K; for (int i = 0; i < MAX_INTR; ++i) K.k[i] = intr[i];
   unproject_kernel<<<(n + 127) / 128, 128, 0, st>>>(model, K, n, uv, xy, ok);
   count_launch();
 }
 
-void launch_bearings(int model, const double* intr10, int n, const double2* uv, double4* b, int* ok, cudaStream_t st) {
+void launch_bearings(int model, const double* intr, int n, const double2* uv, double4* b, int* ok, cudaStream_t st) {
   if (n <= 0) return;
-  Intr K; for (int i = 0; i < 10; ++i) K.k[i] = intr10[i];
+  Intr K; for (int i = 0; i < MAX_INTR; ++i) K.k[i] = intr[i];
   bearing_kernel<<<(n + 127) / 128, 128, 0, st>>>(model, K, n, uv, b, ok);
   count_launch();
 }
@@ -719,11 +719,11 @@ icc_status refine_board_points(cudaStream_t st, PointProblem Q, int nc, const in
 
 // un-projection of every corner and the PoseProblem of EstimatePosesFromJson / OptimizeAllPoses for a W x H camera (pose_estimator.cc:97-101, :181).
 // Tangent mode: bearings into B.bear (B.xy and B.okh are the start's scratch); the thresholds keep their values, now on the tangent error.
-static PoseProblem unproject_corners(cudaStream_t st, int model, const double intr[10], int W, int H, const BoardViews& B, double max_reproj_error, int min_points, int pose_error) {
+static PoseProblem unproject_corners(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int W, int H, const BoardViews& B, double max_reproj_error, int min_points, int pose_error) {
   if (pose_error == ICC_POSE_ERROR_TANGENT) launch_bearings(model, intr, B.nc, B.uv.p, B.bear.p, B.ok.p, st);
   else launch_unproject(model, intr, B.nc, B.uv.p, B.xy.p, B.ok.p, st);
   PoseProblem Q; memset(&Q, 0, sizeof Q);
-  Q.model = model; for (int i = 0; i < 10; ++i) Q.intr[i] = intr[i];
+  Q.model = model; for (int i = 0; i < MAX_INTR; ++i) Q.intr[i] = intr[i];
   Q.n_frames = B.nf; Q.n_points = B.np; Q.min_points = min_points > 0 ? min_points : 8;
   Q.board = B.board.p; Q.f_off = B.off.p; Q.pid = B.pid.p;
   const double max_px = max_reproj_error > 0.0 ? max_reproj_error : 0.004 * H;            // pose_estimator.cc:97
@@ -732,7 +732,7 @@ static PoseProblem unproject_corners(cudaStream_t st, int model, const double in
   return Q;
 }
 
-icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err) {
+icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int n, const double* uv, double* xy_out, int32_t* ok, std::string& err) {
   DevBuf<double2> d_uv, d_xy; DevBuf<int> d_ok;
   CU(d_uv.upload(uv, n, st)); CU(d_xy.alloc(n)); CU(d_ok.alloc(n));
   launch_unproject(model, intr, n, d_uv.p, d_xy.p, d_ok.p, st);
@@ -742,7 +742,7 @@ icc_status pixels_to_normalized(cudaStream_t st, int model, const double intr[10
   return ICC_OK;
 }
 
-icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[10], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err) {
+icc_status pixels_to_bearings(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int n, const double* uv, double* xyz_out, int32_t* ok, std::string& err) {
   DevBuf<double2> d_uv; DevBuf<double4> d_b; DevBuf<int> d_ok;
   CU(d_uv.upload(uv, n, st)); CU(d_b.alloc(n)); CU(d_ok.alloc(n));
   launch_bearings(model, intr, n, d_uv.p, d_b.p, d_ok.p, st);
@@ -808,7 +808,7 @@ static icc_status rs_read(cudaStream_t st, int nf, RsState& R, const PoseShutter
   return ICC_OK;
 }
 
-icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off,
+icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int W, int H, int np, const double* points, int nf, const int32_t* off,
                                 const int32_t* ids, const double* uv, double max_reproj_error, int min_points, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc, double* mean_err,
                                 int32_t* valid, std::string& err) {
   BoardViews B;
@@ -828,7 +828,7 @@ icc_status estimate_board_poses(cudaStream_t st, int model, const double intr[10
   return ICC_OK;
 }
 
-icc_status optimize_board_points(cudaStream_t st, int model, const double intr[10], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
+icc_status optimize_board_points(cudaStream_t st, int model, const double intr[ICC_MAX_INTRINSICS], int W, int H, int np, const double* points, int nf, const int32_t* off, const int32_t* ids,
                                  const double* uv, double max_reproj_error, int min_points, int min_observations, int pose_error, const PoseShutter& shutter, double* q_wc, double* p_wc,
                                  double* mean_err, int32_t* valid, std::vector<double>& points_out, int32_t* n_opt_out, std::string& err) {
   BoardViews B;
@@ -856,7 +856,7 @@ icc_status optimize_board_points(cudaStream_t st, int model, const double intr[1
   DevBuf<double> d_qcw, d_c; DevBuf<double4> d_board2;
   CU(d_qcw.upload(qh)); CU(d_c.upload(ph));
   PointProblem PQ; memset(&PQ, 0, sizeof PQ);
-  PQ.model = model; for (int i = 0; i < 10; ++i) PQ.intr[i] = intr[i];
+  PQ.model = model; for (int i = 0; i < MAX_INTR; ++i) PQ.intr[i] = intr[i];
   PQ.normalized = 1; PQ.n_points = np; PQ.min_obs = min_observations > 0 ? min_observations : 30; PQ.huber = 1.345;
   PQ.board_in = B.board.p; PQ.meas = B.xy.p; PQ.q_cw = d_qcw.p; PQ.cam_c = d_c.p;
   int n_opt = 0;

@@ -44,9 +44,10 @@ ICC_HD bool rs_pose_residual(double4 b, Q4 q, V3 t, V3 X, const RsMotion& m, dou
 //   r = project(model, k, P(tau)) - uv.
 // With J0 / J1 (nullable) the 2x6 rows for the right increment R_cw exp(delta) and the camera centre c, the columns of camcal_accumulate_kernel:
 // (d x (R_cw^T A^T a), -(R_cw^T A^T a)), with a0, a1 the rows of the projection's 2x3 Jacobian at P(tau) and d = X - c.  With Jk0 / Jk1
-// (nullable) the 2x10 intrinsic rows d(u,v)/dk in Theia's order (zero beyond the model's parameters).  Returns the projection's ok flag.
+// (nullable) the intrinsic rows d(u,v)/dk in Theia's order, max(10, camera_num_params(model)) entries each (zero beyond the model's
+// parameters).  Returns the projection's ok flag.
 ICC_HD bool rs_camera_residual(int model, const double* k, Q4 q, V3 c, V3 X, const RsMotion& m, double tau, double2 uv, double& r0, double& r1,
-                               double J0[6], double J1[6], double Jk0[10], double Jk1[10]) {
+                               double J0[6], double J1[6], double* Jk0, double* Jk1) {
   const Q4 A = rs_rotation(m, tau);
   const V3 d = X - c;
   const V3 P = rs_point(A, m, tau, qrot(q, d));
@@ -60,7 +61,7 @@ ICC_HD bool rs_camera_residual(int model, const double* k, Q4 q, V3 c, V3 X, con
     J1[0] = b1.x; J1[1] = b1.y; J1[2] = b1.z; J1[3] = -t1.x; J1[4] = -t1.y; J1[5] = -t1.z;
   }
   if (Jk0)
-    for (int i = 0; i < 10; ++i) { Jk0[i] = pk.Jk[i]; Jk1[i] = pk.Jk[10 + i]; }
+    for (int i = 0; i < 10 || i < camera_num_params(model); ++i) { Jk0[i] = pk.Jk[jk_at(0, i)]; Jk1[i] = pk.Jk[jk_at(1, i)]; }
   return pr.ok;
 }
 

@@ -31,7 +31,7 @@ struct FrameWin {
   double u_so3, u_r3;     // normalised knot times of the frame (CalcTimes, impl.h:763-788)
 };
 struct VisConst {
-  double intr[10];
+  double intr[MAX_INTR];
   M3 Ric;                 // rotation matrix of T_i_c
   V3 tic;
   double ld;              // line delay

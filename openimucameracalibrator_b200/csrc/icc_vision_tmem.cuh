@@ -111,7 +111,7 @@ ICC_D void tile_part(const NeLayout& L, double* __restrict__ tile, int k0, int k
 
 // shared-memory constants of the vision items (written once per CTA)
 ICC_D void init_const(VisConst* K, const DeviceProblem& P, const DeviceState& S, int model) {
-  if (threadIdx.x < 10) K->intr[threadIdx.x] = S.glob[G_CAM_INTR + threadIdx.x];
+  if (threadIdx.x < MAX_INTR) K->intr[threadIdx.x] = S.glob[G_CAM_INTR + threadIdx.x];
   if (threadIdx.x == 32) {
     const Q4 q_ic = q4(S.glob[G_TIC + 0], S.glob[G_TIC + 1], S.glob[G_TIC + 2], S.glob[G_TIC + 3]);
     K->Ric = qmat(q_ic); K->tic = v3(S.glob[G_TIC + 4], S.glob[G_TIC + 5], S.glob[G_TIC + 6]);

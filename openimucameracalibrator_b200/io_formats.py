@@ -117,6 +117,9 @@ _INTR_KEYS = {
     cm.EXTENDED_UNIFIED: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], alpha=k[5], beta=k[6]),
     cm.SCARAMUZZA: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=0.0, principal_pt_x=k[3], principal_pt_y=k[4], stretch_d=k[8], stretch_e=k[2],
                                   polynomial_a2=k[5], polynomial_a3=k[6], polynomial_a4=k[7]),
+    cm.PINHOLE_RATIONAL: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], radial_distortion_1=k[5],
+                                        radial_distortion_2=k[6], radial_distortion_3=k[7], tangential_distortion_1=k[8], tangential_distortion_2=k[9],
+                                        radial_distortion_4=k[10], radial_distortion_5=k[11], radial_distortion_6=k[12]),
     cm.OMNI_RADIAL_TANGENTIAL: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], xi=k[5], radial_distortion_1=k[6],
                                               radial_distortion_2=k[7], tangential_distortion_1=k[8], tangential_distortion_2=k[9]),
 }
