@@ -213,7 +213,7 @@ class CameraCalibrator:
         """scene_json: the corner file as a dictionary (io_formats.ubjson_loads of extract_board_to_json's output).  Writes
         `<output_path>.json` in the layout of io::write_camera_calibration when output_path is given."""
         import json
-        from . import camera_models as cm
+        from .io_formats import intrinsics_dict
         pts = scene_json["scene_pts"]
         n = max(int(i) for i in pts) + 1
         board = np.zeros((n, 4)); board[:, 3] = 1.0
@@ -240,20 +240,8 @@ class CameraCalibrator:
         if not s["success"]:
             return False
         if output_path:
-            k = self.result["intrinsics"]
-            noskew = self.model in (cm.FOV, cm.DIVISION_UNDISTORTION)
-            intr = {"skew": 0.0, "principal_pt_x": k[2] if noskew else k[3], "principal_pt_y": k[3] if noskew else k[4], "aspect_ratio": k[1], "focal_length": k[0]}
-            extra = {cm.DIVISION_UNDISTORTION: {"div_undist_distortion": 4}, cm.DOUBLE_SPHERE: {"xi": 5, "alpha": 6}, cm.EXTENDED_UNIFIED: {"alpha": 5, "beta": 6},
-                     cm.FISHEYE: {f"radial_distortion_{i + 1}": 5 + i for i in range(4)}, cm.FOV: {"radial_distortion_1": 4},
-                     cm.PINHOLE_RADIAL_TANGENTIAL: {"radial_distortion_1": 5, "radial_distortion_2": 6, "radial_distortion_3": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9},
-                     cm.OMNI_RADIAL_TANGENTIAL: {"xi": 5, "radial_distortion_1": 6, "radial_distortion_2": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9},
-                     cm.SCARAMUZZA: {"stretch_d": 8, "stretch_e": 2, "polynomial_a2": 5, "polynomial_a3": 6, "polynomial_a4": 7},
-                     cm.PINHOLE_RATIONAL: {"radial_distortion_1": 5, "radial_distortion_2": 6, "radial_distortion_3": 7, "tangential_distortion_1": 8, "tangential_distortion_2": 9,
-                                           "radial_distortion_4": 10, "radial_distortion_5": 11, "radial_distortion_6": 12}}
-            for name, idx in extra.get(self.model, {}).items():
-                intr[name] = k[idx]
             doc = {"stabelized": False, "fps": scene_json["camera_fps"], "nr_calib_images": s["n_views_used"], "final_reproj_error": s["final_reproj_error"],
-                   "image_width": W, "image_height": H, "intrinsic_type": self.camera_model, "intrinsics": {a: float(b) for a, b in intr.items()}}
+                   "image_width": W, "image_height": H, "intrinsic_type": self.camera_model, "intrinsics": intrinsics_dict(self.model, self.result["intrinsics"])}
             with open(output_path + ".json", "w") as f:
                 json.dump(doc, f, indent=2)
         return True
@@ -261,23 +249,10 @@ class CameraCalibrator:
     def PrintResult(self):
         from . import camera_models as cm
         k = self.result["intrinsics"]
-        noskew = self.model in (cm.FOV, cm.DIVISION_UNDISTORTION)
-        print(f"Focal Length:{k[0]}px Principal Point: {k[2] if noskew else k[3]}/{k[3] if noskew else k[4]}px.")
-        if self.model == cm.DIVISION_UNDISTORTION:
-            print(f"DIVISION_UNDISTORTION model: Distortion: {k[4]}")
-        elif self.model == cm.DOUBLE_SPHERE:
-            print(f"DOUBLE_SPHERE model: XI: {k[5]} ALPHA: {k[6]}")
-        elif self.model == cm.EXTENDED_UNIFIED:
-            print(f"EXTENDED_UNIFIED model: {k[5]} BETA: {k[6]}")
-        elif self.model == cm.OMNI_RADIAL_TANGENTIAL:
-            print(f"OMNI_RADIAL_TANGENTIAL model: XI: {k[5]} Radial distortion 1: {k[6]} Radial distortion 2: {k[7]} Tangential distortion 1: {k[8]} Tangential distortion 2: {k[9]}")
-        elif self.model == cm.PINHOLE_RATIONAL:
-            print("PINHOLE_RATIONAL model: " + " ".join(f"Radial distortion {i + 1}: {k[(5, 6, 7, 10, 11, 12)[i]]}" for i in range(6))
-                  + f" Tangential distortion 1: {k[8]} Tangential distortion 2: {k[9]}")
-        elif self.model == cm.SCARAMUZZA:
-            print(f"SCARAMUZZA model: A2: {k[5]} A3: {k[6]} A4: {k[7]} Stretch c: {k[1]} d: {k[8]} e: {k[2]}")
-        elif self.model == cm.FISHEYE:
-            print("FISHEYE model: " + " ".join(f"Radial distortion {i + 1}: {k[5 + i]}" for i in range(4)))
+        cam = cm.CAMERAS[self.model]
+        print(f"Focal Length:{k[0]}px Principal Point: {k[cam.keys['principal_pt_x']]}/{k[cam.keys['principal_pt_y']]}px.")
+        if cam.printed:
+            print(f"{cam.name} model: " + " ".join(f"{label}: {k[i]}" if label else f"{k[i]}" for label, i in cam.printed.items()))
 
 
 class StaticImuCalibrator:

@@ -7,6 +7,8 @@ values; JSON names follow src/io/read_camera_calibration.cc:59-116.
 """
 from __future__ import annotations
 
+from typing import NamedTuple
+
 import numpy as np
 
 PINHOLE, PINHOLE_RADIAL_TANGENTIAL, FISHEYE, FOV, DIVISION_UNDISTORTION, DOUBLE_SPHERE, EXTENDED_UNIFIED = range(7)
@@ -14,21 +16,43 @@ OMNI_RADIAL_TANGENTIAL = 7   # extension without a Theia counterpart: Kalibr's o
 SCARAMUZZA = 8               # extension without a Theia counterpart: Scaramuzza's omnidirectional polynomial model (OCamCalib)
 PINHOLE_RATIONAL = 9         # extension without a Theia counterpart: OpenCV's rational polynomial model (k1..k6, p1, p2)
 
-MODEL_NAMES = {
-    PINHOLE: "PINHOLE",
-    PINHOLE_RADIAL_TANGENTIAL: "PINHOLE_RADIAL_TANGENTIAL",
-    FISHEYE: "FISHEYE",
-    FOV: "FOV",
-    DIVISION_UNDISTORTION: "DIVISION_UNDISTORTION",
-    DOUBLE_SPHERE: "DOUBLE_SPHERE",
-    EXTENDED_UNIFIED: "EXTENDED_UNIFIED",
-    OMNI_RADIAL_TANGENTIAL: "OMNI_RADIAL_TANGENTIAL",
-    SCARAMUZZA: "SCARAMUZZA",
-    PINHOLE_RATIONAL: "PINHOLE_RATIONAL",
-}
-MODEL_IDS = {v: k for k, v in MODEL_NAMES.items()}
-NUM_PARAMS = {PINHOLE: 7, PINHOLE_RADIAL_TANGENTIAL: 10, FISHEYE: 9, FOV: 5, DIVISION_UNDISTORTION: 5,
-              DOUBLE_SPHERE: 7, EXTENDED_UNIFIED: 7, OMNI_RADIAL_TANGENTIAL: 10, SCARAMUZZA: 9, PINHOLE_RATIONAL: 13}
+
+class CameraLayout(NamedTuple):
+    """One camera model in the camera JSON and the tools' printed summary.  The same table, row for row, is kCameraLayouts in
+    csrc/icc_cli_common.hpp."""
+    name: str          # `intrinsic_type`
+    id: int            # ICC_CAM_* / theia::CameraIntrinsicsModelType
+    num_params: int
+    keys: dict         # JSON key -> Theia index of every intrinsic the file carries, in file order; `skew` only where index 2 is the skew
+    printed: dict      # label -> index of the model's PrintResult line, "" for an unlabelled value; empty when the tools print none
+
+
+_AFFINE = {"focal_length": 0, "aspect_ratio": 1, "skew": 2, "principal_pt_x": 3, "principal_pt_y": 4}
+_AFFINE_NOSKEW = {"focal_length": 0, "aspect_ratio": 1, "principal_pt_x": 2, "principal_pt_y": 3}
+CAMERAS = {c.id: c for c in (
+    CameraLayout("PINHOLE", PINHOLE, 7, _AFFINE, {}),
+    CameraLayout("PINHOLE_RADIAL_TANGENTIAL", PINHOLE_RADIAL_TANGENTIAL, 10,
+                 dict(_AFFINE, radial_distortion_1=5, radial_distortion_2=6, radial_distortion_3=7, tangential_distortion_1=8, tangential_distortion_2=9), {}),
+    CameraLayout("FISHEYE", FISHEYE, 9, dict(_AFFINE, radial_distortion_1=5, radial_distortion_2=6, radial_distortion_3=7, radial_distortion_4=8),
+                 {"Radial distortion 1": 5, "Radial distortion 2": 6, "Radial distortion 3": 7, "Radial distortion 4": 8}),
+    CameraLayout("FOV", FOV, 5, dict(_AFFINE_NOSKEW, radial_distortion_1=4), {}),
+    CameraLayout("DIVISION_UNDISTORTION", DIVISION_UNDISTORTION, 5, dict(_AFFINE_NOSKEW, div_undist_distortion=4), {"Distortion": 4}),
+    CameraLayout("DOUBLE_SPHERE", DOUBLE_SPHERE, 7, dict(_AFFINE, xi=5, alpha=6), {"XI": 5, "ALPHA": 6}),
+    CameraLayout("EXTENDED_UNIFIED", EXTENDED_UNIFIED, 7, dict(_AFFINE, alpha=5, beta=6), {"": 5, "BETA": 6}),
+    CameraLayout("OMNI_RADIAL_TANGENTIAL", OMNI_RADIAL_TANGENTIAL, 10,
+                 dict(_AFFINE, xi=5, radial_distortion_1=6, radial_distortion_2=7, tangential_distortion_1=8, tangential_distortion_2=9),
+                 {"XI": 5, "Radial distortion 1": 6, "Radial distortion 2": 7, "Tangential distortion 1": 8, "Tangential distortion 2": 9}),
+    CameraLayout("SCARAMUZZA", SCARAMUZZA, 9,   # index 2 is the stretch e, not a skew
+                 dict(focal_length=0, aspect_ratio=1, principal_pt_x=3, principal_pt_y=4, stretch_d=8, stretch_e=2, polynomial_a2=5, polynomial_a3=6, polynomial_a4=7),
+                 {"A2": 5, "A3": 6, "A4": 7, "Stretch c": 1, "d": 8, "e": 2}),
+    CameraLayout("PINHOLE_RATIONAL", PINHOLE_RATIONAL, 13, dict(_AFFINE, radial_distortion_1=5, radial_distortion_2=6, radial_distortion_3=7, tangential_distortion_1=8,
+                                                                tangential_distortion_2=9, radial_distortion_4=10, radial_distortion_5=11, radial_distortion_6=12),
+                 {"Radial distortion 1": 5, "Radial distortion 2": 6, "Radial distortion 3": 7, "Radial distortion 4": 10, "Radial distortion 5": 11,
+                  "Radial distortion 6": 12, "Tangential distortion 1": 8, "Tangential distortion 2": 9}),
+)}
+MODEL_NAMES = {m: c.name for m, c in CAMERAS.items()}
+MODEL_IDS = {c.name: m for m, c in CAMERAS.items()}
+NUM_PARAMS = {m: c.num_params for m, c in CAMERAS.items()}
 MAX_INTRINSICS = 13   # ICC_MAX_INTRINSICS: the longest intrinsic vector
 
 

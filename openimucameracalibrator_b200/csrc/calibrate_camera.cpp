@@ -22,22 +22,6 @@
 
 using iccjson::Value;
 
-namespace {
-int model_from_string(const std::string& s) {   // theia::StringToCameraIntrinsicsModelType for the names the app documents (:27-31)
-  if (s == "PINHOLE") return ICC_CAM_PINHOLE;
-  if (s == "PINHOLE_RADIAL_TANGENTIAL") return ICC_CAM_PINHOLE_RADIAL_TANGENTIAL;
-  if (s == "DIVISION_UNDISTORTION") return ICC_CAM_DIVISION_UNDISTORTION;
-  if (s == "DOUBLE_SPHERE") return ICC_CAM_DOUBLE_SPHERE;
-  if (s == "EXTENDED_UNIFIED") return ICC_CAM_EXTENDED_UNIFIED;
-  if (s == "FISHEYE") return ICC_CAM_FISHEYE;
-  if (s == "FOV") return ICC_CAM_FOV;
-  if (s == "OMNI_RADIAL_TANGENTIAL") return ICC_CAM_OMNI_RADIAL_TANGENTIAL;   // extension: Kalibr's omni-radtan
-  if (s == "SCARAMUZZA") return ICC_CAM_SCARAMUZZA;                           // extension: Scaramuzza's omnidirectional model (OCamCalib)
-  if (s == "PINHOLE_RATIONAL") return ICC_CAM_PINHOLE_RATIONAL;               // extension: OpenCV's rational polynomial model
-  return -1;
-}
-}  // namespace
-
 int main(int argc, char** argv) {
   icccli::Flags F;
   F.str = {{"input_corners", ""}, {"camera_model_to_calibrate", "DOUBLE_SPHERE"}, {"save_path_calib_dataset", ""}, {"pose_shutter", "global"}};
@@ -49,8 +33,9 @@ int main(int argc, char** argv) {
     Value scene_json; icccli::SceneViews sv;
     try { scene_json = icccli::load_scene(F.str["input_corners"], sv); } catch (const std::exception& e) { std::cerr << "Check failed: Failed to load " << F.str["input_corners"] << ": " << e.what() << std::endl; return 1; }
     const std::string model_name = F.str["camera_model_to_calibrate"];
-    const int model = model_from_string(model_name);
-    if (model < 0) { std::cerr << "ERROR: unknown camera model '" << model_name << "'" << std::endl; return 1; }
+    const icccli::CameraLayout* cam = icccli::find_camera(model_name);
+    if (!cam) { std::cerr << "ERROR: unknown camera model '" << model_name << "'" << std::endl; return 1; }
+    const int model = cam->id;
     const int width = (int)scene_json.at("image_width").num(), height = (int)scene_json.at("image_height").num();
     const double fps = scene_json.at("camera_fps").num();
     int np = 0;
@@ -85,33 +70,14 @@ int main(int argc, char** argv) {
     if (opt.optimize_board_points && S.success) std::cout << "Optimized " << S.n_points_optimized << " board points.\n";
     if (!S.success) { std::cerr << "Not enough views for proper calibration!\nCalibration failed.\n"; return 3; }
     std::cout << "Final camera calibration reprojection error: " << S.final_reproj_error << " from " << S.n_views_used << " view." << std::endl;
-    const bool noskew = model == ICC_CAM_FOV || model == ICC_CAM_DIVISION_UNDISTORTION;
-    const double cx = noskew ? intr[2] : intr[3], cy = noskew ? intr[3] : intr[4];
     const std::string out = F.str["save_path_calib_dataset"];
     if (!out.empty()) {
       // io::write_camera_calibration (src/io/write_camera_calibration.cc:33-133)
-      Value j = Value::object(), in = Value::object();
+      Value j = Value::object();
       j["stabelized"] = Value(false); j["fps"] = Value(fps); j["nr_calib_images"] = Value((int64_t)S.n_views_used); j["final_reproj_error"] = Value(S.final_reproj_error);
       j["image_width"] = Value((int64_t)width); j["image_height"] = Value((int64_t)height);   // integers, like io::write_camera_calibration
       j["intrinsic_type"] = Value(model_name);
-      in["skew"] = Value(0.0); in["principal_pt_x"] = Value(cx); in["principal_pt_y"] = Value(cy); in["aspect_ratio"] = Value(intr[1]); in["focal_length"] = Value(intr[0]);
-      switch (model) {
-        case ICC_CAM_DIVISION_UNDISTORTION: in["div_undist_distortion"] = Value(intr[4]); break;
-        case ICC_CAM_DOUBLE_SPHERE: in["xi"] = Value(intr[5]); in["alpha"] = Value(intr[6]); break;
-        case ICC_CAM_EXTENDED_UNIFIED: in["alpha"] = Value(intr[5]); in["beta"] = Value(intr[6]); break;
-        case ICC_CAM_FISHEYE: for (int i = 0; i < 4; ++i) in["radial_distortion_" + std::to_string(i + 1)] = Value(intr[5 + i]); break;
-        case ICC_CAM_PINHOLE_RADIAL_TANGENTIAL: for (int i = 0; i < 3; ++i) in["radial_distortion_" + std::to_string(i + 1)] = Value(intr[5 + i]);
-                                                in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
-        case ICC_CAM_FOV: in["radial_distortion_1"] = Value(intr[4]); break;   // extension: the layout this repository's readers use for FOV
-        case ICC_CAM_OMNI_RADIAL_TANGENTIAL: in["xi"] = Value(intr[5]); in["radial_distortion_1"] = Value(intr[6]); in["radial_distortion_2"] = Value(intr[7]);
-                                             in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
-        case ICC_CAM_SCARAMUZZA: in["stretch_e"] = Value(intr[2]); in["stretch_d"] = Value(intr[8]);   // `skew` stays 0: the stretch is e, d
-                                 in["polynomial_a2"] = Value(intr[5]); in["polynomial_a3"] = Value(intr[6]); in["polynomial_a4"] = Value(intr[7]); break;
-        case ICC_CAM_PINHOLE_RATIONAL: for (int i = 0; i < 3; ++i) { in["radial_distortion_" + std::to_string(i + 1)] = Value(intr[5 + i]); in["radial_distortion_" + std::to_string(i + 4)] = Value(intr[10 + i]); }
-                                       in["tangential_distortion_1"] = Value(intr[8]); in["tangential_distortion_2"] = Value(intr[9]); break;
-        default: break;
-      }
-      j["intrinsics"] = in;
+      j["intrinsics"] = icccli::write_intrinsics(*cam, intr.data());
       std::ofstream f(out + ".json");
       if (!f.is_open()) { std::cerr << "Could not open: " << out << ".json\nCheck failed: Could not write calibration file.\n"; return 1; }
       f << iccjson::dump(j, 2) << std::endl;
@@ -139,18 +105,7 @@ int main(int argc, char** argv) {
       for (int i = 0; i < np; ++i) { const double w = board_out[4 * i + 3]; ply << board_out[4 * i] / w << " " << board_out[4 * i + 1] / w << " " << board_out[4 * i + 2] / w << " 255 255 255\n"; }
     }
     // CameraCalibrator::PrintResult (:391-458)
-    std::cout << "Focal Length:" << intr[0] << "px Principal Point: " << cx << "/" << cy << "px.\n";
-    if (model == ICC_CAM_DIVISION_UNDISTORTION) std::cout << "DIVISION_UNDISTORTION model: Distortion: " << intr[4] << "\n";
-    else if (model == ICC_CAM_DOUBLE_SPHERE) std::cout << "DOUBLE_SPHERE model: XI: " << intr[5] << " ALPHA: " << intr[6] << "\n";
-    else if (model == ICC_CAM_EXTENDED_UNIFIED) std::cout << "EXTENDED_UNIFIED model: " << intr[5] << " BETA: " << intr[6] << "\n";
-    else if (model == ICC_CAM_OMNI_RADIAL_TANGENTIAL) std::cout << "OMNI_RADIAL_TANGENTIAL model: XI: " << intr[5] << " Radial distortion 1: " << intr[6] << " Radial distortion 2: " << intr[7]
-                                                                << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
-    else if (model == ICC_CAM_PINHOLE_RATIONAL) std::cout << "PINHOLE_RATIONAL model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7]
-                                                          << " Radial distortion 4: " << intr[10] << " Radial distortion 5: " << intr[11] << " Radial distortion 6: " << intr[12]
-                                                          << " Tangential distortion 1: " << intr[8] << " Tangential distortion 2: " << intr[9] << "\n";
-    else if (model == ICC_CAM_SCARAMUZZA) std::cout << "SCARAMUZZA model: A2: " << intr[5] << " A3: " << intr[6] << " A4: " << intr[7] << " Stretch c: " << intr[1]
-                                                    << " d: " << intr[8] << " e: " << intr[2] << "\n";
-    else if (model == ICC_CAM_FISHEYE) std::cout << "FISHEYE model: Radial distortion 1: " << intr[5] << " Radial distortion 2: " << intr[6] << " Radial distortion 3: " << intr[7] << " Radial distortion 4: " << intr[8] << "\n";
+    icccli::print_camera(std::cout, *cam, intr.data());
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
   return 0;
 }

@@ -7,8 +7,10 @@
 #include <algorithm>
 #include <cstdint>
 #include <map>
+#include <ostream>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace icccli {
@@ -68,28 +70,82 @@ inline void parse_flags(int argc, char** argv, Flags& f) {
 }
 
 
-inline // src/io/read_camera_calibration.cc:35-119 -> (model id, Theia-ordered intrinsics).  Like the reference, `skew` is never read.
-int read_camera(const Value& j, std::vector<double>& k, int& width, int& height, double& fps) {
+// The camera JSON (src/io/read_camera_calibration.cc:35-119, src/io/write_camera_calibration.cc:33-133) and the model line of
+// CameraCalibrator::PrintResult (src/core/camera_calibrator.cc:391-458), one row per model.  The same table, row for row, is CAMERAS in
+// openimucameracalibrator_b200/camera_models.py.
+using CameraKeys = std::vector<std::pair<std::string, int>>;
+struct CameraLayout {
+  std::string name;     // `intrinsic_type`, --camera_model_to_calibrate
+  int id, num_params;
+  CameraKeys keys;      // (JSON key, Theia index) of every intrinsic the file carries; `skew` only where index 2 is the skew
+  CameraKeys printed;   // (label, index) of the model's PrintResult line, "" for an unlabelled value; empty when the tools print none
+  int index(const std::string& key) const { for (const auto& [k, i] : keys) if (k == key) return i; throw std::runtime_error("no intrinsic " + key); }
+};
+inline CameraKeys affine_keys(bool skew, CameraKeys own) {   // focal length, aspect ratio, [skew,] principal point, then the model's own keys
+  CameraKeys k = skew ? CameraKeys{{"focal_length", 0}, {"aspect_ratio", 1}, {"skew", 2}, {"principal_pt_x", 3}, {"principal_pt_y", 4}}
+                      : CameraKeys{{"focal_length", 0}, {"aspect_ratio", 1}, {"principal_pt_x", 2}, {"principal_pt_y", 3}};
+  k.insert(k.end(), own.begin(), own.end());
+  return k;
+}
+inline const std::vector<CameraLayout> kCameraLayouts = {
+  {"PINHOLE", ICC_CAM_PINHOLE, 7, affine_keys(true, {}), {}},
+  {"PINHOLE_RADIAL_TANGENTIAL", ICC_CAM_PINHOLE_RADIAL_TANGENTIAL, 10,
+   affine_keys(true, {{"radial_distortion_1", 5}, {"radial_distortion_2", 6}, {"radial_distortion_3", 7}, {"tangential_distortion_1", 8}, {"tangential_distortion_2", 9}}), {}},
+  {"FISHEYE", ICC_CAM_FISHEYE, 9, affine_keys(true, {{"radial_distortion_1", 5}, {"radial_distortion_2", 6}, {"radial_distortion_3", 7}, {"radial_distortion_4", 8}}),
+   {{"Radial distortion 1", 5}, {"Radial distortion 2", 6}, {"Radial distortion 3", 7}, {"Radial distortion 4", 8}}},
+  {"FOV", ICC_CAM_FOV, 5, affine_keys(false, {{"radial_distortion_1", 4}}), {}},
+  {"DIVISION_UNDISTORTION", ICC_CAM_DIVISION_UNDISTORTION, 5, affine_keys(false, {{"div_undist_distortion", 4}}), {{"Distortion", 4}}},
+  {"DOUBLE_SPHERE", ICC_CAM_DOUBLE_SPHERE, 7, affine_keys(true, {{"xi", 5}, {"alpha", 6}}), {{"XI", 5}, {"ALPHA", 6}}},
+  {"EXTENDED_UNIFIED", ICC_CAM_EXTENDED_UNIFIED, 7, affine_keys(true, {{"alpha", 5}, {"beta", 6}}), {{"", 5}, {"BETA", 6}}},
+  {"OMNI_RADIAL_TANGENTIAL", ICC_CAM_OMNI_RADIAL_TANGENTIAL, 10,
+   affine_keys(true, {{"xi", 5}, {"radial_distortion_1", 6}, {"radial_distortion_2", 7}, {"tangential_distortion_1", 8}, {"tangential_distortion_2", 9}}),
+   {{"XI", 5}, {"Radial distortion 1", 6}, {"Radial distortion 2", 7}, {"Tangential distortion 1", 8}, {"Tangential distortion 2", 9}}},
+  {"SCARAMUZZA", ICC_CAM_SCARAMUZZA, 9,   // index 2 is the stretch e, not a skew
+   {{"focal_length", 0}, {"aspect_ratio", 1}, {"principal_pt_x", 3}, {"principal_pt_y", 4}, {"stretch_d", 8}, {"stretch_e", 2}, {"polynomial_a2", 5}, {"polynomial_a3", 6}, {"polynomial_a4", 7}},
+   {{"A2", 5}, {"A3", 6}, {"A4", 7}, {"Stretch c", 1}, {"d", 8}, {"e", 2}}},
+  {"PINHOLE_RATIONAL", ICC_CAM_PINHOLE_RATIONAL, 13,
+   affine_keys(true, {{"radial_distortion_1", 5}, {"radial_distortion_2", 6}, {"radial_distortion_3", 7}, {"tangential_distortion_1", 8}, {"tangential_distortion_2", 9},
+                      {"radial_distortion_4", 10}, {"radial_distortion_5", 11}, {"radial_distortion_6", 12}}),
+   {{"Radial distortion 1", 5}, {"Radial distortion 2", 6}, {"Radial distortion 3", 7}, {"Radial distortion 4", 10}, {"Radial distortion 5", 11}, {"Radial distortion 6", 12},
+    {"Tangential distortion 1", 8}, {"Tangential distortion 2", 9}}},
+};
+
+// theia::StringToCameraIntrinsicsModelType: the row of a model name, nullptr for an unknown one
+inline const CameraLayout* find_camera(const std::string& name) {
+  for (const CameraLayout& c : kCameraLayouts) if (c.name == name) return &c;
+  return nullptr;
+}
+
+// camera JSON -> (model id, Theia-ordered intrinsics).  Like the reference, `skew` is never read; FOV's aspect_ratio may be absent (1.0).
+inline int read_camera(const Value& j, std::vector<double>& k, int& width, int& height, double& fps) {
   const std::string type = j.at("intrinsic_type").str();
   const Value& in = j.at("intrinsics");
   width = (int)j.at("image_width").num(); height = (int)j.at("image_height").num(); fps = j.at("fps").num();
-  const double f = in.at("focal_length").num(), cx = in.at("principal_pt_x").num(), cy = in.at("principal_pt_y").num();
-  auto ar = [&]() { return in.at("aspect_ratio").num(); };
-  if (type == "DIVISION_UNDISTORTION") { k = {f, ar(), cx, cy, in.at("div_undist_distortion").num()}; return ICC_CAM_DIVISION_UNDISTORTION; }
-  if (type == "DOUBLE_SPHERE") { k = {f, ar(), 0.0, cx, cy, in.at("xi").num(), in.at("alpha").num()}; return ICC_CAM_DOUBLE_SPHERE; }
-  if (type == "EXTENDED_UNIFIED") { k = {f, ar(), 0.0, cx, cy, in.at("alpha").num(), in.at("beta").num()}; return ICC_CAM_EXTENDED_UNIFIED; }
-  if (type == "FISHEYE") { k = {f, ar(), 0.0, cx, cy, in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("radial_distortion_3").num(), in.at("radial_distortion_4").num()}; return ICC_CAM_FISHEYE; }
-  if (type == "PINHOLE_RADIAL_TANGENTIAL") { k = {f, ar(), 0.0, cx, cy, in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("radial_distortion_3").num(), in.at("tangential_distortion_1").num(), in.at("tangential_distortion_2").num()}; return ICC_CAM_PINHOLE_RADIAL_TANGENTIAL; }
-  if (type == "PINHOLE") { k = {f, ar(), 0.0, cx, cy, 0.0, 0.0}; return ICC_CAM_PINHOLE; }
-  if (type == "OMNI_RADIAL_TANGENTIAL") { k = {f, ar(), 0.0, cx, cy, in.at("xi").num(), in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("tangential_distortion_1").num(), in.at("tangential_distortion_2").num()}; return ICC_CAM_OMNI_RADIAL_TANGENTIAL; }
-  if (type == "SCARAMUZZA") { k = {f, ar(), in.at("stretch_e").num(), cx, cy, in.at("polynomial_a2").num(), in.at("polynomial_a3").num(), in.at("polynomial_a4").num(), in.at("stretch_d").num()}; return ICC_CAM_SCARAMUZZA; }
-  if (type == "PINHOLE_RATIONAL") {   // extension: OpenCV's rational polynomial model, k1..k6 = radial_distortion_1..6, p1, p2 = tangential_distortion_1, 2
-    k = {f, ar(), 0.0, cx, cy, in.at("radial_distortion_1").num(), in.at("radial_distortion_2").num(), in.at("radial_distortion_3").num(), in.at("tangential_distortion_1").num(),
-         in.at("tangential_distortion_2").num(), in.at("radial_distortion_4").num(), in.at("radial_distortion_5").num(), in.at("radial_distortion_6").num()};
-    return ICC_CAM_PINHOLE_RATIONAL;
+  const CameraLayout* c = find_camera(type);
+  if (!c) throw std::runtime_error("unknown intrinsic_type " + type);
+  k.assign(c->num_params, 0.0);
+  for (const auto& [key, i] : c->keys) {
+    if (key == "skew") continue;
+    k[i] = c->id == ICC_CAM_FOV && key == "aspect_ratio" && !in.contains(key) ? 1.0 : in.at(key).num();
   }
-  if (type == "FOV") { k = {f, in.contains("aspect_ratio") ? ar() : 1.0, cx, cy, in.at("radial_distortion_1").num()}; return ICC_CAM_FOV; }
-  throw std::runtime_error("unknown intrinsic_type " + type);
+  return c->id;
+}
+
+// the `intrinsics` object of the camera JSON: every key of the layout, and `skew` 0 for the models whose index 2 is no skew
+inline Value write_intrinsics(const CameraLayout& c, const double* k) {
+  Value in = Value::object();
+  in["skew"] = Value(0.0);
+  for (const auto& [key, i] : c.keys) in[key] = Value(k[i]);
+  return in;
+}
+
+// CameraCalibrator::PrintResult: the focal length and principal point line, then the model's line if it has one
+inline void print_camera(std::ostream& os, const CameraLayout& c, const double* k) {
+  os << "Focal Length:" << k[0] << "px Principal Point: " << k[c.index("principal_pt_x")] << "/" << k[c.index("principal_pt_y")] << "px.\n";
+  if (c.printed.empty()) return;
+  os << c.name << " model:";
+  for (const auto& [label, i] : c.printed) os << " " << label << (label.empty() ? "" : ": ") << k[i];
+  os << "\n";
 }
 
 // Corner file (src/core/board_extractor.cc:294-296,325-333,375-380): scene_pts {"id": [x,y,z]} -> homogeneous board points by id.

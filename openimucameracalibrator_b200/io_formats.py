@@ -105,24 +105,12 @@ def ubjson_loads(data: bytes):
 
 
 # ---- dataset -> files -----------------------------------------------------------------------------------------------------
-_INTR_KEYS = {
-    cm.PINHOLE: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4]),
-    cm.PINHOLE_RADIAL_TANGENTIAL: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], radial_distortion_1=k[5],
-                                                 radial_distortion_2=k[6], radial_distortion_3=k[7], tangential_distortion_1=k[8], tangential_distortion_2=k[9]),
-    cm.FISHEYE: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], radial_distortion_1=k[5], radial_distortion_2=k[6],
-                               radial_distortion_3=k[7], radial_distortion_4=k[8]),
-    cm.FOV: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=0.0, principal_pt_x=k[2], principal_pt_y=k[3], radial_distortion_1=k[4]),
-    cm.DIVISION_UNDISTORTION: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=0.0, principal_pt_x=k[2], principal_pt_y=k[3], div_undist_distortion=k[4]),
-    cm.DOUBLE_SPHERE: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], xi=k[5], alpha=k[6]),
-    cm.EXTENDED_UNIFIED: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], alpha=k[5], beta=k[6]),
-    cm.SCARAMUZZA: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=0.0, principal_pt_x=k[3], principal_pt_y=k[4], stretch_d=k[8], stretch_e=k[2],
-                                  polynomial_a2=k[5], polynomial_a3=k[6], polynomial_a4=k[7]),
-    cm.PINHOLE_RATIONAL: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], radial_distortion_1=k[5],
-                                        radial_distortion_2=k[6], radial_distortion_3=k[7], tangential_distortion_1=k[8], tangential_distortion_2=k[9],
-                                        radial_distortion_4=k[10], radial_distortion_5=k[11], radial_distortion_6=k[12]),
-    cm.OMNI_RADIAL_TANGENTIAL: lambda k: dict(focal_length=k[0], aspect_ratio=k[1], skew=k[2], principal_pt_x=k[3], principal_pt_y=k[4], xi=k[5], radial_distortion_1=k[6],
-                                              radial_distortion_2=k[7], tangential_distortion_1=k[8], tangential_distortion_2=k[9]),
-}
+def intrinsics_dict(model: int, k) -> dict:
+    """The `intrinsics` object of the camera JSON for Theia-ordered intrinsics k: every key of the model's layout, and `skew` 0.0 for
+    the models whose index 2 is no skew (the readers never read `skew`)."""
+    intr = {key: float(k[i]) for key, i in cm.CAMERAS[model].keys.items()}
+    intr.setdefault("skew", 0.0)
+    return intr
 
 
 def view_key(t_s: float) -> str:
@@ -134,7 +122,6 @@ def write_dataset_files(ds: dict, out_dir: str) -> dict:
     """Write every input file of the hot CLI for a synthetic dataset; returns {flag name: path}."""
     os.makedirs(out_dir, exist_ok=True)
     W, H = ds["image_size"]
-    k = [float(v) for v in ds["intrinsics"]]
     paths = {}
     # corners (UBJSON)
     off, ids, uv = ds["corner_offsets"], ds["point_ids"], ds["uv"]
@@ -147,7 +134,7 @@ def write_dataset_files(ds: dict, out_dir: str) -> dict:
     with open(paths["input_corners"], "wb") as f:
         f.write(ubjson_dumps(scene))
     # camera calibration
-    cam = {"fps": float(ds["fps"]), "image_width": int(W), "image_height": int(H), "intrinsic_type": cm.MODEL_NAMES[ds["model"]], "intrinsics": _INTR_KEYS[ds["model"]](k)}
+    cam = {"fps": float(ds["fps"]), "image_width": int(W), "image_height": int(H), "intrinsic_type": cm.MODEL_NAMES[ds["model"]], "intrinsics": intrinsics_dict(ds["model"], ds["intrinsics"])}
     paths["camera_calibration_json"] = os.path.join(out_dir, "cam_calib.json")
     json.dump(cam, open(paths["camera_calibration_json"], "w"), indent=4)
     # telemetry (timestamps as integer nanoseconds like telemetry_converter.py)

@@ -60,7 +60,7 @@ def scaramuzza_intrinsics(ocam: dict) -> list:
 def camera_document(ocam: dict, fps: float) -> dict:
     k = scaramuzza_intrinsics(ocam)
     return {"fps": float(fps), "image_width": int(ocam["width"]), "image_height": int(ocam["height"]), "intrinsic_type": cm.MODEL_NAMES[cm.SCARAMUZZA],
-            "intrinsics": {a: float(b) for a, b in iof._INTR_KEYS[cm.SCARAMUZZA](k).items()}}
+            "intrinsics": iof.intrinsics_dict(cm.SCARAMUZZA, k)}
 
 
 def main(argv=None) -> dict:

@@ -150,7 +150,7 @@ def camera_document(doc: dict, fps: float, width=None, height=None) -> dict:
     if W is None or H is None:
         raise ValueError("the file gives no image size: pass --width and --height")
     return {"fps": float(fps), "image_width": int(W), "image_height": int(H), "intrinsic_type": cm.MODEL_NAMES[model],
-            "intrinsics": {a: float(b) for a, b in iof._INTR_KEYS[model](k).items()}}
+            "intrinsics": iof.intrinsics_dict(model, k)}
 
 
 def main(argv=None) -> dict:
