@@ -162,6 +162,21 @@ icc_status icc_set_imu(icc_handle* h, int n_samples, const double* timestamps_s,
 /* BatchInitSpline (imu_camera_calibrator.cc:21-124): spline time range, knot counts, knot initialisation, bias
  * splines, measurement wiring (CalcTimes impl.h:763-788), gravity initialisation; uploads everything to HBM. */
 icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* p);
+/* ---- bias splines (extension: the reference fixes InitBiasSplines(bias, bias, 10 s, 10 s, 1.0, 0.1), imu_camera_calibrator.cc:79-85) ----
+ * icc_set_bias_splines: knot spacing [s] of the accelerometer / gyroscope bias splines; a value <= 0 selects the reference's 10 s, and so does
+ * never calling it.  Knot counts stay duration / dt + 3.  icc_set_bias_random_walk: random-walk densities per axis in SI units, Kalibr's
+ * accelerometer_random_walk [m/s^3/sqrt(Hz)] and gyroscope_random_walk [rad/s^2/sqrt(Hz)]; NULL turns that sensor's prior off (the default).
+ * Both are read by the next icc_batch_init_spline.  A sensor with densities adds, per bias-spline segment s = 0 .. n-3, Gauss-Legendre node
+ * g = 0, 1 (u_g = 1/2 -+ 1/(2 sqrt 3)) and axis a, the residual r = sqrt(dt / 2) b'_a(u_g) / q_a, so that 1/2 sum r^2 is the Wiener-process
+ * negative log-likelihood 1/2 int |b'|^2 / q^2 dt of the whole spline.  The rows are part of the problem under every flag set (their cost
+ * always counts); they have columns where ACC_BIAS / GYR_BIAS / IMU_BIASES free the knots.  Residual order of icc_evaluate: [vision | accel |
+ * gyro | acc-bias prior | gyr-bias prior], segment-major, then node, then axis.  Under sharding only shard 0 holds the rows.  The bias box
+ * (|b| <= 1.0 / 0.1) is unchanged.  Free bias knots are border columns of the solver: too many give ICC_ERR_UNSUPPORTED from the solve.
+ * Non-finite, zero or negative densities, or a spacing that is not finite or outside [1 ns, 1e9 s]: ICC_ERR_INVALID_ARGUMENT.  Host state only. */
+icc_status icc_set_bias_splines(icc_handle* h, double acc_dt_s, double gyr_dt_s);
+icc_status icc_set_bias_random_walk(icc_handle* h, const double acc_q[3] /* nullable */, const double gyr_q[3] /* nullable */);
+/* prior rows of this shard's problem (0 without densities, and on shards other than 0) */
+icc_status icc_num_bias_prior_residuals(const icc_handle* h, int* n);
 /* SetKnownGravityDir (imu_camera_calibrator.cc:126-128) */
 icc_status icc_set_known_gravity_dir(icc_handle* h, const double g[3]);
 /* Residual sharding: keep only frames/IMU samples in shard `rank` of `world` (time-sliced, equal residual counts);
@@ -253,7 +268,7 @@ icc_status icc_num_tangent(const icc_handle* h, int flags, int* n);
 /* One evaluation at the current state.  Canonical tangent order: so3 knots (3 each), r3 knots (3 each), T_i_c (6: upsilon,
  * omega), gravity (3), line delay (1), acc-bias knots (3 each), gyr-bias knots (3 each), accelerometer intrinsics (6),
  * gyroscope intrinsics (9), camera intrinsics (model count), time-offset increment (1) — only blocks active under `flags`.
- * residuals: [vision 2/corner in frame order | accel 3/sample | gyro 3/sample].  hessian_dense: n x n row-major J^T J
+ * residuals: [vision 2/corner in frame order | accel 3/sample | gyro 3/sample | bias random-walk prior rows (icc_set_bias_random_walk)].  hessian_dense: n x n row-major J^T J
  * (small problems only).  Any output may be NULL. */
 icc_status icc_evaluate(icc_handle* h, int flags, double* cost, double* residuals, double* gradient, double* hessian_dense);
 /* Run exactly `n` LM iterations (no convergence test) from the current state; used by bench.py as the timed "step". */

@@ -568,8 +568,23 @@ class CApi:
     def num_tangent(self, flags):
         n = C.c_int(); self._call("num_tangent", [C.c_int, C.POINTER(C.c_int)], int(flags), C.byref(n)); return n.value
 
+    def set_bias_splines(self, acc_dt_s=0.0, gyr_dt_s=0.0):
+        """Knot spacing [s] of the accelerometer / gyroscope bias splines for the next batch_init_spline (<= 0: the reference's 10 s)."""
+        self._call("set_bias_splines", [C.c_double, C.c_double], float(acc_dt_s), float(gyr_dt_s))
+
+    def set_bias_random_walk(self, acc_q=None, gyr_q=None):
+        """Random-walk densities per axis (Kalibr's units: m/s^3/sqrt(Hz), rad/s^2/sqrt(Hz)) of the bias prior for the next
+        batch_init_spline; None turns that sensor's prior off."""
+        arrs = [None if q is None else _f64(np.broadcast_to(np.asarray(q, dtype=np.float64), (3,))) for q in (acc_q, gyr_q)]
+        self._call("set_bias_random_walk", [c_double_p, c_double_p], *[_dp(x) for x in arrs])
+
+    def num_bias_prior_residuals(self) -> int:
+        """Rows of the bias random-walk prior in this shard's problem (they follow the gyroscope rows of evaluate's residuals)."""
+        n = C.c_int(); self._call("num_bias_prior_residuals", [C.POINTER(C.c_int)], C.byref(n)); return n.value
+
     def evaluate(self, flags, residuals=True, gradient=True, hessian=False):
-        nres = sum(self.num_residuals()); n = self.num_tangent(flags)
+        nres = sum(self.num_residuals()) + (self.num_bias_prior_residuals() if hasattr(self.lib, self.prefix + "num_bias_prior_residuals") else 0)
+        n = self.num_tangent(flags)
         cost = C.c_double()
         r = np.zeros(nres) if residuals else None
         g = np.zeros(n) if gradient else None

@@ -87,6 +87,15 @@ class ImuCameraCalibrator:
         self.last_summary = self.api.optimize(iterations, int(optim_flags))
         return self.last_summary.mean_reproj_error
 
+    def SetBiasSplines(self, acc_dt_s: float, gyr_dt_s: float):
+        """Bias-spline knot spacing [s] for the next BatchInitSpline (<= 0: the reference's 10 s)."""
+        self.api.set_bias_splines(acc_dt_s, gyr_dt_s)
+
+    def SetBiasRandomWalk(self, acc_q, gyr_q):
+        """Random-walk prior on the bias splines for the next BatchInitSpline: per-axis densities in Kalibr's units (scalar or 3-vector,
+        m/s^3/sqrt(Hz) and rad/s^2/sqrt(Hz); io_formats.bias_random_walk_from_allan derives them from an Allan fit); None: no prior."""
+        self.api.set_bias_random_walk(acc_q, gyr_q)
+
     def GetCornerErrors(self):
         """Per-corner reprojection error |(rx, ry)| [px, or scaled tangent units] of the corners in the solve, in frame order."""
         return self.api.corner_errors()

@@ -24,6 +24,11 @@
 // icc_reject_outlier_corners (corners whose reprojection error exceeds max(m, k * rms) leave the solve) each followed by stage 1 again with
 // the same flags and iteration limit, until a round rejects nothing; stage 2 then runs as before.  With k > 0 the result JSON also holds
 // "outlier_corners_rejected" (all rounds) and "outlier_threshold_px" (the last round's threshold).
+// --bias_knot_spacing_s dt (default 10, the reference's), --accl_random_walk / --gyro_random_walk q (Kalibr's names and units, m/s^3/sqrt(Hz)
+// and rad/s^2/sqrt(Hz), default 0 = no prior) or --imu_noise_json (the --output_json document of fit_allan_variance, per axis q = sqrt(3) |K| /
+// scale): both bias splines at spacing dt with a random-walk prior of density q (icc_set_bias_splines, icc_set_bias_random_walk).  They act
+// through --reestimate_biases only, so without it they are refused, as are the scalars together with the JSON.  When given, the tool prints
+// the knot counts, spacing and densities, and the result JSON gains "bias_knot_spacing_s", "accl_random_walk" and "gyro_random_walk".
 #include "../../include/icc_b200.h"
 #include "icc_cli_common.hpp"
 
@@ -49,10 +54,10 @@ icccli::Flags default_flags() {
   f.str = {{"telemetry_json", ""}, {"input_pose_dataset", ""}, {"input_corners", ""}, {"camera_calibration_json", ""},
     {"gyro_to_cam_initial_calibration", ""}, {"imu_intrinsics", ""}, {"imu_bias_file", ""}, {"spline_error_weighting_json", ""}, {"output_path", ""},
     {"result_output_json", ""}, {"known_grav_dir_axis", "Z"}, {"debug_video_path", ""}, {"comm_id_hex", ""}, {"pose_error", "normalized"},
-    {"pose_shutter", "global"}, {"reprojection_error", "pixel"}};
+    {"pose_shutter", "global"}, {"reprojection_error", "pixel"}, {"imu_noise_json", ""}};
   f.boolean = {{"global_shutter", false}, {"calibrate_cam_line_delay", false}, {"reestimate_biases", false}, {"parse_only", false}, {"json_selftest", false}};
   f.num = {{"max_t", 1000.0}, {"gravity_const", 9.81}, {"device", 0.0}, {"gpus", 1.0}, {"shard_rank", 0.0}, {"shard_world", 1.0},
-    {"outlier_sigma", 0.0}, {"outlier_min_px", 1.0}, {"outlier_rounds", 2.0}};
+    {"outlier_sigma", 0.0}, {"outlier_min_px", 1.0}, {"outlier_rounds", 2.0}, {"bias_knot_spacing_s", 10.0}, {"accl_random_walk", 0.0}, {"gyro_random_walk", 0.0}};
   return f;
 }
 
@@ -171,6 +176,7 @@ int main(int argc, char** argv) {
   int pose_error = ICC_POSE_ERROR_NORMALIZED, reproj_error = ICC_REPROJ_ERROR_PIXEL;
   bool pose_rolling = false;
   double outlier_sigma = 0.0, outlier_min_px = 1.0; int outlier_rounds = 2;
+  bool bias_walk = false; double bias_dt = 10.0, acc_q[3] = {0, 0, 0}, gyr_q[3] = {0, 0, 0};   // --bias_knot_spacing_s / --*_random_walk / --imu_noise_json
   try {
     icccli::parse_flags(argc, argv, F); pose_error = icccli::parse_pose_error(F.str["pose_error"]); pose_rolling = icccli::parse_pose_shutter(F.str["pose_shutter"]);
     reproj_error = icccli::parse_reprojection_error(F.str["reprojection_error"]);
@@ -180,6 +186,17 @@ int main(int argc, char** argv) {
     if (!(F.num["outlier_rounds"] >= 0.0) || F.num["outlier_rounds"] > 1000.0 || F.num["outlier_rounds"] != std::floor(F.num["outlier_rounds"]))
       throw std::runtime_error("--outlier_rounds must be a whole number >= 0");
     outlier_rounds = (int)F.num["outlier_rounds"];
+    bias_dt = F.num["bias_knot_spacing_s"];
+    const double aq = F.num["accl_random_walk"], gq = F.num["gyro_random_walk"];
+    if (!(bias_dt > 0.0) || !std::isfinite(bias_dt)) throw std::runtime_error("--bias_knot_spacing_s must be a finite number > 0");
+    if (!(aq >= 0.0) || !std::isfinite(aq) || !(gq >= 0.0) || !std::isfinite(gq)) throw std::runtime_error("--accl_random_walk / --gyro_random_walk must be finite numbers >= 0 (0 = no prior)");
+    const bool scalars = aq > 0.0 || gq > 0.0, noise_json = !F.str["imu_noise_json"].empty();
+    if (scalars && noise_json) throw std::runtime_error("--imu_noise_json and --accl_random_walk / --gyro_random_walk both give the random-walk densities: use one");
+    bias_walk = scalars || noise_json || bias_dt != 10.0;
+    if (bias_walk && !F.boolean["reestimate_biases"])
+      throw std::runtime_error("--bias_knot_spacing_s, --accl_random_walk, --gyro_random_walk and --imu_noise_json shape the bias splines, which only --reestimate_biases frees: add it");
+    for (int a = 0; a < 3; ++a) { acc_q[a] = aq; gyr_q[a] = gq; }
+    if (noise_json) icccli::bias_random_walk_from_allan(iccjson::load_json(F.str["imu_noise_json"]), acc_q, gyr_q);
     if (pose_rolling && F.boolean["global_shutter"]) throw std::runtime_error("--pose_shutter rolling contradicts --global_shutter");
     if (pose_rolling && !F.str["input_pose_dataset"].empty()) throw std::runtime_error("--pose_shutter rolling applies to the in-process pose step, which --input_pose_dataset skips");
   } catch (const std::exception& e) { std::cerr << "ERROR: " << e.what() << std::endl; return 1; }
@@ -331,6 +348,10 @@ int main(int argc, char** argv) {
       s["board_points"] = Value((int64_t)(max_id + 1)); s["camera_model"] = Value(model); s["intrinsics"] = Value::array();
       for (double v : intr) s["intrinsics"].push_back(Value(v));
       if (outlier_sigma > 0.0) { s["outlier_sigma"] = Value(outlier_sigma); s["outlier_min_px"] = Value(outlier_min_px); s["outlier_rounds"] = Value((int64_t)outlier_rounds); }
+      if (bias_walk) {
+        s["bias_knot_spacing_s"] = Value(bias_dt); s["accl_random_walk"] = Value::array(); s["gyro_random_walk"] = Value::array();
+        for (int a = 0; a < 3; ++a) { s["accl_random_walk"].push_back(Value(acc_q[a])); s["gyro_random_walk"].push_back(Value(gyr_q[a])); }
+      }
       s["init_line_delay_s"] = Value(init_line_delay); s["dt_so3"] = Value(ip.dt_so3_s); s["dt_r3"] = Value(ip.dt_r3_s); s["first_view_t_s"] = Value(frame_t.front());
       s["uv_sum"] = Value([&] { double a = 0; for (double v : uv) a += v; return a; }());
       // order-sensitive digests: the views must arrive in std::map key order, the corners of a view in the order of their id strings
@@ -350,7 +371,16 @@ int main(int argc, char** argv) {
     ICC(icc_set_board_points(h, max_id + 1, board.data()));
     ICC(icc_set_frames(h, (int)frame_t.size(), frame_t.data(), off.data(), ids.data(), uv.data(), q_wc.data(), p_wc.data()));
     ICC(icc_set_imu(h, (int)imu_t.size(), imu_t.data(), acc.data(), gyr.data()));
+    if (bias_walk) {   // a sensor whose density is 0 keeps no prior
+      ICC(icc_set_bias_splines(h, bias_dt, bias_dt));
+      ICC(icc_set_bias_random_walk(h, acc_q[0] > 0.0 ? acc_q : nullptr, gyr_q[0] > 0.0 ? gyr_q : nullptr));
+    }
     ICC(icc_batch_init_spline(h, &ip));
+    if (bias_walk) {
+      int nba = 0, nbg = 0; ICC(icc_get_num_knots(h, nullptr, nullptr, &nba, &nbg));
+      std::cout << "Bias splines: " << nba << " accelerometer and " << nbg << " gyroscope knots at " << bias_dt << " s spacing; random walk accel ["
+                << acc_q[0] << ", " << acc_q[1] << ", " << acc_q[2] << "] m/s^3/sqrt(Hz), gyro [" << gyr_q[0] << ", " << gyr_q[1] << ", " << gyr_q[2] << "] rad/s^2/sqrt(Hz)\n";
+    }
     const int grav_dir_axis = grav_dir_string_to_int(F.str["known_grav_dir_axis"]);
     int flags = ICC_FLAG_SPLINE | ICC_FLAG_T_I_C;
     if (F.boolean["reestimate_biases"]) flags |= ICC_FLAG_IMU_BIASES;
@@ -428,6 +458,10 @@ int main(int argc, char** argv) {
     out["init_line_delay_us"] = Value(init_line_delay * S_TO_US); out["calib_line_delay_us"] = Value(calib_line_delay_us);
     out["time_offset_imu_to_cam_s"] = Value(time_offset_imu_to_cam);
     if (outlier_sigma > 0.0) { out["outlier_corners_rejected"] = Value(outliers_rejected); out["outlier_threshold_px"] = Value(outlier_threshold); }
+    if (bias_walk) {
+      out["bias_knot_spacing_s"] = Value(bias_dt); out["accl_random_walk"] = Value::array(); out["gyro_random_walk"] = Value::array();
+      for (int a = 0; a < 3; ++a) { out["accl_random_walk"].push_back(Value(acc_q[a])); out["gyro_random_walk"].push_back(Value(gyr_q[a])); }
+    }
     int n_used = 0; ICC(icc_get_num_imu_used(h, &n_used));
     std::vector<double> ut(n_used), ua(3 * (size_t)n_used), ug(3 * (size_t)n_used);
     ICC(icc_get_imu_used(h, ut.data(), ua.data(), ug.data()));

@@ -9,6 +9,7 @@
 // and applies the trust-region accept/reject logic to a few scalars read back per iteration.  There is no CPU fallback.
 #include "../../include/icc_b200.h"
 #include "icc_allan_math.cuh"
+#include "icc_bias_prior.cuh"
 #include "icc_bearing_math.cuh"
 #include "icc_camera.cuh"
 #include "icc_host.h"
@@ -126,6 +127,11 @@ struct icc_handle {
   bool initialised = false;
   icc_init_params ip;
   int64_t dt_so3_ns = 0, dt_r3_ns = 0, dt_ba_ns = 0, dt_bg_ns = 0, start_ns = 0, end_ns = 0;
+  // bias splines: spacing [s] of icc_set_bias_splines (<= 0: the reference's 10 s) and the random-walk densities of icc_set_bias_random_walk
+  // (walk_set[s] = false: no prior rows), both read by the next icc_batch_init_spline into `prior` (0 = accelerometer, 1 = gyroscope)
+  double bias_dt_s_set[2] = {0.0, 0.0}; bool walk_set[2] = {false, false}; double walk_q_set[2][3] = {{0.0}};
+  BiasPrior prior{};        // the prior of the assembled problem (on[s] only on shard 0, which owns the rows)
+  int n_res_prior = 0;      // its rows in this shard
   double t0_s = 0, tend_s = 0, max_ba = 1.0, max_bg = 0.1;
   std::vector<double> so3, r3, ba, bg;       // host mirror of the state (4/3/3/3 doubles per knot)
   double glob[G_COUNT] = {0};
@@ -454,16 +460,27 @@ icc_status cross_rank_sum(icc_handle* h, double* dev, int64_t n) {
 // the tangent measurements the evaluation kernels take in tangent mode; nullptr selects the pixel residual
 const TangentMeas* tangent_meas(const icc_handle* h) { return h->reproj_error == ICC_REPROJ_ERROR_TANGENT ? &h->tan : nullptr; }
 
-// One Jacobian evaluation on the current state: zero the packed normal equations, run the kernels, cross-rank reduce.
+// The random-walk prior of the bias splines with its rows placed after the gyroscope rows of the residual vector
+BiasPrior prior_at(const icc_handle* h) {
+  BiasPrior B = h->prior;
+  const int base = h->P.n_res_vis + h->P.n_res_acc + h->P.n_res_gyr;
+  B.res_off[0] += base; B.res_off[1] += base;
+  return B;
+}
+
+// One Jacobian evaluation on the current state: zero the packed normal equations, run the kernels, add the bias prior (when set),
+// cross-rank reduce.
 icc_status eval_jacobian(icc_handle* h, const DeviceState& S, double* residuals_dev) {
   h->ne_flags = -1;
   CU(cudaMemsetAsync(h->P.ne, 0, (size_t)h->P.ne_size * sizeof(double), h->stream));
   if (launch_eval(h->P, S, true, nullptr, residuals_dev, nullptr, h->stream, h->aux_ok ? &h->aux : nullptr, tangent_meas(h))) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
   if (h->P.col_pts >= 0 && h->P.rolling) launch_points_jac(h->P, S, S.pjac, h->P.col_pts, h->sm_count, h->stream, tangent_meas(h));   // board-point columns (POINTS)
+  launch_bias_prior(prior_at(h), h->P, S, true, nullptr, residuals_dev, h->stream);
   return cross_rank_sum(h, h->P.ne, h->P.ne_size);
 }
 icc_status eval_cost(icc_handle* h, const DeviceState& S, double* cost_dev, double* residuals_dev, double* reproj_dev) {
   if (launch_eval(h->P, S, false, cost_dev, residuals_dev, reproj_dev, h->stream, h->aux_ok ? &h->aux : nullptr, tangent_meas(h))) return fail(h, ICC_ERR_CUDA, std::string("eval launch: ") + cudaGetErrorString(cudaGetLastError()));
+  launch_bias_prior(prior_at(h), h->P, S, false, cost_dev, residuals_dev, h->stream);
   return cost_dev ? cross_rank_sum(h, cost_dev, 1) : ICC_OK;
 }
 
@@ -484,11 +501,18 @@ icc_status mean_reproj(icc_handle* h, double* out) {
   return ICC_OK;
 }
 
-// configure() accepted the knot band, so a plan that does not fit is the border's doing
-std::string border_too_wide_message(const DeviceProblem& P) {
-  char msg[256];
-  snprintf(msg, sizeof msg, "the border of %d columns (globals, bias knots, board points) is too wide for the solver's shared-memory plans "
-           "(half bandwidth %d, %d knot columns)", P.nb, P.kd, P.nk);
+// configure() accepted the knot band, so a plan that does not fit is the border's doing; with free bias knots the message names their
+// count and spacing, the usual cause (icc_set_bias_splines)
+std::string border_too_wide_message(const icc_handle* h) {
+  const DeviceProblem& P = h->P;
+  char msg[512];
+  int len = snprintf(msg, sizeof msg, "the border of %d columns (globals, bias knots, board points) is too wide for the solver's shared-memory plans "
+                     "(half bandwidth %d, %d knot columns)", P.nb, P.kd, P.nk);
+  const bool ab = !h->ba_col.empty() && h->ba_col[0] >= 0, gb = !h->bg_col.empty() && h->bg_col[0] >= 0;
+  if ((ab || gb) && len > 0 && len < (int)sizeof msg)
+    snprintf(msg + len, sizeof msg - len, "; %d of them are columns of free bias knots: %d accelerometer knots at %g s spacing, %d gyroscope knots at %g s spacing "
+             "(a wider spacing, icc_set_bias_splines, gives fewer)", 3 * ((ab ? P.n_ba : 0) + (gb ? P.n_bg : 0)), ab ? P.n_ba : 0, double(h->dt_ba_ns) / S_TO_NS,
+             gb ? P.n_bg : 0, double(h->dt_bg_ns) / S_TO_NS);
   return msg;
 }
 
@@ -503,7 +527,7 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
   icc_summary S; memset(&S, 0, sizeof S);
   const DeviceProblem& P = h->P;
   const int n = P.nk + P.nb;
-  S.num_residuals = P.n_res_vis + P.n_res_acc + P.n_res_gyr; S.num_tangent = n;
+  S.num_residuals = P.n_res_vis + P.n_res_acc + P.n_res_gyr + h->n_res_prior; S.num_tangent = n;
   const int launches0 = kernel_launch_count();
   std::vector<cudaEvent_t> ev;
   auto mark = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, h->stream); ev.push_back(e); return (int)ev.size() - 1; };
@@ -547,7 +571,7 @@ icc_status run_lm(icc_handle* h, int max_iters, int flags, bool check_convergenc
     SolveParams sp; sp.radius = T.radius; sp.min_diag = to.min_diagonal; sp.max_diag = to.max_diagonal; sp.jacobi_scaling = h->opt.jacobi_scaling;
     const int a = mark();
     { const int se = launch_solve(P, h->d_scale.p, sp, h->d_ws.p, h->d_delta.p, h->d_scal.p, h->stream, 0);
-      if (se == 1) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(P));
+      if (se == 1) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(h));
       if (se) return fail(h, ICC_ERR_CUDA, std::string("solver launch: ") + cudaGetErrorString(cudaGetLastError())); }
     const int b = mark(); lin_spans.push_back({a, b});
     const int cand = 1 - h->cur;
@@ -609,9 +633,23 @@ icc_status init_globals_and_knot_counts(icc_handle* h, KnotCounts& n) {
   h->end_ns = (int64_t)(h->tend_s * S_TO_NS + 0.01 * S_TO_NS + ip.init_line_delay_s);
   h->dt_so3_ns = (int64_t)(ip.dt_so3_s * S_TO_NS); h->dt_r3_ns = (int64_t)(ip.dt_r3_s * S_TO_NS);
   if (h->dt_so3_ns <= 0 || h->dt_r3_ns <= 0) return fail(h, ICC_ERR_INVALID_ARGUMENT, "knot spacing must be positive");
-  h->dt_ba_ns = h->dt_bg_ns = (int64_t)(10 * 1e9); h->max_ba = 1.0; h->max_bg = 1e-1;
+  // the bias spacing of icc_set_bias_splines in place of the reference's constant 10 s; the bias box stays the reference's
+  auto bias_dt_ns = [](double dt_s) { return dt_s > 0.0 ? (int64_t)(dt_s * S_TO_NS) : (int64_t)(10 * 1e9); };
+  h->dt_ba_ns = bias_dt_ns(h->bias_dt_s_set[0]); h->dt_bg_ns = bias_dt_ns(h->bias_dt_s_set[1]); h->max_ba = 1.0; h->max_bg = 1e-1;
   const int64_t duration = h->end_ns - h->start_ns;
   n = {(int)(duration / h->dt_so3_ns) + SPLINE_N, (int)(duration / h->dt_r3_ns) + SPLINE_N, (int)(duration / h->dt_ba_ns) + BIAS_N, (int)(duration / h->dt_bg_ns) + BIAS_N};
+  {   // the prior rows: shard 0 owns them, so that the cross-rank sums count them once
+    BiasPrior& B = h->prior; B = BiasPrior{};
+    const int nk[2] = {n.ba, n.bg}; const int64_t dt[2] = {h->dt_ba_ns, h->dt_bg_ns};
+    int off = 0;
+    for (int s = 0; s < 2; ++s) {
+      B.on[s] = h->walk_set[s] && h->shard_rank == 0 ? 1 : 0;
+      for (int a = 0; a < 3; ++a) B.c[s][a] = B.on[s] ? bias_prior_scale(double(dt[s]) / S_TO_NS, h->walk_q_set[s][a]) : 0.0;
+      B.res_off[s] = off;                                       // relative to the end of the gyroscope rows (see prior_at)
+      if (B.on[s]) off += 3 * BIAS_PRIOR_NODES * (nk[s] - 2);
+    }
+    h->n_res_prior = off;
+  }
   h->so3.assign(4 * (size_t)n.so3, 0.0); h->r3.assign(3 * (size_t)n.r3, 0.0);
   h->ba.resize(3 * (size_t)n.ba); h->bg.resize(3 * (size_t)n.bg);
   for (int i = 0; i < n.ba; ++i) for (int d = 0; d < 3; ++d) h->ba[3 * i + d] = ip.acc_bias[d];
@@ -1229,6 +1267,25 @@ icc_status icc_set_comm(icc_handle* h, icc_comm* c) {
 }
 icc_status icc_set_allreduce(icc_handle* h, icc_allreduce_fn fn, void* user) { if (!h) return ICC_ERR_INVALID_ARGUMENT; h->allreduce = fn; h->allreduce_user = user; return ICC_OK; }
 
+icc_status icc_set_bias_splines(icc_handle* h, double acc_dt_s, double gyr_dt_s) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  for (const double dt : {acc_dt_s, gyr_dt_s})   // <= 0 selects the reference's 10 s; a spacing must be a whole number of nanoseconds >= 1
+    if (!std::isfinite(dt) || (dt > 0.0 && (dt * S_TO_NS < 1.0 || dt > 1e9)))
+      return fail(h, ICC_ERR_INVALID_ARGUMENT, "bias knot spacing must be finite and either <= 0 (the default 10 s) or in [1 ns, 1e9 s]");
+  h->bias_dt_s_set[0] = acc_dt_s; h->bias_dt_s_set[1] = gyr_dt_s;
+  return ICC_OK;
+}
+icc_status icc_set_bias_random_walk(icc_handle* h, const double acc_q[3], const double gyr_q[3]) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  const double* q[2] = {acc_q, gyr_q};
+  for (int s = 0; s < 2; ++s)
+    if (q[s]) for (int a = 0; a < 3; ++a)
+      if (!(q[s][a] > 0.0) || !std::isfinite(q[s][a])) return fail(h, ICC_ERR_INVALID_ARGUMENT, "random-walk densities must be finite and > 0 (NULL turns a sensor's prior off)");
+  for (int s = 0; s < 2; ++s) { h->walk_set[s] = q[s] != nullptr; for (int a = 0; a < 3; ++a) h->walk_q_set[s][a] = q[s] ? q[s][a] : 0.0; }
+  return ICC_OK;
+}
+icc_status icc_num_bias_prior_residuals(const icc_handle* h, int* n) { if (!h || !n) return ICC_ERR_INVALID_ARGUMENT; *n = h->n_res_prior; return ICC_OK; }
+
 icc_status icc_batch_init_spline(icc_handle* h, const icc_init_params* ipp) {
   if (!h || !ipp) return ICC_ERR_INVALID_ARGUMENT;
   if (h->model < 0 || h->frame_t.empty() || h->points.empty()) return fail(h, ICC_ERR_STATE, "camera, board points and frames must be set before batch_init_spline");
@@ -1419,7 +1476,7 @@ icc_status icc_evaluate(icc_handle* h, int flags, double* cost, double* residual
   CU(cudaSetDevice(h->device));
   icc_status s = configure(h, flags); if (s != ICC_OK) return s;
   const DeviceProblem& P = h->P;
-  const int nres = P.n_res_vis + P.n_res_acc + P.n_res_gyr, n = h->n_tan;
+  const int nres = P.n_res_vis + P.n_res_acc + P.n_res_gyr + h->n_res_prior, n = h->n_tan;
   double* res_dev = nullptr;
   if (residuals) { CU(h->d_res.alloc((size_t)std::max(1, nres))); CU(cudaMemsetAsync(h->d_res.p, 0, (size_t)nres * sizeof(double), h->stream)); res_dev = h->d_res.p; }
   if (!gradient && !hessian) {
@@ -1513,7 +1570,7 @@ icc_status icc_solve_normal_equations(icc_handle* h, int flags, double radius, i
   const int n = P.nk + P.nb;
   icc_solver_plan_info pi; solver_plan_info(P, chunks, &pi);
   if (plan) *plan = pi;
-  if (!pi.valid) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(P));
+  if (!pi.valid) return fail(h, ICC_ERR_UNSUPPORTED, border_too_wide_message(h));
   if (n == 0) { if (model_change) *model_change = 0.0; if (step_ok) *step_ok = 1; return ICC_OK; }
   DevBuf<double> ws; CU(ws.alloc((size_t)pi.workspace_doubles));
   CU(cudaMemsetAsync(h->d_scal.p, 0, SC_COUNT * sizeof(double), h->stream));

@@ -9,6 +9,7 @@
 #include <map>
 #include <ostream>
 #include <stdexcept>
+#include <cmath>
 #include <string>
 #include <utility>
 #include <vector>
@@ -47,6 +48,17 @@ inline bool parse_pose_shutter(const std::string& v) {
 inline double pose_line_delay(double fps, int height) {
   if (!(fps > 0.0) || height <= 0) throw std::runtime_error("--pose_shutter rolling needs fps > 0 and an image height in the camera calibration");
   return 1.0 / fps / height;
+}
+
+// Random-walk densities in Kalibr's units (m/s^3/sqrt(Hz), rad/s^2/sqrt(Hz)) from a fit_allan_variance --output_json document: per axis
+// q = sqrt(3) |K| / scale, K the channel's fitted rate-random-walk term, scale 1 for the accelerometer (m/s^2) and 57.3 * 3600 for the
+// gyroscope (deg/h).  The Python statement is io_formats.bias_random_walk_from_allan.
+inline void bias_random_walk_from_allan(const Value& doc, double acc_q[3], double gyr_q[3]) {
+  const char* axes[3] = {"x", "y", "z"};
+  for (int a = 0; a < 3; ++a) {
+    acc_q[a] = std::sqrt(3.0) * std::fabs(doc.at("channels").at(std::string("acc_") + axes[a]).at("params").at("K").num()) / 1.0;
+    gyr_q[a] = std::sqrt(3.0) * std::fabs(doc.at("channels").at(std::string("gyr_") + axes[a]).at("params").at("K").num()) / (57.3 * 3600);
+  }
 }
 
 inline bool parse_bool(const std::string& v) { return v == "true" || v == "1" || v == "t" || v == "yes" || v == "y" || v == "True"; }

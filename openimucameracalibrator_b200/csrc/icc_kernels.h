@@ -179,6 +179,12 @@ struct CornerCompaction {
   double2* uv_out; int* pid_out; double4* bear_out; int* bear_ok_out; int* src_out;
 };
 void launch_compact_corners(const CornerCompaction& C, cudaStream_t st);
+// ---- random-walk prior on the bias splines (icc_bias_prior.cu) -------------------------------------------------------
+// on[s]: the rows of sensor s (0 = accelerometer, 1 = gyroscope) are part of the problem; c[s][a] = 1 / (q_a sqrt(2 dt_s)); res_off[s] = index of
+// its first row in the residual vector.  Adds the rows' cost to P.ne's cost slot (with_jacobian) and / or *cost_out, writes them to residuals_out
+// (nullable) and, with the Jacobian, J^T r and J^T J at the bias columns P.ba_col / P.bg_col that are free.  Launches nothing when both are off.
+struct BiasPrior { int on[2]; int res_off[2]; double c[2][3]; };
+void launch_bias_prior(const BiasPrior& B, const DeviceProblem& P, const DeviceState& S, bool with_jacobian, double* cost_out, double* residuals_out, cudaStream_t st);
 int kernel_launch_count();   // kernels launched so far in this process (icc_eval.cu)
 void count_launch();         // every launcher calls it once per kernel it enqueues
 

@@ -225,6 +225,18 @@ def allan_variance_document(result: dict, curves: list) -> dict:
     return doc
 
 
+# Allan-deviation scale of each sensor's fit: the accelerometer in m/s^2, the gyroscope in deg/h (57.3 deg/rad, 3600 s/h)
+ALLAN_RATE_SCALE = {"acc": 1.0, "gyr": 57.3 * 3600}
+
+
+def bias_random_walk_from_allan(doc: dict):
+    """(acc_q[3], gyr_q[3]) random-walk densities in Kalibr's units (m/s^3/sqrt(Hz), rad/s^2/sqrt(Hz)) from a fit_allan_variance
+    --output_json document: per axis q = sqrt(3) |K| / scale, K the fitted rate-random-walk term of that channel's Allan variance."""
+    ch = doc["channels"]
+    q = {s: np.array([np.sqrt(3.0) * abs(float(ch[f"{s}_{a}"]["params"]["K"])) / ALLAN_RATE_SCALE[s] for a in "xyz"]) for s in ("acc", "gyr")}
+    return q["acc"], q["gyr"]
+
+
 def write_allan_variance_json(path: str, result: dict, curves: list) -> None:
     with open(path, "w") as f:
         json.dump(allan_variance_document(result, curves), f, indent=1)
