@@ -53,6 +53,11 @@ typedef enum {
  *                             R = (1 + k1 s + k2 s^2 + k3 s^3) / (1 + k4 s + k5 s^2 + k6 s^3), dx = xn R + 2 t1 xn yn + t2 (s + 2 xn^2),
  *                             dy = yn R + t1 (s + 2 yn^2) + 2 t2 xn yn, then the skewed affine; valid iff z > 0 and s < s_max, the first
  *                             s > 0 at which r R(r^2) stops increasing (a root of d(r R)/dr or a pole of R), +inf when there is none)
+ *   FISHEYE_RADIAL_TANGENTIAL [f, ar, skew, cx, cy, k1, k2, k3, k4, k5, k6, t1, t2]   (extension, no Theia counterpart: Kannala-Brandt with
+ *                             six radial and two tangential terms, Fisheye62; theta = atan2(|(x, y)|, z), theta_d = theta (1 + k1 theta^2 + ...
+ *                             + k6 theta^12), (xr, yr) = (theta_d / |(x, y)|) (x, y), s = xr^2 + yr^2, dx = xr + 2 t1 xr yr + t2 (s + 2 xr^2),
+ *                             dy = yr + t1 (s + 2 yr^2) + 2 t2 xr yr, then the skewed affine; t1, t2 as PINHOLE_RADIAL_TANGENTIAL's (OpenCV's p1,
+ *                             p2); k1..k4 sit where FISHEYE keeps them; valid iff z > 0 and d theta_d / d theta has no root in (0, theta])
  * ICC_MAX_INTRINSICS is the longest of these vectors. */
 #define ICC_MAX_INTRINSICS 13
 typedef enum {
@@ -65,7 +70,8 @@ typedef enum {
   ICC_CAM_EXTENDED_UNIFIED = 6,
   ICC_CAM_OMNI_RADIAL_TANGENTIAL = 7,
   ICC_CAM_SCARAMUZZA = 8,
-  ICC_CAM_PINHOLE_RATIONAL = 9
+  ICC_CAM_PINHOLE_RATIONAL = 9,
+  ICC_CAM_FISHEYE_RADIAL_TANGENTIAL = 10
 } icc_camera_model;
 
 /* OpenICC::core::SplineOptimFlags (core/spline_trajectory_estimator.h:17-27), same numeric values. */
@@ -454,7 +460,7 @@ icc_status icc_spline_error_weighting(icc_handle* h, int n, const double* times_
  * utils::initialize_radial_undistortion_camera hands the reference, :283-306) before the target model takes over.
  * Needs icc_set_board_points (planar board for the internal initialiser).
  * Outputs (caller-owned): intrinsics in Theia's order for `model`, max(10, its parameter count) entries (10 for every model but
- * PINHOLE_RATIONAL, 13 for it; unused entries zero); per view q_wc / p_wc (as icc_set_frames consumes them),
+ * PINHOLE_RATIONAL and FISHEYE_RADIAL_TANGENTIAL, 13 for them; unused entries zero); per view q_wc / p_wc (as icc_set_frames consumes them),
  * the mean reprojection error [px] (GetReprojErrorOfView) and used[v] = 1 for the views that survive to the end.
  * summary->success = 0 (status still ICC_OK) when fewer than min_num_views views remain, like RunCalibration returning false. */
 typedef struct icc_camcal_options {

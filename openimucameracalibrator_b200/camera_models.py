@@ -15,6 +15,7 @@ PINHOLE, PINHOLE_RADIAL_TANGENTIAL, FISHEYE, FOV, DIVISION_UNDISTORTION, DOUBLE_
 OMNI_RADIAL_TANGENTIAL = 7   # extension without a Theia counterpart: Kalibr's omni-radtan
 SCARAMUZZA = 8               # extension without a Theia counterpart: Scaramuzza's omnidirectional polynomial model (OCamCalib)
 PINHOLE_RATIONAL = 9         # extension without a Theia counterpart: OpenCV's rational polynomial model (k1..k6, p1, p2)
+FISHEYE_RADIAL_TANGENTIAL = 10   # extension without a Theia counterpart: Kannala-Brandt with k1..k6 and tangential t1, t2 (Fisheye62)
 
 
 class CameraLayout(NamedTuple):
@@ -49,6 +50,11 @@ CAMERAS = {c.id: c for c in (
                                                                 tangential_distortion_2=9, radial_distortion_4=10, radial_distortion_5=11, radial_distortion_6=12),
                  {"Radial distortion 1": 5, "Radial distortion 2": 6, "Radial distortion 3": 7, "Radial distortion 4": 10, "Radial distortion 5": 11,
                   "Radial distortion 6": 12, "Tangential distortion 1": 8, "Tangential distortion 2": 9}),
+    CameraLayout("FISHEYE_RADIAL_TANGENTIAL", FISHEYE_RADIAL_TANGENTIAL, 13,
+                 dict(_AFFINE, radial_distortion_1=5, radial_distortion_2=6, radial_distortion_3=7, radial_distortion_4=8, radial_distortion_5=9,
+                      radial_distortion_6=10, tangential_distortion_1=11, tangential_distortion_2=12),
+                 {"Radial distortion 1": 5, "Radial distortion 2": 6, "Radial distortion 3": 7, "Radial distortion 4": 8, "Radial distortion 5": 9,
+                  "Radial distortion 6": 10, "Tangential distortion 1": 11, "Tangential distortion 2": 12}),
 )}
 MODEL_NAMES = {m: c.name for m, c in CAMERAS.items()}
 MODEL_IDS = {c.name: m for m, c in CAMERAS.items()}
@@ -205,6 +211,73 @@ def rational_unproject(k, uv):
     return np.stack([x, y], axis=-1), ok
 
 
+def fisheye_radtan_theta_max(k) -> float:
+    """FISHEYE_RADIAL_TANGENTIAL's [f, ar, skew, cx, cy, k1, k2, k3, k4, k5, k6, t1, t2]: the first theta > 0 at which theta_d = theta (1 +
+    k1 theta^2 + ... + k6 theta^12) stops increasing, i.e. sqrt of the smallest positive real root t of d theta_d / d theta = 1 + 3 k1 t +
+    5 k2 t^2 + ... + 13 k6 t^6 (np.roots), inf when there is none."""
+    k = np.asarray(k, dtype=np.float64)
+    q = np.trim_zeros(np.concatenate([[1.0], np.arange(3, 15, 2) * k[5:11]]), "b")
+    if q.size < 2:
+        return np.inf
+    roots = np.roots(q[::-1])
+    pos = roots.real[(np.abs(roots.imag) <= 1e-9 * np.maximum(np.abs(roots), 1.0)) & (roots.real > 0.0)]
+    return float(np.sqrt(pos.min())) if pos.size else np.inf
+
+
+def fisheye_radtan_distort(k, x, y, z):
+    """FISHEYE_RADIAL_TANGENTIAL's distorted point (dx, dy) of camera-frame points (x, y, z), z > 0: the radial stage (xr, yr) = (theta_d / r)
+    (x, y) ((x, y) / z on the axis), then the tangential terms of PINHOLE_RADIAL_TANGENTIAL"""
+    r = np.hypot(x, y)
+    th = np.arctan2(r, z); t = th * th
+    P = 1.0 + t * (k[5] + t * (k[6] + t * (k[7] + t * (k[8] + t * (k[9] + t * k[10])))))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        g = np.where(r > 0.0, th * P / np.where(r > 0.0, r, 1.0), 1.0 / z)
+    xr, yr = g * x, g * y
+    s = xr * xr + yr * yr
+    return (xr + 2.0 * k[11] * xr * yr + k[12] * (s + 2.0 * xr * xr),
+            yr + k[11] * (s + 2.0 * yr * yr) + 2.0 * k[12] * xr * yr)
+
+
+def fisheye_radtan_unproject(k, uv):
+    """FISHEYE_RADIAL_TANGENTIAL: (xn, yn) = (x / z, y / z) of pixels uv (..., 2) and ok (...,): the skewed affine inverted, then damped
+    Newton's method on the normalised plane over whole arrays (Jacobian by central differences), started at the equidistant reading of the
+    distorted point; ok iff the point converged to 1e-12 of the distorted point and its ray lies inside the domain theta < theta_max."""
+    k = np.asarray(k, dtype=np.float64)
+    uv = np.asarray(uv, dtype=np.float64)
+    dy = (uv[..., 1] - k[4]) / (k[0] * k[1])
+    dx = (uv[..., 0] - k[3] - k[2] * dy) / k[0]
+    thmax = min(fisheye_radtan_theta_max(k), 0.5 * np.pi)
+    rd = np.hypot(dx, dy)
+    th0 = np.minimum(rd, 0.9 * thmax)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        sc = np.where(rd > 0.0, np.tan(th0) / np.where(rd > 0.0, rd, 1.0), 1.0)
+    x, y = dx * sc, dy * sc                                 # a start inside the domain
+
+    def err(x, y):
+        fx, fy = fisheye_radtan_distort(k, x, y, 1.0)
+        return np.where(np.arctan(np.hypot(x, y)) < thmax, np.hypot(fx - dx, fy - dy), np.inf), fx - dx, fy - dy
+
+    with np.errstate(all="ignore"):
+        for _ in range(100):                                 # Newton's method, each step halved until it stays inside and improves
+            e, ex, ey = err(x, y)
+            h = 1e-7 * np.maximum(1.0, np.hypot(x, y))
+            ax = (np.array(fisheye_radtan_distort(k, x + h, y, 1.0)) - np.array(fisheye_radtan_distort(k, x - h, y, 1.0))) / (2.0 * h)
+            ay = (np.array(fisheye_radtan_distort(k, x, y + h, 1.0)) - np.array(fisheye_radtan_distort(k, x, y - h, 1.0))) / (2.0 * h)
+            det = ax[0] * ay[1] - ay[0] * ax[1]
+            sx, sy = -(ay[1] * ex - ay[0] * ey) / det, -(-ax[1] * ex + ax[0] * ey) / det
+            t = np.ones_like(x)
+            for _ in range(40):
+                bad = ~(err(x + t * sx, y + t * sy)[0] <= e)
+                if not bad.any():
+                    break
+                t = np.where(bad, 0.5 * t, t)
+            moved = err(x + t * sx, y + t * sy)[0] <= e
+            x, y = np.where(moved, x + t * sx, x), np.where(moved, y + t * sy, y)
+        fx, fy = fisheye_radtan_distort(k, x, y, 1.0)
+        ok = (np.hypot(fx - dx, fy - dy) <= 1e-12 * np.maximum(1.0, np.hypot(dx, dy))) & (np.arctan(np.hypot(x, y)) < thmax)
+    return np.stack([x, y], axis=-1), ok
+
+
 def project(model: int, intr, pts):
     """pts: (..., 3) camera-frame points -> (uv (..., 2), valid (...,))."""
     k = np.asarray(intr, dtype=np.float64)
@@ -293,5 +366,11 @@ def project(model: int, intr, pts):
             s = xn * xn + yn * yn
             dx, dy = rational_distort(k, xn, yn)
             valid = (z > 0.0) & (s < rational_s_max(k)) & (1.0 + s * (k[10] + s * (k[11] + s * k[12])) > 0.0)
+        return _affine_skew(k, dx, dy), valid
+    if model == FISHEYE_RADIAL_TANGENTIAL:
+        # Kannala-Brandt with k1..k6, then the tangential terms (t1, t2 = OpenCV's p1, p2); valid iff z > 0 and theta < theta_max
+        with np.errstate(divide="ignore", invalid="ignore"):
+            dx, dy = fisheye_radtan_distort(k, x, y, z)
+            valid = (z > 0.0) & (np.arctan2(np.hypot(x, y), z) < fisheye_radtan_theta_max(k))
         return _affine_skew(k, dx, dy), valid
     raise ValueError(f"unknown camera model {model}")

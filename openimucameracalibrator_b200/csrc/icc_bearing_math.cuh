@@ -68,10 +68,11 @@ ICC_HD double tangent_scale(int model, const double* k, bool dispatch_fov) {
 }
 
 // Unit ray b with project(b) within 1e-6 px of (px, py); false otherwise.  Pinhole, PinholeRadialTangential, FOV and DivisionUndistortion
-// cannot see past 90 degrees: their ray is unproject_gn's normalised-plane point, normalised.  Fisheye, DoubleSphere, ExtendedUnified and OmniRadtan run
+// cannot see past 90 degrees: their ray is unproject_gn's normalised-plane point, normalised.  Fisheye, FisheyeRadtan, DoubleSphere,
+// ExtendedUnified and OmniRadtan run
 // damped Gauss-Newton on the sphere: the step lives in the tangent plane of the current b, its 2x2 Jacobian is the 2x3 projection Jacobian
 // times (e1, e2), and the new ray is b + dx e1 + dy e2 renormalised.  Theia's Fisheye projects p and -p to the same pixel, so its ray is held
-// in z > 0; the three unified models reach their whole forward domain, z <= 0 included (OmniRadtan: past 90 degrees for any xi > 0).
+// in z > 0, and so is FisheyeRadtan's, whose domain is z > 0; the three unified models reach their whole forward domain, z <= 0 included (OmniRadtan: past 90 degrees for any xi > 0).
 // Scaramuzza's model back-projects in closed form: the sensor point (u', v') = A^-1 (u - cx, v - cy) sees (u', v', F(rho)), for every
 // rho = |(u', v')| below rho_max (beyond it the pixel is not the image of any point) and det A = c - d e != 0.
 ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, V3& b) {
@@ -85,7 +86,7 @@ ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, 
     b = (1.0 / sqrt(dot(ray, ray))) * ray;
     return true;
   }
-  if (model != CAM_FISHEYE && model != CAM_DOUBLE_SPHERE && model != CAM_EXTENDED_UNIFIED && model != CAM_OMNI_RADTAN) {
+  if (model != CAM_FISHEYE && model != CAM_FISHEYE_RADTAN && model != CAM_DOUBLE_SPHERE && model != CAM_EXTENDED_UNIFIED && model != CAM_OMNI_RADTAN) {
     double x = 0.0, y = 0.0;
     const bool good = unproject_gn(model, k, px, py, x, y);
     const double in = 1.0 / sqrt(x * x + y * y + 1.0);
@@ -103,7 +104,7 @@ ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, 
     const double x = (d * du - bb * dv) / det, y = (-c * du + a * dv) / det, rho = sqrt(x * x + y * y);
     if (rho > 0.0) {
       double th = 2.0 * atan(0.5 * rho);
-      if (model == CAM_FISHEYE) th = fmin(th, 1.5);
+      if (model == CAM_FISHEYE || model == CAM_FISHEYE_RADTAN) th = fmin(th, 1.5);
       const double s = sin(th) / rho;
       b = v3(x * s, y * s, cos(th));
     }
@@ -124,7 +125,7 @@ ICC_HD bool unproject_bearing(int model, const double* k, double px, double py, 
     for (int bt = 0; bt < 30; ++bt, t *= 0.5) {
       V3 bn = b + (t * dx) * e1 + (t * dy) * e2;
       bn = (1.0 / sqrt(dot(bn, bn))) * bn;
-      if (model == CAM_FISHEYE && !(bn.z > 0.0)) continue;
+      if ((model == CAM_FISHEYE || model == CAM_FISHEYE_RADTAN) && !(bn.z > 0.0)) continue;
       const Proj pn = project(model, k, bn, true);
       if (!pn.ok) continue;
       const double r0 = pn.u - px, r1 = pn.v - py, en = r0 * r0 + r1 * r1;

@@ -371,6 +371,7 @@ IntrinsicSubsets intrinsic_subsets(int model) {
     case CAM_OMNI_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({8, 9})};   // radial = xi, k1, k2
     case CAM_SCARAMUZZA: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7}), bits({2, 8})};    // radial = a2, a3, a4; the stretch e, d as tangential
     case CAM_PINHOLE_RATIONAL: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7, 10, 11, 12}), bits({8, 9})};   // radial = k1..k6
+    case CAM_FISHEYE_RADTAN: return {bits({0}), bits({1}), bits({3, 4}), bits({5, 6, 7, 8, 9, 10}), bits({11, 12})};      // radial = k1..k6
     default: return {0u, 0u, 0u, 0u, 0u};
   }
 }
@@ -634,7 +635,8 @@ icc_status calibrate_camera(cudaStream_t st, int model, int W, int H, int np, co
   rc = bundle_adjust(sub.principal, false, 1); if (rc != ICC_OK) return rc;
   if ((int)active.size() < o.min_num_views) return finish(false);                               // :176-179
   // 3. full optimisation (:181-198)
-  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN || model == CAM_SCARAMUZZA || model == CAM_PINHOLE_RATIONAL ? sub.tangential : 0u);
+  const unsigned stage3_mask = sub.principal | sub.focal | sub.aspect | (model == CAM_PINHOLE ? sub.radial : 0u) | (model == CAM_PINHOLE_RADTAN || model == CAM_OMNI_RADTAN || model == CAM_SCARAMUZZA || model == CAM_PINHOLE_RATIONAL ||
+                                                                                               model == CAM_FISHEYE_RADTAN ? sub.tangential : 0u);
   rc = bundle_adjust(stage3_mask, true, 2);
   if (rc != ICC_OK) return rc;
   rc = remove_views(o.max_view_error_final_px); if (rc != ICC_OK) return rc;                     // :200

@@ -13,7 +13,8 @@ namespace icc {
 enum CameraModel { CAM_PINHOLE = 0, CAM_PINHOLE_RADTAN = 1, CAM_FISHEYE = 2, CAM_FOV = 3, CAM_DIVISION_UNDISTORTION = 4, CAM_DOUBLE_SPHERE = 5, CAM_EXTENDED_UNIFIED = 6,
                    CAM_OMNI_RADTAN = 7 /* extension: Kalibr's omni-radtan, no Theia counterpart */,
                    CAM_SCARAMUZZA = 8 /* extension: Scaramuzza's omnidirectional polynomial model (OCamCalib), no Theia counterpart */,
-                   CAM_PINHOLE_RATIONAL = 9 /* extension: OpenCV's rational polynomial model (k1..k6, p1, p2), no Theia counterpart */ };
+                   CAM_PINHOLE_RATIONAL = 9 /* extension: OpenCV's rational polynomial model (k1..k6, p1, p2), no Theia counterpart */,
+                   CAM_FISHEYE_RADTAN = 10 /* extension: Kannala-Brandt with k1..k6 and tangential t1, t2 (Fisheye62), no Theia counterpart */ };
 
 // Width of every intrinsic vector, buffer and Jacobian row in this library: the longest model's parameter count.
 constexpr int MAX_INTR = ICC_MAX_INTRINSICS;
@@ -21,12 +22,13 @@ constexpr int MAX_INTR = ICC_MAX_INTRINSICS;
 ICC_HD int camera_num_params(int model) {
   switch (model) { case CAM_PINHOLE: return 7; case CAM_PINHOLE_RADTAN: return 10; case CAM_FISHEYE: return 9; case CAM_FOV: return 5;
                    case CAM_DIVISION_UNDISTORTION: return 5; case CAM_DOUBLE_SPHERE: return 7; case CAM_EXTENDED_UNIFIED: return 7;
-                   case CAM_OMNI_RADTAN: return 10; case CAM_SCARAMUZZA: return 9; case CAM_PINHOLE_RATIONAL: return 13; default: return -1; }
+                   case CAM_OMNI_RADTAN: return 10; case CAM_SCARAMUZZA: return 9; case CAM_PINHOLE_RATIONAL: return 13;
+                   case CAM_FISHEYE_RADTAN: return 13; default: return -1; }
 }
 
 // J is row-major 2x3: J[0..2] = d px / d(x,y,z), J[3..5] = d py / d(x,y,z).
 // Jk (only filled when requested): d(u,v)/d intrinsics in Theia's parameter order, unused entries zero.  The first ten columns are
-// row-major 2 x 10 in Jk[0..19]; the columns past ten (CAM_PINHOLE_RATIONAL's k4..k6) follow as row-major 2 x (MAX_INTR - 10): jk_at.
+// row-major 2 x 10 in Jk[0..19]; the columns past ten (CAM_PINHOLE_RATIONAL's k4..k6, CAM_FISHEYE_RADTAN's k6, t1, t2) follow as row-major 2 x (MAX_INTR - 10): jk_at.
 struct Proj { double u, v; double J[6]; bool ok; };
 struct ProjK { double Jk[2 * MAX_INTR]; };
 ICC_HD constexpr int jk_at(int row, int col) { return col < 10 ? 10 * row + col : 20 + (MAX_INTR - 10) * row + (col - 10); }
@@ -183,6 +185,16 @@ ICC_HD bool rational_in_domain(const double* k, double s) {
     h[j] = acc;
   }
   return poly_root_free<3>(m, s) && poly_root_free<6>(h, s);
+}
+
+// ---- Kannala-Brandt with six radial and two tangential terms (Fisheye62), [f, ar, skew, cx, cy, k1, k2, k3, k4, k5, k6, t1, t2] ---------
+// theta = atan2(r, z), theta_d = theta P(theta^2), P(t) = 1 + k1 t + ... + k6 t^6, (xr, yr) = (theta_d / r) (x, y), then the tangential
+// terms of PINHOLE_RADIAL_TANGENTIAL on (xr, yr) and the skewed affine.  Valid iff z > 0 and theta_d is still increasing on (0, theta]:
+// d theta_d / d theta = Q(theta^2) = 1 + 3 k1 t + 5 k2 t^2 + ... + 13 k6 t^6 has no root in (0, theta^2] (t = theta^2 is the test's
+// variable).  The tangential stage is not fold-checked, as for PINHOLE_RADIAL_TANGENTIAL.
+__host__ __device__ inline __noinline__ bool fisheye_radtan_in_domain(const double* k, double t) {   // out of line: see project_fisheye_radtan
+  const double q[7] = {1.0, 3.0 * k[5], 5.0 * k[6], 7.0 * k[7], 9.0 * k[8], 11.0 * k[9], 13.0 * k[10]};
+  return poly_root_free<6>(q, t);
 }
 
 template <int MODEL, bool WITH_K = false>
@@ -364,6 +376,40 @@ ICC_HD Proj project_model(const double* k, V3 p, bool dispatch_fov, ProjK* pk = 
       const double ddy[5] = {-am1 * d * in, my * r2, my * r2 * r2, r2 + 2.0 * my * my, 2.0 * mx * my};
       affine_skew_k(k, dx, dy, 5, idx, ddx, ddy, *pk);
     }
+  } else if (MODEL == CAM_FISHEYE_RADTAN) {   // [f, ar, skew, cx, cy, k1, k2, k3, k4, k5, k6, t1, t2]
+    if (!(p.z > 0.0)) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
+    const double r2 = p.x * p.x + p.y * p.y, z2 = p.z * p.z, rho2 = r2 + z2, iz = 1.0 / p.z;
+    // tr = theta / r and c = (Q z / rho^2 - g) / r^2 (g = theta_d / r: d g / d(x, y) = c (x, y)).  Near the axis (a^2 = r^2 / z^2 < 1e-8) both
+    // from their series in a: theta / a = 1 - a^2 / 3 + a^4 / 5 (next term a^6 / 7 < 2e-25) and c = (2 k1 - 2 / 3) / z^3 (+ O(a^2), which
+    // enters the Jacobian times x^2 <= r^2 only); exact on the axis itself.
+    const bool axis = !(r2 > 1e-8 * z2);
+    const double a2 = r2 * iz * iz;
+    const double tr = axis ? (1.0 + a2 * (-1.0 / 3.0 + 0.2 * a2)) * iz : atan2(sqrt(r2), p.z) / sqrt(r2);
+    const double t = tr * tr * r2;                                   // theta^2
+    if (!fisheye_radtan_in_domain(k, t)) { o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
+    const double P = 1.0 + t * (k[5] + t * (k[6] + t * (k[7] + t * (k[8] + t * (k[9] + t * k[10])))));
+    const double Q = 1.0 + t * (3.0 * k[5] + t * (5.0 * k[6] + t * (7.0 * k[7] + t * (9.0 * k[8] + t * (11.0 * k[9] + t * 13.0 * k[10])))));
+    const double g = tr * P;
+    const double c = axis ? (2.0 * k[5] - 2.0 / 3.0) * iz * iz * iz : (Q * p.z / rho2 - g) / r2;
+    const double gz = -Q / rho2;
+    const double xr = g * p.x, yr = g * p.y;
+    const double M[6] = {g + p.x * p.x * c, p.x * p.y * c, p.x * gz, p.x * p.y * c, g + p.y * p.y * c, p.y * gz};   // d(xr, yr)/dp
+    const double t1 = k[11], t2 = k[12], s = xr * xr + yr * yr;
+    const double dx = xr + 2.0 * t1 * xr * yr + t2 * (s + 2.0 * xr * xr);
+    const double dy = yr + t1 * (s + 2.0 * yr * yr) + 2.0 * t2 * xr * yr;
+    const double a00 = 1.0 + 2.0 * t1 * yr + 6.0 * t2 * xr, a01 = 2.0 * t1 * xr + 2.0 * t2 * yr;   // a = d(dx, dy)/d(xr, yr), symmetric
+    const double a11 = 1.0 + 2.0 * t2 * xr + 6.0 * t1 * yr;
+    double Dd[6];
+    for (int j = 0; j < 3; ++j) { Dd[j] = a00 * M[j] + a01 * M[3 + j]; Dd[3 + j] = a01 * M[j] + a11 * M[3 + j]; }
+    affine_skew(k, dx, dy, Dd, o);
+    if (WITH_K) {   // d(xr, yr)/dk_i = theta^(2i) (theta / r) (x, y) = t^i tr (x, y), through a; d(dx, dy)/dt1, dt2 directly
+      const int idx[8] = {5, 6, 7, 8, 9, 10, 11, 12};
+      double ddx[8], ddy[8], w = tr;
+      for (int i = 0; i < 6; ++i) { w *= t; const double ex = w * p.x, ey = w * p.y; ddx[i] = a00 * ex + a01 * ey; ddy[i] = a01 * ex + a11 * ey; }
+      ddx[6] = 2.0 * xr * yr; ddy[6] = s + 2.0 * yr * yr;
+      ddx[7] = s + 2.0 * xr * xr; ddy[7] = 2.0 * xr * yr;
+      affine_skew_k(k, dx, dy, 8, idx, ddx, ddy, *pk);
+    }
   } else if (MODEL == CAM_SCARAMUZZA) {   // [a0, c, e, cx, cy, a2, a3, a4, d]: (u', v') = s (x, y), G(s) = 0; u = u' + e v' + cx, v = d u' + c v' + cy
     const double r = sqrt(p.x * p.x + p.y * p.y);
     double s, gs;
@@ -401,6 +447,11 @@ __host__ __device__ inline __noinline__ Proj project_out_of_line(int model, cons
 __host__ __device__ inline __noinline__ Proj project_out_of_line_with_k(int model, const double* k, V3 p, ProjK* pk) {
   return model == CAM_SCARAMUZZA ? project_model<CAM_SCARAMUZZA, true>(k, p, true, pk) : project_model<CAM_PINHOLE_RATIONAL, true>(k, p, true, pk);
 }
+// CAM_FISHEYE_RADTAN out of line as well, on calls of its own from the dispatchers' default branch, with its domain test out of line in
+// turn.  Of the arrangements tried, this is the one that leaves every kernel of the other models with no more registers or spills than
+// before the model existed (-Xptxas -v); behind project_out_of_line it grew them.
+__host__ __device__ inline __noinline__ Proj project_fisheye_radtan(const double* k, V3 p) { return project_model<CAM_FISHEYE_RADTAN>(k, p, true); }
+__host__ __device__ inline __noinline__ Proj project_fisheye_radtan_with_k(const double* k, V3 p, ProjK* pk) { return project_model<CAM_FISHEYE_RADTAN, true>(k, p, true, pk); }
 
 // Same dispatch, additionally returning d(u,v)/d(intrinsics) (CAM_INTRINSICS extension).
 ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, ProjK* pk) {
@@ -414,11 +465,14 @@ ICC_HD Proj project_with_k(int model, const double* k, V3 p, bool dispatch_fov, 
     case CAM_FOV: return project_model<CAM_FOV, true>(k, p, dispatch_fov, pk);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN, true>(k, p, dispatch_fov, pk);
     case CAM_SCARAMUZZA: case CAM_PINHOLE_RATIONAL: return project_out_of_line_with_k(model, k, p, pk);
-    default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 2 * MAX_INTR; ++j) pk->Jk[j] = 0; return o; }
+    default: {
+      if (model == CAM_FISHEYE_RADTAN) return project_fisheye_radtan_with_k(k, p, pk);
+      Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; for (int j = 0; j < 2 * MAX_INTR; ++j) pk->Jk[j] = 0; return o; }
   }
 }
 
-// Runtime dispatch in the reference's order (residuals.h:366-389), then the extensions CAM_OMNI_RADTAN, CAM_SCARAMUZZA and CAM_PINHOLE_RATIONAL.
+// Runtime dispatch in the reference's order (residuals.h:366-389), then the extensions CAM_OMNI_RADTAN, CAM_SCARAMUZZA, CAM_PINHOLE_RATIONAL
+// and CAM_FISHEYE_RADTAN.
 ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
   switch (model) {
     case CAM_DIVISION_UNDISTORTION: return project_model<CAM_DIVISION_UNDISTORTION>(k, p, dispatch_fov);
@@ -430,7 +484,9 @@ ICC_HD Proj project(int model, const double* k, V3 p, bool dispatch_fov) {
     case CAM_FOV: return project_model<CAM_FOV>(k, p, dispatch_fov);
     case CAM_OMNI_RADTAN: return project_model<CAM_OMNI_RADTAN>(k, p, dispatch_fov);
     case CAM_SCARAMUZZA: case CAM_PINHOLE_RATIONAL: return project_out_of_line(model, k, p);
-    default: { Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
+    default: {
+      if (model == CAM_FISHEYE_RADTAN) return project_fisheye_radtan(k, p);
+      Proj o; o.ok = false; o.u = o.v = 0; for (int j = 0; j < 6; ++j) o.J[j] = 0; return o; }
   }
 }
 

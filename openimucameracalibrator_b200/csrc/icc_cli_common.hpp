@@ -120,6 +120,11 @@ inline const std::vector<CameraLayout> kCameraLayouts = {
                       {"radial_distortion_4", 10}, {"radial_distortion_5", 11}, {"radial_distortion_6", 12}}),
    {{"Radial distortion 1", 5}, {"Radial distortion 2", 6}, {"Radial distortion 3", 7}, {"Radial distortion 4", 10}, {"Radial distortion 5", 11}, {"Radial distortion 6", 12},
     {"Tangential distortion 1", 8}, {"Tangential distortion 2", 9}}},
+  {"FISHEYE_RADIAL_TANGENTIAL", ICC_CAM_FISHEYE_RADIAL_TANGENTIAL, 13,
+   affine_keys(true, {{"radial_distortion_1", 5}, {"radial_distortion_2", 6}, {"radial_distortion_3", 7}, {"radial_distortion_4", 8}, {"radial_distortion_5", 9},
+                      {"radial_distortion_6", 10}, {"tangential_distortion_1", 11}, {"tangential_distortion_2", 12}}),
+   {{"Radial distortion 1", 5}, {"Radial distortion 2", 6}, {"Radial distortion 3", 7}, {"Radial distortion 4", 8}, {"Radial distortion 5", 9}, {"Radial distortion 6", 10},
+    {"Tangential distortion 1", 11}, {"Tangential distortion 2", 12}}},
 };
 
 // theia::StringToCameraIntrinsicsModelType: the row of a model name, nullptr for an unknown one

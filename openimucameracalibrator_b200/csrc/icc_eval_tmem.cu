@@ -145,6 +145,7 @@ int launch_eval_tmem(const DeviceProblem& P, const DeviceState& S, double* resid
       case CAM_OMNI_RADTAN: e = launch_model<CAM_OMNI_RADTAN>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       case CAM_SCARAMUZZA: e = launch_model<CAM_SCARAMUZZA>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       case CAM_PINHOLE_RATIONAL: e = launch_model<CAM_PINHOLE_RATIONAL>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
+      case CAM_FISHEYE_RADTAN: e = launch_model<CAM_FISHEYE_RADTAN>(Q, S, residuals_out, nv, nc, sm_count, st, T, true); break;
       default: return 1;
     }
     if (e) return 1;
