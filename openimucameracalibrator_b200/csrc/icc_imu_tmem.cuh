@@ -11,7 +11,7 @@
 //    and 2 go entry by entry to the warp's lane-private shared-memory park (icc_park.cuh; 43 / 38 doubles) and are expanded into
 //    the same tile after the previous row has been contracted.  The park holds only these deferred rows, which is what lets
 //    eight warps' tiles and parks fit in one block's shared memory;
-//  * the samples of all knot-interval cells form ONE packed stream (cells padded to a multiple of 4 = one m8n8k4 k-step) cut into
+//  * the samples of all knot-interval cells form ONE packed stream (cells padded to a multiple of 4 = one tensor-core k-step) cut into
 //    equal runs of 32-lane chunks, one run per warp: a 50-sample cell (1 kHz, dt = 0.05 s) no longer costs two passes with 18 of 32
 //    lanes idle in the second; a chunk may straddle two cells (two staged windows, lanes pick theirs).
 #pragma once

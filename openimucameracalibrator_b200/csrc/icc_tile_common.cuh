@@ -10,11 +10,23 @@ namespace icc {
 constexpr int TILE_LD = 36;            // rows per tile column (32 + 4 pad: conflict-free fragment loads)
 constexpr int TILE_COLS = 48;
 
+// one 8 x 8 block: c (m8n8 fragment) += a b^T over one k-step of 4 rows
 __device__ __forceinline__ void tile_mma_f64(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
-// acc += T^T T over tile rows [4 k0, 4 k1), NB column blocks of 8 (upper block triangle, NB (NB + 1) / 2 fragments of 2 doubles)
+// two 8 x 8 blocks of one block column in one m16n8k4: A rows g and g + 8 are a0 and a1, so (c0, c1) += a0 b^T and (c2, c3) += a1 b^T
+// are the m8n8 fragments of the two blocks in the same lane layout as tile_mma_f64's.  One DMMA.16x8x4 holds the H100's FP64 pipe
+// as long as one DMMA.8x8x4 (16 cycles per SM sub-partition, tools/fp64_peaks.cu; DESIGN §5), so a pair costs half.
+__device__ __forceinline__ void tile_mma2_f64(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b));
+}
+
+// acc += T^T T over tile rows [4 k0, 4 k1), NB column blocks of 8: the upper block triangle, NB (NB + 1) / 2 fragments of 2 doubles
+// stored block column by block column (bj outer, bi = 0..bj inner).  Within a block column the blocks bi = 2p and 2p + 1 are
+// adjacent fragments and share one m16n8k4; the diagonal block of an even block column is left over and takes one m8n8k4
+// (NB = 6: 9 + 3 instructions per k-step instead of 21).
 template <int NB>
 __device__ __forceinline__ void tile_syrk(const double* __restrict__ tile, int k0, int k1, double (&acc)[NB * (NB + 1)]) {
   const int lane = threadIdx.x & 31;
@@ -25,9 +37,11 @@ __device__ __forceinline__ void tile_syrk(const double* __restrict__ tile, int k
     for (int b = 0; b < NB; ++b) f[b] = base[(8 * b) * TILE_LD + 4 * s];
     int idx = 0;
 #pragma unroll
-    for (int bi = 0; bi < NB; ++bi)
+    for (int bj = 0; bj < NB; ++bj) {
 #pragma unroll
-      for (int bj = bi; bj < NB; ++bj) { tile_mma_f64(acc[2 * idx], acc[2 * idx + 1], f[bi], f[bj]); ++idx; }
+      for (int bi = 0; bi < bj; bi += 2) { tile_mma2_f64(acc[2 * idx], acc[2 * idx + 1], acc[2 * idx + 2], acc[2 * idx + 3], f[bi], f[bi + 1], f[bj]); idx += 2; }
+      if (bj % 2 == 0) { tile_mma_f64(acc[2 * idx], acc[2 * idx + 1], f[bj], f[bj]); ++idx; }
+    }
   }
 }
 
@@ -46,9 +60,9 @@ __device__ __forceinline__ void tile_flush(const NeLayout& L, const int* __restr
   const int ldbm1 = L.ldb - 1;
   int idx = 0;
 #pragma unroll
-  for (int bi = 0; bi < NB; ++bi)
+  for (int bj = 0; bj < NB; ++bj)                                                 // tile_syrk's fragment order
 #pragma unroll
-    for (int bj = bi; bj < NB; ++bj) {
+    for (int bi = 0; bi <= bj; ++bi) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         double v = acc[2 * idx + e];

@@ -10,7 +10,7 @@
 //    expanded into the same tile after the x rows have been contracted.  Neither row is held in registers, so chain and
 //    accumulators fit in 255 registers together and nothing spills; the park is 36 instead of 78 doubles per lane, which is what
 //    lets eight warps' tiles and parks fit in one block's shared memory.
-//  * The corners of all frames form ONE packed stream (frames padded to a multiple of 4 = one m8n8k4 k-step) that is cut into
+//  * The corners of all frames form ONE packed stream (frames padded to a multiple of 4 = one tensor-core k-step) that is cut into
 //    equal runs of 32-lane chunks, one run per warp: no partial last wave, no half-empty chunk at the end of a 144-corner frame.
 //    A chunk may straddle two frames (two staged knot windows, lanes pick theirs); the k-steps of the first frame finish its
 //    tile, which is flushed, before the k-steps of the second start a new one.
