@@ -9,6 +9,7 @@ from helpers import F_STAGE1, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_scaled_parity
 
 F_CI, F_TO = capi.FLAG_CAM_INTRINSICS, capi.FLAG_TIME_OFFSET
 
@@ -69,6 +70,7 @@ def test_gpu_extension_columns_match_oracle(oracle_factory, gpu_factory, k):
         co, ro, go, Ho = o.evaluate(flags, hessian=True)
         cg, rg, gg, Hg = g.evaluate(flags, hessian=True)
         assert abs(cg - co) <= 1e-9 * co and rel(rg, ro) < 1e-9 and rel(gg, go) < 1e-9 and rel(Hg, Ho) < 1e-9
+        assert_scaled_parity(g, flags, (co, ro, go, Ho), (cg, rg, gg, Hg))
 
 
 @pytest.mark.gpu

@@ -11,6 +11,7 @@ import pytest
 
 from bias_walk_support import DRIFT, drifting_dataset, new_bias_walk_oracle, prior_rows_of
 from openimucameracalibrator_b200 import _capi as capi, calibrator, io_formats, synthetic as syn
+from scaled_parity import assert_block_probes, assert_scaled_parity, probe_reference
 from test_tangent_spline import set_oracle_bearings
 
 pytestmark = pytest.mark.gpu
@@ -68,6 +69,7 @@ def test_prior_parity_dense(spacing, sensors, free, tangent):
     co, ro, go, Ho = o.evaluate(FLAGS[free], hessian=True)
     assert abs(cg - co) <= 1e-9 * abs(co)
     assert _rel(rg, ro) < 1e-9 and _rel(gg, go) < 1e-9 and _rel(Hg, Ho) < 1e-9
+    assert_scaled_parity(g, FLAGS[free], (co, ro, go, Ho), (cg, rg, gg, Hg))      # the prior rows and bias columns at their own scale
     nres = sum(g.num_residuals())
     assert np.abs(rg[nres:]).min() > 0.0
     cc, rc, _, _ = g.evaluate(FLAGS[free], gradient=False)                  # the cost-only kernel path
@@ -106,6 +108,7 @@ def test_config4_normal_equations_and_border_limit():
     Vb = np.zeros((1, n)); Vb[0, n - 6 * g.num_knots()[2]:] = 1.0              # the bias columns (last in the canonical order here)
     V = np.concatenate([V, Vb])
     assert _rel(g.normal_matvec(F_BIAS, V), o.normal_matvec(F_BIAS, V)) < 1e-9
+    assert_block_probes(g, probe_reference(o, F_BIAS, rng))
     assert abs(g.evaluate(F_BIAS, residuals=False, gradient=False)[0] - o.evaluate(F_BIAS, residuals=False, gradient=False)[0]) <= 1e-9 * o.evaluate(F_BIAS, residuals=False, gradient=False)[0]
     s = g.lm_iterations(2, F_BIAS)                                              # 2 s: 2 * 3 * 52 + 6 = 318 border columns, solved
     assert s.iterations == 2 and np.isfinite(s.final_cost)

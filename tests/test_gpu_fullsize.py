@@ -15,6 +15,7 @@ import pytest
 from helpers import F_STAGE1, TangentWalker, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_block_probes, probe_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -91,6 +92,7 @@ def test_config4_jacobian_parity_against_oracle(oracle_factory, gpu_factory, ds4
     Hg, Ho = g.normal_matvec(F_STAGE1, V), o.normal_matvec(F_STAGE1, V)
     for a, b in zip(Hg, Ho):
         assert rel(a, b) < 1e-9
+    assert_block_probes(g, probe_reference(o, F_STAGE1, rng))       # each column block and the end knots at their own scale
 
 
 def test_config4_lm_parity_against_oracle(oracle_factory, gpu_factory, ds4):

@@ -1,5 +1,6 @@
 """Parity of the CUDA path (through the C-ABI) against the CPU oracle on identical seeded inputs.
-FP64 tolerances: residuals / cost / J^T r / J^T J relative 1e-9 (observed ~1e-14); LM end state relative 1e-8;
+FP64 tolerances: residuals / cost / J^T r / J^T J relative 1e-9 (observed ~1e-14), and 1e-9 again with every block at its own scale
+(scaled_parity.py: Jacobi-scaled J^T J, J^T r against |r| sqrt(diag), residuals per kind; observed <= 4e-14 on an H100); LM end state relative 1e-8;
 north-star bar on converged T_cam_imu / line delay: 1e-4 relative."""
 import os
 
@@ -11,6 +12,7 @@ from helpers import F_ALL, F_STAGE1, F_STAGE2, TangentWalker, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_scaled_parity
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-9
@@ -30,6 +32,7 @@ def _assert_eval_parity(o, g, flags, hessian=True):
     if hessian:
         assert rel(Hg, Ho) < TOL
         assert np.array_equal(Hg, Hg.T)
+        assert_scaled_parity(g, flags, (co, ro, go, Ho), (cg, rg, gg, Hg))   # each block at its own scale
     c2 = g.evaluate(flags, residuals=False, gradient=False)[0]     # cost-only kernels agree with the Jacobian kernels
     assert abs(c2 - cg) <= 1e-12 * abs(cg)
 
@@ -84,6 +87,8 @@ def test_gpu_matches_committed_golden(gpu_factory, path, eval_path):
         c, r, gr, H = g.evaluate(flags, hessian=True)
         assert abs(c - float(ds[f"{tag}_cost"])) <= TOL * abs(c)
         assert rel(r, ds[f"{tag}_residuals"]) < TOL and rel(gr, ds[f"{tag}_gradient"]) < TOL and rel(H, ds[f"{tag}_hessian"]) < TOL
+        golden = tuple(ds[f"{tag}_{x}"] for x in ("cost", "residuals", "gradient", "hessian"))
+        assert_scaled_parity(g, flags, golden, (c, r, gr, H))
     g2 = gpu_factory(); capi.load_dataset(g2, ds, known_gravity=True)
     s1 = g2.optimize(50, F_STAGE1)
     assert s1.iterations == int(ds["lm_stage1_iterations"]) and s1.gpu_launches > 0

@@ -12,6 +12,7 @@ from helpers import F_STAGE1, TangentWalker, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_block_probes, probe_reference
 
 pytestmark = pytest.mark.gpu
 FLAGS = F_STAGE1 | capi.FLAG_POINTS
@@ -41,6 +42,7 @@ def test_points_jacobian_parity(oracle_factory, gpu_factory, eval_path, model, i
     V = rng.normal(size=(4, n)); V[1, : n - 3 * npts] = 0.0; V[2, n - 3 * npts:] = 0.0
     for a, b in zip(g.normal_matvec(FLAGS, V), o.normal_matvec(FLAGS, V)):
         assert rel(a, b) < 1e-9
+    assert_block_probes(g, probe_reference(o, FLAGS, rng))
 
 
 def test_points_gradient_against_finite_differences(gpu_factory):

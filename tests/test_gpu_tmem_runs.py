@@ -19,6 +19,7 @@ from helpers import F_ALL, F_STAGE1, F_STAGE2, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_block_probes, probe_reference
 
 CHUNK = 32
 CTA_WARPS = 6                   # warps per CTA of the persistent kernel (eval_tmem_warps)
@@ -385,6 +386,7 @@ def test_config2_schedule_invariance(oracle_factory, gpu_factory, tmem_runs):
         n = o.num_tangent(flags)
         V = rng.normal(size=(4, n)); V[1, : n - 9] = 0.0; V[2, n - 9:] = 0.0      # all columns / border only / band only / all
         ref[flags] = (co, go, V, o.normal_matvec(flags, V))
+    probes = {flags: probe_reference(o, flags, rng) for flags in ref}           # each column block and the end knots at their own scale
     for cap in (None, 96, 7):
         tmem_runs(cap)
         g = gpu_factory(); capi.load_dataset(g, ds, known_gravity=False)
@@ -396,6 +398,7 @@ def test_config2_schedule_invariance(oracle_factory, gpu_factory, tmem_runs):
             assert abs(cg - co) <= 1e-9 * co and rel(gg, go) < 1e-9, (cap, flags)
             for a, b in zip(g.normal_matvec(flags, V), Ho):
                 assert rel(a, b) < 1e-9, (cap, flags)
+            assert_block_probes(g, probes[flags])
         g.close()
 
 
@@ -432,3 +435,4 @@ def test_points_in_multi_chunk_runs(oracle_factory, gpu_factory, tmem_runs):
     V = rng.normal(size=(4, n)); V[1, : n - 3 * npts] = 0.0; V[2, n - 3 * npts:] = 0.0
     for a, b in zip(g.normal_matvec(flags, V), o.normal_matvec(flags, V)):
         assert rel(a, b) < 1e-9
+    assert_block_probes(g, probe_reference(o, flags, rng))

@@ -17,6 +17,7 @@ import pytest
 from helpers import F_STAGE1, qexp, qmul, rel
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_block_probes, probe_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "..", "openimucameracalibrator_b200", "csrc")
@@ -117,3 +118,4 @@ def test_table_follows_set_knots(oracle_factory, gpu_factory, monkeypatch):
     V = rng.normal(size=(2, n)); V[1, : n - 6] = 0.0
     for a, b in zip(g.normal_matvec(F_STAGE1, V), o.normal_matvec(F_STAGE1, V)):
         assert rel(a, b) < 1e-9
+    assert_block_probes(g, probe_reference(o, F_STAGE1, rng))

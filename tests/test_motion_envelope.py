@@ -12,6 +12,7 @@ from motion_support import R_IC, branch_census, make_motion_dataset, truth_knots
 from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_scaled_parity
 
 TOL = 1e-9
 INCREMENT = 2.4                      # rad per SO(3) knot interval at full spin: |lambda theta / 2| reaches 1.2 > pi/4
@@ -139,6 +140,7 @@ def _assert_eval_parity(o, g, flags):
     assert np.isfinite(cg) and np.isfinite(rg).all() and np.isfinite(gg).all() and np.isfinite(Hg).all()
     assert abs(cg - co) <= TOL * abs(co)
     assert rel(rg, ro) < TOL and rel(gg, go) < TOL and rel(Hg, Ho) < TOL
+    assert_scaled_parity(g, flags, (co, ro, go, Ho), (cg, rg, gg, Hg))
     c2 = g.evaluate(flags, residuals=False, gradient=False)[0]
     assert abs(c2 - cg) <= 1e-12 * abs(cg)
     return rg

@@ -22,6 +22,7 @@ from openimucameracalibrator_b200 import _capi as capi
 from openimucameracalibrator_b200 import camera_models as cm
 from openimucameracalibrator_b200 import io_formats as iof
 from openimucameracalibrator_b200 import synthetic as syn
+from scaled_parity import assert_scaled_parity
 from test_camera_models import CASES
 from test_host_device_math import _B6, _qexp, _qmat, _qmul, _spline_rotation
 from wide_angle_support import oracle_bearings
@@ -341,6 +342,7 @@ def _parity(g, o, flags):
     co, ro, go, Ho = o.evaluate(flags, hessian=True)
     assert abs(cg - co) <= 1e-9 * abs(co), (cg, co)
     assert rel(rg, ro) < 1e-9 and rel(gg, go) < 1e-9 and rel(Hg, Ho) < 1e-9, (rel(rg, ro), rel(gg, go), rel(Hg, Ho))
+    assert_scaled_parity(g, flags, (co, ro, go, Ho), (cg, rg, gg, Hg))
 
 
 @pytest.mark.gpu
