@@ -627,6 +627,32 @@ icc_status icc_allan_variance(icc_handle* h, int n, const double* t_s, const dou
  * every factor.  `factors` NULL returns F in *len; otherwise *len is the capacity of each array. */
 icc_status icc_get_allan_curves(const icc_handle* h, int channel, int32_t* factors, double* tau, double* sigma2, double* fit_deviation, int32_t* len);
 
+/* ---- upstream: radon checkerboard corners (extract_board_to_json --board_type radon) ---------------------------------------------------
+ * BoardExtractor::ExtractBoard for BoardType::RADON (src/core/board_extractor.cc): cv::resize(frame, 1/f, INTER_LINEAR), then
+ * cv::findChessboardCornersSB(CALIB_CB_LARGER | CALIB_CB_MARKER | CALIB_CB_EXHAUSTIVE) on the board of resource/checkerboard_radon.png
+ * (corners_x x corners_y inner corners, 14 x 9 for the printed board, three circle markers next to the centre).  frames: n_frames 8-bit
+ * gray images of width x height, row pitch pitch_bytes, frame k at frames + k height pitch_bytes, in host or device memory (detected
+ * with cudaPointerGetAttributes; device frames are not copied through the host).  A frame is found iff exactly corners_x x
+ * corners_y corners form one grid and the three markers sit in their squares; then uv_out holds its corners in the downsampled
+ * image's pixels in id order id = i corners_x + j (row i, column j; the reference's continuous_board_indices_), in the corner order
+ * findChessboardCornersSB returns.  Frames that are not found get found = 0 and their uv_out is left untouched.
+ * ICC_ERR_INVALID_ARGUMENT, with nothing launched: corners_x or corners_y < 3, a factor < 1 or not finite, pitch < width, a NULL
+ * frame or output pointer. */
+typedef struct icc_board_summary {
+  int32_t width, height;             /* the downsampled frame size */
+  int32_t n_found;
+  int32_t n_no_grid;                 /* too few candidates, or no grid grew from the seed */
+  int32_t n_wrong_count;             /* the grid is not exactly corners_x x corners_y (a partial or a larger board) */
+  int32_t n_no_markers;              /* the grid is complete but the three markers are not where the board has them */
+  int64_t candidate_overflow;        /* candidates dropped because a frame's list (1024) was full, summed over the frames */
+  int32_t gpu_launches;
+  int32_t reserved;
+  double seconds;                    /* host wall clock of the call */
+} icc_board_summary;
+icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int height, int64_t pitch_bytes, const uint8_t* frames, int corners_x,
+                                   int corners_y, double downsample_factor, double* uv_out /* n_frames * corners_x * corners_y * 2 */,
+                                   int32_t* found /* n_frames */, icc_board_summary* summary /* nullable */);
+
 /* Device blocks of destroyed handles are cached process-wide for the next job; this returns them to the CUDA driver. */
 void icc_trim_device_cache(void);
 

@@ -150,6 +150,38 @@ def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
+class BoardSummary(C.Structure):
+    """icc_board_summary (include/icc_b200.h): what one icc_extract_radon_board call did."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_found", C.c_int32), ("n_no_grid", C.c_int32), ("n_wrong_count", C.c_int32),
+                ("n_no_markers", C.c_int32), ("candidate_overflow", C.c_int64), ("gpu_launches", C.c_int32), ("reserved", C.c_int32),
+                ("seconds", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
+def _frames_pointer(frames):
+    """(pointer, n, height, width, pitch in bytes) of 8-bit frames: an (N, H, W) or (H, W) uint8 NumPy array, or a torch CUDA tensor,
+    whose rows are contiguous and whose frames are `height` rows of one pitch apart."""
+    if hasattr(frames, "data_ptr"):   # torch tensor: passed by pointer, never copied through the host
+        t = frames if frames.dim() == 3 else frames.unsqueeze(0)
+        assert str(t.dtype) == "torch.uint8", t.dtype
+        n, h, w = t.shape
+        s0, s1, s2 = t.stride()
+        ptr = t.data_ptr()
+    else:
+        a = np.asarray(frames)
+        if a.ndim == 2:
+            a = a[None]
+        assert a.dtype == np.uint8, a.dtype
+        n, h, w = a.shape
+        s0, s1, s2 = a.strides
+        ptr = a.ctypes.data
+    if s2 != 1 or (n > 1 and s0 != h * s1) or s1 < w:
+        raise ValueError("frames need contiguous rows, one row pitch >= width, and frames `height` rows apart")
+    return ptr, n, h, w, s1
+
+
 class CApi:
     """Thin object wrapper around one solver handle of a loaded library."""
 
@@ -410,6 +442,19 @@ class CApi:
         self._call("get_allan_curves", args, int(channel), f.ctypes.data_as(c_int32_p), _dp(t), _dp(s2), _dp(d), C.byref(n))
         k = n.value
         return dict(factors=f[:k].astype(np.int64), tau=t[:k], sigma2=s2[:k], fit_deviation=d[:k])
+
+    # ---- upstream: radon checkerboard corners (src/core/board_extractor.cc, BoardType::RADON) ----------------------------------
+    def extract_radon_board(self, frames, corners_x, corners_y, downsample_factor=1.0):
+        """-> (uv (N, corners_y * corners_x, 2) in id order, NaN for frames not found, found (N,) bool, summary dict).  frames: (N, H, W)
+        or (H, W) uint8 NumPy array, or a torch CUDA uint8 tensor (read on the device by pointer)."""
+        ptr, n, h, w, pitch = _frames_pointer(frames)
+        uv = np.full((n, corners_x * corners_y, 2), np.nan)
+        found = np.zeros(n, dtype=np.int32)
+        s = BoardSummary()
+        self._call("extract_radon_board", [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_double, c_double_p, c_int32_p,
+                                           C.POINTER(BoardSummary)], n, w, h, pitch, C.c_void_p(ptr), int(corners_x), int(corners_y),
+                   float(downsample_factor), _dp(uv), found.ctypes.data_as(c_int32_p), C.byref(s))
+        return uv, found.astype(bool), s.as_dict()
 
     # ---- upstream row f2: spline error weighting (python/sew.py:knot_spacing_and_variance) ------------------------------------
     def spline_error_weighting(self, times_s, signal_xyz, quality, min_dt=0.0, max_dt=0.0, want_spectrum=False):

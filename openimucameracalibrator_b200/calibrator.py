@@ -333,3 +333,37 @@ class AllanVarianceFitter:
 
     def curves(self, channel: int) -> dict:
         return self._api.allan_curves(channel)
+
+
+class BoardExtractor:
+    """BoardExtractor for BoardType::RADON (src/core/board_extractor.cc) on the GPU: InitializeRadonBoard, then frames -> the scene
+    dictionary of the corner file (the layout io_formats.write_dataset_files writes and icccli::load_scene reads)."""
+
+    def __init__(self, square_length_m: float, corners_x: int = 14, corners_y: int = 9, device: int = 0):
+        self.square_length_m, self.corners_x, self.corners_y = float(square_length_m), int(corners_x), int(corners_y)
+        self.api = CApi(load_library(), "icc_", device)
+
+    def scene_points(self) -> dict:
+        """id -> (i s, j s, 0): the reference puts the row index i on x (InitializeRadonBoard)."""
+        s, W = self.square_length_m, self.corners_x
+        return {str(i * W + j): [float(i * s), float(j * s), 0.0] for i in range(self.corners_y) for j in range(W)}
+
+    def extract(self, frames, timestamps_s, downsample_factor: float = 1.0) -> dict:
+        """Corner-file dictionary of the frames: views named io_formats.view_key(t), written only for frames where the board was found."""
+        from .io_formats import view_key
+        uv, found, summary = self.api.extract_radon_board(frames, self.corners_x, self.corners_y, downsample_factor)
+        views = {}
+        for k, t in enumerate(timestamps_s):
+            if found[k]:
+                views[view_key(float(t))] = {"image_points": {str(c): [float(uv[k, c, 0]), float(uv[k, c, 1])] for c in range(uv.shape[1])}}
+        self.summary = summary
+        return {"calibration_board_type": 1, "square_size_meter": self.square_length_m, "image_width": int(summary["width"]),
+                "image_height": int(summary["height"]), "scene_pts": self.scene_points(), "views": views}
+
+    def write(self, path: str, frames, timestamps_s, downsample_factor: float = 1.0) -> dict:
+        """extract(), written as UBJSON with io_formats.ubjson_dumps; returns the dictionary."""
+        from .io_formats import ubjson_dumps
+        scene = self.extract(frames, timestamps_s, downsample_factor)
+        with open(path, "wb") as f:
+            f.write(ubjson_dumps(scene))
+        return scene

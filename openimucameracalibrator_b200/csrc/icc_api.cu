@@ -1926,6 +1926,26 @@ icc_status icc_get_corner_status(const icc_handle* hc, int n_input, int32_t* sta
   return ICC_OK;
 }
 
+// ---- upstream: radon checkerboard corners (icc_board.cu) -------------------------------------------------------------------------------
+icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, int corners_x, int corners_y,
+                                   double f, double* uv_out, int32_t* found, icc_board_summary* summary) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (n_frames < 0 || width < 1 || height < 1 || pitch < width || corners_x < 3 || corners_y < 3 || !(f >= 1.0) || !std::isfinite(f) ||
+      (n_frames > 0 && (!frames || !uv_out || !found)))
+    return fail(h, ICC_ERR_INVALID_ARGUMENT, "icc_extract_radon_board needs corners_x, corners_y >= 3, a finite downsample factor >= 1, pitch >= width and non-NULL frames and outputs");
+  NEED_DEVICE();
+  icc_board_summary S;
+  memset(&S, 0, sizeof S);
+  if (n_frames == 0) { if (summary) *summary = S; return ICC_OK; }
+  cudaPointerAttributes at;
+  bool on_device = false;
+  if (cudaPointerGetAttributes(&at, frames) == cudaSuccess) on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  else cudaGetLastError();
+  const icc_status rc = drive(h, [&](std::string& err) { return extract_radon_board(h->stream, n_frames, width, height, pitch, frames, on_device, corners_x, corners_y, f, uv_out, found, S, err); });
+  if (rc == ICC_OK && summary) *summary = S;
+  return rc;
+}
+
 void icc_trim_device_cache(void) { block_cache().trim(); pinned_cache().trim(); }
 
 }  // extern "C"

@@ -342,3 +342,133 @@ def allan_small(seed=5) -> dict:
 def allan_full_size(seed=6) -> dict:
     """2 hours at 400 Hz (2.88 M samples)."""
     return make_allan_log(400.0, 7200.0, seed)
+
+
+# ---- radon checkerboard renderer ------------------------------------------------------------------------------------
+# The board of the reference's resource/checkerboard_radon.png: (W + 1) x (H + 1) squares around W x H inner corners (14 x 9
+# for the printed board), the top-left square white, black squares on the border rounded outward by a half disk, and three
+# circle markers of diameter 0.36 squares near the centre.  In the board frame corner (i, j) sits at (i s, j s, 0) like the
+# reference's scene points: x runs up the printed sheet (i = 0 is the bottom inner row), y runs right, z points into the sheet.
+RADON_MARKER_RADIUS = 0.18   # squares
+
+
+def radon_marker_cell(corners_x: int, corners_y: int):
+    """Board cell (i, j) (corners (i..i+1, j..j+1)) of the L-shaped marker triple's vertex: a black circle in a white square.
+    The arms are the cells (i + 1, j) and (i, j + 1), white circles in black squares."""
+    return corners_y // 2 - 1, corners_x // 2 - 1
+
+
+def radon_board_points(corners_x: int, corners_y: int, square_m: float):
+    """(H W, 3) board points in id order id = i W + j."""
+    i, j = np.meshgrid(np.arange(corners_y), np.arange(corners_x), indexing="ij")
+    return np.stack([i.ravel() * square_m, j.ravel() * square_m, np.zeros(i.size)], -1)
+
+
+def radon_board_shade(xb, yb, corners_x: int, corners_y: int, square_m: float, markers: bool = True, marker_cell=None):
+    """Reflectance in [0, 1] (0 black) at board-frame points (xb, yb).  `marker_cell` moves the marker triple's vertex to another
+    cell (a board that is not the radon board)."""
+    W, H = corners_x, corners_y
+    u = yb / square_m + 1.0                     # printed columns from the left edge, 0 .. W + 1
+    v = (H - 1) - xb / square_m + 1.0           # printed rows from the top edge, 0 .. H + 1
+    C, R = np.floor(u), np.floor(v)
+    inside = (C >= 0) & (C <= W) & (R >= 0) & (R <= H)
+    black = ((R + C) % 2 == 1) & inside
+    du, dv = u - C - 0.5, v - R - 0.5           # offset from the square's centre, squares
+    outward = ((C == 0) & (du < 0)) | ((C == W) & (du > 0)) | ((R == 0) & (dv < 0)) | ((R == H) & (dv > 0))
+    black &= ~outward | (du * du + dv * dv <= 0.25)
+    if markers:
+        mi, mj = radon_marker_cell(W, H) if marker_cell is None else marker_cell
+        dot = du * du + dv * dv <= RADON_MARKER_RADIUS ** 2
+        for ci, cj in ((mi, mj), (mi + 1, mj), (mi, mj + 1)):
+            black ^= dot & (C == cj + 1) & (R == H - 1 - ci)
+    return np.where(black, 0.0, 1.0)
+
+
+def unproject_grid(model: int, intr, uv, iters: int = 30):
+    """Camera-frame rays (x, y, 1) of pixels uv (..., 2) by damped Newton on cm.project with a central-difference Jacobian."""
+    uv = np.asarray(uv, dtype=np.float64)
+    k = np.asarray(intr, dtype=np.float64)
+    f = k[0]
+    cx, cy = (k[2], k[3]) if model in (cm.FOV, cm.DIVISION_UNDISTORTION) else (k[3], k[4])
+    x = np.stack([(uv[..., 0] - cx) / f, (uv[..., 1] - cy) / f], -1)
+    one = np.ones(uv.shape[:-1])
+
+    def proj(xy):
+        return cm.project(model, k, np.stack([xy[..., 0], xy[..., 1], one], -1))[0]
+    h = 1e-6
+    for _ in range(iters):
+        r = proj(x) - uv
+        J = np.stack([(proj(x + [h, 0]) - proj(x - [h, 0])) / (2 * h), (proj(x + [0, h]) - proj(x - [0, h])) / (2 * h)], -1)
+        det = J[..., 0, 0] * J[..., 1, 1] - J[..., 0, 1] * J[..., 1, 0]
+        dx = (J[..., 1, 1] * r[..., 0] - J[..., 0, 1] * r[..., 1]) / det
+        dy = (-J[..., 1, 0] * r[..., 0] + J[..., 0, 0] * r[..., 1]) / det
+        step = np.stack([dx, dy], -1)
+        n = np.linalg.norm(step, axis=-1, keepdims=True)
+        x = x - step * np.minimum(1.0, 0.5 / np.maximum(n, 1e-300))   # damped: at most 0.5 in normalised units per step
+        if np.nanmax(np.abs(r)) < 1e-9:
+            break
+    ok = np.linalg.norm(proj(x) - uv, axis=-1) < 1e-6
+    return np.stack([x[..., 0], x[..., 1], one], -1), ok
+
+
+def radon_view_pose(corners_x: int, corners_y: int, square_m: float, distance_m: float, tilt_deg: float = 0.0, tilt_axis_deg: float = 0.0,
+                    roll_deg: float = 0.0, offset_m=(0.0, 0.0)):
+    """(R_cb, t_cb) of a camera `distance_m` in front of the board centre: the printed sheet upright in the image at roll 0, tilted
+    by `tilt_deg` about an in-plane axis at `tilt_axis_deg`, rolled about the optical axis, and the board shifted by `offset_m`."""
+    R_bc0 = np.array([[0.0, -1.0, 0.0], [1.0, 0.0, 0.0], [0.0, 0.0, 1.0]])   # camera x = board y, camera y = -board x, camera z = board z
+    a = np.deg2rad(tilt_axis_deg)
+    tilt = so3_exp(np.deg2rad(tilt_deg) * np.array([np.cos(a), np.sin(a), 0.0]))
+    roll = so3_exp(np.array([0.0, 0.0, np.deg2rad(roll_deg)]))
+    R_cb = roll @ tilt @ R_bc0.T
+    centre = np.array([(corners_y - 1) * square_m / 2, (corners_x - 1) * square_m / 2, 0.0])
+    t_cb = np.array([offset_m[0], offset_m[1], distance_m]) - R_cb @ centre
+    return R_cb, t_cb
+
+
+def render_radon_board(model: int, intr, size, R_cb, t_cb, corners_x: int = 14, corners_y: int = 9, square_m: float = 0.03,
+                       supersample: int = 4, blur_sigma_px: float = 0.0, noise_sigma_dn: float = 0.0, seed: int = 0, markers: bool = True,
+                       black_dn: float = 30.0, white_dn: float = 220.0, rays=None, marker_cell=None):
+    """uint8 (height, width) image of the radon board seen by the camera (model, intr) at board-to-camera pose (R_cb, t_cb), by
+    supersampled ray casting (supersample^2 stratified, jittered rays per pixel, pixel centres at integer coordinates); optional
+    Gaussian blur and noise.  Returns (image, truth uv (H W, 2) in id order, truth valid).  `rays` reuses camera_rays(...) of the same camera."""
+    width, height = size
+    if rays is None:
+        rays = camera_rays(model, intr, size, supersample)
+    d, ok = rays
+    R_cb, t_cb = np.asarray(R_cb, float), np.asarray(t_cb, float)
+    n = R_cb[:, 2]
+    lam = (n @ t_cb) / (d @ n)
+    pb = (lam[..., None] * d - t_cb) @ R_cb                       # R_cb^T (lam d - t)
+    hit = ok & (lam > 0)
+    shade = np.where(hit, radon_board_shade(pb[..., 0], pb[..., 1], corners_x, corners_y, square_m, markers, marker_cell), 1.0)
+    img = shade.reshape(height, supersample, width, supersample).mean(axis=(1, 3))
+    img = black_dn + (white_dn - black_dn) * img
+    if blur_sigma_px > 0:
+        from scipy.ndimage import gaussian_filter
+        img = gaussian_filter(img, blur_sigma_px, mode="nearest")
+    if noise_sigma_dn > 0:
+        img = img + np.random.default_rng(seed).normal(0.0, noise_sigma_dn, img.shape)
+    img = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+    pc = radon_board_points(corners_x, corners_y, square_m) @ R_cb.T + t_cb
+    uv, valid = cm.project(model, intr, pc)
+    valid = valid & (pc[:, 2] > 0) & (uv[:, 0] >= 0) & (uv[:, 0] <= width - 1) & (uv[:, 1] >= 0) & (uv[:, 1] <= height - 1)
+    return img, uv, valid
+
+
+_RAYS = {}
+
+
+def camera_rays(model: int, intr, size, supersample: int = 4):
+    """Rays of the supersampled pixel grid (height * ss, width * ss, 3) and their validity, cached per camera.  Each pixel's ss x ss
+    cells get one ray at a uniformly random point inside the cell (a fixed seed): a regular grid would put every edge of an
+    axis-aligned square at the same sub-cell phase and bias its rendered position by up to 1 / (2 ss) px."""
+    key = (model, tuple(float(x) for x in intr), tuple(size), supersample)
+    if key not in _RAYS:
+        width, height = size
+        cells = np.arange(supersample) / supersample - 0.5
+        jit = np.random.default_rng(12345).uniform(0.0, 1.0 / supersample, (2, height * supersample, width * supersample))
+        uu = (np.arange(width)[:, None] + cells[None]).ravel()[None, :] + jit[0]
+        vv = (np.arange(height)[:, None] + cells[None]).ravel()[:, None] + jit[1]
+        _RAYS.clear()
+        _RAYS[key] = unproject_grid(model, intr, np.stack([uu, vv], -1))
+    return _RAYS[key]
