@@ -652,6 +652,18 @@ typedef struct icc_board_summary {
 icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int height, int64_t pitch_bytes, const uint8_t* frames, int corners_x,
                                    int corners_y, double downsample_factor, double* uv_out /* n_frames * corners_x * corners_y * 2 */,
                                    int32_t* found /* n_frames */, icc_board_summary* summary /* nullable */);
+/* The same for colour frames: rows hold width interleaved B, G, R bytes (cv::imread's order), pitch_bytes >= 3 width.  The first stage is the
+ * reference's order, cv::resize of the colour image (each channel as icc_extract_radon_board resizes gray) and then cv::cvtColor(BGR2GRAY)
+ * with OpenCV's 15-bit rule (B 3735 + G 19235 + R 9798 + 16384) >> 15; at a factor of 1 only the conversion.  Every later step, the
+ * argument checks, the chunking and the summary are those of icc_extract_radon_board.  A gray frame replicated to B = G = R gives the
+ * same corners through either entry. */
+icc_status icc_extract_radon_board_bgr(icc_handle* h, int n_frames, int width, int height, int64_t pitch_bytes, const uint8_t* frames_bgr, int corners_x,
+                                       int corners_y, double downsample_factor, double* uv_out /* n_frames * corners_x * corners_y * 2 */,
+                                       int32_t* found /* n_frames */, icc_board_summary* summary /* nullable */);
+/* Page-locked host memory (cudaHostAlloc) for frames that a host program fills and hands to the extraction entries; *p = NULL for 0 bytes.
+ * ICC_ERR_NO_DEVICE without a GPU, ICC_ERR_CUDA when the allocation fails.  Free with icc_host_free_pinned (NULL is accepted). */
+icc_status icc_host_alloc_pinned(uint64_t bytes, void** p);
+icc_status icc_host_free_pinned(void* p);
 
 /* Device blocks of destroyed handles are cached process-wide for the next job; this returns them to the CUDA driver. */
 void icc_trim_device_cache(void);

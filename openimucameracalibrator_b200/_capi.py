@@ -182,6 +182,28 @@ def _frames_pointer(frames):
     return ptr, n, h, w, s1
 
 
+def _bgr_frames_pointer(frames):
+    """(pointer, n, height, width, pitch in bytes) of 8-bit B, G, R frames: an (N, H, W, 3) or (H, W, 3) uint8 NumPy array, or a torch CUDA
+    tensor, whose pixels are interleaved and contiguous along each row and whose frames are `height` rows of one pitch apart."""
+    if hasattr(frames, "data_ptr"):
+        t = frames if frames.dim() == 4 else frames.unsqueeze(0)
+        assert str(t.dtype) == "torch.uint8", t.dtype
+        n, h, w, c = t.shape
+        s0, s1, s2, s3 = t.stride()
+        ptr = t.data_ptr()
+    else:
+        a = np.asarray(frames)
+        if a.ndim == 3:
+            a = a[None]
+        assert a.dtype == np.uint8, a.dtype
+        n, h, w, c = a.shape
+        s0, s1, s2, s3 = a.strides
+        ptr = a.ctypes.data
+    if c != 3 or s3 != 1 or s2 != 3 or (n > 1 and s0 != h * s1) or s1 < 3 * w:
+        raise ValueError("colour frames need 3 interleaved channels, contiguous rows, one row pitch >= 3 width, and frames `height` rows apart")
+    return ptr, n, h, w, s1
+
+
 class CApi:
     """Thin object wrapper around one solver handle of a loaded library."""
 
@@ -453,6 +475,18 @@ class CApi:
         s = BoardSummary()
         self._call("extract_radon_board", [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_double, c_double_p, c_int32_p,
                                            C.POINTER(BoardSummary)], n, w, h, pitch, C.c_void_p(ptr), int(corners_x), int(corners_y),
+                   float(downsample_factor), _dp(uv), found.ctypes.data_as(c_int32_p), C.byref(s))
+        return uv, found.astype(bool), s.as_dict()
+
+    def extract_radon_board_bgr(self, frames, corners_x, corners_y, downsample_factor=1.0):
+        """extract_radon_board for colour frames, resized and then converted to gray as the reference does (icc_extract_radon_board_bgr).
+        frames: (N, H, W, 3) or (H, W, 3) uint8 in B, G, R order (cv2.imread's), a NumPy array or a torch CUDA tensor."""
+        ptr, n, h, w, pitch = _bgr_frames_pointer(frames)
+        uv = np.full((n, corners_x * corners_y, 2), np.nan)
+        found = np.zeros(n, dtype=np.int32)
+        s = BoardSummary()
+        self._call("extract_radon_board_bgr", [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_double, c_double_p, c_int32_p,
+                                               C.POINTER(BoardSummary)], n, w, h, pitch, C.c_void_p(ptr), int(corners_x), int(corners_y),
                    float(downsample_factor), _dp(uv), found.ctypes.data_as(c_int32_p), C.byref(s))
         return uv, found.astype(bool), s.as_dict()
 

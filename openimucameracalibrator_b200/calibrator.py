@@ -224,6 +224,8 @@ class CameraCalibrator:
         import json
         from .io_formats import intrinsics_dict
         pts = scene_json["scene_pts"]
+        if isinstance(pts, (list, tuple)):                         # the reference's radon files: an array indexed by id
+            pts = {i: p for i, p in enumerate(pts)}
         n = max(int(i) for i in pts) + 1
         board = np.zeros((n, 4)); board[:, 3] = 1.0
         for i, p in pts.items():

@@ -1927,12 +1927,15 @@ icc_status icc_get_corner_status(const icc_handle* hc, int n_input, int32_t* sta
 }
 
 // ---- upstream: radon checkerboard corners (icc_board.cu) -------------------------------------------------------------------------------
-icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, int corners_x, int corners_y,
-                                   double f, double* uv_out, int32_t* found, icc_board_summary* summary) {
+namespace {
+icc_status extract_radon(icc_handle* h, const char* name, bool bgr, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, int corners_x,
+                         int corners_y, double f, double* uv_out, int32_t* found, icc_board_summary* summary) {
   if (!h) return ICC_ERR_INVALID_ARGUMENT;
-  if (n_frames < 0 || width < 1 || height < 1 || pitch < width || corners_x < 3 || corners_y < 3 || !(f >= 1.0) || !std::isfinite(f) ||
+  const int64_t row = (bgr ? 3 : 1) * (int64_t)width;
+  if (n_frames < 0 || width < 1 || height < 1 || pitch < row || corners_x < 3 || corners_y < 3 || !(f >= 1.0) || !std::isfinite(f) ||
       (n_frames > 0 && (!frames || !uv_out || !found)))
-    return fail(h, ICC_ERR_INVALID_ARGUMENT, "icc_extract_radon_board needs corners_x, corners_y >= 3, a finite downsample factor >= 1, pitch >= width and non-NULL frames and outputs");
+    return fail(h, ICC_ERR_INVALID_ARGUMENT, std::string(name) + " needs corners_x, corners_y >= 3, a finite downsample factor >= 1, pitch >= " +
+                                                 (bgr ? "3 width" : "width") + " and non-NULL frames and outputs");
   NEED_DEVICE();
   icc_board_summary S;
   memset(&S, 0, sizeof S);
@@ -1941,9 +1944,33 @@ icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int h
   bool on_device = false;
   if (cudaPointerGetAttributes(&at, frames) == cudaSuccess) on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
   else cudaGetLastError();
-  const icc_status rc = drive(h, [&](std::string& err) { return extract_radon_board(h->stream, n_frames, width, height, pitch, frames, on_device, corners_x, corners_y, f, uv_out, found, S, err); });
+  const icc_status rc = drive(h, [&](std::string& err) { return extract_radon_board(h->stream, n_frames, width, height, pitch, frames, on_device, bgr, corners_x, corners_y, f, uv_out, found, S, err); });
   if (rc == ICC_OK && summary) *summary = S;
   return rc;
+}
+}  // namespace
+
+icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, int corners_x, int corners_y,
+                                   double f, double* uv_out, int32_t* found, icc_board_summary* summary) {
+  return extract_radon(h, "icc_extract_radon_board", false, n_frames, width, height, pitch, frames, corners_x, corners_y, f, uv_out, found, summary);
+}
+icc_status icc_extract_radon_board_bgr(icc_handle* h, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames_bgr, int corners_x, int corners_y,
+                                       double f, double* uv_out, int32_t* found, icc_board_summary* summary) {
+  return extract_radon(h, "icc_extract_radon_board_bgr", true, n_frames, width, height, pitch, frames_bgr, corners_x, corners_y, f, uv_out, found, summary);
+}
+
+icc_status icc_host_alloc_pinned(uint64_t bytes, void** p) {
+  if (!p) return ICC_ERR_INVALID_ARGUMENT;
+  *p = nullptr;
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ICC_ERR_NO_DEVICE; }
+  if (bytes == 0) return ICC_OK;
+  if (cudaHostAlloc(p, bytes, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); *p = nullptr; return ICC_ERR_CUDA; }
+  return ICC_OK;
+}
+icc_status icc_host_free_pinned(void* p) {
+  if (p && cudaFreeHost(p) != cudaSuccess) { cudaGetLastError(); return ICC_ERR_CUDA; }
+  return ICC_OK;
 }
 
 void icc_trim_device_cache(void) { block_cache().trim(); pinned_cache().trim(); }

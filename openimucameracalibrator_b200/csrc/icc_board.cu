@@ -4,7 +4,8 @@
 //
 // Frames go through in chunks of kChunk (ICC_BOARD_CHUNK_FRAMES overrides it), so device memory stays bounded whatever the count.
 // Per chunk:
-//   resize_kernel     cv::resize INTER_LINEAR (icc_board_math.cuh), skipped at f = 1;
+//   resize_kernel     cv::resize INTER_LINEAR (icc_board_math.cuh), skipped at f = 1; for colour frames bgr_gray_kernel instead:
+//                     cv::resize of each B, G, R channel, then OpenCV's BGR2GRAY (at f = 1 only the conversion);
 //   box_kernel        the 3x3 box mean, FP32;
 //   response_kernel   the localized Radon response, and the frame's maximum (atomicMax on the float's bits: responses are >= 0);
 //   candidate_kernel  one CTA per 32x32 tile: a pixel is a candidate when its response is >= kRelThreshold x the frame maximum and
@@ -46,6 +47,12 @@ __global__ void resize_kernel(const uint8_t* __restrict__ src, int sw, int sh, d
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, n = blockIdx.z;
   if (x >= dw || y >= dh) return;
   dst[((size_t)n * dh + y) * dw + x] = board::resize_pixel(src + (size_t)n * sw * sh, sw, sw, sh, f, x, y);
+}
+
+__global__ void bgr_gray_kernel(const uint8_t* __restrict__ src, int sw, int sh, double f, uint8_t* __restrict__ dst, int dw, int dh) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, n = blockIdx.z;
+  if (x >= dw || y >= dh) return;
+  dst[((size_t)n * dh + y) * dw + x] = board::bgr_resize_gray_pixel(src + (size_t)n * 3 * sw * sh, 3 * (int64_t)sw, sw, sh, f, x, y);
 }
 
 __global__ void box_kernel(const uint8_t* __restrict__ img, int w, int h, float* __restrict__ box) {
@@ -293,7 +300,7 @@ __global__ void __launch_bounds__(128) refine_kernel(const uint8_t* __restrict__
 
 #define CU(call) ICC_CUDA_CHECK(call, err)
 
-icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, int W, int H,
+icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, bool bgr, int W, int H,
                                double f, double* uv_out, int32_t* found, icc_board_summary& S, std::string& err) {
   const auto t0 = std::chrono::steady_clock::now();
   const int launches0 = kernel_launch_count();
@@ -306,22 +313,23 @@ icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int hei
   int chunk = kChunk;
   if (const char* e = getenv("ICC_BOARD_CHUNK_FRAMES")) chunk = std::max(1, atoi(e));
   chunk = std::min(chunk, std::max(n_frames, 1));
-  const size_t in_px = (size_t)width * height, px = (size_t)w * h, per = (size_t)W * H;
+  const size_t row = (size_t)width * (bgr ? 3 : 1), in_bytes = row * height, px = (size_t)w * h, per = (size_t)W * H;
   DevBuf<uint8_t> d_in, d_small; DevBuf<float> d_box, d_resp, d_spacing; DevBuf<unsigned> d_max; DevBuf<Cand> d_cand;
   DevBuf<int> d_count, d_over, d_status; DevBuf<float2> d_corner; DevBuf<double2> d_uv;
-  CU(d_in.alloc(chunk * in_px)); CU(d_box.alloc(chunk * px)); CU(d_resp.alloc(chunk * px)); CU(d_max.alloc(chunk));
-  if (scaled) CU(d_small.alloc(chunk * px));
+  CU(d_in.alloc(chunk * in_bytes)); CU(d_box.alloc(chunk * px)); CU(d_resp.alloc(chunk * px)); CU(d_max.alloc(chunk));
+  if (scaled || bgr) CU(d_small.alloc(chunk * px));
   CU(d_cand.alloc((size_t)chunk * kMaxCandidates)); CU(d_count.alloc(chunk)); CU(d_over.alloc(chunk)); CU(d_status.alloc(chunk));
   CU(d_corner.alloc(chunk * per)); CU(d_spacing.alloc(chunk * per)); CU(d_uv.alloc(chunk * per));
   std::vector<int> status(chunk), over(chunk);
   std::vector<double2> uv(chunk * per);
   for (int f0 = 0; f0 < n_frames; f0 += chunk) {
     const int nb = std::min(chunk, n_frames - f0);
-    CU(cudaMemcpy2DAsync(d_in.p, width, frames + (size_t)f0 * height * pitch, pitch, width, (size_t)nb * height,
+    CU(cudaMemcpy2DAsync(d_in.p, row, frames + (size_t)f0 * height * pitch, pitch, row, (size_t)nb * height,
                          frames_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     const uint8_t* img = d_in.p;
     const dim3 blk(32, 8), grd((w + 31) / 32, (h + 7) / 8, nb);
-    if (scaled) { resize_kernel<<<grd, blk, 0, st>>>(d_in.p, width, height, f, d_small.p, w, h); count_launch(); img = d_small.p; }
+    if (bgr) { bgr_gray_kernel<<<grd, blk, 0, st>>>(d_in.p, width, height, f, d_small.p, w, h); count_launch(); img = d_small.p; }
+    else if (scaled) { resize_kernel<<<grd, blk, 0, st>>>(d_in.p, width, height, f, d_small.p, w, h); count_launch(); img = d_small.p; }
     CU(cudaMemsetAsync(d_max.p, 0, nb * sizeof(unsigned), st)); CU(cudaMemsetAsync(d_count.p, 0, nb * sizeof(int), st)); CU(cudaMemsetAsync(d_over.p, 0, nb * sizeof(int), st));
     box_kernel<<<grd, blk, 0, st>>>(img, w, h, d_box.p); count_launch();
     response_kernel<<<grd, blk, 0, st>>>(d_box.p, w, h, d_resp.p, d_max.p); count_launch();

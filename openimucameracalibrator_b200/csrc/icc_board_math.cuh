@@ -32,17 +32,19 @@ ICC_HD void resize_coeff(int d, double scale, int ssize, bool clamp_hi, int& s, 
   w1 = (int)rintf(fx * 2048.f);
 }
 
-ICC_HD uint8_t resize_pixel(const uint8_t* src, int64_t pitch, int sw, int sh, double f, int dx, int dy) {
+// one channel of pixels STEP bytes apart (1: gray; 3: one channel of interleaved B, G, R, src pointing at that channel's first byte)
+template <int STEP>
+ICC_HD uint8_t resize_channel(const uint8_t* src, int64_t pitch, int sw, int sh, double f, int dx, int dy) {
   const double scale = resize_scale(f);
   if (scale == 2.0) {
     const int sx = 2 * dx, sy = 2 * dy;
     if (sx + 1 < sw && sy + 1 < sh) {
-      const uint8_t* r0 = src + (int64_t)sy * pitch + sx;
-      return (uint8_t)((r0[0] + r0[1] + r0[pitch] + r0[pitch + 1] + 2) >> 2);
+      const uint8_t* r0 = src + (int64_t)sy * pitch + (int64_t)sx * STEP;
+      return (uint8_t)((r0[0] + r0[STEP] + r0[pitch] + r0[pitch + STEP] + 2) >> 2);
     }
     int sum = 0, cnt = 0;   // resizeAreaFast_'s border: the mean of the block's pixels inside the image
     for (int y = sy; y < sy + 2 && y < sh; ++y)
-      for (int x = sx; x < sx + 2 && x < sw; ++x) { sum += src[(int64_t)y * pitch + x]; ++cnt; }
+      for (int x = sx; x < sx + 2 && x < sw; ++x) { sum += src[(int64_t)y * pitch + (int64_t)x * STEP]; ++cnt; }
     return (uint8_t)min(255, max(0, (int)rintf((float)sum / (float)cnt)));
   }
   int sx, a0, a1, sy, b0, b1;
@@ -51,8 +53,26 @@ ICC_HD uint8_t resize_pixel(const uint8_t* src, int64_t pitch, int sw, int sh, d
   const int sx1 = min(sx + 1, sw - 1), y0 = min(max(sy, 0), sh - 1), y1 = min(max(sy + 1, 0), sh - 1);
   const uint8_t* r0 = src + (int64_t)y0 * pitch;
   const uint8_t* r1 = src + (int64_t)y1 * pitch;
-  const int S0 = r0[sx] * a0 + r0[sx1] * a1, S1 = r1[sx] * a0 + r1[sx1] * a1;
+  const int S0 = r0[sx * STEP] * a0 + r0[sx1 * STEP] * a1, S1 = r1[sx * STEP] * a0 + r1[sx1 * STEP] * a1;
   return (uint8_t)((((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2);
+}
+
+ICC_HD uint8_t resize_pixel(const uint8_t* src, int64_t pitch, int sw, int sh, double f, int dx, int dy) {
+  return resize_channel<1>(src, pitch, sw, sh, f, dx, dy);
+}
+
+// ---- colour frames: cv::resize on the BGR image, then cv::cvtColor(BGR2GRAY) ----------------------------------------------------
+// The reference resizes the colour image and converts afterwards (BoardExtractor::ExtractImageFolderToJson), which is not the same
+// image as converting first.  OpenCV's 8UC3 resize is three independent single-channel resizes.  OpenCV 4.13's 8-bit BGR2GRAY is the
+// 15-bit fixed-point rule (B 3735 + G 19235 + R 9798 + 2^14) >> 15 (with or without IPP); the often-quoted 14-bit weights
+// 1868 / 9617 / 4899 differ on about 0.26 % of pixels.  B = G = R = v gives v exactly, so a gray image converts to itself.
+ICC_HD uint8_t bgr_to_gray(int b, int g, int r) { return (uint8_t)((b * 3735 + g * 19235 + r * 9798 + 16384) >> 15); }
+
+// output pixel (dx, dy) of cvtColor(resize(bgr, 1/f), BGR2GRAY); pitch in bytes (>= 3 sw); at f = 1 only the conversion
+ICC_HD uint8_t bgr_resize_gray_pixel(const uint8_t* bgr, int64_t pitch, int sw, int sh, double f, int dx, int dy) {
+  if (f == 1.0) { const uint8_t* p = bgr + (int64_t)dy * pitch + 3 * (int64_t)dx; return bgr_to_gray(p[0], p[1], p[2]); }
+  return bgr_to_gray(resize_channel<3>(bgr, pitch, sw, sh, f, dx, dy), resize_channel<3>(bgr + 1, pitch, sw, sh, f, dx, dy),
+                     resize_channel<3>(bgr + 2, pitch, sw, sh, f, dx, dy));
 }
 
 // ---- corner response: a localized Radon transform on a 3x3 box mean (Duda & Frese, BMVC 2018) -------------------------------------

@@ -166,8 +166,18 @@ inline void print_camera(std::ostream& os, const CameraLayout& c, const double* 
 }
 
 // Corner file (src/core/board_extractor.cc:294-296,325-333,375-380): scene_pts {"id": [x,y,z]} -> homogeneous board points by id.
+// The reference writes the radon board's points with an integer index, so there scene_pts is an array [[x,y,z], ...] whose index is the
+// id; read_scene.cc iterates items(), which takes either form, and so does this.
 inline std::vector<double> read_scene_points(const Value& scene_json, int& n_points) {
   const Value& pts = scene_json.at("scene_pts");
+  if (pts.is_array()) {
+    const int n = (int)pts.size();
+    std::vector<double> board(4 * (size_t)n, 0.0);
+    for (int id = 0; id < n; ++id) { for (int d = 0; d < 3; ++d) board[4 * id + d] = pts.at(id).at(d).num(); board[4 * id + 3] = 1.0; }
+    n_points = n;
+    return board;
+  }
+  if (!pts.is_object()) throw std::runtime_error("scene_pts must be an object or an array");
   int max_id = -1; for (const auto& kv : *pts.o) max_id = std::max(max_id, std::stoi(kv.first));
   std::vector<double> board(4 * (size_t)(max_id + 1), 0.0);
   for (int i = 0; i <= max_id; ++i) board[4 * i + 3] = 1.0;

@@ -123,7 +123,8 @@ namespace allan { struct Curves; }   // icc_allan_math.cuh
 void default_allan_options(icc_allan_options* o);
 icc_status allan_variance(cudaStream_t st, int n, const double* t, const double* acc, const double* gyr, const icc_allan_options& o,
                           double params[30], icc_allan_noise noise[6], icc_allan_summary summary[6], allan::Curves& curves, std::string& err);
-icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, int W, int H,
+// bgr: rows hold width interleaved B, G, R bytes (icc_extract_radon_board_bgr); else width gray bytes
+icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, bool bgr, int W, int H,
                                double f, double* uv_out, int32_t* found, icc_board_summary& S, std::string& err);
 
 }  // namespace icc

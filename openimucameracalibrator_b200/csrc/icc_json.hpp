@@ -244,4 +244,33 @@ class UbjsonParser {
 };
 inline Value load_ubjson(const std::string& path) { const std::string d = read_file(path, true); return UbjsonParser(d).parse(); }
 
+// nlohmann::json::to_ubjson(j) with its defaults (no count or type optimisation): keys in std::map order, every floating-point number as
+// 'D' (big-endian double), every integer in the smallest of i, U, I, l, L that holds it, strings and keys with such a length prefix.
+class UbjsonWriter {
+ public:
+  static std::string dump(const Value& v) { std::string s; write(s, v); return s; }
+  static void write(std::string& out, const Value& v) {
+    switch (v.type) {
+      case Value::Null: out += 'Z'; break;
+      case Value::Bool: out += v.b ? 'T' : 'F'; break;
+      case Value::Int: integer(out, v.i); break;
+      case Value::Float: out += 'D'; be(out, v.d); break;
+      case Value::String: out += 'S'; string(out, *v.sp); break;
+      case Value::Arr: out += '['; for (const Value& e : *v.a) write(out, e); out += ']'; break;
+      case Value::Obj: out += '{'; for (const auto& kv : *v.o) { string(out, kv.first); write(out, kv.second); } out += '}'; break;
+    }
+  }
+ private:
+  template <class T> static void be(std::string& out, T v) { unsigned char b[sizeof(T)]; memcpy(b, &v, sizeof(T)); for (size_t k = 0; k < sizeof(T); ++k) out += (char)b[sizeof(T) - 1 - k]; }
+  static void integer(std::string& out, int64_t n) {
+    if (n >= INT8_MIN && n <= INT8_MAX) { out += 'i'; be(out, (int8_t)n); }
+    else if (n >= 0 && n <= UINT8_MAX) { out += 'U'; be(out, (uint8_t)n); }
+    else if (n >= INT16_MIN && n <= INT16_MAX) { out += 'I'; be(out, (int16_t)n); }
+    else if (n >= INT32_MIN && n <= INT32_MAX) { out += 'l'; be(out, (int32_t)n); }
+    else { out += 'L'; be(out, n); }
+  }
+  static void string(std::string& out, const std::string& s) { integer(out, (int64_t)s.size()); out += s; }
+};
+inline std::string dump_ubjson(const Value& v) { return UbjsonWriter::dump(v); }
+
 }  // namespace iccjson
