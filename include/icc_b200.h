@@ -660,6 +660,39 @@ icc_status icc_extract_radon_board(icc_handle* h, int n_frames, int width, int h
 icc_status icc_extract_radon_board_bgr(icc_handle* h, int n_frames, int width, int height, int64_t pitch_bytes, const uint8_t* frames_bgr, int corners_x,
                                        int corners_y, double downsample_factor, double* uv_out /* n_frames * corners_x * corners_y * 2 */,
                                        int32_t* found /* n_frames */, icc_board_summary* summary /* nullable */);
+/* ---- upstream: Kalibr AprilGrid corners (extract_board_to_json --board_type apriltag) ------------------------------------------------
+ * BoardExtractor::ExtractBoard for BoardType::APRILTAG (src/core/board_extractor.cc): cv::resize(frame, 1/f, INTER_LINEAR), then the
+ * Kalibr/Basalt wrapper ApriltagDetector::detectTags (third_party/apriltag/apriltag.cpp) on tag36h11 with a 2-bit black border.  The board
+ * has tags_x x tags_y tags; tag t = tags_x y + x has its corners i = 0..3 (bottom-left, bottom-right, top-right, top-left with the
+ * board's y up) at point id (t << 2) + i.  frames: n_frames 8-bit gray images as for icc_extract_radon_board (host or device memory).
+ * Per frame and point id (n_frames x 4 tags_x tags_y): uv_out (x, y) in the downsampled image's pixels and status_out 1 (kept),
+ * 0 (not seen; uv NaN) or -1 (seen, but cornerSubPix moved it further than the wrapper's radius; uv is where it moved to).
+ * found[k] = 1 iff frame k gives a view: it has >= 4 tags left after the wrapper's rules, in this order: a corner within 4 px of the
+ * border, a Hamming distance > 1, an id >= 36 (the wrapper's limit whatever the board size), and no id appears twice.  A tag with an
+ * id the board does not have (tags_x tags_y <= id < 36) counts for those rules but has no point ids.  Frames that are not found have
+ * every status 0.  ICC_ERR_INVALID_ARGUMENT, with nothing launched: tags_x or tags_y outside 1..64, a factor < 1 or not finite,
+ * pitch < width, a NULL frame or output pointer. */
+typedef struct icc_aprilgrid_summary {
+  int32_t width, height;             /* the downsampled frame size */
+  int32_t n_found;                   /* frames with a view */
+  int32_t n_few_tags;                /* frames with fewer than 4 tags after the tag rules */
+  int32_t n_duplicate;               /* frames dropped because an id appeared twice */
+  int32_t n_quads;                   /* dark components examined, summed over the frames */
+  int32_t n_not_decoded;             /* quads whose 36 bits were not all inside the image */
+  int32_t n_border;                  /* decoded tags dropped: a corner within 4 px of the border */
+  int32_t n_not_good;                /* decoded tags dropped: Hamming distance > 1 (most quads that are not tags) */
+  int32_t n_id_range;                /* decoded tags dropped: id >= 36 */
+  int32_t n_corners_kept;            /* status 1 */
+  int32_t n_corners_moved;           /* status -1 */
+  int64_t quad_overflow;             /* components dropped because a frame's 1024 quad slots were full */
+  int32_t gpu_launches;
+  int32_t reserved;
+  double seconds;                    /* host wall clock of the call */
+} icc_aprilgrid_summary;
+icc_status icc_extract_aprilgrid(icc_handle* h, int n_frames, int width, int height, int64_t pitch_bytes, const uint8_t* frames, int tags_x, int tags_y,
+                                 double downsample_factor, double* uv_out /* n_frames * 4 tags_x tags_y * 2 */,
+                                 int32_t* status_out /* n_frames * 4 tags_x tags_y */, int32_t* found /* n_frames */,
+                                 icc_aprilgrid_summary* summary /* nullable */);
 /* Page-locked host memory (cudaHostAlloc) for frames that a host program fills and hands to the extraction entries; *p = NULL for 0 bytes.
  * ICC_ERR_NO_DEVICE without a GPU, ICC_ERR_CUDA when the allocation fails.  Free with icc_host_free_pinned (NULL is accepted). */
 icc_status icc_host_alloc_pinned(uint64_t bytes, void** p);

@@ -160,6 +160,17 @@ class BoardSummary(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
 
 
+class AprilGridSummary(C.Structure):
+    """icc_aprilgrid_summary (include/icc_b200.h): what one icc_extract_aprilgrid call did."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n_found", C.c_int32), ("n_few_tags", C.c_int32), ("n_duplicate", C.c_int32),
+                ("n_quads", C.c_int32), ("n_not_decoded", C.c_int32), ("n_border", C.c_int32), ("n_not_good", C.c_int32), ("n_id_range", C.c_int32),
+                ("n_corners_kept", C.c_int32), ("n_corners_moved", C.c_int32), ("quad_overflow", C.c_int64), ("gpu_launches", C.c_int32),
+                ("reserved", C.c_int32), ("seconds", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 def _frames_pointer(frames):
     """(pointer, n, height, width, pitch in bytes) of 8-bit frames: an (N, H, W) or (H, W) uint8 NumPy array, or a torch CUDA tensor,
     whose rows are contiguous and whose frames are `height` rows of one pitch apart."""
@@ -489,6 +500,21 @@ class CApi:
                                                C.POINTER(BoardSummary)], n, w, h, pitch, C.c_void_p(ptr), int(corners_x), int(corners_y),
                    float(downsample_factor), _dp(uv), found.ctypes.data_as(c_int32_p), C.byref(s))
         return uv, found.astype(bool), s.as_dict()
+
+    # ---- upstream: Kalibr AprilGrid corners (src/core/board_extractor.cc, BoardType::APRILTAG) -----------------------------------
+    def extract_aprilgrid(self, frames, tags_x=6, tags_y=6, downsample_factor=1.0):
+        """-> (uv (N, 4 tags_x tags_y, 2) per point id (t << 2) + i, NaN where not seen, status (N, 4 tags_x tags_y) int32: 1 kept,
+        0 not seen, -1 moved too far by the refinement, found (N,) bool, summary dict).  frames as for extract_radon_board."""
+        ptr, n, h, w, pitch = _frames_pointer(frames)
+        n_pts = 4 * int(tags_x) * int(tags_y)
+        uv = np.full((n, n_pts, 2), np.nan)
+        status = np.zeros((n, n_pts), dtype=np.int32)
+        found = np.zeros(n, dtype=np.int32)
+        s = AprilGridSummary()
+        self._call("extract_aprilgrid", [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_double, c_double_p, c_int32_p,
+                                         c_int32_p, C.POINTER(AprilGridSummary)], n, w, h, pitch, C.c_void_p(ptr), int(tags_x), int(tags_y),
+                   float(downsample_factor), _dp(uv), status.ctypes.data_as(c_int32_p), found.ctypes.data_as(c_int32_p), C.byref(s))
+        return uv, status, found.astype(bool), s.as_dict()
 
     # ---- upstream row f2: spline error weighting (python/sew.py:knot_spacing_and_variance) ------------------------------------
     def spline_error_weighting(self, times_s, signal_xyz, quality, min_dt=0.0, max_dt=0.0, want_spectrum=False):

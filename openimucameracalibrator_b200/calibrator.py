@@ -369,3 +369,43 @@ class BoardExtractor:
         with open(path, "wb") as f:
             f.write(ubjson_dumps(scene))
         return scene
+
+
+class AprilGridExtractor(BoardExtractor):
+    """BoardExtractor for BoardType::APRILTAG (src/core/board_extractor.cc) on the GPU: InitializeAprilBoard(tag_size_m, 0.3, tags_x,
+    tags_y), then frames -> the corner file's scene dictionary.  A view holds only the kept corners (status 1) of its frame; frames
+    without a view (fewer than 4 tags, or a duplicate id) are left out.  write() is BoardExtractor's."""
+
+    def __init__(self, tag_size_m: float, tags_x: int = 6, tags_y: int = 6, device: int = 0):
+        self.tag_size_m, self.tags_x, self.tags_y = float(tag_size_m), int(tags_x), int(tags_y)
+        self.api = CApi(load_library(), "icc_", device)
+
+    def scene_points(self) -> dict:
+        """str((t << 2) + i) -> the corner as cv::Point3f: tag t = tags_x y + x, corner i at (1.3 s x + {0, s, s, 0}[i],
+        1.3 s y + {0, 0, s, s}[i], 0), each coordinate rounded to float32 as the reference stores it."""
+        import numpy as np
+        s, nx = self.tag_size_m, self.tags_x
+        out = {}
+        for t in range(nx * self.tags_y):
+            x, y = t % nx, t // nx
+            for i in range(4):
+                p = np.array([x * s * 1.3 + (0.0, s, s, 0.0)[i], y * s * 1.3 + (0.0, 0.0, s, s)[i], 0.0], dtype=np.float32)
+                out[str((t << 2) + i)] = [float(v) for v in p]
+        return out
+
+    def extract(self, frames, timestamps_s, downsample_factor: float = 1.0) -> dict:
+        import numpy as np
+        from .io_formats import view_key
+        uv, status, found, summary = self.api.extract_aprilgrid(frames, self.tags_x, self.tags_y, downsample_factor)
+        views = {}
+        for k, t in enumerate(timestamps_s):
+            if found[k]:
+                ids = [int(c) for c in range(status.shape[1]) if status[k, c] == 1]
+                views[view_key(float(t))] = {"image_points": {str(c): [float(uv[k, c, 0]), float(uv[k, c, 1])] for c in ids}}
+        self.summary = summary
+        scene = {"calibration_board_type": 2, "square_size_meter": self.tag_size_m, "image_width": int(summary["width"]),
+                 "image_height": int(summary["height"]), "scene_pts": self.scene_points(), "views": views}
+        t = np.asarray(timestamps_s, dtype=np.float64)
+        if t.size >= 3:   # the reference's camera_fps: 1 / the median frame interval, the last interval left out
+            scene["camera_fps"] = float(1.0 / np.median(np.diff(t)[:-1]))
+        return scene

@@ -1959,6 +1959,29 @@ icc_status icc_extract_radon_board_bgr(icc_handle* h, int n_frames, int width, i
   return extract_radon(h, "icc_extract_radon_board_bgr", true, n_frames, width, height, pitch, frames_bgr, corners_x, corners_y, f, uv_out, found, summary);
 }
 
+// ---- upstream: Kalibr AprilGrid corners (icc_aprilgrid.cu) ------------------------------------------------------------------------------
+icc_status icc_extract_aprilgrid(icc_handle* h, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, int tags_x, int tags_y,
+                                 double f, double* uv_out, int32_t* status_out, int32_t* found, icc_aprilgrid_summary* summary) {
+  if (!h) return ICC_ERR_INVALID_ARGUMENT;
+  if (n_frames < 0 || width < 1 || height < 1 || pitch < width || tags_x < 1 || tags_y < 1 || tags_x > 64 || tags_y > 64 || !(f >= 1.0) || !std::isfinite(f) ||
+      (n_frames > 0 && (!frames || !uv_out || !status_out || !found)))
+    return fail(h, ICC_ERR_INVALID_ARGUMENT, "icc_extract_aprilgrid needs tags_x, tags_y in 1..64, a finite downsample factor >= 1, pitch >= width "
+                                             "and non-NULL frames and outputs");
+  NEED_DEVICE();
+  icc_aprilgrid_summary S;
+  memset(&S, 0, sizeof S);
+  if (n_frames == 0) { if (summary) *summary = S; return ICC_OK; }
+  cudaPointerAttributes at;
+  bool on_device = false;
+  if (cudaPointerGetAttributes(&at, frames) == cudaSuccess) on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  else cudaGetLastError();
+  const icc_status rc = drive(h, [&](std::string& err) {
+    return extract_aprilgrid(h->stream, n_frames, width, height, pitch, frames, on_device, tags_x, tags_y, f, uv_out, status_out, found, S, err);
+  });
+  if (rc == ICC_OK && summary) *summary = S;
+  return rc;
+}
+
 icc_status icc_host_alloc_pinned(uint64_t bytes, void** p) {
   if (!p) return ICC_ERR_INVALID_ARGUMENT;
   *p = nullptr;

@@ -127,4 +127,7 @@ icc_status allan_variance(cudaStream_t st, int n, const double* t, const double*
 icc_status extract_radon_board(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, bool bgr, int W, int H,
                                double f, double* uv_out, int32_t* found, icc_board_summary& S, std::string& err);
 
+// 8-bit gray frames; uv_out / status_out per frame and point id (icc_extract_aprilgrid)
+icc_status extract_aprilgrid(cudaStream_t st, int n_frames, int width, int height, int64_t pitch, const uint8_t* frames, bool frames_on_device, int tags_x, int tags_y,
+                             double f, double* uv_out, int32_t* status_out, int32_t* found, icc_aprilgrid_summary& S, std::string& err);
 }  // namespace icc

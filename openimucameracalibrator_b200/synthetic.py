@@ -8,6 +8,7 @@ writers in `io_formats.py`.
 """
 from __future__ import annotations
 
+import os
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -472,3 +473,88 @@ def camera_rays(model: int, intr, size, supersample: int = 4):
         _RAYS.clear()
         _RAYS[key] = unproject_grid(model, intr, np.stack([uu, vv], -1))
     return _RAYS[key]
+
+
+# ---- Kalibr AprilGrid (BoardType::APRILTAG) ------------------------------------------------------------------------------------------
+# tags_x x tags_y tag36h11 tags of side s, spacing 0.3 s: tag t = tags_x y + x has its lower-left corner at (1.3 s x, 1.3 s y) in the
+# board frame (x right, y up the printed sheet, z out of it), and a black square of side 0.3 s fills every gap crossing, the outer
+# ones included (Kalibr's corner squares, which make every tag corner an X-junction).
+def tag36h11_codes():
+    """The 587 codes of csrc/icc_tag36h11.h (the codebook the GPU decoder uses)."""
+    import re
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc", "icc_tag36h11.h")
+    return np.array([int(x, 16) for x in re.findall(r"0x([0-9a-f]+)ull", open(path).read())], dtype=np.uint64)
+
+
+def aprilgrid_board_points(tags_x: int, tags_y: int, tag_m: float):
+    """(4 tags_x tags_y, 3) board points in point-id order (t << 2) + i, i = bottom-left, bottom-right, top-right, top-left."""
+    i = np.arange(4 * tags_x * tags_y)
+    t, c = i >> 2, i & 3
+    x = (t % tags_x) * tag_m * 1.3 + np.array([0.0, tag_m, tag_m, 0.0])[c]
+    y = (t // tags_x) * tag_m * 1.3 + np.array([0.0, 0.0, tag_m, tag_m])[c]
+    return np.stack([x, y, np.zeros_like(x)], -1)
+
+
+def aprilgrid_shade(xb, yb, tags_x: int, tags_y: int, tag_m: float, tag_ids=None, codes=None):
+    """Reflectance in [0, 1] (0 black) at board-frame points.  tag_ids[t] is the id drawn at position t (default t).  A code's first
+    (most significant) bit is the top-left data cell with the board's y up; 1 is white."""
+    codes = tag36h11_codes() if codes is None else codes
+    ids = np.arange(tags_x * tags_y) if tag_ids is None else np.asarray(tag_ids)
+    pitch = 1.3 * tag_m
+    tx, ty = np.floor(xb / pitch), np.floor(yb / pitch)
+    fx, fy = (xb - tx * pitch) / tag_m, (yb - ty * pitch) / tag_m
+    in_x, in_y = (tx >= 0) & (tx < tags_x), (ty >= 0) & (ty < tags_y)
+    tag = in_x & in_y & (fx < 1) & (fy < 1)
+    crossing = (tx >= -1) & (tx < tags_x) & (ty >= -1) & (ty < tags_y) & (fx >= 1) & (fy >= 1)
+    cx = np.clip(np.floor(fx * 10), 0, 9).astype(np.int64)
+    cy = 9 - np.clip(np.floor(fy * 10), 0, 9).astype(np.int64)          # cell row from the tag's top
+    data = tag & (cx >= 2) & (cx <= 7) & (cy >= 2) & (cy <= 7)
+    t = (np.clip(ty, 0, tags_y - 1) * tags_x + np.clip(tx, 0, tags_x - 1)).astype(np.int64)
+    code = codes[ids[t]]
+    k = ((cy - 2) * 6 + (cx - 2)).clip(0, 35)
+    bit = (code >> (35 - k).astype(np.uint64)) & np.uint64(1)
+    white = ~(tag | crossing) | (data & (bit == 1))
+    return np.where(white, 1.0, 0.0)
+
+
+def aprilgrid_view_pose(tags_x: int, tags_y: int, tag_m: float, distance_m: float, tilt_deg: float = 0.0, tilt_axis_deg: float = 0.0,
+                        roll_deg: float = 0.0, offset_m=(0.0, 0.0)):
+    """(R_cb, t_cb) of a camera `distance_m` in front of the grid's centre: the sheet upright (board y up the image) at roll 0,
+    tilted by `tilt_deg` about an in-plane axis at `tilt_axis_deg`, rolled about the optical axis, and the board shifted by `offset_m`."""
+    a = np.deg2rad(tilt_axis_deg)
+    tilt = so3_exp(np.deg2rad(tilt_deg) * np.array([np.cos(a), np.sin(a), 0.0]))
+    roll = so3_exp(np.array([0.0, 0.0, np.deg2rad(roll_deg)]))
+    R_cb = roll @ tilt @ np.diag([1.0, -1.0, -1.0])
+    centre = np.array([(tags_x * 1.3 - 0.3) * tag_m / 2, (tags_y * 1.3 - 0.3) * tag_m / 2, 0.0])
+    t_cb = np.array([offset_m[0], offset_m[1], distance_m]) - R_cb @ centre
+    return R_cb, t_cb
+
+
+def render_aprilgrid(model: int, intr, size, R_cb, t_cb, tags_x: int = 6, tags_y: int = 6, tag_m: float = 0.04, supersample: int = 4,
+                     blur_sigma_px: float = 0.0, noise_sigma_dn: float = 0.0, seed: int = 0, black_dn: float = 30.0, white_dn: float = 220.0,
+                     tag_ids=None, rays=None):
+    """uint8 (height, width) image of the AprilGrid seen by the camera (model, intr) at board-to-camera pose (R_cb, t_cb), by the
+    supersampled ray casting of render_radon_board; optional Gaussian blur and noise.  Returns (image, truth uv (4 tags_x tags_y, 2)
+    in point-id order, truth valid)."""
+    width, height = size
+    if rays is None:
+        rays = camera_rays(model, intr, size, supersample)
+    d, ok = rays
+    R_cb, t_cb = np.asarray(R_cb, float), np.asarray(t_cb, float)
+    n = R_cb[:, 2]
+    lam = (n @ t_cb) / (d @ n)
+    pb = (lam[..., None] * d - t_cb) @ R_cb
+    hit = ok & (lam > 0)
+    shade = np.where(hit, aprilgrid_shade(pb[..., 0], pb[..., 1], tags_x, tags_y, tag_m, tag_ids), 1.0)
+    img = shade.reshape(height, supersample, width, supersample).mean(axis=(1, 3))
+    img = black_dn + (white_dn - black_dn) * img
+    if blur_sigma_px > 0:
+        from scipy.ndimage import gaussian_filter
+        img = gaussian_filter(img, blur_sigma_px, mode="nearest")
+    if noise_sigma_dn > 0:
+        img = img + np.random.default_rng(seed).normal(0.0, noise_sigma_dn, img.shape)
+    img = np.clip(np.rint(img), 0, 255).astype(np.uint8)
+    pc = aprilgrid_board_points(tags_x, tags_y, tag_m) @ R_cb.T + t_cb
+    uv, valid = cm.project(model, intr, pc)
+    valid = valid & (pc[:, 2] > 0) & (uv[:, 0] >= 0) & (uv[:, 0] <= width - 1) & (uv[:, 1] >= 0) & (uv[:, 1] <= height - 1)
+    return img, uv, valid
